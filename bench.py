@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the OccDepth forward hot path (BASELINE.json metric: forward voxels/sec).
 
-  python bench.py --gpus N --steps K --warmup W            # B200 arm (one process per GPU under torchrun)
+  python bench.py --gpus N --steps K --warmup W            # GPU arm (one process per GPU under torchrun)
   python bench.py --impl reference --steps K --warmup W    # the reference algorithm on the host CPU cores
 
 Workload (BASELINE.json configs[1]): synthetic 1370x376 stereo pair, tf_efficientnet_b7_ns 2D backbone,
@@ -19,6 +19,10 @@ metric with pinned host inputs copied H2D and the logits read back D2H inside th
 occdepth_b200.serving.FramePipeline (copies on their own streams, double-buffered); the back-to-back figure is listed
 beside it.  Prints ONE JSON line (rank 0) on the original stdout; everything else this process or its libraries print
 goes to stderr.
+
+--dump-outputs DIR writes what the timed forward returned in its last step as DIR/<key>.npy (float32): arrays of up to
+1 Mi elements whole, larger ones as a fixed seeded sample of 1 Mi elements (DIR/<key>.sample_index.npy holds the flat
+int32 indices); under 64 MB in all for this workload.  The inputs depend on the arguments only, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -37,8 +41,8 @@ N_OUT = FULL[0] * FULL[1] * FULL[2]
 PROJECT_RES = ["1", "2", "4", "8"]
 WORKLOAD = ("configs[1]: 1370x376 stereo, tf_efficientnet_b7_ns, flosp lift to 128x128x16/64ch, "
             "UNet3D+CRP+cascade head -> 256x256x32x20 logits, B=1 per GPU")
-# stated parity of the two arithmetic modes vs the CPU fp32 oracle at this configuration (tests/test_gpu_config2.py,
-# profiles/r02_config2_parity_*.json): max-abs logit diff relative to max |logit|, arg-max agreement
+# stated parity of the two arithmetic modes vs the CPU fp32 oracle at this configuration (tests/test_gpu_config2.py):
+# max-abs logit diff relative to max |logit|, arg-max agreement
 TOLERANCE = {"tf32": {"rel": 1.5e-3, "argmax": 0.9984}, "bf16": {"rel": 1.4e-2, "argmax": 0.984}}
 
 
@@ -148,8 +152,8 @@ def oracle_inputs(device=None):
 
 
 def host_cores():
-    """physical cores of the host (one oneDNN thread per hyper-thread pair: 128 threads on the 64-core B200 hosts run
-    the forward 15x SLOWER than 64, measured); torchrun's OMP_NUM_THREADS=1 is overridden on purpose"""
+    """physical cores of the host (one oneDNN thread per hyper-thread pair: one thread per logical core oversubscribes
+    the cores); torchrun's OMP_NUM_THREADS=1 is overridden on purpose"""
     try:
         import psutil
         n = psutil.cpu_count(logical=False)
@@ -161,7 +165,7 @@ def host_cores():
 
 
 def cpu_forward_seconds(steps=1, warmup=0):
-    """the reference algorithm (oracle/functional.py, pinned against /root/reference) on ALL host cores.
+    """the reference algorithm (oracle/functional.py, pinned against the original project) on ALL host cores.
     torchrun exports OMP_NUM_THREADS=1: the thread count is set explicitly."""
     import torch
     from oracle import functional as OF      # bench.py executes oracle/ code only in the baseline legs
@@ -233,8 +237,8 @@ def eager_cuda_baseline(dev, steps=3):
 
 
 def tf32_matmul_peak(dev, seconds=2.0):
-    """TF32 tensor-core roofline denominator, measured the way MEASURED_PEAKS.json measures bf16 (the driver file has
-    no TF32 entry): torch.matmul fp32 with allow_tf32, 8192^3, best of 10 (burst) and back to back (sustained)."""
+    """TF32 tensor-core roofline denominator, measured on this GPU: torch.matmul fp32 with allow_tf32, 8192^3, best of
+    10 (burst) and back to back (sustained)."""
     import torch
     old = torch.backends.cuda.matmul.allow_tf32
     torch.backends.cuda.matmul.allow_tf32 = True
@@ -266,6 +270,32 @@ def tf32_matmul_peak(dev, seconds=2.0):
         return {"burst": best, "sustained": iters * 2 * n ** 3 / (e0.elapsed_time(e1) * 1e-3) / 1e12}
     finally:
         torch.backends.cuda.matmul.allow_tf32 = old
+
+
+DUMP_SAMPLE = 1 << 20
+
+
+def dump_outputs(out, directory):
+    """the arrays the timed path returned (dict of tensors) -> DIR/<key>.npy, float32; arrays above DUMP_SAMPLE
+    elements as a fixed seeded sample (<key>.sample_index.npy: the flat indices), at most 64 MB in all"""
+    import numpy as np
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    for k in sorted(out):
+        v = out[k]
+        if not torch.is_tensor(v) or not v.is_floating_point():
+            continue
+        a = v.detach().float().cpu().reshape(-1)
+        if a.numel() > DUMP_SAMPLE:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(1234))[:DUMP_SAMPLE].sort().values
+            np.save(os.path.join(directory, k + ".sample_index.npy"), idx.to(torch.int32).numpy())
+            a = a[idx]
+            dump_outputs.sampled.append(k)
+        np.save(os.path.join(directory, k + ".npy"), a.numpy() if v.numel() > DUMP_SAMPLE else
+                v.detach().float().cpu().numpy())
+
+
+dump_outputs.sampled = []
 
 
 def time_forwards(m, batch, steps, barrier, dev):
@@ -318,9 +348,8 @@ def run_b200(args):
 
     # The K-step timed region (barrier + synchronize on both sides, CUDA events, max over ranks) is run REPS times and
     # the fastest repetition is reported; every repetition is listed in the JSON line.  Reason: on a fresh box the
-    # first process sees one 35-240 ms stall of the whole GPU somewhere in its first seconds of work, with or without
-    # this script's own NVML sampler and however long the warm-up is (profiles/r02f_bench_first_process.json,
-    # r02g: one step of 46-88 ms among steps of 13.9 ms) -- an event outside this process.
+    # first process can see a stall of the whole GPU somewhere in its first seconds of work, an event outside this
+    # process that one repetition absorbs.
     REPS = 3
     reps = []
     for _ in range(REPS):
@@ -328,6 +357,9 @@ def run_b200(args):
         reps.append((ms_r, dict(time_forwards.last_steps)))
     ms_total, step_spread = min(reps, key=lambda r: r[0])   # rank 0's per-step device times of that repetition
     step_spread["timed_region_repetitions_ms_per_step"] = [r[0] / args.steps for r in reps]
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        dump_outputs(out, args.dump_outputs)
 
     # ---- end-to-end arm: host buffers, H2D of the inputs and D2H of the logits inside the timed region ----
     img_h, pix_h, fov_h = img.pin_memory(), pix.pin_memory(), fov.pin_memory()
@@ -491,22 +523,17 @@ def run_b200(args):
         conv_fl = sum(f for n, t, f in prof if f > 0)
         lift_ms = sum(t for n, t, f in prof if n == "sfa_lift")
         tot_ms = sum(t for n, t, f in prof)
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:  # noqa: BLE001
-            pass
-        src = "measured" if peaks else "fallback"
-        hpeak = peaks.get("hbm_gbs", 6650.0)
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- denominators, not reached figures
+        src = "H100 SXM data sheet"
+        hpeak = 3350.0
         if prec == "tf32":
             tp = tf32_matmul_peak(dev)
             tpeak = tp["sustained"]
-            tsrc = ("measured in this run (torch.matmul fp32, allow_tf32, 8192^3: sustained %.0f / burst %.0f TFLOP/s; "
-                    "MEASURED_PEAKS.json has no TF32 entry, its bf16 sustained figure is %.0f)"
-                    % (tp["sustained"], tp["burst"], peaks.get("bf16_tflops_sustained", float("nan"))))
+            tsrc = ("measured in this run (torch.matmul fp32, allow_tf32, 8192^3: sustained %.0f / burst %.0f TFLOP/s)"
+                    % (tp["sustained"], tp["burst"]))
         else:
-            tpeak = peaks.get("bf16_tflops_sustained", 1400.0)
-            tsrc = src + " bf16_tflops_sustained"
+            tpeak = 989.0
+            tsrc = src + " dense bf16"
         esize = 4 if prec == "tf32" else 2
         # lift algorithmic bytes (SURVEY 8d formula with the element size actually moved)
         import synthetic as synth
@@ -522,11 +549,6 @@ def run_b200(args):
         ach_h = lift_bytes / (lift_ms * 1e-3) / 1e9 if lift_ms > 0 else 0.0
         frames = 1 if slab_only else world
         value = frames * N_OUT * args.steps / (ms_total * 1e-3)
-        ncu = {}
-        try:
-            ncu = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(prec, {})
-        except Exception:  # noqa: BLE001
-            pass
         line = {
             "metric": "forward voxels/sec", "value": value, "unit": "voxels/s", "n_gpus": world,
             "steps": args.steps, "warmup": warm, "ms_per_step": ms_total / args.steps,
@@ -534,11 +556,11 @@ def run_b200(args):
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "frames_per_step": frames,
                        "partition": "x-slab of one frame + NCCL halo exchange" if slab_only else "frame replicas",
-                       "precision": {"mode": prec, "operands": "TF32 (tcgen05 kind::tf32)" if prec == "tf32" else "bf16 (tcgen05 kind::f16)",
-                                     "accumulate": "fp32 (TMEM)", "activations": "fp32 holding TF32 values" if prec == "tf32" else "bf16",
+                       "precision": {"mode": prec, "operands": "TF32 (wgmma .tf32)" if prec == "tf32" else "bf16 (wgmma .bf16)",
+                                     "accumulate": "fp32 (registers)", "activations": "fp32 holding TF32 values" if prec == "tf32" else "bf16",
                                      "stated_tolerance_vs_fp32_oracle": TOLERANCE[prec],
                                      "backbone_parity": "EfficientNet oracle pinned vs torchvision, unpinned vs geffnet (un-vendored)"},
-                       "l2": "per-step working set (weights + activations, >2 GB) exceeds the 126 MB L2; no flush",
+                       "l2": "per-step working set (weights + activations, >2 GB) exceeds the 50 MB L2; no flush",
                        "timing": "K steps between barrier + synchronize, CUDA events, max over ranks; the region is "
                                  "run 3 times and the fastest is reported (all three in step_ms)",
                        "cuda_graph": os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1"},
@@ -563,18 +585,17 @@ def run_b200(args):
                             if ms_cls != float("inf") and ms_cls > 0 else {"error": cls_err}),
             "gpu_launches": n_ops * args.steps,
             "clocks": sampler.summary(),
-            "roofline": {"kernel": "conv_tc_kernel + conv_halo_kernel (tcgen05 implicit GEMM family, %d launches/step)" % sum(1 for n, t, f in prof if f > 0),
+            "roofline": {"kernel": "conv_tc_kernel + conv_halo_kernel (wgmma implicit GEMM family, %d launches/step)" % sum(1 for n, t, f in prof if f > 0),
                          "bound": "tensor", "achieved": ach_t, "peak": tpeak, "unit": "TFLOP/s",
-                         "frac": ach_t / tpeak if prof else None, "traffic": ncu.get("conv_family_dram_bytes"),
+                         "frac": ach_t / tpeak if prof else None,
                          "peak_source": tsrc,
                          "note": "achieved = sum of algorithmic FLOPs (2*MACs of the reference convs) / sum of the family's "
-                                 "launch durations (CUDA events, back-to-back); traffic = sum over the family of ncu "
-                                 "dram__bytes_read+write per launch (profiles/ncu_traffic.json)",
+                                 "launch durations (CUDA events, back-to-back)",
                          "share_of_step": conv_ms / tot_ms if tot_ms else None,
                          "algorithmic_flops_per_step": conv_fl},
             "roofline_lift": {"kernel": "sfa_lift_p1_kernel", "bound": "hbm", "achieved": ach_h, "peak": hpeak,
-                              "unit": "GB/s", "frac": ach_h / hpeak, "traffic": ncu.get("lift_dram_bytes"),
-                              "peak_source": src + " hbm_gbs",
+                              "unit": "GB/s", "frac": ach_h / hpeak,
+                              "peak_source": src + " HBM3 bandwidth",
                               "algorithmic_bytes": lift_bytes, "ms": lift_ms,
                               "share_of_step": lift_ms / tot_ms if tot_ms else None},
             "step_ms": step_spread,
@@ -592,9 +613,19 @@ def run_b200(args):
             times, cores = cpu_forward_seconds(1, 0)
             line["cpu_baseline"] = {"value": N_OUT / times[0], "unit": "voxels/s", "cores": cores, "kind": "port",
                                     "sample": "1 full forward of the workload (oracle/functional.py, PyTorch CPU fp32), %.1f s" % times[0]}
+        try:      # the card's power limit is part of every number above
+            plim = float(subprocess.run(["nvidia-smi", "-i", str(ClockSampler._physical_index(local)),
+                                         "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                                        capture_output=True, text=True, timeout=10).stdout.strip())
+        except Exception:  # noqa: BLE001
+            plim = None
+        line["gpu"] = {"name": torch.cuda.get_device_name(dev), "power_limit_w": plim}
+        if args.dump_outputs:
+            line["dump_outputs"] = {"dir": args.dump_outputs, "sampled": dump_outputs.sampled,
+                                    "sample_size": DUMP_SAMPLE}
         if args.dump_profile:
-            os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-            with open(os.path.join(ROOT, "gpurun_out", "plan_profile_%s.json" % prec), "w") as f:
+            os.makedirs(args.dump_profile, exist_ok=True)
+            with open(os.path.join(args.dump_profile, "plan_profile_%s.json" % prec), "w") as f:
                 json.dump([{"name": n, "ms": t, "flops": fl} for n, t, fl in prof], f)
     if world > 1:
         dist.barrier()
@@ -690,7 +721,10 @@ def main():
     ap.add_argument("--partition", default="frames", choices=["frames", "slab"],
                     help="frames: one frame per GPU (default, weak scaling; N > 1 adds a `slab` block); slab: the "
                          "X-slab partition of one frame as the headline")
-    ap.add_argument("--dump-profile", action="store_true")
+    ap.add_argument("--dump-profile", metavar="DIR", default=None,
+                    help="write the per-kernel profile of the plan as DIR/plan_profile_<precision>.json")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * occdepth_b200 -- C ABI of the B200 (sm_100a) kernels behind the OccDepth forward hot path.
+ * occdepth_b200 -- C ABI of the H100 (sm_90a) kernels behind the OccDepth forward hot path.
  *
  * The reference (megvii-research/OccDepth) has no FFI: its "operator interface" for this path is the
  * sequence of PyTorch library calls inside occdepth/models/*.py.  Each entry point below names the
@@ -22,10 +22,10 @@ extern "C" {
 
 /* Activation / GEMM-operand element types.  Every kernel that touches channels-last activations takes one of:    */
 /*   OCCD_DTYPE_F32  : fp32 storage holding TF32-representable values (each store rounds to the 10-bit TF32        */
-/*                     mantissa, round-to-nearest-away); convolutions run as tcgen05 kind::tf32 with fp32          */
+/*                     mantissa, round-to-nearest-away); convolutions run as wgmma .tf32 with fp32          */
 /*                     accumulation -- the reference-precision mode (the reference's fp32 nn.Conv*d under PyTorch's */
 /*                     CUDA default, TF32 tensor cores)                                                             */
-/*   OCCD_DTYPE_BF16 : bf16 storage, tcgen05 kind::f16 -- the throughput mode                                       */
+/*   OCCD_DTYPE_BF16 : bf16 storage, wgmma .bf16 -- the throughput mode                                       */
 /* One channel "vector" is 8 consecutive channels (32 / 16 bytes): cstride, coff and C are multiples of 8.         */
 #define OCCD_DTYPE_F32 0
 #define OCCD_DTYPE_BF16 1
@@ -81,7 +81,7 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
 
 
 /* -------------------------------------------------------------------------------------------- */
-/* Generalised N-d convolution as implicit GEMM on tcgen05 (sm_100a)                              */
+/* Generalised N-d convolution as implicit GEMM on wgmma (sm_90a)                              */
 /* replaces, with BatchNorm folded into weights/bias and the activation / residual adds fused:    */
 /*   nn.Conv3d / nn.Conv2d (+BN +ReLU/LeakyReLU/SiLU)  modules.py:6-48,51-235; DDR.py:51-139;      */
 /*     unet2d.py:24-46,65-165; CRP3D.py:22-52; flosp_depth.py:201-257; geffnet 1x1 convs           */
@@ -100,9 +100,9 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
 #define OCCD_ACT_LEAKY 2 /* slope 0.01 */
 #define OCCD_ACT_SILU 3
 #define OCCD_ACT_SIGMOID 4
-#define OCCD_CONV_IMPL_TC 0   /* tcgen05 + TMA implicit GEMM                                       */
+#define OCCD_CONV_IMPL_TC 0   /* wgmma + TMA implicit GEMM                                       */
 #define OCCD_CONV_IMPL_SIMT 1 /* CUDA-core direct convolution (cross-check / odd shapes)           */
-#define OCCD_CONV_IMPL_HALO 2 /* tcgen05, halo tile loaded once + row-shifted smem views per tap:    */
+#define OCCD_CONV_IMPL_HALO 2 /* wgmma, halo tile loaded once + row-shifted smem views per tap:    */
                               /* stride-1 {-d,0,d}-tap convs, Cin <= 64, resident weights; returns  */
                               /* OCCD_ERR_UNSUPPORTED from plan_create when the shape does not fit   */
 #define OCCD_CONV_IMPL_HALOX 3 /* halo tile for grids whose innermost extent W is 8 / 16 / 32 (one warp row): the   */

@@ -1,4 +1,4 @@
-"""occdepth_b200 -- B200 (sm_100a) native forward hot path of OccDepth.
+"""occdepth_b200 -- H100 (sm_90a) native forward hot path of OccDepth.
 
 Module surface mirrors the reference's `occdepth.models` (same class names, constructor signatures, forward
 inputs/outputs and state_dict keys); `install_as_occdepth()` registers this package under the reference's

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a kernel library (nvcc -> occdepth_b200/lib/libocc_b200.so).
+"""In-tree build of the sm_90a kernel library (nvcc -> occdepth_b200/lib/libocc_b200.so).
 
 No torch extension machinery: the product boundary is a plain C ABI (include/occdepth_b200.h), so the
 library is compiled with nvcc directly and loaded through ctypes (occdepth_b200/_lib.py).
@@ -17,7 +17,7 @@ OBJDIR = os.path.join(LIBDIR, "obj")
 LIBNAME = "libocc_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -55,7 +55,7 @@ def lib_path():
 
 
 def build(verbose=False, force=False):
-    """Compile every csrc/*.cu for sm_100a and link lib/libocc_b200.so (incremental by content hash)."""
+    """Compile every csrc/*.cu for sm_90a and link lib/libocc_b200.so (incremental by content hash)."""
     os.makedirs(OBJDIR, exist_ok=True)
     nvcc = _nvcc()
     srcs = _sources()
@@ -92,7 +92,7 @@ def build(verbose=False, force=False):
             list(ex.map(compile_one, jobs))
     out = lib_path()
     if jobs or not os.path.exists(out):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out] + objs
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

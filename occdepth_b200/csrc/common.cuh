@@ -1,4 +1,4 @@
-// Shared device/host helpers for the occdepth_b200 sm_100a kernels.
+// Shared device/host helpers for the occdepth_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -43,8 +43,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 
 // activation over 8 values with ONE uniform branch (keeps the epilogues free of per-element switches)
 // SiLU with ONE MUFU op per element: x sigmoid(x) = h + h tanh(h), h = x / 2 (tanh.approx.f32: max relative error
-// 2^-11).  Used by the bf16 mode only, whose stores round to 2^-9; the tf32 mode keeps ex2 + rcp (two MUFU ops):
-// a SiLU epilogue runs within 2x of the MUFU pipe (16 lanes / cycle / SM), see DESIGN.md section 4
+// 2^-11).  Used by the bf16 mode only, whose stores round to 2^-9; the tf32 mode keeps ex2 + rcp (two MUFU ops)
 __device__ __forceinline__ float silu_tanh(float x) {
   const float h = 0.5f * x;
   float t;
@@ -106,9 +105,9 @@ __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // Activation element types.  Two precision modes share every kernel (template parameter T):
-//   __nv_bfloat16 : bf16 storage, tcgen05 kind::f16 operands ("bf16" throughput mode)
+//   __nv_bfloat16 : bf16 storage, wgmma .bf16 operands ("bf16" throughput mode)
 //   float         : fp32 storage holding TF32-representable values (10-bit mantissa, round-to-nearest-away at every
-//                   store), tcgen05 kind::tf32 operands -- the reference-precision mode: the reference's convolutions
+//                   store), wgmma .tf32 operands -- the reference-precision mode: the reference's convolutions
 //                   are fp32 nn.Conv*d (modules.py:158-175, DDR.py:111-139) which PyTorch itself runs as TF32 on CUDA
 // One "vector" is always 8 consecutive channels: 16 bytes of bf16 or 32 bytes of fp32.
 __device__ __forceinline__ float round_tf32(float v) {
@@ -117,28 +116,20 @@ __device__ __forceinline__ float round_tf32(float v) {
   return __uint_as_float(u);
 }
 
+// 8 fp32 values as two 16-byte accesses (sm_90 has no 256-bit global loads / stores)
 __device__ __forceinline__ void ld256_f(const float* p, float* f) {
-  uint32_t r[8];
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(r[i]);
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+  f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 __device__ __forceinline__ void ld256_nc_f(const float* p, float* f) {
-  uint32_t r[8];
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(r[i]);
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p + 4));
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+  f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 __device__ __forceinline__ void st256_f(float* p, const float* f) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(__float_as_uint(f[0])),
-               "r"(__float_as_uint(f[1])), "r"(__float_as_uint(f[2])), "r"(__float_as_uint(f[3])),
-               "r"(__float_as_uint(f[4])), "r"(__float_as_uint(f[5])), "r"(__float_as_uint(f[6])),
-               "r"(__float_as_uint(f[7]))
-               : "memory");
+  *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
 }
 
 template <typename T> struct Elem;

@@ -1,12 +1,12 @@
 // Generalised N-d convolution as implicit GEMM.
 //   TC path  : TMA (5-D tiled tensor maps, zero-filled halos, traversal strides) -> swizzled smem ->
-//              tcgen05.mma (M=128 positions x N<=256 channels, fp32 accumulators in TMEM) ->
-//              tcgen05.ld epilogue (bias + residuals + activation, channels-last / fp32 planar stores)
+//              wgmma (M=128 positions as two warpgroups x 64, N<=256 channels, fp32 accumulators in registers) ->
+//              epilogue (bias + residuals + activation, channels-last / fp32 planar stores)
 //   SIMT path: CUDA-core direct convolution with identical semantics (cross-check and odd shapes)
 // Two operand types share every kernel (template parameter T, see Elem<T> / tc::Mma<T>):
-//   float (TF32 values, tcgen05 kind::tf32, K chunk = 32 / 16 / 8 channels)  -- reference-precision mode
-//   __nv_bfloat16 (tcgen05 kind::f16, K chunk = 64 / 32 / 16 channels)       -- throughput mode
-// A K chunk is always one swizzled smem row of RB = 128 / 64 / 32 bytes; one tcgen05.mma consumes 32 bytes of it.
+//   float (TF32 values, wgmma .tf32, K chunk = 32 / 16 / 8 channels)  -- reference-precision mode
+//   __nv_bfloat16 (wgmma .bf16, K chunk = 64 / 32 / 16 channels)      -- throughput mode
+// A K chunk is always one swizzled smem row of RB = 128 / 64 / 32 bytes; one wgmma step consumes 32 bytes of it.
 // See include/occdepth_b200.h for the reference call sequences this replaces.
 #include "conv_common.cuh"
 #include "conv_tc.cuh"
@@ -18,8 +18,18 @@
 
 namespace {
 
-constexpr int kTcThreads = 576;  // warp 0: TMA producer, warp 1: MMA issuer (+TMEM alloc), warps 2-17: four epilogue groups
+// 384 threads: warpgroup 0 is the TMA producer (one lane issues, the rest give their registers away), warpgroups 1
+// and 2 issue wgmma and run the epilogue, each for 64 of the 128 rows of an M tile (fp32 accumulators in registers)
+constexpr int kTcThreads = 384;
 constexpr int kMaxStages = 24;
+constexpr int kEmptyArrivals = 8;   // one per MMA warp: a stage is free when both MMA warpgroups are done with it
+// accumulator staging for the epilogue: [2 warpgroups][64 rows][LD floats].  The per-tap kernel stages rounds of
+// 32 columns (LD = kStageWide); the halo kernels, whose resident weights leave less shared memory, rounds of 16
+// (x-packed: three groups of 8, LD = kStageNarrow) or 8 columns (LD = kStageHalo)
+constexpr int kStageWide = 36;
+constexpr int kStageNarrow = 18;
+constexpr int kStageHalo = 10;
+__host__ __device__ constexpr int staging_bytes(int ld) { return 2 * 64 * ld * 4; }
 
 struct TcParams {
   ConvEpi epi;
@@ -34,9 +44,8 @@ struct TcParams {
   int Cout_pad, N_tile;
   int stages, group;
   int a_bytes, b_stride, b_bytes;
-  int tmem_cols;
+  int rb;            // bytes per K chunk row: 128 / 64 / 32 == the swizzle mode
   int pdl;           // launched with programmatic stream serialization: wait for the producer grid after the prologue
-  long long* trace;  // optional [tile][8] clock64 stamps of CTA 0 (occd_conv_debug_trace, tools/conv_trace.py)
   signed char tap_src[OCCD_CONV_MAX_TAPS];
   short tap_dz[OCCD_CONV_MAX_TAPS], tap_dy[OCCD_CONV_MAX_TAPS], tap_dx[OCCD_CONV_MAX_TAPS];
   // tap groups: n_groups convolutions over the same sources and iteration space in one launch (the sub-pixel phases
@@ -48,75 +57,172 @@ struct TcParams {
   signed char grp_oadd[OCCD_CONV_MAX_GROUPS][3];
 };
 
+// One pipeline item (one K chunk of RB bytes per row) of a warpgroup's 64 x (32 * nc) accumulator tile: RB / 32
+// wgmma steps per 32-column block.  first: the item's first step overwrites the accumulators.
+template <typename T, int NC>
+__device__ __forceinline__ void mma_item(float (&acc)[NC][16], uint64_t da, uint64_t db, int nmma, int nc,
+                                         uint32_t b_chunk16, bool first) {
+  for (int k = 0; k < nmma; ++k) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+      if (c < nc)
+        tc::Mma<T>::issue(acc[c], da + 2 * k, db + (uint64_t)(c * b_chunk16) + 2 * k, (first && k == 0) ? 0u : 1u);
+  }
+}
+
+template <int NC>
+__device__ __forceinline__ void acc_fence_all(float (&acc)[NC][16]) {
+#pragma unroll
+  for (int c = 0; c < NC; ++c) tc::acc_fence(acc[c]);
+}
+
+// This thread's part of the 8-column block `blk` of the accumulator tile -> st[row][col0, col0 + 8).  wgmma m64nN
+// fragment: warp w of the warpgroup holds rows 16w + lane/4 and 16w + lane/4 + 8, columns 2 (lane % 4) + {0, 1} of
+// every 8-column block.
+template <int LD, int NC>
+__device__ __forceinline__ void stage8(float* st, const float (&acc)[NC][16], int blk, int col0, int warp4,
+                                       int lane) {
+  const int r0 = 16 * warp4 + (lane >> 2), cc = col0 + 2 * (lane & 3);
+#pragma unroll
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (4 * c + i == blk) {
+        *reinterpret_cast<float2*>(st + r0 * LD + cc) = make_float2(acc[c][4 * i], acc[c][4 * i + 1]);
+        *reinterpret_cast<float2*>(st + (r0 + 8) * LD + cc) = make_float2(acc[c][4 * i + 2], acc[c][4 * i + 3]);
+      }
+}
+
+// Epilogue of one warpgroup's 64-row tile, columns [0, ncols) of output channels n0 + [0, ncols): rounds of 32
+// (LD = kStageWide), 16 (kStageNarrow) or 8 (kStageHalo) columns go through shared memory so that thread t owns
+// row t / 2 and 16 (8) consecutive channels -- with 8-column rounds threads 0..63 own row t -- the vector width of
+// the channels-last stores.  The caller gives the position of the thread's row; oa:
+// per-launch output offset (tap groups) or nullptr for e.oadd.
+template <typename T, int NC, int LD>
+__device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&acc)[NC][16], float* st, int bar_id,
+                                              int warp4, int lane, int t, int ncols, bool valid, int b, int od,
+                                              int oh, int ow, int n0, const signed char* oa) {
+  constexpr int ROUND = LD == kStageWide ? 32 : (LD == kStageNarrow ? 16 : 8);
+  constexpr int TPR = ROUND == 8 ? 1 : 2, VW = ROUND / TPR;   // threads per row, channels per thread
+  const int row = t / TPR, h = t % TPR;
+  const bool fast = VW == 16 && epi_fast_ok(e);
+  EpiRow<T> er;
+  if (fast)
+    er = oa ? epi_row<T>(e, valid, b, od, oh, ow, n0, oa[0], oa[1], oa[2]) : epi_row<T>(e, valid, b, od, oh, ow, n0);
+  for (int c0 = 0; c0 < ncols; c0 += ROUND) {
+    tc::wg_sync(bar_id);   // the previous round's reads are done
+#pragma unroll
+    for (int j = 0; j < ROUND / 8; ++j) stage8<LD, NC>(st, acc, (c0 >> 3) + j, 8 * j, warp4, lane);
+    tc::wg_sync(bar_id);
+    const int cc = c0 + VW * h;
+    if (row < 64 && cc < ncols) {
+      float v[VW];
+      // staged rows are 8-byte aligned (LD is even, not a multiple of 4 for kStageNarrow)
+      const float2* sp = reinterpret_cast<const float2*>(st + row * LD + VW * h);
+#pragma unroll
+      for (int i = 0; i < VW / 2; ++i) {
+        const float2 x = sp[i];
+        v[2 * i] = x.x; v[2 * i + 1] = x.y;
+      }
+      if constexpr (VW == 16) {
+        if (fast) {
+          EpiPre q;
+          epi_prefetch<T>(er, cc, q);
+          epi_finish_v<T>(er, cc, v, q.b, q.r);
+          continue;
+        }
+      }
+      if (valid) conv_epilogue_row<T, VW>(e, b, od, oh, ow, n0 + cc, v);
+    }
+  }
+}
+
+// Epilogue of the x-packed kernels: the accumulator holds three column groups Q_c (c = 0, 1, 2: the W taps -d, 0,
+// +d) of CP columns each and out[r] = Q_0[r - d] + Q_1[r] + Q_2[r + d], where r -+ d stays inside the line of PW
+// rows (lo_ok / hi_ok false: the neighbour is the conv's zero padding).  Rounds of 8 channels: Q_0 and Q_1 are
+// staged side by side, then Q_2, and threads 0..63 (one per row) form the sums and store.
+template <typename T, int NC>
+__device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[NC][16], float* st, int bar_id,
+                                            int warp4, int lane, int t, int CP, int d, bool lo_ok, bool hi_ok,
+                                            bool valid, int b, int od, int oh, int ow) {
+  constexpr int LD = kStageNarrow;
+  for (int c0 = 0; c0 < CP; c0 += 8) {
+    float v[8];
+    tc::wg_sync(bar_id);
+    stage8<LD, NC>(st, acc, c0 >> 3, 0, warp4, lane);
+    stage8<LD, NC>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
+    tc::wg_sync(bar_id);
+    if (t < 64 && valid) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = st[t * LD + 8 + i] + (lo_ok ? st[(t - d) * LD + i] : 0.f);
+    }
+    tc::wg_sync(bar_id);
+    stage8<LD, NC>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
+    tc::wg_sync(bar_id);
+    if (t < 64 && valid) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] += hi_ok ? st[(t + d) * LD + i] : 0.f;
+      conv_epilogue_row<T, 8>(e, b, od, oh, ow, c0, v);
+    }
+  }
+}
+
+__device__ __forceinline__ void pdl_prologue_done(int pdl) {
+  if (pdl) {
+    // programmatic dependent launch: everything above (barrier init, tensor-map prefetch) overlapped the tail of the
+    // producer grid; its results are only touched below this point
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  }
+}
+
 // XP: x-packed variant: the pipeline items are (source, dz, dy) groups whose B operand stacks the three W taps
 // (N_tile = 3 * Cout_pad: with taps in lexicographic order that is 3 consecutive tap slices of the ordinary weight
-// tensor), tiles are 32 wide with one halo column on each side so that one smem row == one TMEM lane == one lane of
-// an epilogue warp, and the epilogue forms out[r] = Q_0[r-1] + Q_1[r] + Q_2[r+1] from the three column groups with
-// two warp shuffles per channel.  One A fetch then feeds 3x the output columns (measured on B200, round 2: the
-// Cout = 80 decoder convs 0.154 -> 0.102 ms).
-template <typename T, int RB, bool XP>
-__global__ void __launch_bounds__(kTcThreads)
+// tensor), tiles are 32 wide with one halo column on each side, and the epilogue forms
+// out[r] = Q_0[r-1] + Q_1[r] + Q_2[r+1] from the three column groups.  One A fetch then feeds 3x the output columns.
+// NC: 32-column accumulator blocks compiled in (N_tile <= 32 * NC).
+template <typename T, int NC, bool XP>
+__global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUtensorMap tmA0,
                const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmW) {
   // Persistent, warp-specialised implicit GEMM.  Each CTA walks tiles blockIdx.x, +gridDim.x, ...:
   //   warp 0 (one lane): TMA producer -- runs ahead across tile boundaries, the smem ring never drains
-  //   warp 1 (one lane): tcgen05.mma issuer, accumulating into one of TWO TMEM accumulators
-  //   warps 2-17       : four epilogue groups of 4 warps: group g drains accumulator (g & 1) -- even / odd
-  //                      tiles -- and column half (g >> 1) of it: TMEM -> regs -> global while the MMAs of the
-  //                      following tiles run (the epilogue is latency bound: 16 warps keep the SM's LSU busy)
-  constexpr int KCH = RB / (int)sizeof(T);  // channels per K chunk
-  constexpr int NMMA = RB / 32;             // tcgen05.mma instructions per chunk (32 bytes of K each)
+  //   warpgroups 1, 2  : wgmma over rows [0, 64) / [64, 128) of the M tile, then the epilogue from registers
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem is only guaranteed 16-byte aligned: round the base up to 1024 (swizzle atom alignment)
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_a + (uint32_t)(p.stages * p.group) * p.a_bytes;
-  const uint32_t bar_base = smem_b + (uint32_t)(p.stages * p.group) * p.b_stride;  // 8-byte aligned (multiples of 1024)
+  constexpr int LD = XP ? kStageNarrow : kStageWide;
+  const uint32_t smem_st = smem_b + (uint32_t)(p.stages * p.group) * p.b_stride;
+  const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
   const uint32_t full_bar = bar_base;
   const uint32_t empty_bar = bar_base + 8u * kMaxStages;
-  const uint32_t tmem_full_bar = bar_base + 16u * kMaxStages;       // [2]
-  const uint32_t tmem_empty_bar = tmem_full_bar + 16u;              // [2]
-  const uint32_t tmem_slot = tmem_empty_bar + 16u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n_tiles_n = XP ? 1 : p.Cout_pad / p.N_tile;
   const int tiles_per_group = p.num_m_tiles * n_tiles_n;
   const int num_tiles = tiles_per_group * p.n_groups;
+  const int RB = p.rb;
+  const int KCH = RB / (int)sizeof(T);  // channels per K chunk
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmA0);
     tc::prefetch_tmap(&tmW);
     for (int s = 0; s < p.stages; ++s) {
       tc::mbar_init(full_bar + 8u * s, 1);
-      tc::mbar_init(empty_bar + 8u * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      tc::mbar_init(tmem_full_bar + 8u * a, 1);
-      tc::mbar_init(tmem_empty_bar + 8u * a, 256);  // every epilogue thread of the two groups arrives
+      tc::mbar_init(empty_bar + 8u * s, kEmptyArrivals);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  if (p.pdl) {
-    // programmatic dependent launch: everything above (barrier init, TMEM alloc, tensor-map prefetch) overlapped
-    // the tail of the producer grid; its results are only touched below this point
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
-  const uint32_t acc_stride = (uint32_t)p.tmem_cols >> 1;  // column offset of the second accumulator
+  pdl_prologue_done(p.pdl);
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    tc::reg_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       // ===== TMA producer =====
       const CUtensorMap* maps[3] = {&tmA0, &tmA1, &tmA2};
       int s = 0;
@@ -136,8 +242,6 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
         // items (tap, k-chunk) are loaded in groups of p.group per pipeline stage: one barrier hand-off per group
         int g = 0;
         int remaining = p.grp_iters[grp];
-        const int jt = (tile - blockIdx.x) / gridDim.x;
-        if (p.trace && blockIdx.x == 0 && jt < 64) p.trace[jt * 8 + 0] = clock64();
         for (int tp = p.grp_tap0[grp]; tp < p.grp_tap0[grp + 1]; ++tp) {
           const int src = p.tap_src[tp];
           const int cw = iw0 + p.tap_dx[tp], ch = ih0 + p.tap_dy[tp], cd = id0 + p.tap_dz[tp];
@@ -160,164 +264,86 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
             }
           }
         }
-        if (p.trace && blockIdx.x == 0 && jt < 64) p.trace[jt * 8 + 1] = clock64();
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = tc::Mma<T>::idesc(128, p.N_tile);
-      const uint64_t da0 = tc::make_sdesc(smem_a, RB);
-      const uint64_t db0 = tc::make_sdesc(smem_b, RB);
-      int s = 0;
-      uint32_t ph = 0;
-      int j = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
-        const uint32_t acc = (uint32_t)j & 1u;
-        tc::mbar_wait(tmem_empty_bar + 8u * acc, (((uint32_t)j >> 1) & 1u) ^ 1u);  // epilogue drained this buffer
-        tc::fence_after_sync();
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 2] = clock64();
-        const uint32_t d_tmem = tmem_base + acc * acc_stride;
-        const int iters_per_tile = p.grp_iters[tile / tiles_per_group];
-        for (int it = 0; it < iters_per_tile;) {
-          tc::mbar_wait(full_bar + 8u * s, ph);
-          tc::fence_after_sync();
-          const int cnt = (iters_per_tile - it) < p.group ? (iters_per_tile - it) : p.group;
-          for (int g = 0; g < cnt; ++g, ++it) {
-            const uint64_t da = da0 + (uint64_t)((s * p.group + g) * (p.a_bytes >> 4));
-            const uint64_t db = db0 + (uint64_t)((s * p.group + g) * (p.b_stride >> 4));
-            if (it == 0) tc::Mma<T>::template issue<0>(d_tmem, da, db, idesc);
-            else tc::Mma<T>::template issue<1>(d_tmem, da, db, idesc);
-#pragma unroll
-            for (int k = 1; k < NMMA; ++k) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * k, db + 2 * k, idesc);
-          }
-          tc::mma_commit(empty_bar + 8u * s);  // frees the smem stage when these MMAs retire
-          if (++s == p.stages) { s = 0; ph ^= 1u; }
-        }
-        tc::mma_commit(tmem_full_bar + 8u * acc);  // accumulator complete
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 3] = clock64();
-      }
-    }
-  } else {
-    // ===== epilogue: TMEM -> registers -> (bias, residuals, activation) -> global =====
-    // (a shared-memory-staged TMA-store epilogue was measured on B200, round 2: same 4-5 B/cycle/SM as these direct
-    // stores -- the write path, not the store instruction mix, is the limit -- and the 64 KB of staging cost the
-    // large-K convs a third of their smem ring: 4.0 -> 5.4 ms for the decoder 3x3 convs.  Removed.)
-    const int q = warp & 3;                  // TMEM lane quarter this warp may access
-    const int egrp = (warp - 2) >> 2;        // epilogue group 0..3 (128 threads == 128 tile rows)
-    const int grp = egrp & 1;                // accumulator index (tile parity)
-    const int half = egrp >> 1;              // this group takes the first / second half of the 16-column chunks
-    const int ncols = XP ? p.Cout_pad : p.N_tile;        // output channels of one tile
-    const int n_chunks = ncols >> 4;
-    const int c_begin = half == 0 ? 0 : ((n_chunks + 1) >> 1) * 16;   // contiguous per thread: whole lines fill up
-    const int c_end = half == 0 ? ((n_chunks + 1) >> 1) * 16 : ncols;
-    const int row = q * 32 + lane;
-    const int rw = row % p.TW;
-    const int rh = (row / p.TW) % p.TH;
-    const int rd = row / (p.TW * p.TH);
-    const bool tracer = p.trace && blockIdx.x == 0 && threadIdx.x == 64;
-    int j = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
-      if ((j & 1) != grp) continue;
-      const int tgrp = tile / tiles_per_group;       // tap group (sub-pixel phase) of this tile
-      const int tg = tile - tgrp * tiles_per_group;
-      const int nt = tg % n_tiles_n;
-      int t = tg / n_tiles_n;
-      const int tw = t % p.tiles_w; t /= p.tiles_w;
-      const int th = t % p.tiles_h; t /= p.tiles_h;
-      const int td = t % p.tiles_d; t /= p.tiles_d;
-      const int b = t;
-      const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = XP ? tw * 30 + rw - 1 : tw * p.TW + rw;
-      const bool valid = od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && (!XP || (rw >= 1 && rw <= 30));
-      const int n0 = nt * p.N_tile;
-      const uint32_t acc = (uint32_t)grp;
-      if (tracer && j < 64) p.trace[j * 8 + 4] = clock64();
-      tc::mbar_wait(tmem_full_bar + 8u * acc, ((uint32_t)j >> 1) & 1u);
-      tc::fence_after_sync();
-      if (tracer && j < 64) p.trace[j * 8 + 5] = clock64();
-      const uint32_t taddr = tmem_base + acc * acc_stride + ((uint32_t)(q * 32) << 16);
-      if constexpr (XP) {
-        // TW == 32: lane == tile column, so the W neighbours' partial sums sit in the neighbouring lanes
-        for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-          float lo[16], v[16], hi[16];
-          tc::tmem_ld16(taddr + (uint32_t)c0, lo);
-          tc::tmem_ld16(taddr + (uint32_t)(p.Cout_pad + c0), v);
-          tc::tmem_ld16(taddr + (uint32_t)(2 * p.Cout_pad + c0), hi);
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            v[i] += __shfl_up_sync(0xffffffffu, lo[i], 1) + __shfl_down_sync(0xffffffffu, hi[i], 1);
-          if (valid) conv_epilogue_row<T, 16>(p.epi, b, od, oh, ow, c0, v);
-        }
-      } else if (epi_fast_ok(p.epi)) {
-        // fast path (conv_common.cuh): bias / residual loads ahead of the accumulator, pointers formed once per tile
-        const EpiRow<T> er = p.n_groups > 1 ? epi_row<T>(p.epi, valid, b, od, oh, ow, n0, p.grp_oadd[tgrp][0],
-                                                         p.grp_oadd[tgrp][1], p.grp_oadd[tgrp][2])
-                                            : epi_row<T>(p.epi, valid, b, od, oh, ow, n0);
-        uint32_t ra[16];
-        EpiPre q;
-        for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-          tc::tmem_ld16_issue(taddr + (uint32_t)c0, ra);
-          epi_prefetch<T>(er, c0, q);                        // in flight together with the TMEM load of this chunk
-          tc::tmem_ld_wait16(ra);
-          epi_finish<T>(er, c0, ra, q);
-        }
-      } else {
-        // software-pipelined: the tcgen05.ld of this group's next 16 columns is in flight while these are stored
-        uint32_t ra[16], rb[16];
-        int c0 = c_begin;
-        long long t_ld = 0, t_epi = 0, t_a = 0;
-        if (c0 < c_end) tc::tmem_ld16_issue(taddr + (uint32_t)c0, ra);
-        for (; c0 < c_end; c0 += 32) {
-          if (tracer) t_a = clock64();
-          tc::tmem_ld_wait16(ra);
-          if (tracer) t_ld += clock64() - t_a;
-          const bool has_b = c0 + 16 < c_end;
-          if (has_b) tc::tmem_ld16_issue(taddr + (uint32_t)(c0 + 16), rb);
-          if (tracer) t_a = clock64();
-          if (valid) {
-            float v[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(ra[i]);
-            conv_epilogue_row<T, 16>(p.epi, b, od, oh, ow, n0 + c0, v);
-          }
-          if (tracer) t_epi += clock64() - t_a;
-          if (has_b) {
-            tc::tmem_ld_wait16(rb);
-            if (c0 + 32 < c_end) tc::tmem_ld16_issue(taddr + (uint32_t)(c0 + 32), ra);
-            if (valid) {
-              float v[16];
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(rb[i]);
-              conv_epilogue_row<T, 16>(p.epi, b, od, oh, ow, n0 + c0 + 16, v);
-            }
-          }
-        }
-        if (tracer && j < 64) p.trace[j * 8 + 7] = (t_ld << 32) | (t_epi & 0xffffffffll);
-      }
-      tc::fence_before_sync();
-      tc::mbar_arrive(tmem_empty_bar + 8u * acc);  // this thread's TMEM reads of the buffer are done
-      if (tracer && j < 64) p.trace[j * 8 + 6] = clock64();
-    }
+    return;
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+
+  // ===== MMA + epilogue warpgroups =====
+  tc::reg_alloc<232>();
+  const int wg = (warp >> 2) - 1;
+  const int warp4 = warp & 3;
+  const int t = threadIdx.x & 127;
+  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
+  const int nmma = RB / 32;
+  const int nc = (p.N_tile + 31) >> 5;
+  const uint32_t b_chunk16 = (uint32_t)(2 * RB);   // 32 B rows, in 16-byte descriptor units
+  const uint64_t da0 = tc::make_sdesc(smem_a, RB) + (uint64_t)(64 * wg * RB / 16);
+  const uint64_t db0 = tc::make_sdesc(smem_b, RB);
+  float acc[NC][16];
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int tgrp = tile / tiles_per_group;       // tap group (sub-pixel phase) of this tile
+    const int iters = p.grp_iters[tgrp];
+    int prev = -1;
+    for (int it = 0; it < iters;) {
+      tc::mbar_wait(full_bar + 8u * s, ph);
+      const int cnt = (iters - it) < p.group ? (iters - it) : p.group;
+      tc::wg_fence();
+      for (int g = 0; g < cnt; ++g, ++it) {
+        const uint64_t da = da0 + (uint64_t)((s * p.group + g) * (p.a_bytes >> 4));
+        const uint64_t db = db0 + (uint64_t)((s * p.group + g) * (p.b_stride >> 4));
+        mma_item<T, NC>(acc, da, db, nmma, nc, b_chunk16, it == 0);
+      }
+      tc::wg_commit();
+      tc::wg_wait<1>();     // the previous stage's MMAs have retired: hand that stage back to the producer
+      if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar + 8u * prev);
+      prev = s;
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
+    }
+    tc::wg_wait<0>();
+    if (lane == 0) tc::mbar_arrive(empty_bar + 8u * prev);
+    acc_fence_all<NC>(acc);
+
+    const int tg = tile - tgrp * tiles_per_group;
+    const int nt = tg % n_tiles_n;
+    int tt = tg / n_tiles_n;
+    const int tw = tt % p.tiles_w; tt /= p.tiles_w;
+    const int th = tt % p.tiles_h; tt /= p.tiles_h;
+    const int td = tt % p.tiles_d; tt /= p.tiles_d;
+    const int b = tt;
+    if constexpr (XP) {
+      // TW == 32: row == tile column inside each 32-row line, so the W neighbours' partial sums are rows r -+ 1
+      const int row = 64 * wg + t;
+      const int rw = row % 32;
+      const int rh = (row / 32) % p.TH;
+      const int rd = row / (32 * p.TH);
+      const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * 30 + rw - 1;
+      const bool valid = t < 64 && od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && rw >= 1 && rw <= 30;
+      epilogue_xp<T, NC>(p.epi, acc, st, 1 + wg, warp4, lane, t, p.Cout_pad, 1, true, true, valid, b, od, oh, ow);
+    } else {
+      const int row = 64 * wg + (t >> 1);
+      const int rw = row % p.TW;
+      const int rh = (row / p.TW) % p.TH;
+      const int rd = row / (p.TW * p.TH);
+      const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * p.TW + rw;
+      const bool valid = od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW;
+      epilogue_rows<T, NC, LD>(p.epi, acc, st, 1 + wg, warp4, lane, t, p.N_tile, valid, b, od, oh, ow, nt * p.N_tile,
+                           p.n_groups > 1 ? p.grp_oadd[tgrp] : nullptr);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Halo-tile variant for stride-1 3x3x3 convolutions with few channels (the full-resolution head):
-// the per-tap TMA boxes of conv_tc_kernel re-load every input row 27 times and the TMA unit (~1.5 cycles per
-// box row) becomes the limiter.  Here each CTA tile loads ONE zero-filled halo box (PD x PH x PW positions,
-// rows of one K chunk) and feeds all 27 taps from row-shifted views of that box: with smem rows
-// linearised as r = (pd*PH + ph)*PW + pw, the A operand of tap (a,b,c) for output rows [R, R+128) is simply
-// rows [R + (a*PH + b)*PW + c, ...) -- a different UMMA start address, same data.  Rows that fall in the
-// halo produce garbage accumulator rows that the epilogue never stores.  Dilation d runs the same scheme on
-// the d^3 sub-sampled grids (TMA traversal stride d), so the halo is always one position.  Weights for all
-// taps stay resident in shared memory.  The swizzled row-shifted UMMA start addresses use base-offset 0 (measured on
-// B200: the XOR swizzle follows absolute smem address bits for both TMA and UMMA).
+// the per-tap TMA boxes of conv_tc_kernel re-load every input row 27 times and the TMA unit becomes the limiter.
+// Here each CTA tile loads ONE zero-filled halo box (PD x PH x PW positions, rows of one K chunk) and feeds all 27
+// taps from row-shifted views of that box: with smem rows linearised as r = (pd*PH + ph)*PW + pw, the A operand of
+// tap (a,b,c) for output rows [R, R+64) is simply rows [R + (a*PH + b)*PW + c, ...) -- a different wgmma start
+// address, same data.  Rows that fall in the halo produce garbage accumulator rows that the epilogue never stores.
+// Dilation d runs the same scheme on the d^3 sub-sampled grids (TMA traversal stride d), so the halo is always one
+// position.  Weights for all taps stay resident in shared memory.
 struct HaloParams {
   ConvEpi epi;
   int d;                      // dilation (== padding)
@@ -331,63 +357,47 @@ struct HaloParams {
   int a_stage_bytes;          // allocated per stage (box + slack rows read by garbage outputs)
   int stages;
   int n_taps;
-  int N_tile, tmem_cols, set_stride;
+  int N_tile, rb;
   int b_stride, w_bytes;
   int tap_off16[27];          // (R0 + (a*PH + b)*PW + c) * row_bytes / 16: A-descriptor advance per tap
   int pdl;                    // see TcParams::pdl
-  long long* trace;
 };
 
-template <typename T, int RB>
-__global__ void __launch_bounds__(kTcThreads)
+template <typename T>
+__global__ void __launch_bounds__(kTcThreads, 1)
 conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ CUtensorMap tmA,
                  const __grid_constant__ CUtensorMap tmW) {
-  constexpr int NMMA = RB / 32;
+  constexpr int NC = 4;   // N_tile <= 128
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_w = smem_base;                                   // [n_taps][b_stride] resident weights
   const uint32_t smem_a = smem_w + (uint32_t)p.w_bytes;                 // [stages][a_stage_bytes]
-  const uint32_t bar_base = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
+  constexpr int LD = kStageHalo;
+  const uint32_t smem_st = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
+  const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
   const uint32_t full_bar = bar_base;            // [4]
   const uint32_t empty_bar = bar_base + 32u;     // [4]
-  const uint32_t tfull_bar = bar_base + 64u;     // [2]
-  const uint32_t tempty_bar = bar_base + 80u;    // [2]
-  const uint32_t w_bar = bar_base + 96u;
-  const uint32_t tmem_slot = bar_base + 104u;
+  const uint32_t w_bar = bar_base + 64u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int d = p.d;
   const int per_res = p.tilesD * p.tilesH * p.tilesW;
   const int num_tiles = p.epi.B * d * d * d * per_res;
+  const int RB = p.rb;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmA);
     tc::prefetch_tmap(&tmW);
     for (int s = 0; s < p.stages; ++s) {
       tc::mbar_init(full_bar + 8u * s, 1);
-      tc::mbar_init(empty_bar + 8u * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      tc::mbar_init(tfull_bar + 8u * a, 1);
-      tc::mbar_init(tempty_bar + 8u * a, 256);
+      tc::mbar_init(empty_bar + 8u * s, kEmptyArrivals);
     }
     tc::mbar_init(w_bar, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  if (p.pdl) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
+  pdl_prologue_done(p.pdl);
 
   // tile -> (batch, residue class, sub-grid tile origin)
   auto decode = [&](int tile, int& b, int& ra, int& rb, int& rc, int& td, int& th, int& tw) {
@@ -401,8 +411,9 @@ conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ C
     b = t;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    tc::reg_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       // ===== TMA producer: resident weights once, then one halo box per tile =====
       tc::mbar_expect_tx(w_bar, (uint32_t)(p.n_taps * p.N_tile * RB));
       for (int tp = 0; tp < p.n_taps; ++tp)
@@ -420,142 +431,69 @@ conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ C
         if (++s == p.stages) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = tc::Mma<T>::idesc(128, p.N_tile);
-      const uint64_t db_w = tc::make_sdesc(smem_w, RB);
-      const int w_step16 = p.b_stride / 16;
-      tc::mbar_wait(w_bar, 0);
-      int s = 0;
-      uint32_t ph = 0;
-      int j = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
-        const uint32_t set = (uint32_t)j & 1u;
-        const uint32_t use = (uint32_t)j >> 1;
-        tc::mbar_wait(tempty_bar + 8u * set, (use & 1u) ^ 1u);
-        tc::mbar_wait(full_bar + 8u * s, ph);
-        tc::fence_after_sync();
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 2] = clock64();
-        // descriptors advance by plain 64-bit adds on the 16-byte-unit address field (smem < 256 KB: no carry out
-        // of the 14-bit field), so the issue loop is ~4 instructions per tcgen05.mma
-        const uint64_t da_stage = tc::make_sdesc(smem_a + (uint32_t)s * p.a_stage_bytes, RB);
-        for (int m = 0; m < p.nM; ++m) {
-          const uint32_t d_tmem = tmem_base + set * (uint32_t)p.set_stride + (uint32_t)(m * p.N_tile);
-          const uint64_t da_m = da_stage + (uint64_t)(m * (128 * RB / 16));
-          {
-            const uint64_t da = da_m + (uint64_t)p.tap_off16[0];
-            tc::Mma<T>::template issue<0>(d_tmem, da, db_w, idesc);
-#pragma unroll
-            for (int k = 1; k < NMMA; ++k) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * k, db_w + 2 * k, idesc);
-          }
-#pragma unroll 3
-          for (int tp = 1; tp < p.n_taps; ++tp) {
-            const uint64_t da = da_m + (uint64_t)p.tap_off16[tp];
-            const uint64_t db = db_w + (uint64_t)(tp * w_step16);
-#pragma unroll
-            for (int k = 0; k < NMMA; ++k) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * k, db + 2 * k, idesc);
-          }
-        }
-        tc::mma_commit(empty_bar + 8u * s);
-        tc::mma_commit(tfull_bar + 8u * set);
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 3] = clock64();
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else {
-    // ===== epilogue =====
-    const int q = warp & 3;
-    const int grp = ((warp - 2) >> 2) & 1;   // accumulator set (tile parity)
-    const int half = (warp - 2) >> 3;        // even / odd M tiles of the set
-    const bool tracer = p.trace && blockIdx.x == 0 && threadIdx.x == 64;
-    int j = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
-      const uint32_t set = (uint32_t)j & 1u;   // accumulator set == epilogue group
-      const uint32_t use = (uint32_t)j >> 1;
-      if ((int)set != grp) continue;
-      int b, ra, rb, rc, td, th, tw;
-      decode(tile, b, ra, rb, rc, td, th, tw);
-      if (tracer && j < 64) p.trace[j * 8 + 4] = clock64();
-      tc::mbar_wait(tfull_bar + 8u * set, use & 1u);
-      tc::fence_after_sync();
-      if (tracer && j < 64) p.trace[j * 8 + 5] = clock64();
-      for (int m = half; m < p.nM; m += 2) {   // one epilogue group per M tile parity
-        const int R = p.R0 + m * 128 + q * 32 + lane;
-        const int pw = R % p.PW;
-        const int phh = (R / p.PW) % p.PH;
-        const int pd = R / (p.PW * p.PH);
-        const int od = (td * p.BD + pd - p.hd) * d + ra, oh = (th * p.BH + phh - p.hh) * d + rb,
-                  ow = (tw * p.BW + pw - p.hw) * d + rc;
-        const bool valid = pd >= p.hd && pd < p.hd + p.BD && phh >= p.hh && phh < p.hh + p.BH && pw >= p.hw &&
-                           pw < p.hw + p.BW && od < p.D && oh < p.H && ow < p.W;
-        const uint32_t taddr = tmem_base + set * (uint32_t)p.set_stride + (uint32_t)(m * p.N_tile) +
-                               ((uint32_t)(q * 32) << 16);
-        if (epi_fast_ok(p.epi)) {
-          const EpiRow<T> er = epi_row<T>(p.epi, valid, b, od, oh, ow, 0);
-          uint32_t ra[16];
-          EpiPre pre;
-          for (int c0 = 0; c0 < p.N_tile; c0 += 16) {
-            tc::tmem_ld16_issue(taddr + (uint32_t)c0, ra);
-            epi_prefetch<T>(er, c0, pre);
-            tc::tmem_ld_wait16(ra);
-            epi_finish<T>(er, c0, ra, pre);
-          }
-        } else {
-          for (int c0 = 0; c0 < p.N_tile; c0 += 16) {
-            float v[16];
-            tc::tmem_ld16(taddr + (uint32_t)c0, v);
-            if (valid) conv_epilogue_row<T, 16>(p.epi, b, od, oh, ow, c0, v);
-          }
-        }
-      }
-      tc::fence_before_sync();
-      tc::mbar_arrive(tempty_bar + 8u * set);
-      if (tracer && j < 64) p.trace[j * 8 + 6] = clock64();
-    }
+    return;
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+
+  // ===== MMA + epilogue warpgroups: M tile m, rows [64 wg, 64 wg + 64) =====
+  tc::reg_alloc<232>();
+  const int wg = (warp >> 2) - 1;
+  const int warp4 = warp & 3;
+  const int t = threadIdx.x & 127;
+  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
+  const int nmma = RB / 32;
+  const int nc = (p.N_tile + 31) >> 5;
+  const uint32_t b_chunk16 = (uint32_t)(2 * RB);
+  const uint64_t db_w = tc::make_sdesc(smem_w, RB);
+  const int w_step16 = p.b_stride / 16;
+  float acc[NC][16];
+  tc::mbar_wait(w_bar, 0);
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int b, ra, rb, rc, td, th, tw;
+    decode(tile, b, ra, rb, rc, td, th, tw);
+    tc::mbar_wait(full_bar + 8u * s, ph);
+    // descriptors advance by plain 64-bit adds on the 16-byte-unit address field (smem < 256 KB: no carry out of
+    // the 14-bit field)
+    const uint64_t da_stage = tc::make_sdesc(smem_a + (uint32_t)s * p.a_stage_bytes, RB) +
+                              (uint64_t)(64 * wg * RB / 16);
+    for (int m = 0; m < p.nM; ++m) {
+      const uint64_t da_m = da_stage + (uint64_t)(m * (128 * RB / 16));
+      tc::wg_fence();
+      for (int tp = 0; tp < p.n_taps; ++tp)
+        mma_item<T, NC>(acc, da_m + (uint64_t)p.tap_off16[tp], db_w + (uint64_t)(tp * w_step16), nmma, nc, b_chunk16,
+                        tp == 0);
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      if (m == p.nM - 1 && lane == 0) tc::mbar_arrive(empty_bar + 8u * s);   // the box is no longer read
+      acc_fence_all<NC>(acc);
+      const int R = p.R0 + m * 128 + 64 * wg + t;   // epilogue threads t < 64: one row each
+      const int pw = R % p.PW;
+      const int phh = (R / p.PW) % p.PH;
+      const int pd = R / (p.PW * p.PH);
+      const int od = (td * p.BD + pd - p.hd) * d + ra, oh = (th * p.BH + phh - p.hh) * d + rb,
+                ow = (tw * p.BW + pw - p.hw) * d + rc;
+      const bool valid = pd >= p.hd && pd < p.hd + p.BD && phh >= p.hh && phh < p.hh + p.BH && pw >= p.hw &&
+                         pw < p.hw + p.BW && od < p.D && oh < p.H && ow < p.W;
+      epilogue_rows<T, NC, LD>(p.epi, acc, st, 1 + wg, warp4, lane, t, p.N_tile, valid, b, od, oh, ow, 0, nullptr);
+    }
+    if (++s == p.stages) { s = 0; ph ^= 1u; }
   }
 }
 
 
 // ------------------------------------------------------------------------------------------------
 // x-packed halo kernel for grids whose innermost extent W is one warp wide or narrower (W in {8, 16, 32}: every
-// 3-D activation of this network -- Z = 32 / 16 / 8).  Measured on B200 (tools/micro/mma_issue_bench.cu,
-// profiles/r02_mma_issue_bench.txt): one tcgen05.mma costs max(59, N/2) cycles for M = 128 whatever the operand
-// type, so a 32-output-channel conv issued tap by tap runs the tensor pipe at N/2 / 59 = 27 % (bf16) and, with
-// K = 8 per instruction, 14 % (TF32).  Here the three W taps (dx = -d, 0, +d) of each (dz, dy) pair share ONE
-// instruction: its B operand stacks the three taps' weights along N (N = 3 * Cout_pad: three consecutive tap slices
-// of the ordinary weight tensor), its A operand is the un-shifted rows, and the accumulator holds
+// 3-D activation of this network -- Z = 32 / 16 / 8).  A 32-output-channel conv issued tap by tap keeps the tensor
+// core at N = 32; here the three W taps (dx = -d, 0, +d) of each (dz, dy) pair share ONE instruction: its B operand
+// stacks the three taps' weights along N (N = 3 * Cout_pad: three consecutive tap slices of the ordinary weight
+// tensor), its A operand is the un-shifted rows, and the accumulator holds
 //     Q_c[r] = sum_{a,b} W[a][b][c] . in[r + (a*PH + b)*PW]      c = 0, 1, 2
 // from which the epilogue forms out[r] = Q_0[r - d] + Q_1[r] + Q_2[r + d].  Smem rows are linearised with W
-// fastest and PW == W divides 32, so r +- d stays inside the warp: two shuffles per channel, masked where the
-// neighbour would fall outside [0, W) -- which is exactly the convolution's zero padding, so the W axis needs no
-// halo columns and no sub-sampling.  D and H keep the halo-tile scheme (one zero-filled halo position per side on
-// the d-sub-sampled grids, TMA traversal stride d).  27 taps become 9 instructions per 32 bytes of K.
-// out[r] = Q0[r - d] + Q1[r] + Q2[r + d] for 16 channels of this lane's row: the three accumulator column groups of
-// the x-packed MMA (lane == W position; lanes shifted out of [0, W) contribute the conv's zero padding).  The three
-// tcgen05.ld are issued back to back and share ONE wait.
-__device__ __forceinline__ void halox_gather16(uint32_t taddr, int c0, int CP, int d, bool lo_ok, bool hi_ok, float* v) {
-  uint32_t lo[16], mid[16], hi[16];
-  tc::tmem_ld16_issue(taddr + (uint32_t)c0, lo);
-  tc::tmem_ld16_issue(taddr + (uint32_t)(CP + c0), mid);
-  tc::tmem_ld16_issue(taddr + (uint32_t)(2 * CP + c0), hi);
-  tc::tmem_ld_wait16(lo);
-  tc::tmem_ld_dep16(mid);
-  tc::tmem_ld_dep16(hi);
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const float l = __shfl_up_sync(0xffffffffu, __uint_as_float(lo[i]), (unsigned)d);
-    const float h = __shfl_down_sync(0xffffffffu, __uint_as_float(hi[i]), (unsigned)d);
-    v[i] = __uint_as_float(mid[i]) + (lo_ok ? l : 0.f) + (hi_ok ? h : 0.f);
-  }
-}
-
+// fastest and PW == W divides 32, so r +- d stays inside one line of the tile, masked where the neighbour would fall
+// outside [0, W) -- which is exactly the convolution's zero padding, so the W axis needs no halo columns and no
+// sub-sampling.  D and H keep the halo-tile scheme (one zero-filled halo position per side on the d-sub-sampled
+// grids, TMA traversal stride d).  27 taps become 9 instructions per 32 bytes of K.
 struct HaloxParams {
   ConvEpi epi;
   int d;                      // dilation (== padding) of the taps
@@ -568,75 +506,58 @@ struct HaloxParams {
   int mt_row[2], mt_pd[2], mt_ph0[2];
   int box_bytes, a_stage_bytes, stages;
   int n_groups;               // (dz, dy) groups = n_taps / 3
-  int CP, N_tile;             // padded output channels, N_tile = 3 * CP
-  int tmem_cols, set_stride;
+  int CP, N_tile, rb;         // padded output channels, N_tile = 3 * CP, bytes per K chunk row
   int b_stride, w_bytes;
   int grp_off[9];             // (a*PH + b)*PW: smem row offset of a group's A operand relative to the M tile
   int pdl;
-  long long* trace;
   // plane-ring mode (ring == 1; chosen when the halo box leaves room for ONE stage only, i.e. the TF32 head whose
   // resident weights take 110 KB): the output planes of all columns (image, residue class, H tile) form one sequence
   // of n_cols * sD M tiles; every CTA takes a contiguous, equal share of it (at most one column change inside).  The
   // four stages are a ring of single input planes, output plane z reads ring planes z-1, z, z+1, so every M tile costs
-  // ONE new 6-row plane (prefetched a plane ahead) instead of half a 4-plane box loaded while the tensor pipe waits
+  // ONE new plane (prefetched a plane ahead) instead of a whole box loaded while the tensor core waits
   int ring, sD, n_cols;
   signed char grp_dz[9];      // -1 / 0 / +1: which ring plane a group reads
   short grp_row[9];           // (hh + dy) * PW: its row offset inside the plane
 };
 
-template <typename T, int RB>
-__global__ void __launch_bounds__(kTcThreads)
+template <typename T>
+__global__ void __launch_bounds__(kTcThreads, 1)
 conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__ CUtensorMap tmA,
                   const __grid_constant__ CUtensorMap tmW) {
-  constexpr int NMMA = RB / 32;
+  constexpr int NC = 8;   // N_tile = 3 * CP <= 256
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_w = smem_base;                                   // [n_groups][b_stride] resident weights
   const uint32_t smem_a = smem_w + (uint32_t)p.w_bytes;                 // [stages][a_stage_bytes]
-  const uint32_t bar_base = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
+  constexpr int LD = kStageNarrow;
+  const uint32_t smem_st = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
+  const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
   const uint32_t full_bar = bar_base;            // [4]
   const uint32_t empty_bar = bar_base + 32u;     // [4]
-  const uint32_t tfull_bar = bar_base + 64u;     // [2]
-  const uint32_t tempty_bar = bar_base + 80u;    // [2]
-  const uint32_t w_bar = bar_base + 96u;
-  const uint32_t tmem_slot = bar_base + 104u;
+  const uint32_t w_bar = bar_base + 64u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int d = p.d;
+  const int RB = p.rb;
   const int num_tiles = p.epi.B * d * d * p.tilesD * p.tilesH;
   // ring mode: this CTA's share [ring_lo, ring_hi) of the n_cols * sD output planes
   const long long ring_total = (long long)p.n_cols * p.sD;
   const long long ring_lo = p.ring ? ring_total * blockIdx.x / gridDim.x : 0;
   const long long ring_hi = p.ring ? ring_total * (blockIdx.x + 1) / gridDim.x : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&tmA);
     tc::prefetch_tmap(&tmW);
     for (int s = 0; s < p.stages; ++s) {
       tc::mbar_init(full_bar + 8u * s, 1);
-      tc::mbar_init(empty_bar + 8u * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      tc::mbar_init(tfull_bar + 8u * a, 1);
-      tc::mbar_init(tempty_bar + 8u * a, 256);
+      tc::mbar_init(empty_bar + 8u * s, kEmptyArrivals);
     }
     tc::mbar_init(w_bar, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  if (p.pdl) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
+  pdl_prologue_done(p.pdl);
 
   // tile -> (batch, (D, H) residue class, sub-grid tile origin)
   auto decode = [&](int tile, int& b, int& ra, int& rb, int& td, int& th) {
@@ -661,217 +582,125 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
     b = t;
   };
 
-  if (warp == 0) {
-    if (lane == 0 && p.ring) {
-      // ===== TMA producer, ring mode: weights once, then planes z0-1 .. z1 of every unit, one ring slot each =====
+  if (warp < 4) {
+    tc::reg_dealloc<40>();
+    if (warp == 0 && lane == 0) {
+      // ===== TMA producer: resident weights once, then (ring) planes z0-1 .. z1 of every unit, one ring slot each,
+      // or (box) one halo box per tile =====
       tc::mbar_expect_tx(w_bar, (uint32_t)(p.n_groups * p.N_tile * RB));
       for (int g = 0; g < p.n_groups; ++g)
         tc::tma_load_2d(smem_w + (uint32_t)g * p.b_stride, &tmW, w_bar, 0, g * p.N_tile);
-      uint32_t n = 0;
-      for (long long pos = ring_lo; pos < ring_hi;) {
-        int b, ra, rb, th, z0, z1;
-        decode_ring(pos, b, ra, rb, th, z0, z1);
-        pos += z1 - z0;
-        for (int z = z0 - 1; z <= z1; ++z, ++n) {
-          const uint32_t slot = n & 3u;
-          if (p.trace && blockIdx.x == 0 && n < 64) p.trace[n * 8 + 0] = clock64();
-          tc::mbar_wait(empty_bar + 8u * slot, ((n >> 2) & 1u) ^ 1u);
-          if (p.trace && blockIdx.x == 0 && n < 64) p.trace[n * 8 + 1] = clock64();
-          tc::mbar_expect_tx(full_bar + 8u * slot, (uint32_t)p.box_bytes);
-          tc::tma_load_5d(smem_a + slot * (uint32_t)p.a_stage_bytes, &tmA, full_bar + 8u * slot, 0, 0,
-                          (th * p.BH - p.hh) * d + rb, z * d + ra + p.src_d0, b);
-        }
-      }
-    } else if (lane == 0) {
-      // ===== TMA producer: resident weights once, then one halo box per tile =====
-      tc::mbar_expect_tx(w_bar, (uint32_t)(p.n_groups * p.N_tile * RB));
-      for (int g = 0; g < p.n_groups; ++g)
-        tc::tma_load_2d(smem_w + (uint32_t)g * p.b_stride, &tmW, w_bar, 0, g * p.N_tile);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int b, ra, rb, td, th;
-        decode(tile, b, ra, rb, td, th);
-        tc::mbar_wait(empty_bar + 8u * s, ph ^ 1u);
-        tc::mbar_expect_tx(full_bar + 8u * s, (uint32_t)p.box_bytes);
-        tc::tma_load_5d(smem_a + (uint32_t)s * p.a_stage_bytes, &tmA, full_bar + 8u * s, 0, 0,
-                        (th * p.BH - p.hh) * d + rb, (td * p.BD - p.hd) * d + ra + p.src_d0, b);
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && p.ring) {
-      // ===== MMA issuer, ring mode =====
-      const uint32_t idesc = tc::Mma<T>::idesc(128, p.N_tile);
-      const uint64_t db_w = tc::make_sdesc(smem_w, RB);
-      const int w_step16 = p.b_stride / 16;
-      // A descriptors of the nine groups for each of the four ring rotations, built once (the issuing thread must not
-      // spend its ~60 cycles per MMA on address arithmetic)
-      uint64_t* dtab = reinterpret_cast<uint64_t*>(smem_raw + (bar_base - tc::smem_u32(smem_raw)) + 128u);
-      for (int r = 0; r < 4; ++r)
-        for (int g = 0; g < 9; ++g) {
-          const uint32_t slot = (uint32_t)(r + (g < p.n_groups ? p.grp_dz[g] : 0)) & 3u;
-          dtab[r * 9 + g] = tc::make_sdesc(smem_a + slot * (uint32_t)p.a_stage_bytes, RB) +
-                            (uint64_t)((g < p.n_groups ? p.grp_row[g] : 0) * (RB / 16));
-        }
-      tc::mbar_wait(w_bar, 0);
-      uint32_t n0 = 0;     // ring index of this unit's first plane (z0 - 1)
-      uint32_t j = 0;      // output planes so far == accumulator uses
-      for (long long pos = ring_lo; pos < ring_hi;) {
-        int b, ra, rb, th, z0, z1;
-        decode_ring(pos, b, ra, rb, th, z0, z1);
-        pos += z1 - z0;
-        const int K = z1 - z0;
-        for (int k = 0; k < K; ++k, ++j) {
-          const uint32_t set = j & 1u;
-          tc::mbar_wait(tempty_bar + 8u * set, ((j >> 1) & 1u) ^ 1u);
-          for (uint32_t i = (k == 0 ? 0u : 2u); i < 3u; ++i) {     // planes z-1 and z were waited for by plane z-1
-            const uint32_t n = n0 + (uint32_t)k + i;
-            tc::mbar_wait(full_bar + 8u * (n & 3u), (n >> 2) & 1u);
-          }
-          tc::fence_after_sync();
-          if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 2] = clock64();
-          const uint32_t d_tmem = tmem_base + set * (uint32_t)p.set_stride;
-          const uint64_t* drow = dtab + ((n0 + (uint32_t)k + 1u) & 3u) * 9u;
-          uint64_t dg[9];
-#pragma unroll
-          for (int g = 0; g < 9; ++g) dg[g] = drow[g];
-#pragma unroll
-          for (int g = 0; g < 9; ++g) {
-            if (g < p.n_groups) {
-              const uint64_t da = dg[g];
-              const uint64_t db = db_w + (uint64_t)(g * w_step16);
-              if (g == 0) tc::Mma<T>::template issue<0>(d_tmem, da, db, idesc);
-              else tc::Mma<T>::template issue<1>(d_tmem, da, db, idesc);
-#pragma unroll
-              for (int kk = 1; kk < NMMA; ++kk) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * kk, db + 2 * kk, idesc);
-            }
-          }
-          tc::mma_commit(tfull_bar + 8u * set);
-          if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 3] = clock64();
-          tc::mma_commit(empty_bar + 8u * ((n0 + (uint32_t)k) & 3u));            // plane z-1 is done with
-          if (k == K - 1) {                                                       // ... and the unit's last two
-            tc::mma_commit(empty_bar + 8u * ((n0 + (uint32_t)k + 1u) & 3u));
-            tc::mma_commit(empty_bar + 8u * ((n0 + (uint32_t)k + 2u) & 3u));
+      if (p.ring) {
+        uint32_t n = 0;
+        for (long long pos = ring_lo; pos < ring_hi;) {
+          int b, ra, rb, th, z0, z1;
+          decode_ring(pos, b, ra, rb, th, z0, z1);
+          pos += z1 - z0;
+          for (int z = z0 - 1; z <= z1; ++z, ++n) {
+            const uint32_t slot = n & 3u;
+            tc::mbar_wait(empty_bar + 8u * slot, ((n >> 2) & 1u) ^ 1u);
+            tc::mbar_expect_tx(full_bar + 8u * slot, (uint32_t)p.box_bytes);
+            tc::tma_load_5d(smem_a + slot * (uint32_t)p.a_stage_bytes, &tmA, full_bar + 8u * slot, 0, 0,
+                            (th * p.BH - p.hh) * d + rb, z * d + ra + p.src_d0, b);
           }
         }
-        n0 += (uint32_t)K + 2u;
-      }
-    } else if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = tc::Mma<T>::idesc(128, p.N_tile);
-      const uint64_t db_w = tc::make_sdesc(smem_w, RB);
-      const int w_step16 = p.b_stride / 16;
-      tc::mbar_wait(w_bar, 0);
-      int s = 0;
-      uint32_t ph = 0;
-      int j = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++j) {
-        const uint32_t set = (uint32_t)j & 1u;
-        const uint32_t use = (uint32_t)j >> 1;
-        tc::mbar_wait(tempty_bar + 8u * set, (use & 1u) ^ 1u);
-        tc::mbar_wait(full_bar + 8u * s, ph);
-        tc::fence_after_sync();
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 2] = clock64();
-        const uint64_t da_stage = tc::make_sdesc(smem_a + (uint32_t)s * p.a_stage_bytes, RB);
-        for (int m = 0; m < p.nM; ++m) {
-          const uint32_t d_tmem = tmem_base + set * (uint32_t)p.set_stride + (uint32_t)(m * p.N_tile);
-          {
-            const uint64_t da = da_stage + (uint64_t)((p.mt_row[m] + p.grp_off[0]) * (RB / 16));
-            tc::Mma<T>::template issue<0>(d_tmem, da, db_w, idesc);
-#pragma unroll
-            for (int k = 1; k < NMMA; ++k) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * k, db_w + 2 * k, idesc);
-          }
-#pragma unroll 2
-          for (int g = 1; g < p.n_groups; ++g) {
-            const uint64_t da = da_stage + (uint64_t)((p.mt_row[m] + p.grp_off[g]) * (RB / 16));
-            const uint64_t db = db_w + (uint64_t)(g * w_step16);
-#pragma unroll
-            for (int k = 0; k < NMMA; ++k) tc::Mma<T>::template issue<1>(d_tmem, da + 2 * k, db + 2 * k, idesc);
-          }
-        }
-        tc::mma_commit(empty_bar + 8u * s);
-        tc::mma_commit(tfull_bar + 8u * set);
-        if (p.trace && blockIdx.x == 0 && j < 64) p.trace[j * 8 + 3] = clock64();
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else {
-    // ===== epilogue: 16 warps; group (egrp & 1) drains accumulator set (tile parity), (egrp >> 1) picks the work
-    // items (M tile, 16-channel chunk) it takes =====
-    const int q = warp & 3;
-    const int egrp = (warp - 2) >> 2;
-    const int grp = egrp & 1;
-    const int half = egrp >> 1;
-    const int rr = q * 32 + lane;            // row inside an M tile
-    const int hr = rr / p.PW;                // h-row inside the M tile
-    const int pw = rr - hr * p.PW;           // == output w
-    const bool lo_ok = pw >= d, hi_ok = pw + d < p.PW;
-    const int chunks = p.CP >> 4;
-    const int n_items = p.nM * chunks;
-    const bool tracer = p.trace && blockIdx.x == 0 && threadIdx.x == 64;
-    if (p.ring) {
-      // ring mode: one M tile (one plane, 128 / PW h-rows) per accumulator use
-      uint32_t jr = 0;
-      for (long long pos = ring_lo; pos < ring_hi;) {
-        int b, ra, rb, th, z0, z1;
-        decode_ring(pos, b, ra, rb, th, z0, z1);
-        pos += z1 - z0;
-        for (int z = z0; z < z1; ++z, ++jr) {
-          const uint32_t set = jr & 1u;
-          if ((int)set != grp) continue;
-          if (tracer && jr < 64) p.trace[jr * 8 + 4] = clock64();
-          tc::mbar_wait(tfull_bar + 8u * set, (jr >> 1) & 1u);
-          tc::fence_after_sync();
-          if (tracer && jr < 64) p.trace[jr * 8 + 5] = clock64();
-          const int od = z * d + ra;
-          const int oh = (th * p.BH + hr) * d + rb;
-          const bool valid = od < p.D && oh < p.H;
-          const uint32_t taddr = tmem_base + set * (uint32_t)p.set_stride + ((uint32_t)(q * 32) << 16);
-          for (int it = half; it < chunks; it += 2) {
-            const int c0 = it * 16;
-            float v[16];
-            halox_gather16(taddr, c0, p.CP, d, lo_ok, hi_ok, v);
-            if (valid) conv_epilogue_row<T, 16>(p.epi, b, od, oh, pw, c0, v);
-          }
-          tc::fence_before_sync();
-          tc::mbar_arrive(tempty_bar + 8u * set);
-          if (tracer && jr < 64) p.trace[jr * 8 + 6] = clock64();
+      } else {
+        int s = 0;
+        uint32_t ph = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          int b, ra, rb, td, th;
+          decode(tile, b, ra, rb, td, th);
+          tc::mbar_wait(empty_bar + 8u * s, ph ^ 1u);
+          tc::mbar_expect_tx(full_bar + 8u * s, (uint32_t)p.box_bytes);
+          tc::tma_load_5d(smem_a + (uint32_t)s * p.a_stage_bytes, &tmA, full_bar + 8u * s, 0, 0,
+                          (th * p.BH - p.hh) * d + rb, (td * p.BD - p.hd) * d + ra + p.src_d0, b);
+          if (++s == p.stages) { s = 0; ph ^= 1u; }
         }
       }
     }
-    int j = 0;
-    for (int tile = blockIdx.x; !p.ring && tile < num_tiles; tile += gridDim.x, ++j) {
-      const uint32_t set = (uint32_t)j & 1u;
-      const uint32_t use = (uint32_t)j >> 1;
-      if ((int)set != grp) continue;
-      int b, ra, rb, td, th;
-      decode(tile, b, ra, rb, td, th);
-      if (tracer && j < 64) p.trace[j * 8 + 4] = clock64();
-      tc::mbar_wait(tfull_bar + 8u * set, use & 1u);
-      tc::fence_after_sync();
-      if (tracer && j < 64) p.trace[j * 8 + 5] = clock64();
-      for (int it = half; it < n_items; it += 2) {
-        const int m = it / chunks, c0 = (it - m * chunks) * 16;
-        const int od = (td * p.BD + p.mt_pd[m] - p.hd) * d + ra;
-        const int oh = (th * p.BH + p.mt_ph0[m] + hr - p.hh) * d + rb;
-        const bool valid = od < p.D && oh < p.H;
-        const uint32_t taddr = tmem_base + set * (uint32_t)p.set_stride + (uint32_t)(m * p.N_tile) +
-                               ((uint32_t)(q * 32) << 16);
-        float v[16];
-        halox_gather16(taddr, c0, p.CP, d, lo_ok, hi_ok, v);
-        if (valid) conv_epilogue_row<T, 16>(p.epi, b, od, oh, pw, c0, v);
-      }
-      tc::fence_before_sync();
-      tc::mbar_arrive(tempty_bar + 8u * set);
-      if (tracer && j < 64) p.trace[j * 8 + 6] = clock64();
-    }
+    return;
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+
+  // ===== MMA + epilogue warpgroups: rows [64 wg, 64 wg + 64) of each M tile =====
+  tc::reg_alloc<232>();
+  const int wg = (warp >> 2) - 1;
+  const int warp4 = warp & 3;
+  const int t = threadIdx.x & 127;
+  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
+  const int nmma = RB / 32;
+  const int nc = (p.N_tile + 31) >> 5;
+  const uint32_t b_chunk16 = (uint32_t)(2 * RB);
+  const uint64_t db_w = tc::make_sdesc(smem_w, RB);
+  const int w_step16 = p.b_stride / 16;
+  const int rr = 64 * wg + t;              // row inside an M tile (epilogue threads t < 64)
+  const int hr = rr / p.PW;                // h-row inside the M tile
+  const int pw = rr - hr * p.PW;           // == output w
+  const bool lo_ok = pw >= d, hi_ok = pw + d < p.PW;
+  float acc[NC][16];
+  tc::mbar_wait(w_bar, 0);
+  if (p.ring) {
+    // one M tile (one plane, 128 / PW h-rows) per output plane
+    uint32_t n0 = 0;     // ring index of this unit's first plane (z0 - 1)
+    for (long long pos = ring_lo; pos < ring_hi;) {
+      int b, ra, rb, th, z0, z1;
+      decode_ring(pos, b, ra, rb, th, z0, z1);
+      pos += z1 - z0;
+      const int K = z1 - z0;
+      for (int k = 0; k < K; ++k) {
+        for (uint32_t i = (k == 0 ? 0u : 2u); i < 3u; ++i) {     // planes z-1 and z were waited for by plane z-1
+          const uint32_t n = n0 + (uint32_t)k + i;
+          tc::mbar_wait(full_bar + 8u * (n & 3u), (n >> 2) & 1u);
+        }
+        const uint32_t r = n0 + (uint32_t)k + 1u;                 // ring index of plane z
+        tc::wg_fence();
+        for (int g = 0; g < p.n_groups; ++g) {
+          const uint32_t slot = (r + (uint32_t)p.grp_dz[g]) & 3u;
+          const uint64_t da = tc::make_sdesc(smem_a + slot * (uint32_t)p.a_stage_bytes, RB) +
+                              (uint64_t)((p.grp_row[g] + 64 * wg) * (RB / 16));
+          mma_item<T, NC>(acc, da, db_w + (uint64_t)(g * w_step16), nmma, nc, b_chunk16, g == 0);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        if (lane == 0) {
+          tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k) & 3u));          // plane z-1 is done with
+          if (k == K - 1) {                                                     // ... and the unit's last two
+            tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k + 1u) & 3u));
+            tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k + 2u) & 3u));
+          }
+        }
+        acc_fence_all<NC>(acc);
+        const int od = (z0 + k) * d + ra;
+        const int oh = (th * p.BH + hr) * d + rb;
+        const bool valid = t < 64 && od < p.D && oh < p.H;
+        epilogue_xp<T, NC>(p.epi, acc, st, 1 + wg, warp4, lane, t, p.CP, d, lo_ok, hi_ok, valid, b, od, oh, pw);
+      }
+      n0 += (uint32_t)K + 2u;
+    }
+    return;
+  }
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int b, ra, rb, td, th;
+    decode(tile, b, ra, rb, td, th);
+    tc::mbar_wait(full_bar + 8u * s, ph);
+    const uint64_t da_stage = tc::make_sdesc(smem_a + (uint32_t)s * p.a_stage_bytes, RB);
+    for (int m = 0; m < p.nM; ++m) {
+      tc::wg_fence();
+      for (int g = 0; g < p.n_groups; ++g) {
+        const uint64_t da = da_stage + (uint64_t)((p.mt_row[m] + p.grp_off[g] + 64 * wg) * (RB / 16));
+        mma_item<T, NC>(acc, da, db_w + (uint64_t)(g * w_step16), nmma, nc, b_chunk16, g == 0);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      if (m == p.nM - 1 && lane == 0) tc::mbar_arrive(empty_bar + 8u * s);
+      acc_fence_all<NC>(acc);
+      const int od = (td * p.BD + p.mt_pd[m] - p.hd) * d + ra;
+      const int oh = (th * p.BH + p.mt_ph0[m] + hr - p.hh) * d + rb;
+      const bool valid = t < 64 && od < p.D && oh < p.H;
+      epilogue_xp<T, NC>(p.epi, acc, st, 1 + wg, warp4, lane, t, p.CP, d, lo_ok, hi_ok, valid, b, od, oh, pw);
+    }
+    if (++s == p.stages) { s = 0; ph ^= 1u; }
   }
 }
 
@@ -964,14 +793,15 @@ int chunk_channels(int C, int esize) {
   return 128 / esize;
 }
 
-long long* g_trace_buf = nullptr;
-
 }  // namespace
 
-// debug hook (tools/conv_trace.py): plans created while a buffer is set record per-role clock64 stamps of CTA 0
-// into it ([64 tiles][8] int64, device memory owned by the caller); NULL switches tracing off again
+// per-role clock64 tracing of the conv kernels: part of the ABI, not built into the sm_90a kernels.  NULL (tracing
+// off) is accepted; a buffer is refused.
 extern "C" int occd_conv_debug_trace(long long* device_buf) {
-  g_trace_buf = device_buf;
+  if (device_buf) {
+    occd_set_last_error("occd_conv_debug_trace: per-role tracing is not available in this build");
+    return OCCD_ERR_UNSUPPORTED;
+  }
   return OCCD_OK;
 }
 
@@ -1013,8 +843,7 @@ static int fill_epi(const occd_conv_desc* d, ConvEpi* e) {
 }
 
 // Programmatic dependent launch (common.cuh): the conv kernels wait on griddepcontrol after their prologue (barrier
-// init, TMEM alloc, tensor-map prefetch overlap the tail of the previous grid).  Measured on B200 (round 2,
-// profiles/r02_ab_experiments.txt): 1.0 % of the config-2 forward, results bit-identical.
+// init, tensor-map prefetch overlap the tail of the previous grid); results are bit-identical either way.
 static int pdl_enabled() { return occd_pdl_enabled(); }
 
 template <typename... KArgs, typename... Args>
@@ -1036,11 +865,11 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, int threads, 
 static int n_sms_current() {
   static int n_sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (n_sms[dev] == 0) {
     int v = 0;
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n_sms[dev] = v;
-    else n_sms[dev] = 148;
+    else n_sms[dev] = 132;
   }
   return n_sms[dev];
 }
@@ -1087,7 +916,7 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.w_bytes = h.n_taps * h.b_stride;
   HALO_REQUIRE(h.w_bytes <= 112 * 1024, "weights do not fit in shared memory");
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil, sW = (d->IW + dil - 1) / dil;
-  const int smem_total = 224 * 1024 - h.w_bytes - 2048;
+  const int smem_total = 227 * 1024 - staging_bytes(kStageHalo) - h.w_bytes - 2048;   // staging, barriers, slack
   // W extent of the box: the whole sub-sampled line when it fits, else equal splits of at most 62
   const int nW = (sW + 61) / 62;
   const int BW = (sW + nW - 1) / nW;
@@ -1118,15 +947,12 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.box_bytes = h.PD * h.PH * h.PW * row_bytes;
   h.stages = smem_total / h.a_stage_bytes;
   if (h.stages > 4) h.stages = 4;
-  h.set_stride = 32;
-  while (h.set_stride < h.nM * h.N_tile) h.set_stride *= 2;
-  h.tmem_cols = 2 * h.set_stride;
+  h.rb = row_bytes;
   for (int i = 0; i < d->n_taps; ++i)
     h.tap_off16[i] = (h.R0 + ((d->taps[i].dz / dil) * h.PH + d->taps[i].dy / dil) * h.PW + d->taps[i].dx / dil) *
                      row_bytes / 16;
-  h.trace = g_trace_buf;
   h.pdl = pdl_enabled();
-  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + 128 + 1024;
+  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(kStageHalo) + 128 + 1024;
   const long long num_tiles = (long long)d->B * dil * dil * dil * h.tilesD * h.tilesH * h.tilesW;
   HALO_REQUIRE(num_tiles < 2147483647LL, "too many tiles");
   const int n_sms = n_sms_current();
@@ -1172,10 +998,11 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.n_groups = d->n_taps / 3;
   h.CP = d->Cout_pad;
   h.N_tile = 3 * d->Cout_pad;
+  h.rb = RB;
   h.PW = d->IW;
   h.b_stride = round_up(h.N_tile * RB, 1024);
   h.w_bytes = h.n_groups * h.b_stride;
-  const int smem_total = 227 * 1024 - h.w_bytes - 4096;   // barriers, TMEM slot, 1024-byte alignment slack
+  const int smem_total = 227 * 1024 - staging_bytes(kStageNarrow) - h.w_bytes - 2048;   // staging, barriers, slack
   HX_REQUIRE(smem_total > 0, "weights do not fit in shared memory");
   const int HR = 128 / h.PW;                               // h-rows of one plane per M tile
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil;
@@ -1191,9 +1018,6 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
     if (stage > smem_total) continue;
     const int stages = smem_total / stage;
     const int nM = BD * nB;
-    int set_stride = 32;
-    while (set_stride < nM * h.N_tile) set_stride *= 2;
-    if (2 * set_stride > 512) continue;
     // cycles per useful output: MMA issue floor (59 cycles per instruction at N <= 118) plus, single-buffered,
     // the un-overlapped L2 -> smem fill at the chip's ~42 B/cycle/SM
     const double eff_d = (double)(sD < BD ? sD : BD) / BD, eff_h = (double)(sH < BH ? sH : BH) / BH;
@@ -1205,14 +1029,13 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
       best = cost;
       h.BD = BD; h.BH = BH; h.PD = PD; h.PH = PH; h.nM = nM;
       h.a_stage_bytes = stage; h.stages = stages > 4 ? 4 : stages;
-      h.set_stride = set_stride;
     }
   }
   HX_REQUIRE(best >= 0, "no tile shape fits");
   h.ring = 0;
   {
     // plane ring instead of a single-stage box (see HaloxParams): needs D taps and four single-plane stages.
-    // OCCD_HALOX_RING=0 keeps the box (experiment hook, tools/conv_bench.py)
+    // OCCD_HALOX_RING=0 keeps the box (experiment hook)
     static const bool ring_off = [] { const char* e = getenv("OCCD_HALOX_RING"); return e && atoi(e) == 0; }();
     const int PHr = HR + 2 * hal[1];
     const int plane = round_up(PHr * h.PW * RB, 1024);
@@ -1220,8 +1043,6 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
       h.ring = 1;
       h.BD = 1; h.BH = HR; h.PD = 3; h.PH = PHr; h.nM = 1;
       h.a_stage_bytes = plane; h.stages = 4;
-      h.set_stride = 32;
-      while (h.set_stride < h.N_tile) h.set_stride *= 2;
     }
   }
   {
@@ -1234,7 +1055,6 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
         h.mt_row[m] = (h.mt_pd[m] * h.PH + h.mt_ph0[m]) * h.PW;
       }
   }
-  h.tmem_cols = 2 * h.set_stride;
   h.tilesD = (sD + h.BD - 1) / h.BD; h.tilesH = (sH + h.BH - 1) / h.BH;
   h.box_bytes = (h.ring ? 1 : h.PD) * h.PH * h.PW * RB;
   for (int g = 0; g < h.n_groups; ++g) {
@@ -1244,9 +1064,8 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   }
   h.sD = sD;
   h.n_cols = d->B * dil * dil * h.tilesH;
-  h.trace = g_trace_buf;
   h.pdl = pdl_enabled();
-  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + 128 + 512 + 1024;   // barriers, ring-mode descriptor table, alignment slack
+  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(kStageNarrow) + 128 + 1024;
   const long long num_tiles = h.ring ? (long long)h.n_cols * sD      // ring mode: M tiles; each CTA takes a contiguous share
                                      : (long long)d->B * dil * dil * h.tilesD * h.tilesH;
   HX_REQUIRE(num_tiles < 2147483647LL, "too many tiles");
@@ -1423,12 +1242,9 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
   }
   t.TWv = xp ? 30 : t.TW;
   t.tiles_w = (d->OW + t.TWv - 1) / t.TWv; t.tiles_h = (d->OH + t.TH - 1) / t.TH; t.tiles_d = (d->OD + t.TD - 1) / t.TD;
-  // N tile: the divisor of Cout_pad (multiple of 16, <= 256) with the smallest estimated makespan.  Three measured
-  // B200 constants drive the model (profiles/r02_mma_issue_bench.txt, r02_conv_role_traces.txt, r02_membw.txt):
-  //   one tcgen05.mma costs max(59, N/2) cycles for M = 128, any operand type
-  //   an SM pulls ~44 bytes/cycle from L2 when the whole chip does (6300 B/cycle chip-wide)
-  //   the epilogue drains ~7-12 bytes/cycle/SM (fast path; 12 measured best for the whole forward, r02c)
-  // A tile's main loop (TMA + MMA) overlaps the previous tile's epilogue, so a CTA's time is
+  // N tile: the divisor of Cout_pad (multiple of 16, <= 256) with the smallest estimated makespan.  The model's
+  // constants are estimates, not measurements: an M = 128 MMA step costs max(59, N/2) cycles, an SM pulls ~44
+  // bytes/cycle from L2 when the whole chip does, the epilogue drains ~12 bytes/cycle/SM, and a CTA's time is
   // waves * max(mainloop, epilogue) + min(mainloop, epilogue).  Small-M layers (late encoder stages: 9 M tiles) get
   // narrow N tiles that spread the write-bound epilogue over every SM; large-M layers get the widest tile (fewest
   // re-reads of the A operand).
@@ -1441,7 +1257,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     const int n_sms = n_sms_current();
     const double out_bytes_per_col = 128.0 * ((d->out0 ? pl->esize : 0) + (d->out1_mode == OCCD_OUT1_CL ? pl->esize : 0) +
                                               (d->out1_mode == OCCD_OUT1_F32_PLANAR ? 4 : 0));
-    // experiment hook (tools/conv_bench.py, bench.py): OCCD_EPI_RATE overrides the model's epilogue drain rate
+    // experiment hook: OCCD_EPI_RATE overrides the model's epilogue drain rate
     static const double epi_rate = [] { const char* e = getenv("OCCD_EPI_RATE"); const double v = e ? atof(e) : 0.0;
                                         return v > 0.0 ? v : 12.0; }();
     double best = -1.0;
@@ -1462,10 +1278,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     }
   }
   if (xp) t.N_tile = 3 * d->Cout_pad;  // one N tile: the three taps' weights stacked
-  t.tmem_cols = 32;
-  while (t.tmem_cols < t.N_tile) t.tmem_cols *= 2;
-  t.trace = g_trace_buf;
-  t.tmem_cols *= 2;  // two accumulators: the epilogue of tile j overlaps the MMAs of tile j+1
+  t.rb = RB;
   t.pdl = pdl_enabled();
   t.a_bytes = 128 * RB;
   t.b_bytes = t.N_tile * RB;
@@ -1478,7 +1291,9 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     t.grp_iters[g] = (short)it;
     if (it > total_iters) total_iters = it;
   }
-  const int budget = 200 * 1024;  // persistent kernel: one CTA per SM owns the shared memory
+  // persistent kernel: one CTA per SM owns the shared memory (227 KB less the epilogue staging and barriers)
+  const int st_bytes = staging_bytes(xp ? kStageNarrow : kStageWide);
+  const int budget = 227 * 1024 - st_bytes - 16 * kMaxStages - 64 - 1024;
   // (tap, k-chunk) items per pipeline stage: the single-thread producer/MMA hand-off costs ~0.25 us, so a stage
   // must carry >= ~512 tensor-pipe cycles of work (or up to 9 items) while leaving >= 3 stages in flight
   const int mma_cycles_per_item = (RB / 32) * (128 * t.N_tile / 256);
@@ -1499,7 +1314,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
   }
   if (stages < 1) stages = 1;
   t.stages = stages;
-  pl->smem = (size_t)stages * group * stage_bytes + 16 * kMaxStages + 64 + 1024;  // + barriers + alignment slack
+  pl->smem = (size_t)stages * group * stage_bytes + st_bytes + 16 * kMaxStages + 64 + 1024;  // + staging, barriers, alignment slack
   const long long m_tiles = (long long)d->B * t.tiles_d * t.tiles_h * t.tiles_w;
   const long long all_tiles = m_tiles * (xp ? 1 : d->Cout_pad / t.N_tile) * n_groups;
   if (all_tiles > 2147483647LL) {
@@ -1689,68 +1504,24 @@ extern "C" int occd_conv_plan_info(const occd_conv_plan* pl, int* info) {
   return OCCD_OK;
 }
 
-template <typename T, int RB, bool XP>
-static int launch_tc(const occd_conv_plan* pl, cudaStream_t st) {
+template <auto kernel, typename... Args>
+static int launch_conv(const occd_conv_plan* pl, int pdl, cudaStream_t st, Args&&... args) {
   static bool attr_set[64] = {false};  // per instantiation, per device (the attribute is per device)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) dev = 0;
+  cudaError_t e = cudaSuccess;
   if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<T, RB, XP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
     attr_set[dev] = true;
   }
-  if (pl->tc.pdl) {
-    cudaError_t e = launch_pdl(conv_tc_kernel<T, RB, XP>, pl->grid, kTcThreads, pl->smem, st, pl->tc, pl->tmA[0],
-                               pl->tmA[1], pl->tmA[2], pl->tmW);
+  if (pdl) {
+    e = launch_pdl(kernel, pl->grid, kTcThreads, pl->smem, st, std::forward<Args>(args)...);
     if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
     return OCCD_OK;
   }
-  conv_tc_kernel<T, RB, XP><<<pl->grid, kTcThreads, pl->smem, st>>>(pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2], pl->tmW);
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
-}
-
-template <typename T, int RB>
-static int launch_halo(const occd_conv_plan* pl, cudaStream_t st) {
-  static bool attr_set[64] = {false};  // per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<T, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
-    attr_set[dev] = true;
-  }
-  if (pl->halo.pdl) {
-    cudaError_t e = launch_pdl(conv_halo_kernel<T, RB>, pl->grid, kTcThreads, pl->smem, st, pl->halo, pl->tmA[0],
-                               pl->tmW);
-    if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
-    return OCCD_OK;
-  }
-  conv_halo_kernel<T, RB><<<pl->grid, kTcThreads, pl->smem, st>>>(pl->halo, pl->tmA[0], pl->tmW);
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
-}
-
-template <typename T, int RB>
-static int launch_halox(const occd_conv_plan* pl, cudaStream_t st) {
-  static bool attr_set[64] = {false};  // per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_halox_kernel<T, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
-    attr_set[dev] = true;
-  }
-  if (pl->halox.pdl) {
-    cudaError_t e = launch_pdl(conv_halox_kernel<T, RB>, pl->grid, kTcThreads, pl->smem, st, pl->halox, pl->tmA[0],
-                               pl->tmW);
-    if (e != cudaSuccess) { occd_set_last_error(cudaGetErrorString(e)); return OCCD_ERR_CUDA; }
-    return OCCD_OK;
-  }
-  conv_halox_kernel<T, RB><<<pl->grid, kTcThreads, pl->smem, st>>>(pl->halox, pl->tmA[0], pl->tmW);
+  kernel<<<pl->grid, kTcThreads, pl->smem, st>>>(std::forward<Args>(args)...);
   OCCD_CHECK_LAUNCH();
   return OCCD_OK;
 }
@@ -1762,33 +1533,20 @@ static int run_typed(const occd_conv_plan* pl, cudaStream_t st) {
     OCCD_CHECK_LAUNCH();
     return OCCD_OK;
   }
-  if (pl->impl == OCCD_CONV_IMPL_HALO) {
-    switch (pl->rb) {
-      case 128: return launch_halo<T, 128>(pl, st);
-      case 64: return launch_halo<T, 64>(pl, st);
-      case 32: return launch_halo<T, 32>(pl, st);
-    }
-  }
-  if (pl->impl == OCCD_CONV_IMPL_HALOX) {
-    switch (pl->rb) {
-      case 128: return launch_halox<T, 128>(pl, st);
-      case 64: return launch_halox<T, 64>(pl, st);
-      case 32: return launch_halox<T, 32>(pl, st);
-    }
-  }
-  if (pl->impl == OCCD_CONV_IMPL_TCX) {
-    switch (pl->rb) {
-      case 128: return launch_tc<T, 128, true>(pl, st);
-      case 64: return launch_tc<T, 64, true>(pl, st);
-      case 32: return launch_tc<T, 32, true>(pl, st);
-    }
-  }
+  if (pl->impl == OCCD_CONV_IMPL_HALO)
+    return launch_conv<conv_halo_kernel<T>>(pl, pl->halo.pdl, st, pl->halo, pl->tmA[0], pl->tmW);
+  if (pl->impl == OCCD_CONV_IMPL_HALOX)
+    return launch_conv<conv_halox_kernel<T>>(pl, pl->halox.pdl, st, pl->halox, pl->tmA[0], pl->tmW);
+  if (pl->impl == OCCD_CONV_IMPL_TCX)
+    return launch_conv<conv_tc_kernel<T, 8, true>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2],
+                       pl->tmW);
   if (pl->impl == OCCD_CONV_IMPL_TC) {
-    switch (pl->rb) {
-      case 128: return launch_tc<T, 128, false>(pl, st);
-      case 64: return launch_tc<T, 64, false>(pl, st);
-      case 32: return launch_tc<T, 32, false>(pl, st);
-    }
+    // accumulator registers compiled in: 4 blocks of 32 columns when the N tile fits, else 8
+    if (pl->tc.N_tile <= 128)
+      return launch_conv<conv_tc_kernel<T, 4, false>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2],
+                         pl->tmW);
+    return launch_conv<conv_tc_kernel<T, 8, false>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2],
+                       pl->tmW);
   }
   occd_set_last_error("occd_conv_run: bad plan");
   return OCCD_ERR_ARG;

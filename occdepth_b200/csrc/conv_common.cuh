@@ -23,7 +23,7 @@ struct ConvEpi {
   void* out1;
   int out1_cstride, out1_coff, out1_C;
   int dbg;   // experiment switch (OCCD_DEBUG_EPI, tools/conv_bench.py only): 1 = skip the out0 stores, 2 = skip the
-             // whole row epilogue (TMEM drain only)
+             // whole row epilogue (accumulators are read, nothing is stored)
 };
 
 __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, int oh, int ow, int oa0, int oa1,
@@ -112,12 +112,10 @@ __device__ __forceinline__ void conv_epilogue_row(const ConvEpi& e, int b, int o
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// Fast path of the per-tap and halo kernels' epilogue (out0 only: no second output, no post-activation residual).  Measured
-// on B200 (tools/conv_bench.py with OCCD_DEBUG_EPI, round 2): the row epilogue above is LATENCY bound -- 4 epilogue
-// warps per scheduler walk a serial chain tcgen05.ld -> wait -> bias loads -> (residual loads) -> math -> store per
-// 16 columns, at ~15 % of the SM's issue rate.  Here the chunk's bias (and residual) loads are issued BEFORE the wait
-// on its TMEM load, the output / residual row pointers are formed once per tile, and the activation switch runs once
-// per 16 values.
+// Fast path of the per-tap kernel's epilogue (out0 only: no second output, no post-activation residual).  The row
+// epilogue above walks a serial chain bias loads -> (residual loads) -> math -> store per 16 columns; here the
+// chunk's bias (and residual) loads are issued together, the output / residual row pointers are formed once per tile,
+// and the activation switch runs once per 16 values.
 template <typename T>
 struct EpiRow {
   T* out;            // out0 row of this thread: channels [n0, ...) of its output position (nullptr: nothing to store)

@@ -1,5 +1,5 @@
-// tcgen05 / TMA / mbarrier PTX wrappers for sm_100a (hand-written; bit layouts follow the PTX ISA
-// "tcgen05" matrix-descriptor / instruction-descriptor tables).
+// wgmma / TMA / mbarrier PTX wrappers for sm_90a (hand-written; bit layouts follow the PTX ISA "wgmma" matrix
+// descriptor tables).
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -8,28 +8,12 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n"
-      ".reg .b32 rx;\n"
-      ".reg .pred px;\n"
-      "elect.sync rx|px, 0xffffffff;\n"
-      "selp.b32 %0, 1, 0, px;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ---------------- mbarrier ----------------
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -56,6 +40,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// named barrier over the 128 threads of one warpgroup (ids 1.. ; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// register budget hand-off between the producer warpgroup and the MMA warpgroups
+template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------- TMA ----------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -75,158 +66,67 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// ---------------- tcgen05 ----------------
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// whole warp; writes the TMEM base address to *slot (shared memory)
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
+// ---------------- wgmma ----------------
 // shared-memory matrix descriptor, K-major operand, swizzled rows of `row_bytes` (32/64/128):
 //   bits [0,14)  start address >> 4         bits [16,30) leading byte offset >> 4 (unused for swizzled K-major)
-//   bits [32,46) stride byte offset >> 4 (distance between 8-row groups)      bits [46,48) version = 1
-//   bits [61,64) layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
+//   bits [32,46) stride byte offset >> 4 (distance between 8-row groups)
+//   bits [62,64) layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
+// The TMA-written tiles start on 1024-byte boundaries and the XOR swizzle is a function of the absolute shared
+// address bits on both the TMA and the wgmma side, so a start address shifted by whole rows (the halo kernels' tap
+// views) or by 32 bytes of K keeps base offset 0.
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr, uint32_t row_bytes) {
-  const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);
+  const uint32_t layout = row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : 3u);
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((8u * row_bytes) >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
+  d |= (uint64_t)layout << 62;
   return d;
 }
 
-// descriptor for a start address that is NOT aligned to the swizzle repeat (8 rows): bits [49,52) "base offset"
-// would tell the hardware where in the 8-row pattern the first row sits.  Measured on B200 (tools/gpu_diag.py halo):
-// with TMA-written tiles whose stage base is 1024-byte aligned the XOR swizzle is a function of the ABSOLUTE shared
-// address bits on both the TMA and the UMMA side, so a row-shifted start address needs base offset 0 (mode 0,
-// bit-exact); mode 1 = (addr >> 7) & 7 produced wrong results and is kept only for experiments.
-__device__ __forceinline__ uint64_t make_sdesc_shifted(uint32_t saddr, uint32_t row_bytes, int mode) {
-  uint64_t d = make_sdesc(saddr, row_bytes);
-  if (mode == 1) d |= (uint64_t)((saddr >> 7) & 7u) << 49;
-  return d;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// instruction descriptor, both operands K-major, F32 accumulate
-//   bits [4,6) D format (1 = F32)  [7,10) A format  [10,13) B format  [15] A major  [16] B major
-//   bits [17,23) N >> 3            [24,29) M >> 4
-//   A/B format: kind::f16 -> 1 = BF16;  kind::tf32 -> 2 = TF32
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// same, with the accumulate flag as an immediate (no per-instruction setp in the issue loop)
-template <int ACC>
-__device__ __forceinline__ void mma_bf16_imm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "n"(ACC)
-      : "memory");
-}
-
-// kind::tf32: fp32 containers in shared memory, the tensor core reads the TF32 bits (sign, 8-bit exponent, 10-bit
-// mantissa); one instruction consumes K = 8 elements = 32 bytes per row, the same 32 bytes as 16 bf16
-template <int ACC>
-__device__ __forceinline__ void mma_tf32_imm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "n"(ACC)
-      : "memory");
-}
-
-// element-type dispatch: T = __nv_bfloat16 (kind::f16) or float (kind::tf32); a 32-byte K slice per instruction
+// One m64n32 MMA step over a 32-byte K slice: bf16 (K = 16) or TF32 (K = 8, fp32 containers whose TF32 bits the
+// tensor core reads).  D: this thread's 16 fp32 accumulators of the 64 x 32 tile; scale_d == 0 overwrites them.
+#define OCCD_WG_ACC16                                                                                          \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
 template <typename T> struct Mma;
 template <> struct Mma<__nv_bfloat16> {
-  static __host__ __device__ constexpr uint32_t idesc(int M, int N) { return make_idesc_bf16(M, N); }
-  template <int ACC>
-  static __device__ __forceinline__ void issue(uint32_t d, uint64_t a, uint64_t b, uint32_t id) {
-    mma_bf16_imm<ACC>(d, a, b, id);
+  static __device__ __forceinline__ void issue(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
+        "%12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : OCCD_WG_ACC16
+        : "l"(a), "l"(b), "r"(scale_d));
   }
 };
 template <> struct Mma<float> {
-  static __host__ __device__ constexpr uint32_t idesc(int M, int N) { return make_idesc_tf32(M, N); }
-  template <int ACC>
-  static __device__ __forceinline__ void issue(uint32_t d, uint64_t a, uint64_t b, uint32_t id) {
-    mma_tf32_imm<ACC>(d, a, b, id);
+  static __device__ __forceinline__ void issue(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
+        "%12, %13, %14, %15}, %16, %17, p, 1, 1;\n"
+        "}\n"
+        : OCCD_WG_ACC16
+        : "l"(a), "l"(b), "r"(scale_d));
   }
 };
-
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// split form for software pipelining: issue the load of the next 16 columns, process the previous ones, then
-// wait; the wait names the destination registers so the compiler cannot hoist their uses above it
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait16(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-
-// after one tmem_ld_wait16: ties further destination arrays of loads issued before that wait to the wait's position
-// (asm volatile statements keep their order), so their uses cannot be scheduled above it
-__device__ __forceinline__ void tmem_ld_dep16(uint32_t* r) {
-  asm volatile(""
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
+#undef OCCD_WG_ACC16
 
 }  // namespace tc

@@ -143,12 +143,9 @@ DWT_HD void store8(float* p, float* v) {
   *reinterpret_cast<float4*>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
 
+// two IEEE fp32 FMAs (sm_90 has no packed FFMA2; the host emulation and the device compute the same values)
 DWT_HD float2 fma2(float2 a, float2 b, float2 c) {
-#ifdef __CUDA_ARCH__
-  return __ffma2_rn(a, b, c);  // one packed FFMA2 issue slot for two IEEE fp32 FMAs (sm_100)
-#else
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#endif
 }
 
 // activation over one 8-channel vector (device: the same uniform-branch fast-math epilogue as the direct kernel)

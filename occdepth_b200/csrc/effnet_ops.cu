@@ -209,8 +209,7 @@ __global__ void upsample_bilinear_kernel(const T* __restrict__ in, T* __restrict
                                          int out_off, float sy, float sx) {
   pdl_wait();
   // grid: x covers one output row's (column, channel-vector) pairs, y = (image, output row): 32-bit index math only
-  // (the flat 64-bit index this kernel used to decode cost three software 64-bit divisions per 32-byte store:
-  // the five decoder upsamples 0.45 -> 0.37 ms, profiles/r02d vs r02e plan profiles)
+  // (a flat 64-bit index would cost three software 64-bit divisions per 32-byte store)
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (unsigned)(OW * CV)) return;
   const int ox = (int)(i / (unsigned)CV);
@@ -306,8 +305,8 @@ template <typename T, int K, int S>
 int launch_dw_tiled_ks(const dwt::Args& a, int B, dwt::Choice ch, cudaStream_t st) {
   if (ch.cvb == 4) {   // 16 rows per pass: TH = 16 only
     if constexpr (sizeof(T) == 4 && S == 1) {
-      // fp32, stride 1: 8 outputs per thread / 128-thread CTAs (B200, tools/dw_bench.py: b2 5x5 31 -> 26 us, b1 3x3
-      // 50 -> 44 us; the stride-2 layers lose, 82 -> 96 us, and keep 4).  OCCD_DW_PX=4 forces 4 (experiment hook)
+      // fp32, stride 1: 8 outputs per thread / 128-thread CTAs (the stride-2 layers keep 4; tools/dw_bench.py
+      // compares the variants).  OCCD_DW_PX=4 forces 4 (experiment hook)
       static const bool px4 = [] { const char* e = getenv("OCCD_DW_PX"); return e && atoi(e) == 4; }();
       if (!px4) return launch_dw_tiled<T, K, S, 4, 16, 8>(a, B, st);
     }
@@ -346,7 +345,7 @@ extern "C" int occd_dwconv2d_tiled_fwd(const void* in, const float* w, const flo
   if (n_sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sms <= 0) n_sms = 148;
+    if (cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sms <= 0) n_sms = 132;
   }
   dwt::Args a;
   a.in = in; a.w = w; a.bias = bias; a.out = out; a.pool = pool;

@@ -383,11 +383,8 @@ sfa_lift_p1_kernel(const SfaKParams p) {
       off[v][0] = o.x; off[v][1] = o.y; off[v][2] = o.z; off[v][3] = o.w;
       m[v] = (active && s_in[v][ln]) ? 1.f : 0.f;
     }
-    // per scale: the V x NV gathers of a lane are issued back to back, then reduced.  Two or four scales per phase
-    // (more loads in flight per lane, fewer dependent phases) measured the same or slower on B200, as did 1 / 2 / 4
-    // batches per block and a 64-register cap: every variant sits at ~63 us for config 2 in fp32 (53 us in bf16 with
-    // half the bytes), DRAM traffic equals the algorithmic bytes (ncu r02b) -- the floor is the scattered 256-byte
-    // row fetches themselves (profiles/r02_lift_variants.txt)
+    // per scale: the V x NV gathers of a lane are issued back to back, then reduced (the floor is the scattered
+    // 256-byte row fetches themselves)
     float acc[CPL];
 #pragma unroll
     for (int i = 0; i < CPL; ++i) acc[i] = 0.f;
@@ -462,16 +459,15 @@ static bool sfa_fits_int32(const SfaKParams& kp, int n_views) {
 }
 
 // G lanes cooperate on one voxel, each holding NV 16-byte vectors of the C channels.  Fewer lanes per voxel = less
-// redundant index / cosine-scalar work per voxel (the kernel is issue bound: ncu r02: SM throughput 62 %, DRAM 24 %,
-// L2 19 %), more vectors per lane = more independent 16-byte gathers in flight per lane.  Measured on B200 at config 2
-// (fp32, 16 vectors per voxel; profiles/r02_lift_variants.txt): 16 lanes x 1 vector 135 us, 8 x 2 94 us, 4 x 4 80 us.
+// redundant index / cosine-scalar work per voxel, more vectors per lane = more independent 16-byte gathers in flight
+// per lane.
 template <typename T, int V, int NV, int G>
 int launch_g(const SfaKParams& kp, cudaStream_t st) {
   constexpr int VPB = kThreads / G;
   const long long per_block = (long long)VPB * kIters;
   const long long blocks = (kp.N + per_block - 1) / per_block;
   if (kp.P == 1 && sfa_fits_int32(kp, V)) {
-    // two voxel batches per block (1 / 2 / 4 measured within 3 % of each other, profiles/r02_lift_variants.txt)
+    // two voxel batches per block
     constexpr int KI = 2;
     const unsigned nb = (unsigned)((kp.N + VPB * KI - 1) / (VPB * KI));
     OCCD_LAUNCH_CHECKED((sfa_lift_p1_kernel<T, V, NV, G, KI>), dim3(nb), dim3(kThreads), 0, st, kp);

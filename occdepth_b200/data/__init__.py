@@ -40,7 +40,7 @@ def vox2pix(cam_E, cam_k, vox_origin, voxel_size, img_W, img_H, scene_size, patt
     """occdepth.data.utils.helpers.vox2pix on the GPU (see module docstring).  Raises if no CUDA device."""
     dev = torch.device("cuda" if device is None else device)
     if dev.type != "cuda" or not torch.cuda.is_available():
-        raise RuntimeError("occdepth_b200.data.vox2pix runs on CUDA (sm_100a) only -- there is no CPU fallback")
+        raise RuntimeError("occdepth_b200.data.vox2pix runs on CUDA (sm_90a) only -- there is no CPU fallback")
     if not 0 <= int(pattern_id) < len(PIXEL_PATTERNS):
         raise IndexError("pattern_id out of range")        # the reference indexes the same 9-entry list
     X, Y, Z = (int(v) for v in volume_dims(vox_origin, voxel_size, scene_size))
@@ -76,7 +76,7 @@ def normalize_rgb(img_u8, img_H, img_W, mean=IMAGENET_MEAN, std=IMAGENET_STD, de
     (ToTensor + Normalize).  The host->device copy is the uint8 image (4x smaller than the float tensor)."""
     dev = torch.device("cuda" if device is None else device)
     if dev.type != "cuda" or not torch.cuda.is_available():
-        raise RuntimeError("occdepth_b200.data.normalize_rgb runs on CUDA (sm_100a) only -- there is no CPU fallback")
+        raise RuntimeError("occdepth_b200.data.normalize_rgb runs on CUDA (sm_90a) only -- there is no CPU fallback")
     t = torch.as_tensor(np.asarray(img_u8) if not isinstance(img_u8, torch.Tensor) else img_u8)
     if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
         raise ValueError("normalize_rgb: expected a uint8 (H, W, 3) RGB image")

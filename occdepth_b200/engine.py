@@ -28,7 +28,7 @@ LIB_DTYPE = {"tf32": _lib.DTYPE_F32, "bf16": _lib.DTYPE_BF16}
 def default_precision():
     """Arithmetic mode of the planned forward (OCCDEPTH_PRECISION, default 'tf32'):
 
-    'tf32': activations are fp32 tensors holding TF32 values, convolutions run as tcgen05 kind::tf32 with fp32
+    'tf32': activations are fp32 tensors holding TF32 values, convolutions run as wgmma .tf32 with fp32
             accumulation -- the reference's precision (fp32 nn.Conv*d, which PyTorch itself executes on TF32 tensor
             cores on CUDA); this is the mode the parity tests and the bench headline use.
     'bf16': bf16 activations and operands (kind::f16), fp32 accumulation -- the throughput mode, own tolerance."""
@@ -58,8 +58,8 @@ def chunk_channels(C_, esize):
 
 
 def default_impl():
-    """'auto' (default): halo-tile tcgen05 kernel where the shape qualifies, the x-packed per-tap kernel for
-    narrow-output convs with W taps, else the per-tap tcgen05 kernel; 'tc' / 'tcx' / 'halo' / 'simt' force one
+    """'auto' (default): halo-tile wgmma kernel where the shape qualifies, the x-packed per-tap kernel for
+    narrow-output convs with W taps, else the per-tap wgmma kernel; 'tc' / 'tcx' / 'halo' / 'simt' force one
     implementation (simt = CUDA-core cross-check)."""
     v = os.environ.get("OCCDEPTH_CONV_IMPL", "auto").lower()
     if v not in ("auto", "tc", "simt", "halo", "halox", "tcx"):
@@ -91,8 +91,8 @@ def halox_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf):
 
 def tcx_eligible(taps, stride, Cout_pad):
     """(src, dz, dy) groups of three W taps -1, 0, +1 (what conv_taps emits for a dense 3-wide kernel), W stride 1,
-    N = 3*Cout_pad <= 256, and enough output channels that the packed MMA beats three narrow ones (measured on
-    B200, profiles/r02_convbench_tcx.txt: Cout 80 0.154 -> 0.102 ms; Cout 32 loses to the halo kernel)"""
+    N = 3*Cout_pad <= 256, and enough output channels that the packed MMA beats three narrow ones (narrow outputs go
+    to the halo kernel)"""
     if len(taps) % 3 or 3 * Cout_pad > 256 or Cout_pad < 48 or stride[2] != 1:
         return False
     for i in range(0, len(taps), 3):
@@ -116,7 +116,7 @@ def halo_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf):
 
 def require_cuda(t, what):
     if not (isinstance(t, torch.Tensor) and t.is_cuda):
-        raise RuntimeError("%s: occdepth_b200 runs on CUDA (sm_100a) only -- there is no CPU fallback" % what)
+        raise RuntimeError("%s: occdepth_b200 runs on CUDA (sm_90a) only -- there is no CPU fallback" % what)
 
 
 class CL:
@@ -347,7 +347,7 @@ class ConvOp:
             d.impl = _lib.CONV_IMPL_TC
             rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
         if rc != 0 and auto and d.impl == _lib.CONV_IMPL_HALO:
-            d.impl = _lib.CONV_IMPL_TC      # shape did not fit the halo scheme: per-tap tcgen05 kernel
+            d.impl = _lib.CONV_IMPL_TC      # shape did not fit the halo scheme: per-tap wgmma kernel
             rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
         _lib.check(rc, "occd_conv_plan_create(%s)" % name)
         self.handle = h

@@ -1,7 +1,7 @@
 """Drop-in for the reference `occdepth/models/CRP3D.py`: CPMegaVoxels (:9-97), the 3D Context Relation Prior.
 
 ASPP -> stride-2 mega-context conv -> n_relations 1x1x1 relation convs (sigmoid fused, raw logits written
-straight into P_logits) -> the torch.bmm as tcgen05 GEMMs whose "weights" are the transposed mega-context
+straight into P_logits) -> the torch.bmm as wgmma GEMMs whose "weights" are the transposed mega-context
 -> concat buffer written in place -> 1x1x1 resize -> Process.
 """
 import torch

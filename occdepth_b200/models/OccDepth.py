@@ -1,7 +1,7 @@
 """Drop-in for the reference `occdepth/models/OccDepth.py` (class OccDepth, forward path :31-376).
 
 Same constructor, same `forward(batch) -> dict`, same state_dict keys.  The forward is one planned sequence of
-sm_100a launches: both stereo views go through the 2D UNet as one batch, the 4-scale / 2-view Stereo-SFA lift
+sm_90a launches: both stereo views go through the 2D UNet as one batch, the 4-scale / 2-view Stereo-SFA lift
 is a single fused kernel writing the channels-last voxel grid the 3D UNet consumes, and the logits are written
 in the reference's NCDHW fp32 layout by the last convolution's epilogue.
 Training (`step`, losses, optimisers; OccDepth.py:378-600) is out of scope of this package.
@@ -226,7 +226,7 @@ class OccDepth(_Base, B200Module):
         img = batch["img"]
         if not img.is_cuda:
             if not torch.cuda.is_available():
-                raise RuntimeError("OccDepth.forward: occdepth_b200 needs a CUDA (sm_100a) device")
+                raise RuntimeError("OccDepth.forward: occdepth_b200 needs a CUDA (sm_90a) device")
             img = img.cuda(non_blocking=True)          # the reference moves the batch in forward too (:345)
         self._check_mode(img)
         dev = img.device

@@ -1,7 +1,7 @@
 """Stereo-SFA lift -- drop-in for the reference `occdepth/models/SFA.py` (class SFA, :5-106).
 
 `SFA(scene_size, dataset, project_scale).forward(x2d[V,C,h,w] f32, projected_pix[V,N,P,2] int64,
-fov_mask[V,N,P] bool) -> [C,X,Y,Z] f32`, computed by the fused sm_100a kernel `occd_sfa_lift_fwd`.
+fov_mask[V,N,P] bool) -> [C,X,Y,Z] f32`, computed by the fused sm_90a kernel `occd_sfa_lift_fwd`.
 `lift_multiscale` is the fused fast path used by OccDepth.forward (all 2D scales, both views, one launch,
 channels-last bf16 in and out).
 """

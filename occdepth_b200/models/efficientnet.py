@@ -1,5 +1,5 @@
 """tf_efficientnet_b{3,4,5,7}_ns with geffnet's module names (what the reference's torch.hub.load returns at
-occdepth/models/unet2d.py:238-240), as a parameter holder + sm_100a launch emitter.
+occdepth/models/unet2d.py:238-240), as a parameter holder + sm_90a launch emitter.
 
 State-dict keys equal geffnet's (`conv_stem, bn1, blocks.S.B.{conv_pw,bn1,conv_dw,bn2,se.conv_reduce,
 se.conv_expand,conv_pwl,bn3}, conv_head, bn2, classifier`), so reference checkpoints
@@ -59,8 +59,8 @@ class SqueezeExcite(nn.Module):
 
 
 def _dw_entry(L):
-    """depthwise entry point: the shared-memory-tiled kernel by default (2-4x the direct one on every B7 layer
-    shape, profiles/r01_dw_check.txt); OCCDEPTH_DW_IMPL=direct selects the register-window variant."""
+    """depthwise entry point: the shared-memory-tiled kernel by default; OCCDEPTH_DW_IMPL=direct selects the
+    register-window variant."""
     impl = os.environ.get("OCCDEPTH_DW_IMPL", "tiled")
     if impl not in ("tiled", "direct"):
         raise ValueError(f"OCCDEPTH_DW_IMPL must be 'tiled' or 'direct', got {impl!r}")

@@ -1,7 +1,7 @@
 """Drop-in for the reference `occdepth/models/flosp_depth/flosp_depth.py`: Mlp :159, SELayer :186, DepthNet :201-257,
 FlospDepth :324-608 (+ the conf dicts of flosp_depth_conf_{kitti,nyu}.py).
 
-DepthNet's convolutions run on the tcgen05 implicit-GEMM kernel; the frustum grid (f2v/frustum_grid_generator.py) is
+DepthNet's convolutions run on the wgmma implicit-GEMM kernel; the frustum grid (f2v/frustum_grid_generator.py) is
 never materialised -- `occd_frustum_sample_fwd` computes each voxel's sampling coordinate on the fly and fuses the
 trilinear sampling of the depth distribution, of the all-ones mask volume and the per-camera masked mean.
 """

@@ -1,4 +1,4 @@
-"""Drop-in for the reference `occdepth/models/modules.py` (3D building blocks), forward on sm_100a kernels.
+"""Drop-in for the reference `occdepth/models/modules.py` (3D building blocks), forward on sm_90a kernels.
 
 ASPP :6-48, SegmentationHead :51-106, SegmentationHeadCascadeCLS :109-175, SegmentationHeadOccludedCLS
 :178-235, Process :258-275, Upsample :278-296, Convblock3d :299-317, Downsample :320-344.
@@ -14,7 +14,7 @@ from .DDR import Bottleneck3D
 
 def _emit_aspp(plan, m, x, out=None, name="aspp"):
     """relu( sum_i bn2_i(conv2_i(relu(bn1_i(conv1_i(x))))) + x ): 3 launches for conv1, ONE launch for the three
-    conv2 branches (81 taps, one TMEM accumulator) with the residual + ReLU in its epilogue."""
+    conv2 branches (81 taps, one accumulator) with the residual + ReLU in its epilogue."""
     ts, ws, b2s, bs = [], [], [], None
     for i, dl in enumerate(m.conv_list):
         w, b = fold_bn(m.conv1[i].weight, m.conv1[i].bias, m.bn1[i])

@@ -1,8 +1,8 @@
 """Frame pipeline around `OccDepth.forward` for callers that hold their frames in HOST memory (the reference's
 `eval.py` / `scripts/generate_output.py` loops: `model(batch)` then `.cpu()` on the logits, generate_output.py:94-97).
 
-One forward of config 2 computes for ~14.5 ms on a B200 while the PCIe copies either side of it (21 MB of inputs in,
-168 MB of logits out) take ~3.4 ms: run back to back they cost a fifth of the frame time.  `FramePipeline` keeps two
+One forward of config 2 moves 21 MB of inputs in and 168 MB of logits out over PCIe; run back to back with the
+forward, those copies add their whole duration to every frame.  `FramePipeline` keeps two
 pre-allocated input and output buffer sets on the device and two pinned result buffers on the host, and issues the
 H2D copy of frame i+1 and the D2H read of frame i-1 on their own copy streams while frame i computes.  Nothing is
 allocated per frame (a caching-allocator block that changes streams would serialise them again).
@@ -22,7 +22,7 @@ from .engine import require_cuda
 class FramePipeline:
     def __init__(self, model, img_shape, pix_shape, fov_shape, device=None, out_key="ssc_logit"):
         if not torch.cuda.is_available():
-            raise RuntimeError("FramePipeline: occdepth_b200 needs a CUDA (sm_100a) device")
+            raise RuntimeError("FramePipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         require_cuda(torch.empty(0, device=dev), "FramePipeline")
         self.model, self.dev, self.out_key = model, dev, out_key

@@ -4,8 +4,8 @@ Follows occdepth/data/utils/helpers.py:94-169 (`vox2pix`) with fusion.py:201-217
 (`rigid_transform`) and :236-343 (`cam2allpixs`), in plain numpy with the reference's dtypes:
 voxel centres in float64 then cast to float32; pose applied with np.dot in float64 (so the summation order is
 whatever this numpy's BLAS does, exactly as in the reference); intrinsics cast to float32; np.round (half to even);
-int64 pixels.  Pinned against the reference itself (numba-compiled, imported from /root/reference) in
-tests/test_oracle_vs_reference.py and through tests/golden/vox2pix.pt.
+int64 pixels.  Pinned against the reference itself (numba-compiled) through the fixtures of
+tests/test_oracle_vs_reference.py and tests/golden/vox2pix.pt.
 """
 import numpy as np
 

@@ -1,6 +1,8 @@
-"""Import the UNMODIFIED reference (`/root/reference/occdepth`) as the ground-truth oracle.
+"""Import the UNMODIFIED reference (`$OCCDEPTH_REFERENCE/occdepth`, a checkout of the original project) as the
+ground-truth oracle.
 
-Only possible in the build container (the GPU box has no /root/reference).  Third-party imports missing
+Only possible where that checkout exists; oracle/gen_golden.py stores what the tests compare against, so the test
+suite itself never needs it.  Third-party imports missing
 from this image are satisfied by `oracle/shims/` (see its README) and `torch.hub.load` is redirected to the
 geffnet-shaped EfficientNet of `oracle/effnet.py` (random init -- no network for pretrained weights).
 """
@@ -10,17 +12,17 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("OCCDEPTH_REFERENCE", "/root/reference")
+REF_ROOT = os.environ.get("OCCDEPTH_REFERENCE", "")
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims")
 
 
 def available():
-    return os.path.isdir(os.path.join(REF_ROOT, "occdepth", "models"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "occdepth", "models"))
 
 
 def _install():
     if not available():
-        raise RuntimeError("reference tree not found at %s" % REF_ROOT)
+        raise RuntimeError("reference tree not found (set OCCDEPTH_REFERENCE to a checkout of the original project)")
     for p in (_SHIMS, REF_ROOT):
         if p not in sys.path:
             sys.path.insert(0, p)

@@ -25,15 +25,33 @@ def rnd(precision):
     return tf32r if precision == "tf32" else bf16r
 
 
-def record(test, precision, **values):
-    """append measured parity figures to gpurun_out/parity_measured.jsonl (the tolerances in the tests are set to
-    <= 2x what this log shows; profiles/ keeps the log of the round)"""
+def report_dir():
+    """directory for the measured parity figures (the tolerances in the tests are set to <= 2x what they show):
+    $OCCDEPTH_PARITY_DIR, or None -- the tests never write into the source tree"""
+    import os
+    d = os.environ.get("OCCDEPTH_PARITY_DIR")
+    if d:
+        os.makedirs(d, exist_ok=True)
+    return d
+
+
+def write_report(name, rep):
     import json
     import os
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    os.makedirs(os.path.join(root, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(root, "gpurun_out", "parity_measured.jsonl"), "a") as f:
-        f.write(json.dumps(dict(test=test, precision=precision, **values)) + "\n")
+    d = report_dir()
+    if d:
+        with open(os.path.join(d, name), "w") as f:
+            json.dump(rep, f)
+
+
+def record(test, precision, **values):
+    """append measured parity figures to <report_dir()>/parity_measured.jsonl"""
+    import json
+    import os
+    d = report_dir()
+    if d:
+        with open(os.path.join(d, "parity_measured.jsonl"), "a") as f:
+            f.write(json.dumps(dict(test=test, precision=precision, **values)) + "\n")
 
 
 def rel_err(got, want):

@@ -21,7 +21,7 @@ def emul(tmp_path_factory):
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
     out = tmp_path_factory.mktemp("dw_emul") / "libdw_emul.so"
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-std=c++17", "--expt-relaxed-constexpr",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-std=c++17", "--expt-relaxed-constexpr",
            "-shared", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "occdepth_b200", "csrc"),
            "-o", str(out), os.path.join(ROOT, "tests", "host_emul", "dw_tiled_emul.cu")]
     r = subprocess.run(cmd, capture_output=True, text=True)

@@ -1,5 +1,5 @@
 """Oracle (oracle/functional.py) vs the committed golden vectors produced by the UNMODIFIED reference
-(oracle/gen_golden.py).  Runs anywhere (CPU); this is what pins the oracle on machines without /root/reference."""
+(oracle/gen_golden.py).  Runs anywhere (CPU); with tests/test_oracle_vs_reference.py this is what pins the oracle."""
 import os
 
 import torch

@@ -1,4 +1,4 @@
-"""Implicit-GEMM convolution through the C ABI: tcgen05 paths and the SIMT path vs torch fp32 on operands rounded
+"""Implicit-GEMM convolution through the C ABI: wgmma paths and the SIMT path vs torch fp32 on operands rounded
 to the mode's element type (TF32 values in fp32 containers / bf16), both precision modes."""
 import pytest
 
@@ -84,7 +84,7 @@ def test_conv_large_vs_simt(precision):
 @PREC
 @pytest.mark.parametrize("case", sorted(G.HALO_CASES))
 def test_conv_halo(case, precision):
-    """halo-tile tcgen05 kernel (row-shifted swizzled smem views, sub-sampled TMA for dilation)"""
+    """halo-tile wgmma kernel (row-shifted swizzled smem views, sub-sampled TMA for dilation)"""
     from occdepth_b200 import _lib
     kw = G.HALO_CASES[case]
     one_chunk = 32 if precision == "tf32" else 64           # the resident-weight scheme holds ONE K chunk

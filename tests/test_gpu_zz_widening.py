@@ -42,7 +42,7 @@ def test_vox2pix_device_matches_reference_outputs():
         pix, fov, z = vox2pix(c["cam_E"].numpy(), c["cam_k"].numpy(), c["vox_origin"].numpy(), c["voxel_size"],
                               c["img_W"], c["img_H"], c["scene_size"], c["pattern_id"])
         assert pix.is_cuda and pix.dtype == torch.int64 and fov.dtype == torch.bool and z.dtype == c["pix_z"].dtype
-        assert torch.equal(pix.cpu(), c["pix"]), name
+        assert torch.equal(pix.cpu(), c["pix"].long()), name
         assert torch.equal(fov.cpu(), c["fov"]), name
         assert np.array_equal(z.cpu().numpy(), c["pix_z"].numpy(), equal_nan=True), name
 

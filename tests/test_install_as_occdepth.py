@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 WITH_REFERENCE = r"""
 import sys
-sys.path[:0] = [%(root)r, %(shims)r, %(ref)r]
+sys.path[:0] = [%(root)r, %(ref)r]
 import occdepth_b200
 occdepth_b200.install_as_occdepth()
 # the import block of occdepth/scripts/generate_output.py:1-5 and eval.py (minus the third-party trainer)
@@ -25,11 +25,24 @@ from occdepth.models.SFA import SFA
 import occdepth
 assert OccDepth.__module__ == "occdepth_b200.models.OccDepth", OccDepth.__module__
 assert UNet3D.__module__ == "occdepth_b200.models.unet3d_kitti" and SFA.__module__ == "occdepth_b200.models.SFA"
-assert "reference" in sscMetrics.__file__ or %(ref)r in sscMetrics.__file__, sscMetrics.__file__
+assert sscMetrics.__file__.startswith(%(ref)r), sscMetrics.__file__
 assert hasattr(helpers, "vox2pix") and hasattr(collate, "collate_fn")
 assert hasattr(occdepth, "__path__")
 print("OK")
 """
+
+# The original project's package layout as far as the import block above reaches: `occdepth` and every sub-package
+# are namespace packages (no __init__.py); its own `occdepth/models` must never be imported after
+# install_as_occdepth(), so the stand-in's copy raises on import.
+REFERENCE_LAYOUT = {
+    "occdepth/models/OccDepth.py": "raise ImportError('the original occdepth.models was imported')\n",
+    "occdepth/models/SFA.py": "raise ImportError('the original occdepth.models was imported')\n",
+    "occdepth/models/unet3d_kitti.py": "raise ImportError('the original occdepth.models was imported')\n",
+    "occdepth/loss/sscMetrics.py": "class SSCMetrics:\n    pass\n",
+    "occdepth/data/utils/helpers.py": "def vox2pix(*args):\n    raise NotImplementedError\n",
+    "occdepth/data/semantic_kitti/collate.py": "def collate_fn(batch):\n    return batch\n",
+}
+
 
 WITHOUT_REFERENCE = r"""
 import sys
@@ -54,10 +67,13 @@ def _run(code):
     return subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, env=env, cwd="/tmp")
 
 
-@pytest.mark.reference
-def test_install_then_reference_imports():
-    from oracle import ref_import
-    r = _run(WITH_REFERENCE % {"root": ROOT, "shims": os.path.join(ROOT, "oracle", "shims"), "ref": ref_import.REF_ROOT})
+def test_install_then_reference_imports(tmp_path):
+    ref = tmp_path / "reference"
+    for rel, body in REFERENCE_LAYOUT.items():
+        f = ref / rel
+        f.parent.mkdir(parents=True, exist_ok=True)
+        f.write_text(body)
+    r = _run(WITH_REFERENCE % {"root": ROOT, "ref": str(ref)})
     assert r.returncode == 0 and "OK" in r.stdout, r.stderr[-2000:]
 
 

@@ -1,83 +1,65 @@
-"""The drop-in boundary: every module of occdepth_b200.models must expose exactly the reference's state_dict keys
-and shapes (released checkpoints are loaded with strict=True, scripts/eval.py:65-70).  Needs /root/reference."""
+"""The drop-in boundary: every module of occdepth_b200.models must expose exactly the reference's state_dict keys,
+shapes and dtypes, in order (released checkpoints are loaded with strict=True, scripts/eval.py:65-70).  The
+reference's layout is stored in tests/golden/state_dict_layout.json (oracle/gen_golden.py, run where the original
+project is importable)."""
 import copy
+import json
+import os
+import types
 
 import pytest
-import torch
-import torch.nn as nn
 
-from oracle import ref_import, synth
+from oracle import gen_golden
 
-pytestmark = pytest.mark.reference
-
-
-@pytest.fixture(scope="module")
-def ref():
-    return ref_import.modules()
+G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+LAYOUT = json.load(open(os.path.join(G, "state_dict_layout.json")))
+CASES = dict(gen_golden.state_dict_cases())
 
 
-def _same(a, b):
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa.keys()) == list(sb.keys())
-    for k in sa:
-        assert sa[k].shape == sb[k].shape and sa[k].dtype == sb[k].dtype, k
-    a.load_state_dict(sb, strict=True)      # and a reference checkpoint loads
-    return len(sa)
+def _product():
+    import occdepth_b200.models.OccDepth as OccDepth
+    import occdepth_b200.models.flosp_depth as flosp_pkg
+    import occdepth_b200.models.flosp_depth.flosp_depth as flosp_depth
+    import occdepth_b200.models.unet2d as unet2d
+    import occdepth_b200.models.unet3d_kitti as unet3d_kitti
+    import occdepth_b200.models.unet3d_nyu as unet3d_nyu
+    return types.SimpleNamespace(OccDepth=OccDepth, flosp_depth=flosp_depth, unet2d=unet2d, unet3d_kitti=unet3d_kitti,
+                                 unet3d_nyu=unet3d_nyu, flosp_conf=flosp_pkg.flosp_depth_conf_map)
 
 
-def test_unet3d_keys(ref):
-    from occdepth_b200.models import unet3d_kitti, unet3d_nyu
-    with ref_import.quiet():
-        args = (20, nn.BatchNorm3d, (256, 256, 32), 64, 2)
-        kw = dict(context_prior=True, cascade_cls=True, occluded_cls=True)
-        assert _same(unet3d_kitti.UNet3D(*args, **kw), ref.unet3d_kitti.UNet3D(*args, **kw)) > 500
-        args = (12, nn.BatchNorm3d, 200, (60, 36, 60))
-        assert _same(unet3d_nyu.UNet3D(*args), ref.unet3d_nyu.UNet3D(*args)) > 500
-        args = (20, nn.BatchNorm3d, (128, 128, 16), 32, 1)      # project_scale 1 -> Convblock3d
-        assert _same(unet3d_kitti.UNet3D(*args), ref.unet3d_kitti.UNet3D(*args)) > 300
+def _same(name):
+    import occdepth_b200.models.flosp_depth.flosp_depth as mfd
+    saved = copy.deepcopy(mfd.flosp_depth_conf_map)
+    try:
+        m = CASES[name](_product())
+    finally:       # OccDepth mutates the module-level conf dicts in place (as the reference does)
+        for k in mfd.flosp_depth_conf_map:
+            mfd.flosp_depth_conf_map[k].clear()
+            mfd.flosp_depth_conf_map[k].update(saved[k])
+    got = gen_golden.state_dict_layout(m)    # (entries, digest of the ordered keys / shapes / dtypes)
+    assert got == LAYOUT["modules"][name]
+    return got[0]
+
+
+def test_unet3d_keys():
+    assert _same("unet3d_kitti") > 500
+    assert _same("unet3d_nyu") > 500
+    assert _same("unet3d_kitti_ps1") > 300      # project_scale 1 -> Convblock3d
 
 
 @pytest.mark.parametrize("backbone", ["tf_efficientnet_b3_ns", "tf_efficientnet_b4_ns", "tf_efficientnet_b5_ns",
                                       "tf_efficientnet_b7_ns"])
-def test_unet2d_keys(ref, backbone):
-    from occdepth_b200.models import unet2d
-    with ref_import.quiet():
-        kw = dict(out_feature=64, use_decoder=True, backbone_2d_name=backbone, return_up_feats=1)
-        assert _same(unet2d.UNet2D.build(**kw), ref.unet2d.UNet2D.build(**kw)) > 600
+def test_unet2d_keys(backbone):
+    assert _same("unet2d_" + backbone) > 600
 
 
-def test_flosp_depth_keys(ref):
-    import occdepth.models.flosp_depth as rfd
-    from occdepth_b200.models.flosp_depth import FlospDepth, flosp_depth_conf_map
+def test_flosp_depth_keys():
+    from occdepth_b200.models.flosp_depth import flosp_depth_conf_map
     for ds in ("kitti", "NYU"):
-        a = copy.deepcopy(flosp_depth_conf_map[ds])
-        b = copy.deepcopy(rfd.flosp_depth_conf_map[ds])
-        assert a == b
-        scene = (256, 256, 32) if ds == "kitti" else (60, 36, 60)
-        for c in (a, b):
-            c.update(scene_size=scene, project_scale=2 if ds == "kitti" else 1, return_depth=False)
-        assert _same(FlospDepth(**a), ref.flosp_depth.FlospDepth(**b)) == 56
+        assert json.loads(json.dumps(flosp_depth_conf_map[ds])) == LAYOUT["conf_map"][ds]
+        assert _same("flosp_depth_" + ds) == 56
 
 
 @pytest.mark.parametrize("variant", ["kitti_flosp", "kitti_flosp_depth", "nyu_flosp"])
-def test_occdepth_keys(ref, variant):
-    from occdepth_b200.models.OccDepth import OccDepth
-    import occdepth.models.flosp_depth as rfd
-    import occdepth_b200.models.flosp_depth.flosp_depth as mfd
-    if variant == "nyu_flosp":
-        cfg = synth.occdepth_cfg(dataset="NYU", full_scene_size=(60, 36, 60), project_scale=1, feature=200,
-                                 feature_2d_oc=200, n_classes=12, cascade_cls=False)
-    else:
-        cfg = synth.occdepth_cfg(trans_2d_to_3d="flosp_depth" if variant.endswith("depth") else "flosp")
-    saved = copy.deepcopy(rfd.flosp_depth_conf_map), copy.deepcopy(mfd.flosp_depth_conf_map)
-    try:
-        with ref_import.quiet():
-            kw = dict(full_scene_size=cfg.full_scene_size, project_res=["1", "2", "4", "8"], config=cfg)
-            n = _same(OccDepth(["c"] * cfg.n_classes, torch.ones(cfg.n_classes), **kw),
-                      ref.OccDepth.OccDepth(["c"] * cfg.n_classes, torch.ones(cfg.n_classes), **kw))
-    finally:       # the reference mutates the module-level conf dicts in place (OccDepth.py:183-198)
-        for m_, s_ in ((rfd.flosp_depth_conf_map, saved[0]), (mfd.flosp_depth_conf_map, saved[1])):
-            for k in m_:
-                m_[k].clear()
-                m_[k].update(s_[k])
-    assert n > 1800
+def test_occdepth_keys(variant):
+    assert _same("occdepth_" + variant) > 1800
