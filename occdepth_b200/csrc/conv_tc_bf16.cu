@@ -1,0 +1,6 @@
+// The per-tap and x-packed per-tap kernels (conv_tc_kernel), bf16, one per compiled N tile.
+#include "conv_kernels.cuh"
+
+namespace occd_conv {
+template int run_tc_family<__nv_bfloat16>(const occd_conv_plan*, cudaStream_t);
+}  // namespace occd_conv
