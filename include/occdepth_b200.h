@@ -186,6 +186,13 @@ int occd_conv_plan_destroy(occd_conv_plan* plan);
 int occd_conv_run(const occd_conv_plan* plan, void* stream);
 /* introspection for tests / profiling: tile box (TD,TH,TW), N tile, K chunk, stages, grid          */
 int occd_conv_plan_info(const occd_conv_plan* plan, int* info8);
+/* how the plan's tensor-core kernel shares M tiles between its two MMA warpgroups (fixed by the N tile):    */
+/* ping-pong (whole tiles, alternately: one tile's epilogue runs under the next tile's MMAs) or cooperative   */
+/* (both on every tile); OCCD_CONV_SCHED_NONE for the SIMT kernel                                            */
+#define OCCD_CONV_SCHED_NONE 0
+#define OCCD_CONV_SCHED_COOPERATIVE 1
+#define OCCD_CONV_SCHED_PINGPONG 2
+int occd_conv_plan_schedule(const occd_conv_plan* plan, int* schedule);
 /* debug: plans created while a device buffer ([64][8] int64) is set stamp per-role clock64 values of CTA 0  */
 /* into it (tools/conv_trace.py); NULL switches tracing off                                               */
 int occd_conv_debug_trace(long long* device_buf);

@@ -103,6 +103,7 @@ SYMBOLS = {
     "occd_conv_plan_destroy": (C.c_int, [_vp]),
     "occd_conv_run": (C.c_int, [_vp, _vp]),
     "occd_conv_plan_info": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "occd_conv_plan_schedule": (C.c_int, [_vp, C.POINTER(C.c_int)]),
     "occd_conv_debug_trace": (C.c_int, [_vp]),
     "occd_softmax_planar_to_cl": (C.c_int, [_vp, _vp, _i, _ll, _i, _ll, _i, _i, _vp]),
     "occd_argmax_classes": (C.c_int, [_vp, _vp, _ll, _i, _ll, _vp, _vp]),

@@ -1,6 +1,7 @@
 // Generalised N-d convolution as implicit GEMM.
 //   TC path  : TMA (5-D tiled tensor maps, zero-filled halos, traversal strides) -> swizzled smem ->
-//              wgmma (M=128 positions as two warpgroups x 64, N<=256 channels, fp32 accumulators in registers) ->
+//              wgmma (M=128 positions, N<=256 channels, fp32 accumulators in registers; two MMA warpgroups on a
+//              ping-pong or cooperative schedule, see conv_kernels.cuh) ->
 //              epilogue (bias + residuals + activation, channels-last / fp32 planar stores)
 //   SIMT path: CUDA-core direct convolution with identical semantics (cross-check and odd shapes)
 // The tensor-core kernels live in conv_kernels.cuh; this file plans them (tile shapes, N tile, pipeline depth, tensor
@@ -282,7 +283,7 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.PW = d->IW;
   h.b_stride = round_up(h.N_tile * RB, 1024);
   h.w_bytes = h.n_groups * h.b_stride;
-  const int smem_total = 227 * 1024 - staging_bytes(kStageNarrow) - h.w_bytes - 2048;   // staging, barriers, slack
+  const int smem_total = 227 * 1024 - staging_bytes(xp_stage_ld(h.N_tile)) - h.w_bytes - 2048;   // staging, barriers, slack
   HX_REQUIRE(smem_total > 0, "weights do not fit in shared memory");
   const int HR = 128 / h.PW;                               // h-rows of one plane per M tile
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil;
@@ -345,12 +346,13 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.sD = sD;
   h.n_cols = d->B * dil * dil * h.tilesH;
   h.pdl = pdl_enabled();
-  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(kStageNarrow) + 128 + 1024;
+  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(xp_stage_ld(h.N_tile)) + 128 + 1024;
   const long long num_tiles = h.ring ? (long long)h.n_cols * sD      // ring mode: M tiles; each CTA takes a contiguous share
                                      : (long long)d->B * dil * dil * h.tilesD * h.tilesH;
   HX_REQUIRE(num_tiles < 2147483647LL, "too many tiles");
   const int n_sms = n_sms_current();
   pl->grid = dim3((unsigned)(num_tiles < n_sms ? num_tiles : n_sms));
+  h.pp = ping_pong(h.N_tile, h.ring ? num_tiles : num_tiles * h.nM, pl->grid.x);   // M tiles per CTA
 #undef HX_REQUIRE
   return OCCD_OK;
 }
@@ -525,10 +527,14 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
   // N tile: the divisor of Cout_pad (multiple of 16, <= 256) with the smallest estimated makespan.  The model's
   // constants are estimates, not measurements: an M = 128 MMA step costs mma_step_cycles(N), an SM pulls ~44
   // bytes/cycle from L2 when the whole chip does, the epilogue drains ~12 bytes/cycle/SM, and a CTA's time is
-  // waves * max(mainloop, epilogue) + min(mainloop, epilogue).  Small-M layers (late encoder stages: 9 M tiles) get
-  // narrow N tiles that spread the write-bound epilogue over every SM; large-M layers get the widest tile (fewest
-  // re-reads of the A operand).
+  // waves * max(mainloop, epilogue) + min(mainloop, epilogue): the ping-pong schedule's overlap (N <= 128, see
+  // kTcThreads).  For the cooperative widths above 128 that overlap does not happen and the estimate is optimistic;
+  // it is kept because the wide tiles it picks for the large decoder convs measure near the tensor-core rate.
+  // Small-M layers (late encoder stages: 9 M tiles) get narrow N tiles that spread the write-bound epilogue over
+  // every SM; large-M layers get the widest tile (fewest re-reads of the A operand).
   t.Cout_pad = d->Cout_pad;
+  double est_mainloop = 0.0, est_epi = 0.0;   // the final N tile's estimates, for the schedule choice below
+  if (xp) t.N_tile = 3 * d->Cout_pad;  // one N tile: the three taps' weights stacked
   {
     int iters = 0;
     for (int i = 0; i < t.n_taps; ++i) iters += t.n_kchunks[t.tap_src[i]];
@@ -540,14 +546,18 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     // experiment hook: OCCD_EPI_RATE overrides the model's epilogue drain rate
     static const double epi_rate = [] { const char* e = getenv("OCCD_EPI_RATE"); const double v = e ? atof(e) : 0.0;
                                         return v > 0.0 ? v : 12.0; }();
-    double best = -1.0;
-    t.N_tile = 16;
-    for (int n = 16; n <= 256 && n <= d->Cout_pad; n += 16) {
-      if (d->Cout_pad % n) continue;
+    // per-tile mainloop and epilogue of an n-column tile that stores out_cols channels
+    auto estimate = [&](int n, int out_cols, double& mainloop, double& epi) {
       const double mma = (RB / 32) * mma_step_cycles(n);
       const double load = (128.0 + n) * RB / 44.0;
-      const double mainloop = iters * (mma > load ? mma : load);
-      const double epi = out_bytes_per_col * n / epi_rate;
+      mainloop = iters * (mma > load ? mma : load);
+      epi = out_bytes_per_col * out_cols / epi_rate;
+    };
+    double best = -1.0;
+    for (int n = 16; !xp && n <= 256 && n <= d->Cout_pad; n += 16) {
+      if (d->Cout_pad % n) continue;
+      double mainloop, epi;
+      estimate(n, n, mainloop, epi);
       const long long tiles = m_tiles0 * (d->Cout_pad / n);
       const double waves = (double)((tiles + n_sms - 1) / n_sms);
       const double span = waves * (mainloop > epi ? mainloop : epi) + (mainloop > epi ? epi : mainloop);
@@ -556,8 +566,8 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
         t.N_tile = n;
       }
     }
+    estimate(t.N_tile, xp ? d->Cout_pad : t.N_tile, est_mainloop, est_epi);
   }
-  if (xp) t.N_tile = 3 * d->Cout_pad;  // one N tile: the three taps' weights stacked
   if (!(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile))) {
     occd_set_last_error(xp ? "occd_conv_plan_create(tcx): no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)"
                            : "occd_conv_plan_create: no kernel compiled for this N tile");
@@ -577,7 +587,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     if (it > total_iters) total_iters = it;
   }
   // persistent kernel: one CTA per SM owns the shared memory (227 KB less the epilogue staging and barriers)
-  const int st_bytes = staging_bytes(xp ? kStageNarrow : kStageWide);
+  const int st_bytes = staging_bytes(xp ? xp_stage_ld(t.N_tile) : kStageWide);
   const int budget = 227 * 1024 - st_bytes - 16 * kMaxStages - 64 - 1024;
   // (tap, k-chunk) items per pipeline stage: the single-thread producer/MMA hand-off costs ~0.25 us, so a stage
   // must carry >= ~512 tensor-pipe cycles of work (or up to 9 items) while leaving >= 3 stages in flight
@@ -611,6 +621,10 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     const int n_sms = n_sms_current();
     pl->grid = dim3((unsigned)(all_tiles < n_sms ? all_tiles : n_sms));
   }
+  // ping-pong hides a tile's epilogue under the next tile's mainloop, but one warpgroup then stores a whole tile
+  // alone: a launch whose epilogue outweighs its mainloop (1x1 convs over few channels, store-bound) keeps both
+  // warpgroups storing at once
+  t.pp = ping_pong(t.N_tile, all_tiles, pl->grid.x) && est_mainloop >= est_epi;
   return OCCD_OK;
 }
 
@@ -786,6 +800,16 @@ extern "C" int occd_conv_plan_info(const occd_conv_plan* pl, int* info) {
   info[0] = pl->tc.TD; info[1] = pl->tc.TH; info[2] = pl->tc.TW; info[3] = pl->tc.N_tile;
   info[4] = pl->kc; info[5] = pl->tc.stages * 100 + pl->tc.group; info[6] = (int)pl->grid.x;
   info[7] = pl->tc.num_m_tiles * (pl->impl == OCCD_CONV_IMPL_TCX ? 1 : pl->tc.Cout_pad / pl->tc.N_tile);
+  return OCCD_OK;
+}
+
+extern "C" int occd_conv_plan_schedule(const occd_conv_plan* pl, int* schedule) {
+  OCCD_CHECK_ARG(pl && schedule, "occd_conv_plan_schedule: null");
+  // conv_halo_kernel is always cooperative
+  const int pp = pl->impl == OCCD_CONV_IMPL_HALOX ? pl->halox.pp
+                 : (pl->impl == OCCD_CONV_IMPL_TC || pl->impl == OCCD_CONV_IMPL_TCX) ? pl->tc.pp : 0;
+  *schedule = pl->impl == OCCD_CONV_IMPL_SIMT ? OCCD_CONV_SCHED_NONE
+                                              : (pp ? OCCD_CONV_SCHED_PINGPONG : OCCD_CONV_SCHED_COOPERATIVE);
   return OCCD_OK;
 }
 

@@ -39,7 +39,7 @@ __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, in
 // Epilogue arithmetic for one output position `pos` and NV consecutive channels [n0, n0+NV) held in v[] (fp32
 // accumulators): v = acc + bias + res1 (+ res2); the optional second output (pre-activation value: channels-last or
 // fp32 planar) is written here; on return v[] holds the out0 values act(v) (+ res2 when it is added after the
-// activation).  NV is 8 or 16; n0 is a multiple of 8.  T is the activation element type.
+// activation).  NV and n0 are multiples of 8.  T is the activation element type.
 template <typename T, int NV>
 __device__ __forceinline__ void conv_epilogue_compute(const ConvEpi& e, long long pos, int b, int n0, float* v) {
 #pragma unroll

@@ -9,17 +9,40 @@
 namespace occd_conv {
 
 // 384 threads: warpgroup 0 is the TMA producer (one lane issues, the rest give their registers away), warpgroups 1
-// and 2 issue wgmma and run the epilogue, each for 64 of the 128 rows of an M tile (fp32 accumulators in registers)
+// and 2 issue wgmma and run the epilogue (fp32 accumulators in registers) on one of two schedules, chosen by the
+// plan (ping_pong below) and compiled as a template parameter:
+//   ping-pong: each MMA warpgroup owns whole 128-row tiles, alternately (warpgroup 1 the CTA's
+//     tiles 0, 2, 4, ..., warpgroup 2 tiles 1, 3, ...).  A pair of named barriers passes the right to issue wgmma
+//     from one to the other once a tile's last wgmma is issued, so one tile's epilogue runs under the next tile's
+//     MMAs.  The accumulator is N registers per thread (two m64nN halves).
+//   cooperative: both warpgroups work on every tile, each on 64 of its 128 rows (N / 2 registers), and
+//     run their epilogues at the same time.
 constexpr int kTcThreads = 384;
 constexpr int kMaxStages = 24;
-constexpr int kEmptyArrivals = 8;   // one per MMA warp: a stage is free when both MMA warpgroups are done with it
+// Ping-pong needs the N-register accumulator to fit (N <= kPingPongMaxN) and pays off only when every warpgroup
+// has tiles to alternate: a CTA with a single tile would leave one warpgroup idle and the other with the whole
+// tile's epilogue, so plans with fewer than kPingPongMinTiles tiles per CTA stay cooperative.
+constexpr int kPingPongMaxN = 128;
+constexpr int kPingPongMinTiles = 4;
+__host__ __device__ constexpr bool ping_pong(int n) { return n <= kPingPongMaxN; }
+__host__ __device__ constexpr bool ping_pong(int n, long long tiles, long long ctas) {
+  return ping_pong(n) && tiles >= kPingPongMinTiles * ctas;
+}
+// arrivals that free a stage: one per MMA warp that reads it (4 per warpgroup)
+__host__ __device__ constexpr int empty_arrivals(bool pp) { return pp ? 4 : 8; }
+constexpr int kEmptyArrivals = 8;   // the halo kernels: both warpgroups read every stage
+// named barriers: 1 + wg: a warpgroup's epilogue staging; kTurnBar + wg: warpgroup wg may issue wgmma (ping-pong)
+constexpr int kTurnBar = 3;
 // accumulator staging for the epilogue: [2 warpgroups][64 rows][LD floats].  The per-tap kernel stages rounds of
-// 32 columns (LD = kStageWide); the halo kernels, whose resident weights leave less shared memory, rounds of 16
-// (x-packed: three groups of 8, LD = kStageNarrow) or 8 columns (LD = kStageHalo)
+// 32 columns (LD = kStageWide); the x-packed kernels rounds of 8 channels (xp_stage_ld); the halo kernel, whose
+// resident weights leave less shared memory, rounds of 8 columns (LD = kStageHalo)
 constexpr int kStageWide = 36;
-constexpr int kStageNarrow = 18;
 constexpr int kStageHalo = 10;
 __host__ __device__ constexpr int staging_bytes(int ld) { return 2 * 64 * ld * 4; }
+// x-packed staging: the 8-column blocks of all three column groups side by side (two barriers per round) for
+// N <= kPingPongMaxN; the wider tiles, whose resident weights in the halo kernel leave 4 KB less room, stage two
+// blocks and then the third (four barriers per round)
+__host__ __device__ constexpr int xp_stage_ld(int n) { return ping_pong(n) ? 26 : 18; }
 
 struct TcParams {
   ConvEpi epi;
@@ -36,6 +59,7 @@ struct TcParams {
   int a_bytes, b_stride, b_bytes;
   int rb;            // bytes per K chunk row: 128 / 64 / 32 == the swizzle mode
   int pdl;           // launched with programmatic stream serialization: wait for the producer grid after the prologue
+  int pp;            // ping-pong schedule (else cooperative), see kTcThreads
   signed char tap_src[OCCD_CONV_MAX_TAPS];
   short tap_dz[OCCD_CONV_MAX_TAPS], tap_dy[OCCD_CONV_MAX_TAPS], tap_dx[OCCD_CONV_MAX_TAPS];
   // tap groups: n_groups convolutions over the same sources and iteration space in one launch (the sub-pixel phases
@@ -47,22 +71,42 @@ struct TcParams {
   signed char grp_oadd[OCCD_CONV_MAX_GROUPS][3];
 };
 
-// One pipeline item (one K chunk of RB bytes per row) of a warpgroup's 64 x N accumulator tile: RB / 32 wgmma
-// steps, one m64nN instruction each, issued as one wgmma group.  first: the item's first step overwrites the
-// accumulators.  The steps are straight-line code for each of the three chunk widths: a wgmma inside a loop or
-// behind a branch makes ptxas fence and close every instruction on its own.
-template <typename T, int NMMA, int N>
-__device__ __forceinline__ void mma_steps(float (&acc)[N / 2], uint64_t da, uint64_t db, bool first) {
+// One pipeline item (one K chunk of RB bytes per row) of a warpgroup's NH x 64 x N accumulator tile: RB / 32 wgmma
+// steps of NH m64nN instructions each (ping-pong: NH = 2, rows 0-63 and 64-127 with the same B operand, A advanced
+// by a_half), issued as one wgmma group.  first: the item's first step overwrites the accumulators.  The steps are
+// straight-line code for each of the three chunk widths: a wgmma inside a loop or behind a branch makes ptxas fence
+// and close every instruction on its own.
+template <typename T, int NMMA, int N, int NH>
+__device__ __forceinline__ void mma_steps(float (&acc)[NH][N / 2], uint64_t da, uint64_t db, uint64_t a_half,
+                                          bool first) {
   tc::wg_fence();
 #pragma unroll
-  for (int k = 0; k < NMMA; ++k) tc::Mma<T, N>::issue(acc, da + 2 * k, db + 2 * k, (first && k == 0) ? 0u : 1u);
+  for (int k = 0; k < NMMA; ++k)
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+      tc::Mma<T, N>::issue(acc[h], da + h * a_half + 2 * k, db + 2 * k, (first && k == 0) ? 0u : 1u);
   tc::wg_commit();
 }
-template <typename T, int N>
-__device__ __forceinline__ void mma_item(float (&acc)[N / 2], uint64_t da, uint64_t db, int nmma, bool first) {
-  if (nmma == 4) mma_steps<T, 4, N>(acc, da, db, first);
-  else if (nmma == 2) mma_steps<T, 2, N>(acc, da, db, first);
-  else mma_steps<T, 1, N>(acc, da, db, first);
+template <typename T, int N, int NH>
+__device__ __forceinline__ void mma_item(float (&acc)[NH][N / 2], uint64_t da, uint64_t db, uint64_t a_half,
+                                         int nmma, bool first) {
+  if (nmma == 4) mma_steps<T, 4, N, NH>(acc, da, db, a_half, first);
+  else if (nmma == 2) mma_steps<T, 2, N, NH>(acc, da, db, a_half, first);
+  else mma_steps<T, 1, N, NH>(acc, da, db, a_half, first);
+}
+template <int NH, int NA> __device__ __forceinline__ void acc_fence(float (&acc)[NH][NA]) {
+#pragma unroll
+  for (int h = 0; h < NH; ++h) tc::acc_fence(acc[h]);
+}
+
+// Ping-pong turn of the tile with CTA-local index q (owned by warpgroup q & 1): wait for the previous tile's owner to
+// have issued its last wgmma; after the tile's own last wgmma, hand the turn on if the CTA has a next tile.  Every
+// wait is matched by exactly one signal.
+__device__ __forceinline__ void turn_take(int wg, int q) {
+  if (q > 0) tc::pair_wait(kTurnBar + wg);
+}
+__device__ __forceinline__ void turn_pass(int wg, bool has_next) {
+  if (has_next) tc::pair_signal(kTurnBar + (wg ^ 1));
 }
 
 // This thread's part of the 8-column block `blk` (a compile-time index after unrolling) of the accumulator tile ->
@@ -77,15 +121,15 @@ __device__ __forceinline__ void stage8(float* st, const float (&acc)[N / 2], int
 }
 
 // Epilogue of one warpgroup's 64-row tile, columns [0, N) of output channels n0 + [0, N): rounds of 32
-// (LD = kStageWide), 16 (kStageNarrow) or 8 (kStageHalo) columns go through shared memory so that thread t owns
-// row t / 2 and 16 (8) consecutive channels -- with 8-column rounds threads 0..63 own row t -- the vector width of
-// the channels-last stores.  The caller gives the position of the thread's row; oa:
+// (LD = kStageWide) or 8 (kStageHalo) columns go through shared memory so that thread t owns row t / 2 and 16
+// consecutive channels -- with 8-column rounds threads 0..63 own row t -- the vector width of the channels-last
+// stores.  The caller gives the position of the thread's row; oa:
 // per-launch output offset (tap groups) or nullptr for e.oadd.
 template <typename T, int N, int LD>
 __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
                                               int warp4, int lane, int t, bool valid, int b, int od, int oh, int ow,
                                               int n0, const signed char* oa) {
-  constexpr int ROUND = LD == kStageWide ? 32 : (LD == kStageNarrow ? 16 : 8);
+  constexpr int ROUND = LD == kStageWide ? 32 : 8;
   constexpr int TPR = ROUND == 8 ? 1 : 2, VW = ROUND / TPR;   // threads per row, channels per thread
   const int row = t / TPR, h = t % TPR;
   const bool fast = VW == 16 && epi_fast_ok(e);
@@ -102,7 +146,7 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
     const int cc = c0 + VW * h;
     if (row < 64 && cc < N) {
       float v[VW];
-      // staged rows are 8-byte aligned (LD is even, not a multiple of 4 for kStageNarrow)
+      // staged rows are 8-byte aligned (LD is even)
       const float2* sp = reinterpret_cast<const float2*>(st + row * LD + VW * h);
 #pragma unroll
       for (int i = 0; i < VW / 2; ++i) {
@@ -124,33 +168,46 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
 
 // Epilogue of the x-packed kernels: the accumulator holds three column groups Q_c (c = 0, 1, 2: the W taps -d, 0,
 // +d) of CP = N / 3 columns each and out[r] = Q_0[r - d] + Q_1[r] + Q_2[r + d], where r -+ d stays inside the line of PW
-// rows (lo_ok / hi_ok false: the neighbour is the conv's zero padding).  Rounds of 8 channels: Q_0 and Q_1 are
-// staged side by side, then Q_2, and threads 0..63 (one per row) form the sums and store.
+// rows (lo_ok / hi_ok false: the neighbour is the conv's zero padding).  Rounds of 8 channels: the 8-column blocks of
+// Q_0, Q_1 and Q_2 are staged (xp_stage_ld) and threads 0..63 (one per row) form the sums.
+// The sums of up to 32 channels stay in registers and go through the row epilogue together, so that its bias and
+// residual loads are issued once per chunk rather than behind every round's barriers.
 template <typename T, int N>
 __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
                                             int warp4, int lane, int t, int d, bool lo_ok, bool hi_ok, bool valid,
                                             int b, int od, int oh, int ow) {
-  constexpr int LD = kStageNarrow;
+  constexpr int LD = xp_stage_ld(N);
+  constexpr int Q2COL = LD >= 24 ? 16 : 0;   // column of Q_2's block: beside the others, or in Q_0's place later
   constexpr int CP = N / 3;
+  constexpr int CH = CP < 32 ? CP : 32;   // channels per chunk
+  const bool mine = t < 64 && valid;
 #pragma unroll
-  for (int c0 = 0; c0 < CP; c0 += 8) {
-    float v[8];
-    tc::wg_sync(bar_id);
-    stage8<LD, N>(st, acc, c0 >> 3, 0, warp4, lane);
-    stage8<LD, N>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
-    tc::wg_sync(bar_id);
-    if (t < 64 && valid) {
+  for (int c1 = 0; c1 < CP; c1 += CH) {
+    float v[CH];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = st[t * LD + 8 + i] + (lo_ok ? st[(t - d) * LD + i] : 0.f);
+    for (int j = 0; j < CH; j += 8) {
+      const int c0 = c1 + j;
+      if (c0 >= CP) break;
+      tc::wg_sync(bar_id);   // the previous round's reads are done
+      stage8<LD, N>(st, acc, c0 >> 3, 0, warp4, lane);
+      stage8<LD, N>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
+      if constexpr (Q2COL != 0) stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, Q2COL, warp4, lane);
+      tc::wg_sync(bar_id);
+      if (mine) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[j + i] = st[t * LD + 8 + i] + (lo_ok ? st[(t - d) * LD + i] : 0.f);
+      }
+      if constexpr (Q2COL == 0) {
+        tc::wg_sync(bar_id);
+        stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
+        tc::wg_sync(bar_id);
+      }
+      if (mine) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[j + i] += hi_ok ? st[(t + d) * LD + Q2COL + i] : 0.f;
+      }
     }
-    tc::wg_sync(bar_id);
-    stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
-    tc::wg_sync(bar_id);
-    if (t < 64 && valid) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] += hi_ok ? st[(t + d) * LD + i] : 0.f;
-      conv_epilogue_row<T, 8>(e, b, od, oh, ow, c0, v);
-    }
+    if (mine) conv_epilogue_row<T, CH>(e, b, od, oh, ow, c1, v);
   }
 }
 
@@ -168,20 +225,22 @@ __device__ __forceinline__ void pdl_prologue_done(int pdl) {
 // tensor), tiles are 32 wide with one halo column on each side, and the epilogue forms
 // out[r] = Q_0[r-1] + Q_1[r] + Q_2[r+1] from the three column groups.  One A fetch then feeds 3x the output columns.
 // N: the N tile (== p.N_tile), one m64nN wgmma per warpgroup and K step.
-template <typename T, int N, bool XP>
+template <typename T, int N, bool XP, bool PP>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUtensorMap tmA0,
                const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmW) {
   // Persistent, warp-specialised implicit GEMM.  Each CTA walks tiles blockIdx.x, +gridDim.x, ...:
   //   warp 0 (one lane): TMA producer -- runs ahead across tile boundaries, the smem ring never drains
-  //   warpgroups 1, 2  : wgmma over rows [0, 64) / [64, 128) of the M tile, then the epilogue from registers
+  //   warpgroups 1, 2  : wgmma, then the epilogue from registers (ping-pong or cooperative, see kTcThreads)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem is only guaranteed 16-byte aligned: round the base up to 1024 (swizzle atom alignment)
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_a + (uint32_t)(p.stages * p.group) * p.a_bytes;
-  constexpr int LD = XP ? kStageNarrow : kStageWide;
+  constexpr int LD = XP ? xp_stage_ld(N) : kStageWide;
+  static_assert(!PP || ping_pong(N), "ping-pong holds N accumulator registers per thread");
+  constexpr int NH = PP ? 2 : 1;   // 64-row halves of the M tile in one warpgroup's accumulator
   const uint32_t smem_st = smem_b + (uint32_t)(p.stages * p.group) * p.b_stride;
   const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
   const uint32_t full_bar = bar_base;
@@ -200,7 +259,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
     tc::prefetch_tmap(&tmW);
     for (int s = 0; s < p.stages; ++s) {
       tc::mbar_init(full_bar + 8u * s, 1);
-      tc::mbar_init(empty_bar + 8u * s, kEmptyArrivals);
+      tc::mbar_init(empty_bar + 8u * s, empty_arrivals(PP));
     }
     tc::fence_barrier_init();
   }
@@ -263,14 +322,23 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
   const int t = threadIdx.x & 127;
   float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
   const int nmma = RB / 32;
-  const uint64_t da0 = tc::make_sdesc(smem_a, RB) + (uint64_t)(64 * wg * RB / 16);
+  const uint64_t a_half = (uint64_t)(64 * RB / 16);
+  const uint64_t da0 = tc::make_sdesc(smem_a, RB) + (PP ? 0 : wg * a_half);
   const uint64_t db0 = tc::make_sdesc(smem_b, RB);
-  float acc[N / 2];
+  float acc[NH][N / 2];
   int s = 0;
   uint32_t ph = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  int q = 0;   // CTA-local tile index
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++q) {
     const int tgrp = tile / tiles_per_group;       // tap group (sub-pixel phase) of this tile
     const int iters = p.grp_iters[tgrp];
+    if (PP && (q & 1) != wg) {
+      // the other warpgroup's tile: step over the stages the producer fills for it
+      for (int n = (iters + p.group - 1) / p.group; n > 0; --n)
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
+      continue;
+    }
+    if (PP) turn_take(wg, q);
     int prev = -1;
     for (int it = 0; it < iters;) {
       tc::mbar_wait(full_bar + 8u * s, ph);
@@ -278,8 +346,9 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
       for (int g = 0; g < cnt; ++g, ++it) {
         const uint64_t da = da0 + (uint64_t)((s * p.group + g) * (p.a_bytes >> 4));
         const uint64_t db = db0 + (uint64_t)((s * p.group + g) * (p.b_stride >> 4));
-        mma_item<T, N>(acc, da, db, nmma, it == 0);
+        mma_item<T, N, NH>(acc, da, db, a_half, nmma, it == 0);
       }
+      if (PP && it == iters) turn_pass(wg, tile + (int)gridDim.x < num_tiles);   // the tile's last wgmma is issued
       tc::wg_wait_le(cnt);  // only this stage's groups are pending: hand the previous stage back to the producer
       if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar + 8u * prev);
       prev = s;
@@ -287,7 +356,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
     }
     tc::wg_wait<0>();
     if (lane == 0) tc::mbar_arrive(empty_bar + 8u * prev);
-    tc::acc_fence(acc);
+    acc_fence(acc);
 
     const int tg = tile - tgrp * tiles_per_group;
     const int nt = tg % n_tiles_n;
@@ -296,24 +365,28 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
     const int th = tt % p.tiles_h; tt /= p.tiles_h;
     const int td = tt % p.tiles_d; tt /= p.tiles_d;
     const int b = tt;
-    if constexpr (XP) {
-      // TW == 32: row == tile column inside each 32-row line, so the W neighbours' partial sums are rows r -+ 1
-      const int row = 64 * wg + t;
-      const int rw = row % 32;
-      const int rh = (row / 32) % p.TH;
-      const int rd = row / (32 * p.TH);
-      const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * 30 + rw - 1;
-      const bool valid = t < 64 && od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && rw >= 1 && rw <= 30;
-      epilogue_xp<T, N>(p.epi, acc, st, 1 + wg, warp4, lane, t, 1, true, true, valid, b, od, oh, ow);
-    } else {
-      const int row = 64 * wg + (t >> 1);
-      const int rw = row % p.TW;
-      const int rh = (row / p.TW) % p.TH;
-      const int rd = row / (p.TW * p.TH);
-      const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * p.TW + rw;
-      const bool valid = od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW;
-      epilogue_rows<T, N, LD>(p.epi, acc, st, 1 + wg, warp4, lane, t, valid, b, od, oh, ow, nt * N,
-                              p.n_groups > 1 ? p.grp_oadd[tgrp] : nullptr);
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const int r64 = 64 * (PP ? h : wg);   // first row of this 64-row half of the M tile
+      if constexpr (XP) {
+        // TW == 32: row == tile column inside each 32-row line, so the W neighbours' partial sums are rows r -+ 1
+        const int row = r64 + t;
+        const int rw = row % 32;
+        const int rh = (row / 32) % p.TH;
+        const int rd = row / (32 * p.TH);
+        const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * 30 + rw - 1;
+        const bool valid = t < 64 && od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && rw >= 1 && rw <= 30;
+        epilogue_xp<T, N>(p.epi, acc[h], st, 1 + wg, warp4, lane, t, 1, true, true, valid, b, od, oh, ow);
+      } else {
+        const int row = r64 + (t >> 1);
+        const int rw = row % p.TW;
+        const int rh = (row / p.TW) % p.TH;
+        const int rd = row / (p.TW * p.TH);
+        const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * p.TW + rw;
+        const bool valid = od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW;
+        epilogue_rows<T, N, LD>(p.epi, acc[h], st, 1 + wg, warp4, lane, t, valid, b, od, oh, ow, nt * N,
+                                p.n_groups > 1 ? p.grp_oadd[tgrp] : nullptr);
+      }
     }
   }
 }
@@ -426,7 +499,7 @@ conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ C
   const int nmma = RB / 32;
   const uint64_t db_w = tc::make_sdesc(smem_w, RB);
   const int w_step16 = p.b_stride / 16;
-  float acc[N / 2];
+  float acc[1][N / 2];
   tc::mbar_wait(w_bar, 0);
   int s = 0;
   uint32_t ph = 0;
@@ -441,10 +514,11 @@ conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ C
     for (int m = 0; m < p.nM; ++m) {
       const uint64_t da_m = da_stage + (uint64_t)(m * (128 * RB / 16));
       for (int tp = 0; tp < p.n_taps; ++tp)
-        mma_item<T, N>(acc, da_m + (uint64_t)p.tap_off16[tp], db_w + (uint64_t)(tp * w_step16), nmma, tp == 0);
+        mma_item<T, N, 1>(acc, da_m + (uint64_t)p.tap_off16[tp], db_w + (uint64_t)(tp * w_step16), 0, nmma,
+                          tp == 0);
       tc::wg_wait<0>();
       if (m == p.nM - 1 && lane == 0) tc::mbar_arrive(empty_bar + 8u * s);   // the box is no longer read
-      tc::acc_fence(acc);
+      acc_fence(acc);
       const int R = p.R0 + m * 128 + 64 * wg + t;   // epilogue threads t < 64: one row each
       const int pw = R % p.PW;
       const int phh = (R / p.PW) % p.PH;
@@ -453,7 +527,7 @@ conv_halo_kernel(const __grid_constant__ HaloParams p, const __grid_constant__ C
                 ow = (tw * p.BW + pw - p.hw) * d + rc;
       const bool valid = pd >= p.hd && pd < p.hd + p.BD && phh >= p.hh && phh < p.hh + p.BH && pw >= p.hw &&
                          pw < p.hw + p.BW && od < p.D && oh < p.H && ow < p.W;
-      epilogue_rows<T, N, LD>(p.epi, acc, st, 1 + wg, warp4, lane, t, valid, b, od, oh, ow, 0, nullptr);
+      epilogue_rows<T, N, LD>(p.epi, acc[0], st, 1 + wg, warp4, lane, t, valid, b, od, oh, ow, 0, nullptr);
     }
     if (++s == p.stages) { s = 0; ph ^= 1u; }
   }
@@ -494,12 +568,13 @@ struct HaloxParams {
   // four stages are a ring of single input planes, output plane z reads ring planes z-1, z, z+1, so every M tile costs
   // ONE new plane (prefetched a plane ahead) instead of a whole box loaded while the tensor core waits
   int ring, sD, n_cols;
+  int pp;                     // ping-pong schedule (else cooperative), see kTcThreads
   signed char grp_dz[9];      // -1 / 0 / +1: which ring plane a group reads
   short grp_row[9];           // (hh + dy) * PW: its row offset inside the plane
 };
 
 // N: the N tile (== p.N_tile == 3 * CP)
-template <typename T, int N>
+template <typename T, int N, bool PP>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__ CUtensorMap tmA,
                   const __grid_constant__ CUtensorMap tmW) {
@@ -507,7 +582,9 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_w = smem_base;                                   // [n_groups][b_stride] resident weights
   const uint32_t smem_a = smem_w + (uint32_t)p.w_bytes;                 // [stages][a_stage_bytes]
-  constexpr int LD = kStageNarrow;
+  constexpr int LD = xp_stage_ld(N);
+  static_assert(!PP || ping_pong(N), "ping-pong holds N accumulator registers per thread");
+  constexpr int NH = PP ? 2 : 1;
   const uint32_t smem_st = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
   const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
   const uint32_t full_bar = bar_base;            // [4]
@@ -599,7 +676,8 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
     return;
   }
 
-  // ===== MMA + epilogue warpgroups: rows [64 wg, 64 wg + 64) of each M tile =====
+  // ===== MMA + epilogue warpgroups: ping-pong (whole M tiles, alternately) or cooperative (rows [64 wg, 64 wg + 64)
+  // of every M tile) =====
   tc::reg_alloc<232>();
   const int wg = (warp >> 2) - 1;
   const int warp4 = warp & 3;
@@ -608,22 +686,37 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   const int nmma = RB / 32;
   const uint64_t db_w = tc::make_sdesc(smem_w, RB);
   const int w_step16 = p.b_stride / 16;
-  const int rr = 64 * wg + t;              // row inside an M tile (epilogue threads t < 64)
-  const int hr = rr / p.PW;                // h-row inside the M tile
-  const int pw = rr - hr * p.PW;           // == output w
-  const bool lo_ok = pw >= d, hi_ok = pw + d < p.PW;
-  float acc[N / 2];
+  const uint64_t a_half = (uint64_t)(64 * RB / 16);
+  const int row0 = PP ? 0 : 64 * wg;       // first M-tile row of this warpgroup's MMAs
+  float acc[NH][N / 2];
+  // epilogue of this warpgroup's rows of an M tile at output plane od whose first h-row is oh_base (sub-sampled)
+  auto tile_epilogue = [&](int b, int ra, int rb, int od, int oh_base) {
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const int rr = 64 * (PP ? h : wg) + t;   // row inside the M tile (epilogue threads t < 64)
+      const int hr = rr / p.PW;                // h-row inside the M tile
+      const int pw = rr - hr * p.PW;           // == output w
+      const int oh = (oh_base + hr) * d + rb;
+      const bool valid = t < 64 && od < p.D && oh < p.H;
+      epilogue_xp<T, N>(p.epi, acc[h], st, 1 + wg, warp4, lane, t, d, pw >= d, pw + d < p.PW, valid, b, od, oh, pw);
+    }
+  };
   tc::mbar_wait(w_bar, 0);
   if (p.ring) {
     // one M tile (one plane, 128 / PW h-rows) per output plane
+    const int total = (int)(ring_hi - ring_lo);   // this CTA's planes; ping-pong: plane q belongs to warpgroup q & 1
+    int q = 0;
     uint32_t n0 = 0;     // ring index of this unit's first plane (z0 - 1)
     for (long long pos = ring_lo; pos < ring_hi;) {
       int b, ra, rb, th, z0, z1;
       decode_ring(pos, b, ra, rb, th, z0, z1);
       pos += z1 - z0;
       const int K = z1 - z0;
-      for (int k = 0; k < K; ++k) {
-        for (uint32_t i = (k == 0 ? 0u : 2u); i < 3u; ++i) {     // planes z-1 and z were waited for by plane z-1
+      for (int k = 0; k < K; ++k, ++q) {
+        if (PP && (q & 1) != wg) continue;
+        if (PP) turn_take(wg, q);
+        // cooperative: planes z-1 and z were waited for by plane z-1
+        for (uint32_t i = (PP || k == 0 ? 0u : 2u); i < 3u; ++i) {
           const uint32_t n = n0 + (uint32_t)k + i;
           tc::mbar_wait(full_bar + 8u * (n & 3u), (n >> 2) & 1u);
         }
@@ -631,46 +724,63 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
         for (int g = 0; g < p.n_groups; ++g) {
           const uint32_t slot = (r + (uint32_t)p.grp_dz[g]) & 3u;
           const uint64_t da = tc::make_sdesc(smem_a + slot * (uint32_t)p.a_stage_bytes, RB) +
-                              (uint64_t)((p.grp_row[g] + 64 * wg) * (RB / 16));
-          mma_item<T, N>(acc, da, db_w + (uint64_t)(g * w_step16), nmma, g == 0);
+                              (uint64_t)((p.grp_row[g] + row0) * (RB / 16));
+          mma_item<T, N, NH>(acc, da, db_w + (uint64_t)(g * w_step16), a_half, nmma, g == 0);
         }
+        if (PP) turn_pass(wg, q + 1 < total);
         tc::wg_wait<0>();
         if (lane == 0) {
-          tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k) & 3u));          // plane z-1 is done with
-          if (k == K - 1) {                                                     // ... and the unit's last two
-            tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k + 1u) & 3u));
-            tc::mbar_arrive(empty_bar + 8u * ((n0 + (uint32_t)k + 2u) & 3u));
+          // ring planes n0 + k .. n0 + k + 2 are read by the unit's output planes k - 2 .. k + 2; a plane's slot is
+          // free after 8 arrivals, one per MMA warp, each given when its warpgroup's last reader of it has retired
+          const uint32_t nz = n0 + (uint32_t)k;
+          if (PP) {
+            // this warpgroup's next plane is k + 2, which reads only n0 + k + 2 of these; the other warpgroup owns
+            // planes k - 1 and k + 1.  A plane the other warpgroup never reads gets both warpgroups' arrivals here
+            const bool o_prev = k >= 1, o_next = k + 1 < K;
+            tc::mbar_arrive(empty_bar + 8u * (nz & 3u), o_prev ? 1u : 2u);
+            tc::mbar_arrive(empty_bar + 8u * ((nz + 1u) & 3u), (o_prev || o_next) ? 1u : 2u);
+            if (k + 2 >= K) tc::mbar_arrive(empty_bar + 8u * ((nz + 2u) & 3u), o_next ? 1u : 2u);
+          } else {
+            tc::mbar_arrive(empty_bar + 8u * (nz & 3u));                          // plane z-1 is done with
+            if (k == K - 1) {                                                     // ... and the unit's last two
+              tc::mbar_arrive(empty_bar + 8u * ((nz + 1u) & 3u));
+              tc::mbar_arrive(empty_bar + 8u * ((nz + 2u) & 3u));
+            }
           }
         }
-        tc::acc_fence(acc);
-        const int od = (z0 + k) * d + ra;
-        const int oh = (th * p.BH + hr) * d + rb;
-        const bool valid = t < 64 && od < p.D && oh < p.H;
-        epilogue_xp<T, N>(p.epi, acc, st, 1 + wg, warp4, lane, t, d, lo_ok, hi_ok, valid, b, od, oh, pw);
+        acc_fence(acc);
+        tile_epilogue(b, ra, rb, (z0 + k) * d + ra, th * p.BH);
       }
       n0 += (uint32_t)K + 2u;
     }
     return;
   }
+  // box mode: M tile m of CTA tile i is number q = i * nM + m of the CTA; ping-pong: it belongs to warpgroup q & 1
+  const int total = ((num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x) * p.nM;
+  int q = 0;
   int s = 0;
   uint32_t ph = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int b, ra, rb, td, th;
     decode(tile, b, ra, rb, td, th);
-    tc::mbar_wait(full_bar + 8u * s, ph);
     const uint64_t da_stage = tc::make_sdesc(smem_a + (uint32_t)s * p.a_stage_bytes, RB);
-    for (int m = 0; m < p.nM; ++m) {
+    for (int m = 0; m < p.nM; ++m, ++q) {
+      if (PP && (q & 1) != wg) continue;
+      if (PP) turn_take(wg, q);
+      tc::mbar_wait(full_bar + 8u * s, ph);
       for (int g = 0; g < p.n_groups; ++g) {
-        const uint64_t da = da_stage + (uint64_t)((p.mt_row[m] + p.grp_off[g] + 64 * wg) * (RB / 16));
-        mma_item<T, N>(acc, da, db_w + (uint64_t)(g * w_step16), nmma, g == 0);
+        const uint64_t da = da_stage + (uint64_t)((p.mt_row[m] + p.grp_off[g] + row0) * (RB / 16));
+        mma_item<T, N, NH>(acc, da, db_w + (uint64_t)(g * w_step16), a_half, nmma, g == 0);
       }
+      if (PP) turn_pass(wg, q + 1 < total);
       tc::wg_wait<0>();
-      if (m == p.nM - 1 && lane == 0) tc::mbar_arrive(empty_bar + 8u * s);
-      tc::acc_fence(acc);
-      const int od = (td * p.BD + p.mt_pd[m] - p.hd) * d + ra;
-      const int oh = (th * p.BH + p.mt_ph0[m] + hr - p.hh) * d + rb;
-      const bool valid = t < 64 && od < p.D && oh < p.H;
-      epilogue_xp<T, N>(p.epi, acc, st, 1 + wg, warp4, lane, t, d, lo_ok, hi_ok, valid, b, od, oh, pw);
+      // the box is free after 8 arrivals, one per MMA warp that read it (ping-pong with nM == 1: one warpgroup)
+      if (lane == 0) {
+        if (PP) tc::mbar_arrive(empty_bar + 8u * s, p.nM == 2 ? 1u : 2u);
+        else if (m == p.nM - 1) tc::mbar_arrive(empty_bar + 8u * s);
+      }
+      acc_fence(acc);
+      tile_epilogue(b, ra, rb, (td * p.BD + p.mt_pd[m] - p.hd) * d + ra, th * p.BH + p.mt_ph0[m] - p.hh);
     }
     if (++s == p.stages) { s = 0; ph ^= 1u; }
   }
@@ -758,13 +868,21 @@ int launch_conv(const occd_conv_plan* pl, int pdl, cudaStream_t st, Args&&... ar
   return OCCD_OK;
 }
 
-// launch the kernel compiled for the plan's N tile (plan creation has checked that there is one)
+// launch the kernel compiled for the plan's N tile and schedule (plan creation has checked that there is one)
+template <typename T, int N, bool XP>
+int run_tc_n(const occd_conv_plan* pl, cudaStream_t st) {
+  if constexpr (ping_pong(N)) {
+    if (pl->tc.pp)
+      return launch_conv<conv_tc_kernel<T, N, XP, true>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1],
+                                                         pl->tmA[2], pl->tmW);
+  }
+  return launch_conv<conv_tc_kernel<T, N, XP, false>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2],
+                                                      pl->tmW);
+}
 template <typename T, bool XP, int... Ns>
 int run_tc(const occd_conv_plan* pl, cudaStream_t st, NTiles<Ns...>) {
   int rc = OCCD_ERR_UNSUPPORTED;
-  (void)((pl->tc.N_tile == Ns &&
-          (rc = launch_conv<conv_tc_kernel<T, Ns, XP>>(pl, pl->tc.pdl, st, pl->tc, pl->tmA[0], pl->tmA[1], pl->tmA[2],
-                                                       pl->tmW), true)) || ...);
+  (void)((pl->tc.N_tile == Ns && (rc = run_tc_n<T, Ns, XP>(pl, st), true)) || ...);
   if (rc == OCCD_ERR_UNSUPPORTED) occd_set_last_error("occd_conv_run: no kernel compiled for the plan's N tile");
   return rc;
 }
@@ -777,13 +895,18 @@ int run_halo(const occd_conv_plan* pl, cudaStream_t st, NTiles<Ns...>) {
   if (rc == OCCD_ERR_UNSUPPORTED) occd_set_last_error("occd_conv_run: no kernel compiled for the plan's N tile");
   return rc;
 }
+template <typename T, int N>
+int run_halox_n(const occd_conv_plan* pl, cudaStream_t st) {
+  if constexpr (ping_pong(N)) {
+    if (pl->halox.pp)
+      return launch_conv<conv_halox_kernel<T, N, true>>(pl, pl->halox.pdl, st, pl->halox, pl->tmA[0], pl->tmW);
+  }
+  return launch_conv<conv_halox_kernel<T, N, false>>(pl, pl->halox.pdl, st, pl->halox, pl->tmA[0], pl->tmW);
+}
 template <typename T, int... Ns>
 int run_halox(const occd_conv_plan* pl, cudaStream_t st, NTiles<Ns...>) {
   int rc = OCCD_ERR_UNSUPPORTED;
-  (void)((pl->halox.N_tile == Ns &&
-          (rc = launch_conv<conv_halox_kernel<T, Ns>>(pl, pl->halox.pdl, st, pl->halox, pl->tmA[0], pl->tmW),
-           true)) ||
-         ...);
+  (void)((pl->halox.N_tile == Ns && (rc = run_halox_n<T, Ns>(pl, st), true)) || ...);
   if (rc == OCCD_ERR_UNSUPPORTED) occd_set_last_error("occd_conv_run: no kernel compiled for the plan's N tile");
   return rc;
 }

@@ -21,6 +21,10 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// count arrivals at once (count >= 1)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
 // Spin on the phase parity.  A bounded spin: a protocol bug traps (context error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
@@ -42,6 +46,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 
 // named barrier over the 128 threads of one warpgroup (ids 1.. ; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// named barrier shared by two warpgroups: one waits (bar.sync), the other signals without waiting (bar.arrive)
+__device__ __forceinline__ void pair_wait(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void pair_signal(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
 
 // register budget hand-off between the producer warpgroup and the MMA warpgroups
 template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }

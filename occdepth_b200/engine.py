@@ -356,7 +356,11 @@ class ConvOp:
     def info(self):
         arr = (C.c_int * 8)()
         _lib.check(_lib.lib().occd_conv_plan_info(self.handle, arr), "occd_conv_plan_info")
-        return dict(zip(("TD", "TH", "TW", "N_tile", "KC", "stages", "grid_x", "grid_y"), list(arr)))
+        sched = C.c_int()
+        _lib.check(_lib.lib().occd_conv_plan_schedule(self.handle, C.byref(sched)), "occd_conv_plan_schedule")
+        info = dict(zip(("TD", "TH", "TW", "N_tile", "KC", "stages", "grid_x", "grid_y"), list(arr)))
+        info["schedule"] = {0: "none", 1: "cooperative", 2: "pingpong"}[sched.value]
+        return info
 
     def run(self, stream):
         _lib.check(_lib.lib().occd_conv_run(self.handle, stream), "occd_conv_run(%s)" % self.name)
