@@ -72,7 +72,9 @@ typedef struct {
 int occd_sfa_lift_fwd(const occd_sfa_params* p, void* stream);
 
 /* layout helpers at the module boundary: NCHW/NCDHW fp32 <-> channels-last (f32 or bf16)          */
-/* in: [B][C][S] planar fp32, out: [B][S][cstride] channels-last (pad channels zero-filled)        */
+/* in: [B][C][S] planar fp32, out: [B][S][cstride] channels-last (pad channels zero-filled), each   */
+/* value rounded to the activation type: bf16 (round-to-nearest-even) or, for OCCD_DTYPE_F32, TF32  */
+/* (cvt.rna.tf32.f32) like every other F32 activation store                                        */
 int occd_planar_to_cl(const float* in, void* out, int out_dtype, long long B, int C, long long S,
                       int cstride, void* stream);
 /* in: [B][S][cstride] channels-last, out: [B][C][S] planar fp32                                   */

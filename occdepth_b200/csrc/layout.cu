@@ -15,7 +15,7 @@ extern "C" int occd_abi_version(void) { return OCCD_ABI_VERSION; }
 
 namespace {
 
-// 32x32 smem tile transpose: in [C][S] -> out [S][cstride]
+// 32x32 smem tile transpose: in [C][S] -> out [S][cstride], rounded to the activation type (bf16, or TF32 for fp32)
 template <typename OT>
 __global__ void planar_to_cl_kernel(const float* __restrict__ in, OT* __restrict__ out, int C, long long S,
                                     int cstride) {
@@ -37,7 +37,7 @@ __global__ void planar_to_cl_kernel(const float* __restrict__ in, OT* __restrict
     if (s < S && c < cstride) {
       const float v = tile[threadIdx.x][i];
       if constexpr (sizeof(OT) == 2) outb[s * cstride + c] = __float2bfloat16_rn(v);
-      else outb[s * cstride + c] = v;
+      else outb[s * cstride + c] = round_tf32(v);   // F32 activations hold TF32 values (Elem<float>::st8)
     }
   }
 }
