@@ -12,7 +12,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..engine import CL, FnOp, Plan, require_cuda
+from ..engine import CL, FnOp, Plan, _round_up, require_cuda
 from ._base import B200Module, _to_planar
 from .SFA import SFA, lift_multiscale
 from .unet2d import UNet2D
@@ -144,15 +144,20 @@ class OccDepth(_Base, B200Module):
         img = plan.alloc(B * (1 if view_shard else V), 1, H, W, 3)
         Cf = self.feature_2d_oc
         assert Cf == self.feature, "feature_2d_oc must equal feature (the lift feeds the 3D net directly)"
-        assert Cf % 8 == 0, "feature_2d_oc must be a multiple of 8"
+        if Cf % 4 != 0 or not 0 < Cf <= 256:
+            raise NotImplementedError("OccDepth: feature must be a multiple of 4 between 4 and 256 (got %d)" % Cf)
+        # every 2-D feature map the lift reads has channel stride Cp; its pad channels [Cf, Cp) are zero (CL.alloc
+        # zero-fills, convolutions and the virtual-view kernel write zeros there), so the lift runs over Cp channels
+        # and writes zeros into the pad channels of x3d (DESIGN.md section 3)
+        Cp = _round_up(Cf, 8)
         scales = [int(s) for s in self.project_res]
         views = {}
         outs = {}
         if virtual:
-            # view-major buffers [2, B, h, w, C]: the 2D net writes view 0, the virtual-view kernel view 1
+            # view-major buffers [2, B, h, w, Cp]: the 2D net writes view 0, the virtual-view kernel view 1
             for s in scales:
                 h_s, w_s = feature_hw(H, W, s)
-                vb = torch.zeros(2, B, h_s, w_s, Cf, dtype=plan.dtype, device=dev)
+                vb = torch.zeros(2, B, h_s, w_s, Cp, dtype=plan.dtype, device=dev)
                 views[s] = vb
                 outs["1_%d" % s] = CL(vb[0].unsqueeze(1), Cf)
         gathered = None
@@ -165,17 +170,17 @@ class OccDepth(_Base, B200Module):
                 P_tot += h_s * w_s
             slice_len = -(-P_tot // R2)
             P_pad = slice_len * R2
-            packed = torch.zeros(P_pad, Cf, dtype=plan.dtype, device=dev)       # this rank's view, all scales
-            gathered = torch.zeros(2, P_pad, Cf, dtype=plan.dtype, device=dev)  # both views after the all-gather
+            packed = torch.zeros(P_pad, Cp, dtype=plan.dtype, device=dev)       # this rank's view, all scales
+            gathered = torch.zeros(2, P_pad, Cp, dtype=plan.dtype, device=dev)  # both views after the all-gather
             for s, (h_s, w_s), o in zip(scales, hw, offs):
-                outs["1_%d" % s] = CL(packed[o:o + h_s * w_s].view(1, 1, h_s, w_s, Cf), Cf)
+                outs["1_%d" % s] = CL(packed[o:o + h_s * w_s].view(1, 1, h_s, w_s, Cp), Cf)
         x_rgb = self.net_rgb.emit(plan, img, outs)                          # {"1_s": CL [B*V,1,h,w,Cf]}
         if view_shard:
             sl = slab.rank % R2
             plan.add(slab.all_gather_op(packed[sl * slice_len:(sl + 1) * slice_len],
-                                        gathered.view(2 * R2, slice_len, Cf)))
+                                        gathered.view(2 * R2, slice_len, Cp)))
             for s, (h_s, w_s), o in zip(scales, hw, offs):
-                views[s] = gathered[:, o:o + h_s * w_s].view(2, 1, h_s, w_s, Cf)   # [view][B=1][h][w][C]
+                views[s] = gathered[:, o:o + h_s * w_s].view(2, 1, h_s, w_s, Cp)   # [view][B=1][h][w][Cp]
         depth0 = None
         if virtual:
             L = _lib.lib()
@@ -186,7 +191,7 @@ class OccDepth(_Base, B200Module):
                 vb = views[s]
                 _, _, h_s, w_s, _ = vb.shape
                 plan.add(FnOp(lambda st, vb=vb, h_s=h_s, w_s=w_s, s=s: L.occd_virtual_view_fwd(
-                    vb[0].data_ptr(), vb[1].data_ptr(), depth0.data_ptr(), plan.lib_dtype, B, h_s, w_s, Cf, Cf, Cf,
+                    vb[0].data_ptr(), vb[1].data_ptr(), depth0.data_ptr(), plan.lib_dtype, B, h_s, w_s, Cf, Cp, Cp,
                     depth0.shape[0], depth0.shape[1], bf / s, st), "virtual_view_1_%d" % s, keep=(vb, depth0)))
         pix = torch.zeros(B, VL, N, P, 2, dtype=torch.int64, device=dev)
         fov = torch.zeros(B, VL, N, P, dtype=torch.bool, device=dev)
@@ -199,11 +204,11 @@ class OccDepth(_Base, B200Module):
             feats = []
             for s in scales:
                 if virtual or view_shard:
-                    feats.append(views[s][:, b])                            # [2, h, w, Cf], strided views
+                    feats.append(views[s][:, b])                            # [2, h, w, Cp], strided views
                 else:
                     f = x_rgb["1_%d" % s]
-                    assert f.coff == 0 and f.cstride == Cf
-                    feats.append(f.buf[b * V:(b + 1) * V, 0])               # [V, h, w, Cf] contiguous view
+                    assert f.coff == 0 and f.cstride == Cp
+                    feats.append(f.buf[b * V:(b + 1) * V, 0])               # [V, h, w, Cp] contiguous view
             out_b = CL(x3d.buf[b:b + 1], x3d.C, 0, x3d.d0, x3d.dlen)
             pr = prior[b] if prior is not None else None
             plan.add(FnOp(lambda st, feats=feats, pb=pix[b], fb=fov[b], ob=out_b, pr=pr:

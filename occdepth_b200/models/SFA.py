@@ -73,7 +73,8 @@ def lift_multiscale(feats, divs, projected_pix, fov_mask, out, dataset, scene_si
                     scale_const=1.0, stream=None):
     """Fused lift over all 2D scales.  feats: list of channels-last bf16 tensors [V, h_s, w_s, C] whose views may be
     strided (e.g. a [V, B, h, w, C] buffer sliced at one batch item); out: CL with dims (1, X, Y, Z) receiving
-    sum_s SFA_s (x prior x scale_const)."""
+    sum_s SFA_s (x prior x scale_const).  C may be the padded stride round_up(out.C, 8) when channels [out.C, C) of
+    every feature map are zero."""
     p = _lib.SfaParams()
     V = feats[0].shape[0]
     Cch = feats[0].shape[3]
@@ -87,7 +88,9 @@ def lift_multiscale(feats, divs, projected_pix, fov_mask, out, dataset, scene_si
     assert out.buf.dtype == feats[0].dtype
     p.n_scales, p.feat_dtype = len(feats), (_lib.DTYPE_F32 if tf32 else _lib.DTYPE_BF16)
     _fill_common(p, projected_pix, fov_mask, V, Cch)
-    assert out.coff == 0 and out.C == Cch and out.spatial() == p.N
+    # the feature maps may carry zero pad channels beyond out.C (padded channel stride); they are lifted too, and the
+    # zeros they produce land in the output's pad channels
+    assert out.coff == 0 and out.C <= Cch <= out.cstride and out.spatial() == p.N
     p.out, p.out_mode, p.out_cstride = out.ptr, (_lib.SFA_OUT_TF32_CL if tf32 else _lib.SFA_OUT_BF16_CL), out.cstride
     _nyu_perm(p, dataset, scene_size, project_scale)
     if prior is not None:
