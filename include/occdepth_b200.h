@@ -285,6 +285,17 @@ int occd_frustum_sample_fwd(const float* depth, const float* cams, int V, int Dn
 /* normalised (x, y, z) coordinates of F.grid_sample(bilinear, zeros, align_corners=False)                    */
 int occd_grid_sample_prior_fwd(const float* depth, const float* grids, int V, int Dn, int h, int w, int X, int Y,
                                int Z, int mean_mode, float* out, int perm_xzy, void* stream);
+/* X windows of the two entry points above, for the X-slab partition of one frame: the prior of planes        */
+/* [x0, x0 + Xl) of the X-plane grid, written densely as [Xl*Y*Z] in the local voxel order (perm_xzy: as       */
+/* [Xl][Z][Y]).  Voxel coordinates and the index into `grids` ([V][X*Y*Z][3], read at full-grid indices; only  */
+/* the window's rows are read) are those of the whole grid, so a window equals the matching slice of the whole  */
+/* grid's output bit for bit; x0 = 0, Xl = X is the whole grid.  Refused: Xl < 1, x0 < 0, x0 + Xl > X.         */
+int occd_frustum_sample_window_fwd(const float* depth, const float* cams, int V, int Dn, int h, int w, int X, int Y,
+                                   int Z, int x0, int Xl, float img_w, float img_h, float dmin, float dmax,
+                                   int mean_mode, float* out, int perm_xzy, void* stream);
+int occd_grid_sample_prior_window_fwd(const float* depth, const float* grids, int V, int Dn, int h, int w, int X,
+                                      int Y, int Z, int x0, int Xl, int mean_mode, float* out, int perm_xzy,
+                                      void* stream);
 /* softmax over the C planar channels of [B][C][S] fp32 (depth_feature.softmax(1), flosp_depth.py:548) */
 int occd_softmax_planar(const float* in, float* out, long long B, int C, long long S, void* stream);
 /* out[b] = act(W in[b] + bias): the Linear / 1x1-on-a-vector layers of DepthNet.mlp and SELayer    */

@@ -118,6 +118,8 @@ SYMBOLS = {
     "occd_scale_weights": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "occd_frustum_sample_fwd": (C.c_int, [_vp, _vp] + [_i] * 7 + [_f] * 4 + [_i, _vp, _i, _vp]),
     "occd_grid_sample_prior_fwd": (C.c_int, [_vp, _vp] + [_i] * 8 + [_vp, _i, _vp]),
+    "occd_frustum_sample_window_fwd": (C.c_int, [_vp, _vp] + [_i] * 9 + [_f] * 4 + [_i, _vp, _i, _vp]),
+    "occd_grid_sample_prior_window_fwd": (C.c_int, [_vp, _vp] + [_i] * 10 + [_vp, _i, _vp]),
     "occd_softmax_planar": (C.c_int, [_vp, _vp, _ll, _i, _ll, _vp]),
     "occd_fc_fwd": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "occd_channel_scale": (C.c_int, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp]),

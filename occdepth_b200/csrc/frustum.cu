@@ -23,22 +23,27 @@ __device__ __forceinline__ float dehom(float z) {  // kornia 0.5.0 convert_point
 // GIVEN: the normalised sampling coordinates are read from `grids` ([V][N][3] = (x, y, z) of F.grid_sample's grid:
 // the reference's infer_mode / ONNX route feeds pre-computed grids, OccDepth.py:310-317, flosp_depth.py:564-565)
 // instead of being computed from the camera tables.
+// X window: the thread grid covers planes [xw0, xw0 + Xl) of the X-plane grid and writes them densely in the local
+// voxel order (perm_xzy applied inside the window); the voxel coordinate and the index of a given grid are those of
+// the full grid, so a window computes exactly the values of the matching slice of the whole grid.
 template <bool GIVEN>
 __global__ void frustum_sample_kernel(const float* __restrict__ depth, const FrustumCam* __restrict__ cams,
                                       const float* __restrict__ grids, int V,
-                                      int Dn, int h, int w, int X, int Y, int Z, float img_w, float img_h,
-                                      float dmin, float bin_size, int mean_mode, float* __restrict__ out,
-                                      int perm_xzy) {
-  const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+                                      int Dn, int h, int w, int X, int Y, int Z, int xw0, int Xl, float img_w,
+                                      float img_h, float dmin, float bin_size, int mean_mode,
+                                      float* __restrict__ out, int perm_xzy) {
+  const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // local voxel index
   const long long N = (long long)X * Y * Z;
-  if (n >= N) return;
-  const int k = (int)(n % Z), j = (int)((n / Z) % Y), i = (int)(n / ((long long)Z * Y));
+  if (n >= (long long)Xl * Y * Z) return;
+  const int k = (int)(n % Z), j = (int)((n / Z) % Y), il = (int)(n / ((long long)Z * Y));
+  const int i = xw0 + il;
+  const long long nf = n + (long long)xw0 * Y * Z;                         // full-grid voxel index
   const float px = i + 0.5f, py = j + 0.5f, pz = k + 0.5f;
   float fsum = 0.f, msum = 0.f;
   for (int v = 0; v < V; ++v) {
     float nx, ny, nz;
     if constexpr (GIVEN) {
-      const float* g = grids + ((long long)v * N + n) * 3;
+      const float* g = grids + ((long long)v * N + nf) * 3;
       nx = g[0]; ny = g[1]; nz = g[2];
     } else {
     const FrustumCam& c = cams[v];
@@ -94,7 +99,7 @@ __global__ void frustum_sample_kernel(const float* __restrict__ depth, const Fru
   float r = fsum;
   if (V > 1 && mean_mode && msum > 0.f) r = fsum / msum;
   long long no = n;
-  if (perm_xzy) no = ((long long)i * Z + k) * Y + j;  // x3ds_depth.permute(0,1,2,4,3) (OccDepth.py:337)
+  if (perm_xzy) no = ((long long)il * Z + k) * Y + j;  // x3ds_depth.permute(0,1,2,4,3) (OccDepth.py:337)
   out[no] = r;
 }
 
@@ -147,29 +152,64 @@ __global__ void channel_scale_kernel(T* __restrict__ x, const float* __restrict_
 
 }  // namespace
 
+namespace {
+int frustum_window(const float* depth, const float* cams, const float* grids, int V, int Dn, int h, int w, int X,
+                   int Y, int Z, int xw0, int Xl, float img_w, float img_h, float dmin, float dmax, int mean_mode,
+                   float* out, int perm_xzy, void* stream) {
+  const long long N = (long long)Xl * Y * Z;
+  OCCD_CHECK_ARG((N + 255) / 256 <= 2147483647LL, "frustum sampling: too many voxels");
+  if (grids) {
+    frustum_sample_kernel<true><<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        depth, nullptr, grids, V, Dn, h, w, X, Y, Z, xw0, Xl, 0.f, 0.f, 0.f, 1.f, mean_mode, out, perm_xzy);
+  } else {
+    const float bin_size = 2.f * (dmax - dmin) / ((float)Dn * (1.f + (float)Dn));
+    frustum_sample_kernel<false><<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        depth, reinterpret_cast<const FrustumCam*>(cams), nullptr, V, Dn, h, w, X, Y, Z, xw0, Xl, img_w, img_h, dmin,
+        bin_size, mean_mode, out, perm_xzy);
+  }
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+}  // namespace
+
 extern "C" int occd_frustum_sample_fwd(const float* depth, const float* cams, int V, int Dn, int h, int w, int X, int Y,
                                        int Z, float img_w, float img_h, float dmin, float dmax, int mean_mode,
                                        float* out, int perm_xzy, void* stream) {
   OCCD_CHECK_ARG(depth && cams && out && V >= 1 && Dn > 1 && h > 0 && w > 0 && X > 0 && Y > 0 && Z > 0,
                  "occd_frustum_sample_fwd: args");
-  const float bin_size = 2.f * (dmax - dmin) / ((float)Dn * (1.f + (float)Dn));
-  const long long N = (long long)X * Y * Z;
-  frustum_sample_kernel<false><<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      depth, reinterpret_cast<const FrustumCam*>(cams), nullptr, V, Dn, h, w, X, Y, Z, img_w, img_h, dmin, bin_size,
-      mean_mode, out, perm_xzy);
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
+  return frustum_window(depth, cams, nullptr, V, Dn, h, w, X, Y, Z, 0, X, img_w, img_h, dmin, dmax, mean_mode, out,
+                        perm_xzy, stream);
+}
+
+extern "C" int occd_frustum_sample_window_fwd(const float* depth, const float* cams, int V, int Dn, int h, int w,
+                                              int X, int Y, int Z, int x0, int Xl, float img_w, float img_h,
+                                              float dmin, float dmax, int mean_mode, float* out, int perm_xzy,
+                                              void* stream) {
+  OCCD_CHECK_ARG(depth && cams && out && V >= 1 && Dn > 1 && h > 0 && w > 0 && X > 0 && Y > 0 && Z > 0,
+                 "occd_frustum_sample_window_fwd: args");
+  OCCD_CHECK_ARG(Xl > 0 && x0 >= 0 && x0 <= X - Xl, "occd_frustum_sample_window_fwd: the window [x0, x0 + Xl) must "
+                 "hold at least one plane and lie inside the X planes of the grid");
+  return frustum_window(depth, cams, nullptr, V, Dn, h, w, X, Y, Z, x0, Xl, img_w, img_h, dmin, dmax, mean_mode, out,
+                        perm_xzy, stream);
 }
 
 extern "C" int occd_grid_sample_prior_fwd(const float* depth, const float* grids, int V, int Dn, int h, int w, int X,
                                           int Y, int Z, int mean_mode, float* out, int perm_xzy, void* stream) {
   OCCD_CHECK_ARG(depth && grids && out && V >= 1 && Dn > 1 && h > 0 && w > 0 && X > 0 && Y > 0 && Z > 0,
                  "occd_grid_sample_prior_fwd: args");
-  const long long N = (long long)X * Y * Z;
-  frustum_sample_kernel<true><<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      depth, nullptr, grids, V, Dn, h, w, X, Y, Z, 0.f, 0.f, 0.f, 1.f, mean_mode, out, perm_xzy);
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
+  return frustum_window(depth, nullptr, grids, V, Dn, h, w, X, Y, Z, 0, X, 0.f, 0.f, 0.f, 0.f, mean_mode, out,
+                        perm_xzy, stream);
+}
+
+extern "C" int occd_grid_sample_prior_window_fwd(const float* depth, const float* grids, int V, int Dn, int h, int w,
+                                                 int X, int Y, int Z, int x0, int Xl, int mean_mode, float* out,
+                                                 int perm_xzy, void* stream) {
+  OCCD_CHECK_ARG(depth && grids && out && V >= 1 && Dn > 1 && h > 0 && w > 0 && X > 0 && Y > 0 && Z > 0,
+                 "occd_grid_sample_prior_window_fwd: args");
+  OCCD_CHECK_ARG(Xl > 0 && x0 >= 0 && x0 <= X - Xl, "occd_grid_sample_prior_window_fwd: the window [x0, x0 + Xl) "
+                 "must hold at least one plane and lie inside the X planes of the grid");
+  return frustum_window(depth, nullptr, grids, V, Dn, h, w, X, Y, Z, x0, Xl, 0.f, 0.f, 0.f, 0.f, mean_mode, out,
+                        perm_xzy, stream);
 }
 
 extern "C" int occd_softmax_planar(const float* in, float* out, long long B, int C, long long S, void* stream) {

@@ -429,9 +429,11 @@ class Plan:
             return
         left = max(0, -min(t[1] for t in taps))
         right = max(0, (out_d - 1) * stride0 + max(t[1] for t in taps) - (src.dlen - 1))
-        if left == 0 and right == 0:
+        # every rank must insert the same exchanges: a slab that ends on a multiple of the stride reaches
+        # max tap - stride + 1 planes to the right, even where this rank's own slab (the last one) does not
+        if left == 0 and right == 0 and max(t[1] for t in taps) - stride0 + 1 <= 0:
             return
-        if max(left, right) > src.halo or max(left, right) > src.dlen:
+        if max(left, right) > src.halo or max(left, right) > src.dlen or src.dlen < src.halo:
             raise RuntimeError("slab partition: a convolution reaches %d planes across the slab boundary but the slab "
                                "is %d planes thick (halo margin %d): use fewer ranks" % (max(left, right), src.dlen,
                                                                                        src.halo))
@@ -457,6 +459,11 @@ class Plan:
         assert ci == x.C, (ci, x.C, name)
         od = (out_size(ID, kd, s[0], p[0], d[0]), out_size(IH, kh, s[1], p[1], d[1]),
               out_size(IW, kw, s[2], p[2], d[2]))
+        if self.slab is not None and x.halo and s[0] > 1 and self.slab.rank < self.slab.world - 1:
+            # a slab other than the last ends on a multiple of the stride (parallel.slab_bounds): it owns the outputs
+            # anchored on its own planes, whatever the padding; the last slab ends where the grid does
+            assert ID % s[0] == 0, (ID, s[0], name)
+            od = (ID // s[0],) + od[1:]
         if out is None and not no_out0:
             out = self.alloc(B, od[0], od[1], od[2], co)
         taps, ws = conv_taps(weight, d, p)

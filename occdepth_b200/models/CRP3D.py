@@ -8,7 +8,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..engine import ConvOp, FnOp, fold_bn, kpad_for, _round_up
+from ..engine import CL, ConvOp, FnOp, fold_bn, kpad_for, out_size, _round_up
 from ._base import B200Module
 from .modules import ASPP, Process
 
@@ -42,29 +42,53 @@ class CPMegaVoxels(B200Module):
         N, M, R = self.flatten_size, self.flatten_context_size, self.n_relations
         F1, F2 = self.feature, self.context_feature
         slab = plan.slab
+        conv = self.mega_context[0]
+        shards = None
         if slab is None:
             assert D * H * W == N
-        else:   # X-slab partition: this rank holds N / world voxels; the mega-context is all-gathered
-            assert B == 1 and D * H * W * slab.world == N
+        else:   # X-slab partition: this rank holds D of the X planes; the mega-context is all-gathered
+            # each rank's X planes here and its mega-context planes (the stride-2 outputs anchored on its planes)
+            lb = slab.level_bounds(self.size[0]) or [(r * D, (r + 1) * D) for r in range(slab.world)]
+            n_out = out_size(self.size[0], 3, 2, conv.padding[0], 1)
+            shards = [(n_out if r == slab.world - 1 else hi // 2) - lo // 2 for r, (lo, hi) in enumerate(lb)]
+            assert B == 1 and sum(hi - lo for lo, hi in lb) * H * W == N and lb[slab.rank][1] - lb[slab.rank][0] == D
             N = D * H * W
         x_agg = self.aspp.emit(plan, x)
-        conv = self.mega_context[0]
         w, b = fold_bn(conv.weight, conv.bias, None)
-        ctx = plan.conv(x_agg, w, b, stride=2, padding=conv.padding, name="crp.mega_context")   # [B, M pos, F2]
-        if slab is not None:
-            from ..engine import CL
-            _, cd, ch, cw = ctx.dims
-            full = CL.alloc(1, cd * slab.world, ch, cw, F2, plan.device, precision=plan.precision)
-            plan.add(slab.all_gather_op(ctx.interior(), full.buf))
-            ctx = full
-        assert ctx.spatial() == M
-        # mega-context as the K-major B operand of the bmm: wbuf[b][f][m] = ctx[b][m][f]
-        Kp = plan.kpad_for(M)
         F2p = _round_up(F2, 16)
+        Kp = plan.kpad_for(M)
         wbuf = torch.zeros(B, 1, F2p, Kp, dtype=plan.dtype, device=plan.device)
-        plan.add(FnOp(lambda st: L.occd_cl_transpose(ctx.ptr, wbuf.data_ptr(), plan.lib_dtype, B, M, F2, ctx.cstride,
-                                                     ctx.coff, Kp, F2p * Kp, st), "occd_cl_transpose",
-                      keep=(ctx, wbuf)))
+        if shards is not None and min(shards) != max(shards):
+            # uneven shards: every rank gathers max(shards) planes (its own, zero-padded), and the bmm operand is
+            # transposed shard by shard, so the padding never reaches it
+            cd = max(shards)
+            ch, cw = (out_size(e, 3, 2, p, 1) for e, p in zip((H, W), conv.padding[1:]))
+            own = CL.alloc(1, cd, ch, cw, F2, plan.device, precision=plan.precision)
+            ctx = plan.conv(x_agg, w, b, stride=2, padding=conv.padding, name="crp.mega_context",
+                            out=CL(own.buf[:, :shards[slab.rank]], F2))
+            full = CL.alloc(1, cd * slab.world, ch, cw, F2, plan.device, precision=plan.precision)
+            plan.add(slab.all_gather_op(own.buf, full.buf))
+            m0, plane = 0, ch * cw
+            for r, n_r in enumerate(shards):
+                src = full.ptr + full.esize * r * cd * full.plane_elems
+                dst = wbuf.data_ptr() + wbuf.element_size() * m0
+                plan.add(FnOp(lambda st, src=src, dst=dst, P=n_r * plane: L.occd_cl_transpose(
+                    src, dst, plan.lib_dtype, B, P, F2, full.cstride, 0, Kp, F2p * Kp, st), "occd_cl_transpose",
+                    keep=(full, wbuf)))
+                m0 += n_r * plane
+            assert m0 == M
+        else:
+            ctx = plan.conv(x_agg, w, b, stride=2, padding=conv.padding, name="crp.mega_context")   # [B, M pos, F2]
+            if slab is not None:
+                _, cd, ch, cw = ctx.dims
+                full = CL.alloc(1, cd * slab.world, ch, cw, F2, plan.device, precision=plan.precision)
+                plan.add(slab.all_gather_op(ctx.interior(), full.buf))
+                ctx = full
+            assert ctx.spatial() == M
+            # mega-context as the K-major B operand of the bmm: wbuf[b][f][m] = ctx[b][m][f]
+            plan.add(FnOp(lambda st: L.occd_cl_transpose(ctx.ptr, wbuf.data_ptr(), plan.lib_dtype, B, M, F2,
+                                                         ctx.cstride, ctx.coff, Kp, F2p * Kp, st), "occd_cl_transpose",
+                          keep=(ctx, wbuf)))
         P_logits = torch.empty(B, R, M, N, dtype=torch.float32, device=plan.device)
         p_view = P_logits.view(B, R * M, D, H, W)
         cat = plan.alloc(B, D, H, W, F1 + R * F2)

@@ -125,13 +125,21 @@ class OccDepth(_Base, B200Module):
         ps = self.project_scale
         S = [int(s) // ps for s in self.full_scene_size]
         n_lo = 0
+        window = None
         if slab is not None:
             # one frame, X-slab partition: this rank lifts and decodes planes [x_lo, x_hi) of the voxel grid; the
-            # 2D network is replicated (its receptive field is global: SE pooling) -- SURVEY.md section 8e
-            if B != 1 or self.dataset != "kitti":
-                raise NotImplementedError("slab partition: batch size 1, KITTI voxel order (X-major) only")
-            x_lo, x_hi = slab.slab(S[0])
+            # 2D network is replicated (its receptive field is global: SE pooling) -- SURVEY.md section 8e.  Both
+            # datasets' voxel orders are X-major, so the slab is one contiguous range of projected_pix / fov_mask.
+            if B != 1:
+                raise NotImplementedError("slab partition: one frame per forward (batch size 1), got %d" % B)
+            if self.dataset == "NYU" and self.trans_2d_to_3d == "flosp_depth":
+                raise NotImplementedError("slab partition: NYU with the FlospDepth prior is not built (no shipped "
+                                          "configuration uses it)")
+            # boundaries on multiples of 2^stages: the UNet's two Downsamples, plus the CRP mega-context conv
+            stages = 2 + (1 if self.net_3d_decoder.context_prior else 0)
+            x_lo, x_hi = slab.partition(S[0], stages)
             n_lo, N = x_lo * S[1] * S[2], (x_hi - x_lo) * S[1] * S[2]
+            window = (x_lo, x_hi - x_lo)
             S = [x_hi - x_lo, S[1], S[2]]
         virtual = V == 1 and "gt_depth" in batch                          # process_rgbs, OccDepth.py:221-229
         VL = 2 if virtual else V                                           # views seen by the lift
@@ -199,7 +207,21 @@ class OccDepth(_Base, B200Module):
         prior = None
         if self.trans_2d_to_3d == "flosp_depth":
             n_cams = 1 if self.dataset == "NYU" else V                      # OccDepth.py:303-305
-            prior = self.flosp_depth.emit(plan, x_rgb, batch, B, V, n_cams)  # fp32 [B, X*Y*Z]
+            x_depth = x_rgb
+            if view_shard:
+                # DepthNet runs whole on every rank, over both views' 1_8 maps: after the all-gather they are views
+                # of `gathered` with a view stride of P_pad * Cp; one copy per view makes them a dense [2,1,h,w,Cp]
+                L = _lib.lib()
+                g8 = views[8]
+                _, _, h8, w8, _ = g8.shape
+                dense = plan.alloc(2, 1, h8, w8, Cf)
+                for v in range(2):
+                    plan.add(FnOp(lambda st, v=v: L.occd_copy_channels(
+                        g8[v].data_ptr(), dense.buf[v].data_ptr(), plan.lib_dtype, h8 * w8, Cp, Cp, 0, Cp, 0, st),
+                        "depthnet.gather_views", keep=(gathered, dense)))
+                x_depth = {"1_8": dense}
+            prior = self.flosp_depth.emit(plan, x_depth, batch, B, V, n_cams, window=window)  # fp32 [B, X*Y*Z]
+            plan.flosp_state = self.flosp_depth.plan_state()
         for b in range(B):
             feats = []
             for s in scales:
@@ -217,8 +239,6 @@ class OccDepth(_Base, B200Module):
                                            prior=pr, scale_const=100.0, stream=st), 0)[1],
                           "sfa_lift", keep=(feats, pix, fov, out_b)))
         out = self.net_3d_decoder.emit(plan, x3d)
-        if slab is not None and self.trans_2d_to_3d == "flosp_depth":
-            raise NotImplementedError("slab partition with the FlospDepth prior is not built")
         if os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
             try:
                 plan.capture()
@@ -269,7 +289,14 @@ class OccDepth(_Base, B200Module):
             self._plans()[key] = ent
         if self.__dict__.get("_build_only"):
             return None
+        self._stage(ent, batch, img, pp, fm, dev)
+        ent[0].run()
+        return self._outputs(ent)
+
+    def _stage(self, ent, batch, img, pp, fm, dev):
+        """copy this batch's inputs into the static input buffers of plan entry `ent`"""
         plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
+        B, V, _, H, W = img.shape
         CL.from_planar(img.reshape(B * V, 3, H, W) if view_sel is None else img[:, view_sel].reshape(B, 3, H, W),
                        out=img_cl)
         if depth0 is not None:
@@ -279,13 +306,17 @@ class OccDepth(_Base, B200Module):
             pix[b].copy_(pp[b][:, n_lo:n_lo + nl], non_blocking=True)
             fov[b].copy_(fm[b][:, n_lo:n_lo + nl], non_blocking=True)
         if self.trans_2d_to_3d == "flosp_depth":
-            self.flosp_depth.stage_inputs(batch, dev)
-        plan.run()
+            self.flosp_depth.stage_inputs(batch, dev, plan.flosp_state)
+
+    def _outputs(self, ent):
+        """the forward's output dict from plan entry `ent` after it ran (under the slab partition: this rank's
+        X-slab of every 3-D tensor, its columns of P_logits, and the whole depth_pred)"""
+        plan, out = ent[0], ent[4]
         res = _to_planar(out, False)
         # tensors written directly by kernels live in plan-owned static buffers: hand out copies
         res = {k: (v.clone() if isinstance(out[k], torch.Tensor) else v) for k, v in res.items()}
         if self.with_depth_gt and self.trans_2d_to_3d == "flosp_depth":
-            res["depth_pred"] = self.flosp_depth.depth_prob().clone()          # OccDepth.py:374-375
+            res["depth_pred"] = self.flosp_depth.depth_prob(plan.flosp_state).clone()   # OccDepth.py:374-375
         return res
 
     @staticmethod

@@ -140,8 +140,11 @@ class FlospDepth(B200Module):
                 cams[b, v, 24:] = A[v].reshape(-1)
         return cams, sps, vn
 
-    def emit(self, plan, x_rgb, batch, B, V, n_cams=None):
-        """x_rgb: {"1_s": CL [B*V,1,h,w,C]} -> prior fp32 [B, X*Y*Z] (voxel order of the lift output)."""
+    def emit(self, plan, x_rgb, batch, B, V, n_cams=None, window=None):
+        """x_rgb: {"1_s": CL [B*V,1,h,w,C]} -> prior fp32 [B, X*Y*Z] (voxel order of the lift output).
+        window (x0, Xl): only the planes [x0, x0 + Xl) of the X axis, as [B, Xl*Y*Z] (the X-slab partition: DepthNet
+        runs whole on every rank, the frustum sampling on this rank's slab).  The plan's input buffers are kept in
+        self.plan_state() until the next emit."""
         L = _lib.lib()
         dev = plan.device
         n_cams = V if n_cams is None else n_cams
@@ -154,7 +157,6 @@ class FlospDepth(B200Module):
         wr, br = fold_bn(dn.reduce_conv[0].weight, dn.reduce_conv[0].bias, dn.reduce_conv[1])
         x = plan.conv(feat, wr.unsqueeze(2), br, padding=(0, 1, 1), act="relu", name="depthnet.reduce")
         sps = torch.zeros(BV, 1, dtype=torch.float32, device=dev)
-        self.__dict__["_sps"] = sps
 
         def fc(inp, lin_w, lin_b, n_in, n_out, act, nm):
             wt = lin_w.detach().float().reshape(n_out, n_in).contiguous()
@@ -187,53 +189,67 @@ class FlospDepth(B200Module):
         vox_origin = batch.get("vox_origin") if isinstance(batch, dict) else None
         _, vn = self._grid_to_lidar(vox_origin if vox_origin is not None else None)
         X, Y, Z = vn
-        self.__dict__["_vn"] = tuple(vn)         # baked into the plan's buffers; stage_inputs checks every batch
+        x0, Xl = window if window is not None else (0, X)
+        if not (Xl > 0 and 0 <= x0 <= X - Xl):
+            raise ValueError("FlospDepth: window [%d, %d) is outside the %d X planes of the grid" % (x0, x0 + Xl, X))
         cams = torch.zeros(B, n_cams, 40, dtype=torch.float32, device=dev)
-        self.__dict__["_cams"] = cams
-        self.__dict__["_n_cams"] = n_cams
-        prior = torch.empty(B, X * Y * Z, dtype=torch.float32, device=dev)
+        # vn is baked into the plan's buffers; stage_inputs checks every batch against it
+        state = {"sps": sps, "vn": tuple(vn), "cams": cams, "n_cams": n_cams, "window": (x0, Xl),
+                 "prob": prob.view(B, V, Dn, h, w)}
+        self.__dict__["_state"] = state
+        prior = torch.empty(B, Xl * Y * Z, dtype=torch.float32, device=dev)
         perm = 1 if vox_origin is not None else 0      # NYU: x3ds_depth.permute(0,1,2,4,3), OccDepth.py:335-337
         H_img, W_img = self.final_dim
         mean_mode = 1 if self.agg_voxel_mode == "mean" else 0
         if self.infer_mode:
             # the caller supplies batch["grids"] (one (B, X, Y, Z, 3) grid per camera) and batch["scaled_pixel_size"]
             # (flosp_depth.py:564-565, OccDepth.py:310-317): staged into these static buffers before every replay
+            # (only the window's rows are staged and read)
             grids = torch.zeros(B, n_cams, X * Y * Z, 3, dtype=torch.float32, device=dev)
-            self.__dict__["_grids"] = grids
+            state["grids"] = grids
             for b in range(B):
                 pb = prob[b * V:b * V + n_cams]
-                plan.add(FnOp(lambda st, pb=pb, gb=grids[b], ob=prior[b]: L.occd_grid_sample_prior_fwd(
-                    pb.data_ptr(), gb.data_ptr(), n_cams, Dn, h, w, X, Y, Z, mean_mode, ob.data_ptr(), perm, st),
-                    "grid_sample_prior", keep=(prob, grids, prior)))
+                plan.add(FnOp(lambda st, pb=pb, gb=grids[b], ob=prior[b]: L.occd_grid_sample_prior_window_fwd(
+                    pb.data_ptr(), gb.data_ptr(), n_cams, Dn, h, w, X, Y, Z, x0, Xl, mean_mode, ob.data_ptr(), perm,
+                    st), "grid_sample_prior", keep=(prob, grids, prior)))
         for b in range(B if not self.infer_mode else 0):
             pb = prob[b * V:b * V + n_cams]
-            plan.add(FnOp(lambda st, pb=pb, cb=cams[b], ob=prior[b]: L.occd_frustum_sample_fwd(
-                pb.data_ptr(), cb.data_ptr(), n_cams, Dn, h, w, X, Y, Z, float(W_img), float(H_img),
+            plan.add(FnOp(lambda st, pb=pb, cb=cams[b], ob=prior[b]: L.occd_frustum_sample_window_fwd(
+                pb.data_ptr(), cb.data_ptr(), n_cams, Dn, h, w, X, Y, Z, x0, Xl, float(W_img), float(H_img),
                 float(self.d_bound[0]), float(self.d_bound[1]), mean_mode,
                 ob.data_ptr(), perm, st), "frustum_sample", keep=(prob, cams, prior)))
-        self.__dict__["_prob"] = prob.view(B, V, Dn, h, w)
         return prior
 
-    def stage_inputs(self, batch, dev):
+    def plan_state(self):
+        """input buffers and depth distribution of the plan the last emit() built"""
+        return self.__dict__["_state"]
+
+    def stage_inputs(self, batch, dev, state=None):
+        """copy this batch's camera tables (or infer_mode grids) into the buffers of `state` (default: the plan the
+        last emit() built)"""
+        state = self.plan_state() if state is None else state
         if self.infer_mode:
-            g = self.__dict__["_grids"]
+            g = state["grids"]
             B, n_cams = g.shape[:2]
+            x0, Xl = state["window"]
             grids = batch["grids"]
             for v in range(n_cams):
-                g[:, v].copy_(grids[v].to(torch.float32).reshape(B, -1, 3), non_blocking=True)
-            self.__dict__["_sps"].copy_(batch["scaled_pixel_size"].to(torch.float32).reshape(-1, 1), non_blocking=True)
+                gv = grids[v].to(torch.float32).reshape(B, -1, 3)
+                plane = gv.shape[1] // state["vn"][0]
+                g[:, v, x0 * plane:(x0 + Xl) * plane].copy_(gv[:, x0 * plane:(x0 + Xl) * plane], non_blocking=True)
+            state["sps"].copy_(batch["scaled_pixel_size"].to(torch.float32).reshape(-1, 1), non_blocking=True)
             return
         cams, sps, vn = self.camera_tables(batch["cam_k"], batch["T_velo_2_cam"], batch["ida_mats"],
-                                           batch.get("vox_origin"), self.__dict__["_n_cams"])
-        if tuple(vn) != self.__dict__.get("_vn", tuple(vn)):
+                                           batch.get("vox_origin"), state["n_cams"])
+        if tuple(vn) != state["vn"]:
             # NYU: the voxel counts are re-derived from batch item 0's vox_origin every forward (flosp_depth.py:466-518)
             raise RuntimeError("FlospDepth: this batch's vox_origin gives a %r voxel grid, the plan was built for %r; "
-                               "call invalidate_plans()" % (tuple(vn), self.__dict__["_vn"]))
-        self.__dict__["_cams"].copy_(cams, non_blocking=True)
-        self.__dict__["_sps"].copy_(sps, non_blocking=True)
+                               "call invalidate_plans()" % (tuple(vn), state["vn"]))
+        state["cams"].copy_(cams, non_blocking=True)
+        state["sps"].copy_(sps, non_blocking=True)
 
-    def depth_prob(self):
-        return self.__dict__["_prob"]
+    def depth_prob(self, state=None):
+        return (self.plan_state() if state is None else state)["prob"]
 
     def forward(self, img_feat, cam_k=None, T_velo_2_cam=None, ida_mats=None, vox_origin=None, grids=None,
                 scaled_pixel_size=None):
@@ -256,16 +272,17 @@ class FlospDepth(B200Module):
             xin = plan.alloc(B * V, 1, h, w, C_)
             with torch.no_grad():
                 prior = self.emit(plan, {"1_%d" % self.downsample_factor: xin}, batch, B, V)
+            plan.flosp_state = self.plan_state()
             ent = (plan, xin, prior)
             self._plans()[key] = ent
         plan, xin, prior = ent
         CL.from_planar(img_feat.reshape(B * V, C_, h, w), out=xin)
-        self.stage_inputs(batch, img_feat.device)
+        self.stage_inputs(batch, img_feat.device, plan.flosp_state)
         plan.run()
         _, vn = self._grid_to_lidar(vox_origin)
         X, Y, Z = vn
         out = prior.clone().view(B, 1, X, Z, Y).permute(0, 1, 2, 4, 3) if vox_origin is not None \
             else prior.clone().view(B, 1, X, Y, Z)
         if self.return_depth:
-            return out, self.depth_prob().clone()
+            return out, self.depth_prob(plan.flosp_state).clone()
         return out

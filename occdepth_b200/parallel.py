@@ -65,8 +65,55 @@ def gather_counts(count, device=None):
 # camera-depth axis; SURVEY.md section 8e explains why not the literal Z), every 3-D activation carries `halo`
 # margin planes, and the only data-path communication is the neighbour exchange of those planes before a
 # convolution whose taps reach across the slab boundary, plus one all-gather of the CRP mega-context.
+def slab_bounds(n, world, stages=0, halo=0, levels=1):
+    """X-slab partition of an extent-n axis that a network halves `stages` times: planes [lo, hi) per rank.
+
+    Boundaries are multiples of A = 2**stages, so every rank's slab halves exactly at each stride-2 stage.  Whole
+    units of A planes are dealt out as evenly as possible (the first ranks take one more), and a final partial unit
+    goes to the last rank.  Every rank must hold at least `halo` planes at each of the first `levels` levels (level k
+    has ceil(planes / 2**k) planes), where convolutions reach across the slab boundary.  Where the extent divides
+    into world * A planes this is the even split.  Raises SlabPartitionError naming the largest world size that
+    works when a rule cannot hold."""
+    bounds = _deal(n, world, 1 << stages, halo, levels)
+    if bounds is None:
+        ok = [r for r in range(world - 1, 0, -1) if _deal(n, r, 1 << stages, halo, levels) is not None]
+        raise SlabPartitionError(
+            "slab partition: %d X planes in units of %d (%d stride-2 stages) cannot give each of %d ranks at least %d "
+            "planes at every exchanging level; the largest world size that works for this grid is %d"
+            % (n, 1 << stages, stages, world, halo, ok[0] if ok else 1))
+    return bounds
+
+
+class SlabPartitionError(NotImplementedError):
+    pass
+
+
+def _deal(n, world, unit, halo, levels):
+    full, part = divmod(n, unit)
+    base, extra = divmod(full, world)
+    bounds, lo = [], 0
+    for r in range(world):
+        hi = lo + (base + (1 if r < extra else 0)) * unit + (part if r == world - 1 else 0)
+        bounds.append((lo, hi))
+        lo = hi
+    if world > 1:
+        for k in range(levels):
+            if min(level_planes(lo, hi, k) for lo, hi in bounds) < max(halo, 1):
+                return None
+    if min(hi - lo for lo, hi in bounds) < 1:
+        return None
+    return bounds
+
+
+def level_planes(lo, hi, k):
+    """planes of the slab [lo, hi) after k stride-2 stages"""
+    return -(-hi // (1 << k)) - (lo >> k)
+
+
 class HaloExchangeOp:
-    """Plan op: fill the margins of a halo-carrying activation from the two X-neighbours (send/recv pairs)."""
+    """Plan op: fill the margins of a halo-carrying activation from the two X-neighbours (send/recv pairs).
+    Neighbours may hold different numbers of planes: each side moves min(halo, planes) planes, and the plan only
+    exchanges activations every rank holds at least `halo` planes of (Plan.need_halo), so both ends agree."""
 
     def __init__(self, ctx, cl):
         self.ctx, self.name, self.flops = ctx, "halo_exchange", 0
@@ -91,7 +138,8 @@ class HaloExchangeOp:
 
 
 class AllGatherOp:
-    """Plan op: dst (full, contiguous) = concat over ranks of src (this rank's contiguous shard)."""
+    """Plan op: dst (full, contiguous) = concat over ranks of src (this rank's contiguous shard).  Shards are equal in
+    size; a caller with uneven shards pads each to the largest (CPMegaVoxels.emit)."""
 
     def __init__(self, ctx, src, dst):
         self.ctx, self.src, self.dst, self.name, self.flops = ctx, src, dst, "all_gather", 0
@@ -107,6 +155,7 @@ class SlabContext:
         self.world = w if world is None else world
         self.halo = halo
         self.n_exchanges = 0
+        self.bounds = None          # [(lo, hi)] per rank at the lift grid, once partition() has run
 
     def exchange_op(self, cl):
         self.n_exchanges += 1
@@ -121,6 +170,23 @@ class SlabContext:
             raise RuntimeError("slab partition: extent %d is not divisible by %d ranks" % (n, self.world))
         per = n // self.world
         return self.rank * per, (self.rank + 1) * per
+
+    def partition(self, n, stages, levels=3):
+        """planes [lo, hi) of the extent-n lift grid owned by this rank under slab_bounds (the 3-D UNets halve X
+        `stages` times and exchange halo planes at their first `levels` levels); every rank's bounds are kept for
+        the layers that need them (the CRP all-gather)"""
+        self.bounds = slab_bounds(n, self.world, stages, self.halo, levels)
+        return self.bounds[self.rank]
+
+    def level_bounds(self, extent):
+        """every rank's [lo, hi) at the level whose global X extent is `extent`, or None before partition()"""
+        if self.bounds is None:
+            return None
+        n = self.bounds[-1][1]
+        for k in range(8):
+            if -(-n // (1 << k)) == extent:
+                return [(lo >> k, -(-hi // (1 << k))) for lo, hi in self.bounds]
+        raise RuntimeError("slab partition: no level of the %d-plane grid has %d planes" % (n, extent))
 
 
 # --------------------------------------------------------------------------------------------------

@@ -57,10 +57,11 @@ CONFIGS = {
 }
 
 
-def make_case(name=None, spec=None, img_hw=None, full=None, seed=0):
+def make_case(name=None, spec=None, img_hw=None, full=None, seed=0, infer_mode=False):
     """-> (model (CPU, eval), batch (CPU tensors), oracle cfg) for CONFIGS[name] (or an explicit spec) at the shipped
     shapes, or at img_hw / full when given.  KITTI views use KITTI-like calibrations; NYU takes one image and a depth
-    map (virtual stereo) with seeded random projection indices."""
+    map (virtual stereo) with seeded random projection indices.  infer_mode builds the model for the reference's
+    deployment route (OccDepth(infer_mode=True)); the batch then still carries camera matrices, not grids."""
     import torch
     import synthetic as synth
     from occdepth_b200.models.OccDepth import OccDepth
@@ -85,7 +86,8 @@ def make_case(name=None, spec=None, img_hw=None, full=None, seed=0):
                                                    z_bound=[-2, -2 + sm[2], 0.2])
         torch.manual_seed(seed)
         with contextlib.redirect_stdout(io.StringIO()):
-            m = OccDepth(["c"] * ncls, torch.ones(ncls), full_scene_size=full, project_res=PROJECT_RES, config=cfg)
+            m = OccDepth(["c"] * ncls, torch.ones(ncls), full_scene_size=full, project_res=PROJECT_RES, config=cfg,
+                         infer_mode=infer_mode)
         conf = copy.deepcopy(getattr(m, "flosp_depth_conf", None))
     finally:
         fd.flosp_depth_conf_map[ds].clear()
