@@ -268,6 +268,13 @@ int occd_scale_weights(const float* master, const float* gate, void* out, int wd
 /* F.interpolate(mode="bilinear", align_corners=True) of UpSampleBN.forward (unet2d.py:39-44)      */
 int occd_upsample_bilinear_ac(const void* in, void* out, int dtype, int B, int h, int w, int OH, int OW, int C,
                               int cs_in, int in_off, int cs_out, int out_off, void* stream);
+/* UpSampleBN conv1 with the resize behind the 3x3 taps. y: [B][h][w][cs_y], tap t = (dy+1)*3+(dx+1) */
+/* of the coarse per-tap products at channels y_off + t*tap_stride + [0, C).  For every fine pixel p: */
+/* out[b][p][c] = act(pre[b][p][c] + sum_t [p+t inside OH x OW] bilinear_ac(Y_t)(p+t)[c]), fp32 sums;  */
+/* pre may be NULL or equal to out (in place); act is an OCCD_ACT_* code                            */
+int occd_upsample_tapsum_ac(const void* y, const void* pre, void* out, int dtype, int B, int h, int w, int OH,
+                            int OW, int C, int cs_y, int y_off, int tap_stride, int cs_pre, int pre_off, int cs_out,
+                            int out_off, int act, void* stream);
 
 /* -------------------------------------------------------------------------------------------- */
 /* FlospDepth (the "OAD" depth branch, configs with trans_2d_to_3d: "flosp_depth")                */

@@ -125,6 +125,7 @@ SYMBOLS = {
     "occd_channel_scale": (C.c_int, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp]),
     "occd_virtual_view_fwd": (C.c_int, [_vp, _vp, _vp] + [_i] * 9 + [_f, _vp]),
     "occd_upsample_bilinear_ac": (C.c_int, [_vp, _vp] + [_i] * 11 + [_vp]),
+    "occd_upsample_tapsum_ac": (C.c_int, [_vp, _vp, _vp] + [_i] * 15 + [_vp]),
 }
 
 

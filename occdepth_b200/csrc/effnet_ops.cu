@@ -3,10 +3,12 @@
 //   squeeze-excite MLP (reduce FC + SiLU + expand FC + sigmoid)
 //   SE gate folded into the following 1x1 projection's weights (per image)
 //   bilinear resize with align_corners=True (UpSampleBN, unet2d.py:39-44)
+//   the same resize applied to the nine per-tap products of UpSampleBN's conv1, summed on the fine grid
 // replaces geffnet DepthwiseSeparableConv / InvertedResidual internals (conv_dw, bn, act, se) as iterated by
 // Encoder.forward (unet2d.py:188-196) and F.interpolate in UpSampleBN.forward.
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include "common.cuh"
 #include "dwconv_tiled.cuh"
 #include "../../include/occdepth_b200.h"
@@ -233,6 +235,99 @@ __global__ void upsample_bilinear_kernel(const T* __restrict__ in, T* __restrict
   Elem<T>::st8(out + (((long long)b * OH + oy) * OW + ox) * cs_out + out_off + cv * 8, o);
 }
 
+// UpSampleBN conv1 with the resize moved behind the 3x3 taps: bilinear resizing commutes with a channel mix, so the
+// up half of the conv runs as one 1x1 GEMM on the coarse map, Y[b][i][j][t*tap_stride + c] = W_t x[b][i][j] for the
+// nine taps t = (dy+1)*3 + (dx+1), and this kernel resizes and sums them on the fine grid:
+//   out[b][p][c] = act(pre[b][p][c] + sum_t [p+t inside OH x OW] bilinear_ac(Y_t)(p+t)[c])
+// The bilinear weights and the padding mask both factor into rows and columns.  A thread owns one (output column,
+// channel vector) and walks a strip of output rows; per dy it keeps the column-summed partials
+//   H_dy(i) = sum_dx [ox+dx inside] ((1-lx) Y_t[i][x0] + lx Y_t[i][x1])
+// of the two coarse rows its current output row reads.  Consecutive output rows share those rows, so each partial
+// is built once per strip (6 vector loads) instead of costing 36 loads per output vector.
+template <typename T>
+__global__ void __launch_bounds__(256)
+upsample_tapsum_kernel(const T* __restrict__ y, const T* pre, T* out, int h, int w, int OH, int OW, int CV,
+                       int cs_y, int y_off, int tap_stride, int cs_pre, int pre_off, int cs_out, int out_off,
+                       int strip_rows, int n_strips, int act, float sy, float sx) {
+  pdl_wait();
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (unsigned)(OW * CV)) return;
+  const int ox = (int)(i / (unsigned)CV);
+  const int cv = (int)(i - (unsigned)ox * (unsigned)CV);
+  const int b = (int)(blockIdx.y / (unsigned)n_strips);
+  const int oy0 = (int)(blockIdx.y - (unsigned)b * (unsigned)n_strips) * strip_rows;
+  const int oy1 = min(oy0 + strip_rows, OH);
+  // per dx: offsets of the two coarse columns (the fine column ox+dx is resized from) and their weights
+  int xo0[3], xo1[3];
+  float wx0[3], wx1[3];
+  bool xin[3];
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const int fx = ox + d - 1;
+    xin[d] = fx >= 0 && fx < OW;
+    const float f = sx * (float)max(fx, 0);
+    const int x0 = min((int)f, w - 1), x1 = min(x0 + 1, w - 1);
+    wx1[d] = f - (float)x0;
+    wx0[d] = 1.f - wx1[d];
+    xo0[d] = x0 * cs_y;
+    xo1[d] = x1 * cs_y;
+  }
+  const T* yb = y + (long long)b * h * w * cs_y + y_off + cv * 8;
+  // hr[d][k]: H_dy of coarse row row[d] + k (k = 1 clamped to the last row); row[d] = -2: nothing held yet
+  float hr[3][2][8];
+  int row[3] = {-2, -2, -2};
+  auto hsum = [&](int d, int r, float* dst) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) dst[k] = 0.f;
+    const T* yr = yb + r * w * cs_y + 3 * d * tap_stride;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+      if (!xin[e]) continue;
+      float a[8], c[8];
+      Elem<T>::ld8_nc(yr + e * tap_stride + xo0[e], a);
+      Elem<T>::ld8_nc(yr + e * tap_stride + xo1[e], c);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) dst[k] += wx0[e] * a[k] + wx1[e] * c[k];
+    }
+  };
+  const int pix0 = b * OH * OW;   // 32-bit: OCCD_CHECK_ARG bounds B*OH*OW*cs
+#pragma unroll 1
+  for (int oy = oy0; oy < oy1; ++oy) {
+    float acc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const int fy = oy + d - 1;
+      if (fy < 0 || fy >= OH) continue;
+      const float f = sy * (float)fy;
+      const int y0 = min((int)f, h - 1);
+      const float ly = f - (float)y0;
+      if (y0 != row[d]) {
+        if (y0 == row[d] + 1) {
+#pragma unroll
+          for (int k = 0; k < 8; ++k) hr[d][0][k] = hr[d][1][k];
+        } else {
+          hsum(d, y0, hr[d][0]);
+        }
+        hsum(d, min(y0 + 1, h - 1), hr[d][1]);
+        row[d] = y0;
+      }
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += (1.f - ly) * hr[d][0][k] + ly * hr[d][1][k];
+    }
+    const int p = pix0 + oy * OW + ox;
+    if (pre) {
+      float r[8];
+      Elem<T>::ld8(pre + p * cs_pre + pre_off + cv * 8, r);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += r[k];
+    }
+    apply_act8(acc, act);
+    Elem<T>::st8(out + p * cs_out + out_off + cv * 8, acc);
+  }
+}
+
 }  // namespace
 
 template <typename T>
@@ -397,6 +492,39 @@ extern "C" int occd_upsample_bilinear_ac(const void* in, void* out, int dtype, i
                                                     dim3((unsigned)((OW * CV + 255) / 256), (unsigned)(B * OH)),
                                                     dim3(256), 0, (cudaStream_t)stream, (const T*)in, (T*)out, B, h, w,
                                                     OH, OW, CV, cs_in, in_off, cs_out, out_off, sy, sx));
+  return OCCD_OK;
+}
+
+extern "C" int occd_upsample_tapsum_ac(const void* y, const void* pre, void* out, int dtype, int B, int h, int w,
+                                       int OH, int OW, int C, int cs_y, int y_off, int tap_stride, int cs_pre,
+                                       int pre_off, int cs_out, int out_off, int act, void* stream) {
+  OCCD_CHECK_ARG(y && out && B > 0 && h > 0 && w > 0 && OH > 0 && OW > 0 && C > 0, "occd_upsample_tapsum_ac: args");
+  OCCD_CHECK_ARG(act >= ACT_NONE && act <= ACT_SIGMOID, "occd_upsample_tapsum_ac: act");
+  OCCD_CHECK_ARG(cs_y % 8 == 0 && y_off % 8 == 0 && tap_stride % 8 == 0 && cs_out % 8 == 0 && out_off % 8 == 0 &&
+                     (!pre || (cs_pre % 8 == 0 && pre_off % 8 == 0)),
+                 "occd_upsample_tapsum_ac: alignment");
+  const int CV = (C + 7) / 8;
+  OCCD_CHECK_ARG(y_off >= 0 && out_off >= 0 && tap_stride >= CV * 8 &&
+                     (long long)y_off + 8LL * tap_stride + CV * 8 <= cs_y && out_off + CV * 8 <= cs_out &&
+                     (!pre || (pre_off >= 0 && pre_off + CV * 8 <= cs_pre)),
+                 "occd_upsample_tapsum_ac: channel window");
+  OCCD_CHECK_ARG((long long)h * w * cs_y < (1LL << 31) && (long long)B * OH * OW * cs_out < (1LL << 31) &&
+                     (!pre || (long long)B * OH * OW * cs_pre < (1LL << 31)) && (long long)OW * CV < (1LL << 31),
+                 "occd_upsample_tapsum_ac: extent");
+  // strips of output rows: long enough that consecutive rows reuse their coarse-row partials, short enough that
+  // the grid still fills the GPU a few times over (2^19 threads)
+  const long long per_row = (long long)B * OW * CV;
+  int n_strips = (int)std::min<long long>(OH, std::max<long long>(1, ((1LL << 19) + per_row - 1) / per_row));
+  const int strip_rows = (OH + n_strips - 1) / n_strips;
+  n_strips = (OH + strip_rows - 1) / strip_rows;
+  OCCD_CHECK_ARG((long long)B * n_strips <= 65535, "occd_upsample_tapsum_ac: extent");
+  const float sy = OH > 1 ? (float)(h - 1) / (float)(OH - 1) : 0.f;
+  const float sx = OW > 1 ? (float)(w - 1) / (float)(OW - 1) : 0.f;
+  OCCD_DISPATCH_DTYPE(dtype, T, OCCD_LAUNCH_CHECKED(upsample_tapsum_kernel<T>,
+                                                    dim3((unsigned)((OW * CV + 255) / 256), (unsigned)(B * n_strips)),
+                                                    dim3(256), 0, (cudaStream_t)stream, (const T*)y, (const T*)pre,
+                                                    (T*)out, h, w, OH, OW, CV, cs_y, y_off, tap_stride, cs_pre, pre_off,
+                                                    cs_out, out_off, strip_rows, n_strips, act, sy, sx));
   return OCCD_OK;
 }
 

@@ -583,10 +583,11 @@ class Plan:
 
 
 class FnOp:
-    """A prepared non-conv launch: fn(stream) -> rc."""
+    """A prepared non-conv launch: fn(stream) -> rc.  flops: reference-conv 2*MACs the launch stands in for (0 for
+    launches outside the convolution family)."""
 
-    def __init__(self, fn, name, keep=()):
-        self.fn, self.name, self._keep = fn, name, keep
+    def __init__(self, fn, name, keep=(), flops=0):
+        self.fn, self.name, self._keep, self.flops = fn, name, keep, flops
 
     def run(self, stream):
         _lib.check(self.fn(stream), self.name)

@@ -1,8 +1,13 @@
 """Drop-in for the reference `occdepth/models/unet2d.py`: UpSampleBN :24-46, DecoderBN :49-180, Encoder :183-196,
 UNet2D :199-255.
 
-The decoder's `torch.cat([up_x, skip])` is never materialised: each 3x3 conv reads two TMA sources (the
-bilinearly resized map and the encoder skip) into one accumulator.
+The decoder's `torch.cat([up_x, skip])` is never materialised.  Bilinear resizing commutes with a channel mix, so on
+the wide levels (split_pays) UpSampleBN's first 3x3 conv is split by input half: the up half runs as ONE 1x1 GEMM on
+the coarse map producing all nine taps' products (tap-major, pack_tap_weights), occd_upsample_tapsum_ac resizes them
+and sums them on the fine grid (the fine grid's zero padding becomes an in-bounds mask), and the skip half is an
+ordinary 3x3 conv whose pre-activation the tap sum adds to before the LeakyReLU.  That executes about a quarter of the
+up half's reference MACs (DESIGN.md section 4.5).  On the narrow levels the resized map is materialised and the 3x3
+conv reads it and the skip as two TMA sources into one accumulator.
 """
 import os
 
@@ -10,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..engine import CL, ConvOp, FnOp, conv_taps, fold_bn
+from ..engine import ACT, CL, ConvOp, FnOp, conv_taps, fold_bn
 from ._base import B200Module
 from .efficientnet import GenEfficientNet
 
@@ -29,6 +34,29 @@ NUM_FEATURES = {
 }
 
 
+def pack_tap_weights(w_up):
+    """conv1's up-half weights [Cout, C_up, 3, 3] -> the coarse GEMM's [9 * Cp, C_up] matrix in tap-major blocks: row
+    t * Cp + o holds w_up[o, :, dy + 1, dx + 1], t = (dy + 1) * 3 + (dx + 1); Cp = Cout rounded up to 8 (so every
+    tap's channel block starts on a vector), padding rows zero."""
+    co, ci = w_up.shape[:2]
+    cp = (co + 7) // 8 * 8
+    wt = w_up.new_zeros(9, cp, ci)
+    wt[:, :co] = w_up.permute(2, 3, 0, 1).reshape(9, co, ci)
+    return wt.reshape(9 * cp, ci)
+
+
+SPLIT_MIN_COUT = 192
+
+
+def split_pays(co):
+    """Whether UpSampleBN's conv1 runs split (coarse tap GEMM + tap sum + skip conv).  The split saves 3/4 of the up
+    half's MACs but writes and reads the nine per-tap products (about 1.1x the resized map) and a pre-activation map.
+    Every decoder level has C_up = 2 * Cout, so MACs saved per fine pixel grow as Cout^2 and the added bytes as Cout.
+    Measured on the B7 decoder (H100, tf32, DESIGN.md section 7): 1.8x faster at Cout 1280, 1.6x at 640, 1.4x at 320,
+    even at 160, 0.7x at 80."""
+    return co >= SPLIT_MIN_COUT
+
+
 class UpSampleBN(B200Module):
     def __init__(self, skip_input, output_features):
         super(UpSampleBN, self).__init__()
@@ -41,23 +69,51 @@ class UpSampleBN(B200Module):
             nn.LeakyReLU())
 
     def emit(self, plan, x, concat_with, name="up"):
-        L = _lib.lib()
+        """conv1(cat(U(x), skip)) as  act(conv1_skip(skip) + bias + tapsum(Y)),  Y = W_up x on the coarse grid, where
+        that pays (split_pays); else the resize is materialised and conv1 reads it and the skip as two sources."""
         B, _, h, w = x.dims
         _, _, OH, OW = concat_with.dims
-        up = plan.alloc(B, 1, OH, OW, x.C)
-        up_fwd = L.occd_upsample_bilinear_ac
-        plan.add(FnOp(lambda st: up_fwd(x.ptr, up.ptr, plan.lib_dtype, B, h, w, OH, OW, x.C, x.cstride, x.coff,
-                                        up.cstride, up.coff, st),
-                      name + ".bilinear", keep=(x, up)))
         w1, b1 = fold_bn(self._net[0].weight, self._net[0].bias, self._net[1])
         assert w1.shape[1] == x.C + concat_with.C
-        t0, ws0 = conv_taps(w1[:, : x.C].unsqueeze(2), (1, 1, 1), (0, 1, 1), src=0)
-        t1, ws1 = conv_taps(w1[:, x.C:].unsqueeze(2), (1, 1, 1), (0, 1, 1), src=1)
-        y = plan.alloc(B, 1, OH, OW, w1.shape[0])
-        plan.add(ConvOp([up, concat_with], t0 + t1, ws0 + ws1, b1, (1, OH, OW), out0=y, act="leaky",
-                        name=name + ".conv1"))
+        co = w1.shape[0]
+        if split_pays(co):
+            y = self._emit_conv1_split(plan, x, concat_with, w1, b1, name)
+        else:
+            up = plan.alloc(B, 1, OH, OW, x.C)
+            up_fwd = _lib.lib().occd_upsample_bilinear_ac
+            plan.add(FnOp(lambda st: up_fwd(x.ptr, up.ptr, plan.lib_dtype, B, h, w, OH, OW, x.C, x.cstride, x.coff,
+                                            up.cstride, up.coff, st),
+                          name + ".bilinear", keep=(x, up)))
+            t0, ws0 = conv_taps(w1[:, : x.C].unsqueeze(2), (1, 1, 1), (0, 1, 1), src=0)
+            t1, ws1 = conv_taps(w1[:, x.C:].unsqueeze(2), (1, 1, 1), (0, 1, 1), src=1)
+            y = plan.alloc(B, 1, OH, OW, co)
+            plan.add(ConvOp([up, concat_with], t0 + t1, ws0 + ws1, b1, (1, OH, OW), out0=y, act="leaky",
+                            name=name + ".conv1"))
         w2, b2 = fold_bn(self._net[3].weight, self._net[3].bias, self._net[4])
         return plan.conv(y, w2.unsqueeze(2), b2, padding=(0, 1, 1), act="leaky", name=name + ".conv2")
+
+    @staticmethod
+    def _emit_conv1_split(plan, x, concat_with, w1, b1, name):
+        B, _, h, w = x.dims
+        _, _, OH, OW = concat_with.dims
+        co = w1.shape[0]
+        wy = pack_tap_weights(w1[:, : x.C])
+        tap_stride = wy.shape[0] // 9
+        # the up half: nine per-tap 1x1 products in one GEMM on the coarse map, kept unrounded (they only feed a sum)
+        ys = plan.alloc(B, 1, h, w, wy.shape[0])
+        taps = plan.add(ConvOp([x], [(0, 0, 0, 0)], [wy], torch.zeros(wy.shape[0], device=wy.device), (1, h, w),
+                               out0=ys, out0_exact=True, name=name + ".taps"))
+        # the skip half: pre-activation (bias included), exact; the tap sum adds to it, activates and rounds in place
+        t1, ws1 = conv_taps(w1[:, x.C:].unsqueeze(2), (1, 1, 1), (0, 1, 1), src=0)
+        y = plan.alloc(B, 1, OH, OW, co)
+        plan.add(ConvOp([concat_with], t1, ws1, b1, (1, OH, OW), out0=y, out0_exact=True, name=name + ".conv1"))
+        tapsum = _lib.lib().occd_upsample_tapsum_ac
+        # FLOP bookkeeping: the tap sum carries the reference up half's 2*MACs that the coarse GEMM did not execute
+        up_flops = 2 * B * OH * OW * co * 9 * x.C
+        plan.add(FnOp(lambda st: tapsum(ys.ptr, y.ptr, y.ptr, plan.lib_dtype, B, h, w, OH, OW, co, ys.cstride, ys.coff,
+                                        tap_stride, y.cstride, y.coff, y.cstride, y.coff, ACT["leaky"], st),
+                      name + ".tapsum", keep=(ys, y), flops=max(up_flops - taps.flops, 0)))
+        return y
 
     def forward(self, x, concat_with):
         raise RuntimeError("UpSampleBN: use UNet2D.forward (the block has two inputs and is planned as a whole)")
