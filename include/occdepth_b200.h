@@ -118,6 +118,13 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
 #define OCCD_OUT1_CL 1         /* pre-activation copy, channels-last in the plan's dtype            */
 #define OCCD_OUT1_BF16_CL OCCD_OUT1_CL
 #define OCCD_OUT1_F32_PLANAR 2 /* pre-activation copy, fp32 [B][C][positions] (reference layout)   */
+#define OCCD_OUT1_CLASS_U16 3  /* class map, uint16 [B][positions] (positions = ODf*OHf*OWf, the planar mode's      */
+                               /* spatial index): the FIRST index of the largest pre-activation value over the Cout */
+                               /* channels (a NaN in channel 0 wins, later NaNs are skipped), i.e. exactly what     */
+                               /* occd_argmax_classes returns for the OCCD_OUT1_F32_PLANAR logits of the same       */
+                               /* descriptor; optional label remap: occd_conv_plan_set_class_lut.  Needs every     */
+                               /* channel in one N tile and no tap groups (else OCCD_ERR_UNSUPPORTED)               */
+#define OCCD_CLASS_LUT_MAX 64
 
 typedef struct {
   int src;        /* which source tensor                                                          */
@@ -164,7 +171,7 @@ typedef struct {
   const void* res2;
   int res2_cstride, res2_coff;
   int res2_post; /* 1: res2 is added AFTER the activation (modules.py Upsample + skip)            */
-  /* out1: optional second output holding the PRE-activation value                                  */
+  /* out1: optional second output holding the PRE-activation value (or its class map, see above)      */
   int out1_mode;
   void* out1;
   int out1_cstride, out1_coff; /* channels-last mode                                               */
@@ -186,6 +193,9 @@ typedef struct occd_conv_plan occd_conv_plan;
 int occd_conv_plan_create(const occd_conv_desc* desc, occd_conv_plan** plan);
 int occd_conv_plan_destroy(occd_conv_plan* plan);
 int occd_conv_run(const occd_conv_plan* plan, void* stream);
+/* class-map plans (OCCD_OUT1_CLASS_U16): lut (HOST pointer, n == Cout <= 64 ints) or NULL: the map holds     */
+/* uint16(lut[class]) -- the inv_map remap of occd_argmax_classes -- from the next occd_conv_run on             */
+int occd_conv_plan_set_class_lut(occd_conv_plan* plan, const int* lut, int n);
 /* introspection for tests / profiling: tile box (TD,TH,TW), N tile, K chunk, stages, grid          */
 int occd_conv_plan_info(const occd_conv_plan* plan, int* info8);
 /* how the plan's tensor-core kernel shares M tiles between its two MMA warpgroups (fixed by the N tile):    */

@@ -22,50 +22,64 @@ namespace {
 
 using namespace occd_conv;
 
+// one thread per (output position, group of 8 channels); with a class-map output one thread per position walks every
+// channel group, so that one thread holds the position's arg-max
 template <typename T>
 __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ SimtParams p) {
-  const int ngroups = p.epi.Cout_store / 8;
+  const bool cls = p.epi.out1_mode == OCCD_OUT1_CLASS_U16;
+  const int ngroups = cls ? 1 : p.epi.Cout_store / 8;
   const long long total = (long long)p.epi.B * p.epi.OD * p.epi.OH * p.epi.OW * ngroups;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
-  const int g = (int)(idx % ngroups);
+  const int g0 = (int)(idx % ngroups), g1 = cls ? p.epi.Cout_store / 8 : g0 + 1;
   long long pos = idx / ngroups;
   const int ow = (int)(pos % p.epi.OW); pos /= p.epi.OW;
   const int oh = (int)(pos % p.epi.OH); pos /= p.epi.OH;
   const int od = (int)(pos % p.epi.OD); pos /= p.epi.OD;
   const int b = (int)pos;
-  float acc[8];
+  ClassArg ca = class_arg_init();
+  for (int g = g0; g < g1; ++g) {
+    float acc[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-  for (int tp = 0; tp < p.n_taps; ++tp) {
-    const int s = p.tap_src[tp];
-    const int id = od * p.stride[0] + p.tap_dz[tp] + p.src_d0;
-    const int ih = oh * p.stride[1] + p.tap_dy[tp];
-    const int iw = ow * p.stride[2] + p.tap_dx[tp];
-    if (id < 0 || id >= p.ID || ih < 0 || ih >= p.IH || iw < 0 || iw >= p.IW) continue;
-    const T* in = reinterpret_cast<const T*>(p.src[s]) +
-                  ((((long long)b * p.ID + id) * p.IH + ih) * p.IW + iw) * p.src_cstride[s] + p.src_coff[s];
-    const T* w = reinterpret_cast<const T*>(p.weight) +
-                 ((long long)b * p.w_batch_rows + (long long)tp * p.Cout_pad + g * 8) * p.Kpad;
-    const int C = p.src_C[s];
-    for (int c = 0; c < C; c += 8) {
-      float x[8];
-      Elem<T>::ld8(in + c, x);
-      if (c + 8 > C) {
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    for (int tp = 0; tp < p.n_taps; ++tp) {
+      const int s = p.tap_src[tp];
+      const int id = od * p.stride[0] + p.tap_dz[tp] + p.src_d0;
+      const int ih = oh * p.stride[1] + p.tap_dy[tp];
+      const int iw = ow * p.stride[2] + p.tap_dx[tp];
+      if (id < 0 || id >= p.ID || ih < 0 || ih >= p.IH || iw < 0 || iw >= p.IW) continue;
+      const T* in = reinterpret_cast<const T*>(p.src[s]) +
+                    ((((long long)b * p.ID + id) * p.IH + ih) * p.IW + iw) * p.src_cstride[s] + p.src_coff[s];
+      const T* w = reinterpret_cast<const T*>(p.weight) +
+                   ((long long)b * p.w_batch_rows + (long long)tp * p.Cout_pad + g * 8) * p.Kpad;
+      const int C = p.src_C[s];
+      for (int c = 0; c < C; c += 8) {
+        float x[8];
+        Elem<T>::ld8(in + c, x);
+        if (c + 8 > C) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (c + i >= C) x[i] = 0.f;
-      }
+          for (int i = 0; i < 8; ++i)
+            if (c + i >= C) x[i] = 0.f;
+        }
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float wv[8];
-        Elem<T>::ld8_nc(w + (long long)j * p.Kpad + c, wv);
+        for (int j = 0; j < 8; ++j) {
+          float wv[8];
+          Elem<T>::ld8_nc(w + (long long)j * p.Kpad + c, wv);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) acc[j] = fmaf(x[i], wv[i], acc[j]);
+          for (int i = 0; i < 8; ++i) acc[j] = fmaf(x[i], wv[i], acc[j]);
+        }
       }
     }
+    if (!cls) {
+      conv_epilogue_row<T, 8>(p.epi, b, od, oh, ow, g * 8, acc);
+      continue;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (g * 8 + i < p.epi.Cout)
+        class_arg_take(ca, class_value<T>(p.epi, epi_pos(p.epi, b, od, oh, ow), g * 8 + i, acc[i]), g * 8 + i);
   }
-  conv_epilogue_row<T, 8>(p.epi, b, od, oh, ow, g * 8, acc);
+  if (cls) class_store(p.epi, epi_pos(p.epi, b, od, oh, ow), ca);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -541,8 +555,11 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     iters = (iters + n_groups - 1) / n_groups;   // tap groups: the mean group; every CTA gets its share of each
     const long long m_tiles0 = (long long)d->B * t.tiles_d * t.tiles_h * t.tiles_w * n_groups;
     const int n_sms = n_sms_current();
+    // (a class map is costed as the planar logits it stands in for: both plans of one descriptor get the same tiles,
+    // so the map equals the arg-max of the logits bit for bit)
     const double out_bytes_per_col = 128.0 * ((d->out0 ? pl->esize : 0) + (d->out1_mode == OCCD_OUT1_CL ? pl->esize : 0) +
-                                              (d->out1_mode == OCCD_OUT1_F32_PLANAR ? 4 : 0));
+                                              (d->out1_mode == OCCD_OUT1_F32_PLANAR ||
+                                               d->out1_mode == OCCD_OUT1_CLASS_U16 ? 4 : 0));
     // experiment hook: OCCD_EPI_RATE overrides the model's epilogue drain rate
     static const double epi_rate = [] { const char* e = getenv("OCCD_EPI_RATE"); const double v = e ? atof(e) : 0.0;
                                         return v > 0.0 ? v : 12.0; }();
@@ -567,6 +584,10 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
       }
     }
     estimate(t.N_tile, xp ? d->Cout_pad : t.N_tile, est_mainloop, est_epi);
+  }
+  if (d->out1_mode == OCCD_OUT1_CLASS_U16 && !xp && t.N_tile < d->Cout_pad) {
+    occd_set_last_error("occd_conv_plan_create: a class map needs every output channel in one N tile");
+    return OCCD_ERR_UNSUPPORTED;
   }
   if (!(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile))) {
     occd_set_last_error(xp ? "occd_conv_plan_create(tcx): no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)"
@@ -702,6 +723,14 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
                    aligned(d->out1), "occd_conv_plan_create: out1 channel window");
   if (d->out1_mode == OCCD_OUT1_F32_PLANAR)
     OCCD_CHECK_ARG(d->out1 && d->out1_coff + d->Cout <= d->out1_C, "occd_conv_plan_create: out1 planar window");
+  if (d->out1_mode == OCCD_OUT1_CLASS_U16) {
+    OCCD_CHECK_ARG(d->out1 && reinterpret_cast<uintptr_t>(d->out1) % 2 == 0 && d->Cout <= 65535,
+                   "occd_conv_plan_create: a class map needs an aligned uint16 out1 and at most 65535 classes");
+    if (d->out0) {
+      occd_set_last_error("occd_conv_plan_create: a class map is the launch's only output (out0 must be NULL)");
+      return OCCD_ERR_UNSUPPORTED;
+    }
+  }
   for (int i = 0; i < 3; ++i) {
     OCCD_CHECK_ARG(d->stride[i] >= 1 && d->stride[i] <= 8 && d->omul[i] >= 1, "occd_conv_plan_create: stride/omul");
   }
@@ -749,7 +778,8 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
       s.tap_src[i] = (signed char)d->taps[i].src;
       s.tap_dz[i] = (short)d->taps[i].dz; s.tap_dy[i] = (short)d->taps[i].dy; s.tap_dx[i] = (short)d->taps[i].dx;
     }
-    const long long total = (long long)d->B * d->OD * d->OH * d->OW * (s.epi.Cout_store / 8);
+    const long long total = (long long)d->B * d->OD * d->OH * d->OW *
+                            (d->out1_mode == OCCD_OUT1_CLASS_U16 ? 1 : s.epi.Cout_store / 8);
     pl->grid = dim3((unsigned)((total + 127) / 128));
     *out = pl;
     return OCCD_OK;
@@ -773,6 +803,23 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
 
 extern "C" int occd_conv_plan_destroy(occd_conv_plan* plan) {
   delete plan;
+  return OCCD_OK;
+}
+
+extern "C" int occd_conv_plan_set_class_lut(occd_conv_plan* pl, const int* lut, int n) {
+  OCCD_CHECK_ARG(pl != nullptr, "occd_conv_plan_set_class_lut: null plan");
+  ConvEpi* e = pl->impl == OCCD_CONV_IMPL_SIMT ? &pl->simt.epi
+               : pl->impl == OCCD_CONV_IMPL_HALO ? &pl->halo.epi
+               : pl->impl == OCCD_CONV_IMPL_HALOX ? &pl->halox.epi : &pl->tc.epi;
+  OCCD_CHECK_ARG(e->out1_mode == OCCD_OUT1_CLASS_U16, "occd_conv_plan_set_class_lut: the plan writes no class map");
+  if (!lut) {
+    e->class_lut_use = 0;
+    return OCCD_OK;
+  }
+  OCCD_CHECK_ARG(n == e->Cout && n <= OCCD_CLASS_LUT_MAX,
+                 "occd_conv_plan_set_class_lut: one label per class, at most 64 classes");
+  for (int c = 0; c < OCCD_CLASS_LUT_MAX; ++c) e->class_lut[c] = c < n ? (unsigned short)lut[c] : 0;  // .astype(uint16)
+  e->class_lut_use = 1;
   return OCCD_OK;
 }
 

@@ -22,6 +22,8 @@ struct ConvEpi {
   int out1_mode;
   void* out1;
   int out1_cstride, out1_coff, out1_C;
+  int class_lut_use;   // class-map output: store class_lut[class] instead of the class (occd_conv_plan_set_class_lut)
+  unsigned short class_lut[OCCD_CLASS_LUT_MAX];
   int dbg;   // experiment switch (OCCD_DEBUG_EPI, tools/conv_bench.py only): 1 = skip the out0 stores, 2 = skip the
              // whole row epilogue (accumulators are read, nothing is stored)
 };
@@ -34,6 +36,40 @@ __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, in
 }
 __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, int oh, int ow) {
   return epi_pos(e, b, od, oh, ow, e.oadd[0], e.oadd[1], e.oadd[2]);
+}
+
+// Running arg-max of the class-map output (OCCD_OUT1_CLASS_U16) over the channels one thread has seen, taken in
+// ascending channel order.  The rule is argmax_classes_kernel's (elementwise.cu): the first index of the largest value;
+// a NaN in channel 0 wins, a NaN anywhere else is skipped.  A NaN channel 0 is held as +inf, which no later value beats
+// and which wins every tie by its index, so two threads' partial results merge with the same take().
+struct ClassArg {
+  float v;
+  int c;
+};
+__device__ __forceinline__ ClassArg class_arg_init() { return ClassArg{-INFINITY, 0x7fffffff}; }
+__device__ __forceinline__ void class_arg_take(ClassArg& a, float v, int c) {
+  if (c == 0 && v != v) v = INFINITY;
+  if (v > a.v || (v == a.v && c < a.c)) { a.v = v; a.c = c; }
+}
+// the partial result of lane ^ mask joins this lane's (every lane of the warp calls it)
+__device__ __forceinline__ void class_arg_merge_xor(ClassArg& a, int mask) {
+  const float v = __shfl_xor_sync(0xffffffffu, a.v, mask);
+  const int c = __shfl_xor_sync(0xffffffffu, a.c, mask);
+  class_arg_take(a, v, c);
+}
+// out1[pos]: the class map has the planar logits' spatial index, one uint16 per position
+__device__ __forceinline__ void class_store(const ConvEpi& e, long long pos, const ClassArg& a) {
+  reinterpret_cast<unsigned short*>(e.out1)[pos] = e.class_lut_use ? e.class_lut[a.c] : (unsigned short)a.c;
+}
+// Pre-activation value of channel n at position pos from its accumulator sum: acc + bias + res1 (+ res2), the additions
+// of conv_epilogue_compute in its order, one channel at a time.  The class-map epilogues feed the arg-max with it
+// value by value, so that no channel vector has to stay in registers beside the accumulator tile.
+template <typename T>
+__device__ __forceinline__ float class_value(const ConvEpi& e, long long pos, int n, float v) {
+  v += __ldg(e.bias + n);
+  if (e.res1) v += Elem<T>::up(reinterpret_cast<const T*>(e.res1)[pos * e.res1_cstride + e.res1_coff + n]);
+  if (e.res2 && !e.res2_post) v += Elem<T>::up(reinterpret_cast<const T*>(e.res2)[pos * e.res2_cstride + e.res2_coff + n]);
+  return v;
 }
 
 // Epilogue arithmetic for one output position `pos` and NV consecutive channels [n0, n0+NV) held in v[] (fp32

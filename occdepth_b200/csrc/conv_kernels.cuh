@@ -124,7 +124,9 @@ __device__ __forceinline__ void stage8(float* st, const float (&acc)[N / 2], int
 // (LD = kStageWide) or 8 (kStageHalo) columns go through shared memory so that thread t owns row t / 2 and 16
 // consecutive channels -- with 8-column rounds threads 0..63 own row t -- the vector width of the channels-last
 // stores.  The caller gives the position of the thread's row; oa:
-// per-launch output offset (tap groups) or nullptr for e.oadd.
+// per-launch output offset (tap groups) or nullptr for e.oadd.  A class map needs the whole channel range in this
+// tile (n0 == 0, Cout <= N: plan creation refuses anything else); the two threads of a row merge their arg-max by
+// shuffle and the first one stores.
 template <typename T, int N, int LD>
 __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
                                               int warp4, int lane, int t, bool valid, int b, int od, int oh, int ow,
@@ -132,6 +134,28 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
   constexpr int ROUND = LD == kStageWide ? 32 : 8;
   constexpr int TPR = ROUND == 8 ? 1 : 2, VW = ROUND / TPR;   // threads per row, channels per thread
   const int row = t / TPR, h = t % TPR;
+  if (e.out1_mode == OCCD_OUT1_CLASS_U16) {
+    // class map: every value joins the row's running arg-max as it leaves the staging buffer
+    ClassArg ca = class_arg_init();
+    const long long pos = valid ? epi_pos(e, b, od, oh, ow) : 0;
+#pragma unroll
+    for (int c0 = 0; c0 < N; c0 += ROUND) {
+      tc::wg_sync(bar_id);
+#pragma unroll
+      for (int j = 0; j < ROUND / 8; ++j)
+        if (c0 + 8 * j < N) stage8<LD, N>(st, acc, (c0 >> 3) + j, 8 * j, warp4, lane);
+      tc::wg_sync(bar_id);
+      const int cc = c0 + VW * h;
+      if (valid && row < 64 && cc < N) {
+#pragma unroll 1
+        for (int i = 0; i < VW && n0 + cc + i < e.Cout; ++i)
+          class_arg_take(ca, class_value<T>(e, pos, n0 + cc + i, st[row * LD + VW * h + i]), n0 + cc + i);
+      }
+    }
+    if constexpr (TPR == 2) class_arg_merge_xor(ca, 1);
+    if (valid && row < 64 && h == 0) class_store(e, pos, ca);
+    return;
+  }
   const bool fast = VW == 16 && epi_fast_ok(e);
   EpiRow<T> er;
   if (fast)
@@ -171,7 +195,8 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
 // rows (lo_ok / hi_ok false: the neighbour is the conv's zero padding).  Rounds of 8 channels: the 8-column blocks of
 // Q_0, Q_1 and Q_2 are staged (xp_stage_ld) and threads 0..63 (one per row) form the sums.
 // The sums of up to 32 channels stay in registers and go through the row epilogue together, so that its bias and
-// residual loads are issued once per chunk rather than behind every round's barriers.
+// residual loads are issued once per chunk rather than behind every round's barriers.  A class map instead feeds each
+// round's 8 sums straight into the row's running arg-max (one thread sees every channel of its row).
 template <typename T, int N>
 __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
                                             int warp4, int lane, int t, int d, bool lo_ok, bool hi_ok, bool valid,
@@ -181,6 +206,38 @@ __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)
   constexpr int CP = N / 3;
   constexpr int CH = CP < 32 ? CP : 32;   // channels per chunk
   const bool mine = t < 64 && valid;
+  if (e.out1_mode == OCCD_OUT1_CLASS_U16) {
+    ClassArg ca = class_arg_init();
+    const long long pos = mine ? epi_pos(e, b, od, oh, ow) : 0;
+#pragma unroll
+    for (int c0 = 0; c0 < CP; c0 += 8) {
+      tc::wg_sync(bar_id);
+      stage8<LD, N>(st, acc, c0 >> 3, 0, warp4, lane);
+      stage8<LD, N>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
+      if constexpr (Q2COL != 0) stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, Q2COL, warp4, lane);
+      tc::wg_sync(bar_id);
+      // Q_1 + Q_0 goes back into this row's own Q_1 block, which no other thread reads, instead of staying in
+      // registers across the next staging
+      if (mine) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) st[t * LD + 8 + i] += lo_ok ? st[(t - d) * LD + i] : 0.f;
+      }
+      if constexpr (Q2COL == 0) {
+        tc::wg_sync(bar_id);
+        stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
+        tc::wg_sync(bar_id);
+      }
+      if (mine) {
+#pragma unroll 1
+        for (int i = 0; i < 8 && c0 + i < e.Cout; ++i) {
+          const float x = st[t * LD + 8 + i] + (hi_ok ? st[(t + d) * LD + Q2COL + i] : 0.f);
+          class_arg_take(ca, class_value<T>(e, pos, c0 + i, x), c0 + i);
+        }
+      }
+    }
+    if (mine) class_store(e, pos, ca);
+    return;
+  }
 #pragma unroll
   for (int c1 = 0; c1 < CP; c1 += CH) {
     float v[CH];

@@ -232,16 +232,22 @@ def fold_bn(weight, bias, bn, eps=None):
     return w * scale.view(shape), (b - bn.running_mean.detach().float()) * scale + bn.bias.detach().float()
 
 
+class ClassMapUnsupported(RuntimeError):
+    """occd_conv_plan_create refused a class-map output (OCCD_ERR_UNSUPPORTED) for the kernel this launch runs on"""
+
+
 class ConvOp:
     """One planned implicit-GEMM launch (occd_conv_plan_create / occd_conv_run)."""
 
     def __init__(self, srcs, taps, tap_weights, bias, out_dims, out0=None, act="none", res1=None, res2=None,
                  stride=(1, 1, 1), omul=(1, 1, 1), oadd=(0, 0, 0), full_dims=None, out1=None, out1_mode="none",
                  out1_coff=0, impl=None, name="", res2_post=False, weight_buf=None, weight_per_image=False,
-                 out0_exact=False, groups=None):
+                 out0_exact=False, groups=None, lut=None):
         """srcs: list[CL] (same B,D,H,W);  taps: [(src_idx, dz, dy, dx)];  tap_weights: list of fp32 [Cout, C_src]
         bias: fp32 [Cout];  out0/res1/res2: CL on the full output grid;  out1: CL (pre-activation bf16 copy) or
-        fp32 planar tensor [B, C1, D, H, W] (mode "planar", written at channel out1_coff).
+        fp32 planar tensor [B, C1, D, H, W] (mode "planar", written at channel out1_coff), or the uint16 class map
+        [B, D, H, W] of the pre-activation values (mode "classes", no out0; lut: Cout label ids or None, the remap of
+        occd_argmax_classes).  Raises ClassMapUnsupported when the chosen kernel cannot write a class map.
         groups: [(n_taps_of_group, (oadd_d, oadd_h, oadd_w))] -- several convolutions over the same sources in one
         launch, each with its own slice of `taps` and output offset (occd_conv_desc.n_groups; per-tap TC kernel)."""
         self.name = name
@@ -336,6 +342,10 @@ class ConvOp:
             assert out1.dtype == torch.float32 and out1.is_contiguous() and tuple(out1.shape[2:]) == fd
             d.out1_mode, d.out1 = _lib.OUT1_F32_PLANAR, out1.data_ptr()
             d.out1_C, d.out1_coff = out1.shape[1], out1_coff
+        elif out1_mode == "classes":
+            assert out0 is None and out1.dtype == torch.uint16 and out1.is_contiguous()
+            assert tuple(out1.shape) == (B,) + fd
+            d.out1_mode, d.out1 = _lib.OUT1_CLASS_U16, out1.data_ptr()
         self.desc = d
         self.flops = 2 * B * OD * OH * OW * Cout * sum(srcs[t[0]].C for t in taps)
         h = C.c_void_p()
@@ -349,9 +359,15 @@ class ConvOp:
         if rc != 0 and auto and d.impl == _lib.CONV_IMPL_HALO:
             d.impl = _lib.CONV_IMPL_TC      # shape did not fit the halo scheme: per-tap wgmma kernel
             rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
+        if rc == _lib.ERR_UNSUPPORTED and out1_mode == "classes":
+            raise ClassMapUnsupported("occd_conv_plan_create(%s): %s" % (name, _lib.lib().occd_last_error().decode()))
         _lib.check(rc, "occd_conv_plan_create(%s)" % name)
         self.handle = h
         self.impl = d.impl
+        if lut is not None:
+            self._lut = (C.c_int * len(lut))(*[int(v) for v in lut])
+            _lib.check(_lib.lib().occd_conv_plan_set_class_lut(h, self._lut, len(lut)),
+                       "occd_conv_plan_set_class_lut(%s)" % name)
 
     def info(self):
         arr = (C.c_int * 8)()
@@ -451,8 +467,10 @@ class Plan:
     # ---- dense convolution (2-D maps have D == 1) ----
     def conv(self, x, weight, bias, stride=1, padding=0, dilation=1, act="none", out=None, res1=None, res2=None,
              out1=None, out1_mode="none", out1_coff=0, name="conv", impl=None, res2_post=False, no_out0=False,
-             out0_exact=False):
-        """x: CL; weight fp32 [Cout,Cin,kd,kh,kw] (BN already folded); returns the output CL."""
+             out0_exact=False, lut=None):
+        """x: CL; weight fp32 [Cout,Cin,kd,kh,kw] (BN already folded); returns the output CL.
+        out1_mode="classes": out1 is a uint16 [B, D, H, W] class map (no out0), written by the conv's epilogue; where
+        the kernel cannot do that, the logits go to a plan-owned fp32 buffer and occd_argmax_classes maps them."""
         s, p, d = _t3(stride), _t3(padding), _t3(dilation)
         B, ID, IH, IW = x.dims
         co, ci, kd, kh, kw = weight.shape
@@ -468,10 +486,29 @@ class Plan:
             out = self.alloc(B, od[0], od[1], od[2], co)
         taps, ws = conv_taps(weight, d, p)
         self.need_halo(x, taps, s[0], od[0])
-        self.add(ConvOp([x], taps, ws, bias, od, out0=out, act=act, res1=res1, res2=res2, stride=s, out1=out1,
-                        out1_mode=out1_mode, out1_coff=out1_coff, name=name, impl=impl, res2_post=res2_post,
-                        out0_exact=out0_exact))
+        kw = dict(out0=out, act=act, res1=res1, res2=res2, stride=s, name=name, impl=impl, res2_post=res2_post,
+                  out0_exact=out0_exact)
+        if out1_mode == "classes":
+            try:
+                self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode="classes", lut=lut, **kw))
+            except ClassMapUnsupported:
+                self._class_map_fallback(x, taps, ws, bias, od, out1, lut, kw)
+            return out
+        self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode=out1_mode, out1_coff=out1_coff, **kw))
         return out
+
+    def _class_map_fallback(self, x, taps, ws, bias, od, classes, lut, kw):
+        """the class map of a conv whose kernel cannot write one: planar fp32 logits into a plan-owned buffer, then
+        occd_argmax_classes (the same values and rule, so the same map)"""
+        B = x.dims[0]
+        co = int(bias.numel())
+        logits = torch.empty((B, co) + tuple(od), dtype=torch.float32, device=self.device)
+        self.add(ConvOp([x], taps, ws, bias, od, out1=logits, out1_mode="planar", **kw))
+        L = _lib.lib()
+        S = od[0] * od[1] * od[2]
+        lut_c = None if lut is None else (C.c_int * len(lut))(*[int(v) for v in lut])
+        self.add(FnOp(lambda st: L.occd_argmax_classes(logits.data_ptr(), classes.data_ptr(), B, co, S, lut_c, st),
+                      "occd_argmax_classes", keep=(logits, classes, lut_c)))
 
     def conv_multi(self, srcs, weights, bias, paddings, dilations, act="none", out=None, res1=None, res2=None,
                    name="conv_multi", impl=None):

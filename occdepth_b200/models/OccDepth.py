@@ -119,7 +119,9 @@ class OccDepth(_Base, B200Module):
             raise NotImplementedError(f"{self.trans_2d_to_3d} is not supported yet.")
 
     # ------------------------------------------------------------------------------------------
-    def _build(self, B, V, H, W, N, P, dev, batch):
+    def _build(self, B, V, H, W, N, P, dev, batch, classes=None):
+        """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut): the plan of
+        predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor)"""
         slab = self.__dict__.get("slab_ctx")
         plan = Plan(dev, slab=slab, precision=self.precision)
         ps = self.project_scale
@@ -238,7 +240,10 @@ class OccDepth(_Base, B200Module):
                                            [S[0] * ps, S[1] * ps, S[2] * ps], ps,
                                            prior=pr, scale_const=100.0, stream=st), 0)[1],
                           "sfa_lift", keep=(feats, pix, fov, out_b)))
-        out = self.net_3d_decoder.emit(plan, x3d)
+        if classes is None:
+            out = self.net_3d_decoder.emit(plan, x3d)
+        else:
+            out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1])
         if os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
             try:
                 plan.capture()
@@ -248,6 +253,23 @@ class OccDepth(_Base, B200Module):
         return plan, img, pix, fov, out, depth0, n_lo, view_sel
 
     def forward(self, batch):
+        return self._run(batch, None)
+
+    def predict_classes(self, batch, inv_map=None):
+        """uint16 class per voxel [B, X, Y, Z]: bit for bit `class_map(self(batch)["ssc_logit"], inv_map)`, but the
+        classifier's epilogue writes the map, so no logits (and none of the forward's other outputs) are stored,
+        converted or copied.  inv_map: one label id per class (at most 64), the submission writer's remap.  Its plan is
+        cached apart from the forward's (alternating both rebuilds neither); under enable_slab_parallel this rank's
+        X-slab."""
+        lut = None
+        if inv_map is not None:
+            import numpy as np
+            lut = tuple(int(v) for v in np.asarray(inv_map).astype(np.int64).reshape(-1))
+            if len(lut) != self.n_classes:
+                raise ValueError("OccDepth.predict_classes: inv_map must hold one label id per class")
+        return self._run(batch, ("classes", lut))
+
+    def _run(self, batch, classes):
         img = batch["img"]
         if not img.is_cuda:
             if not torch.cuda.is_available():
@@ -267,6 +289,8 @@ class OccDepth(_Base, B200Module):
         key = (B, V, H, W, N, P, str(dev), virtual, float(batch["virtual_bf"][0]) if virtual else 0.0,
                None if slab is None else (slab.rank, slab.world), self.precision, self.param_stamp())
         with torch.cuda.device(dev):           # launches, tensor maps and function attributes follow the tensors
+            if classes is not None:
+                return self._classes_on(batch, key + classes, img, pp, fm, B, V, H, W, N, P, dev, classes)
             return self._forward_on(batch, key, img, pp, fm, B, V, H, W, N, P, dev)
 
     def prepare(self, batch):
@@ -292,6 +316,20 @@ class OccDepth(_Base, B200Module):
         self._stage(ent, batch, img, pp, fm, dev)
         ent[0].run()
         return self._outputs(ent)
+
+    def _classes_on(self, batch, key, img, pp, fm, B, V, H, W, N, P, dev, classes):
+        cache = self._class_plans()
+        ent = cache.get(key)
+        if ent is None:
+            cache.clear()                      # one class-map plan: weights, shapes or inv_map changed
+            with torch.no_grad():
+                ent = self._build(B, V, H, W, N, P, dev, batch, classes=classes)
+            cache[key] = ent
+        if self.__dict__.get("_build_only"):
+            return None
+        self._stage(ent, batch, img, pp, fm, dev)
+        ent[0].run()
+        return ent[4].clone()                  # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
         """copy this batch's inputs into the static input buffers of plan entry `ent`"""

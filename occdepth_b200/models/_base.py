@@ -51,18 +51,26 @@ class B200Module(nn.Module):
             self.__dict__["_stamp_tensors"] = ts
         return hash(tuple((t.data_ptr(), t._version) for t in ts))
 
+    def _class_plans(self):
+        """plans of OccDepth.predict_classes: a cache of their own, so that forward and predict_classes on the same
+        shapes keep one plan each; dropped together with _plans()"""
+        return self.__dict__.setdefault("_class_plan_cache", {})
+
     def invalidate_plans(self):
         for m in self.modules():
             if isinstance(m, B200Module):
                 m.__dict__["_plan_cache"] = {}
+                m.__dict__["_class_plan_cache"] = {}
 
     def _load_from_state_dict(self, *a, **k):
         self.__dict__["_plan_cache"] = {}
+        self.__dict__["_class_plan_cache"] = {}
         self.__dict__["_stamp_tensors"] = None
         return super()._load_from_state_dict(*a, **k)
 
     def _apply(self, fn, *a, **k):
         self.__dict__["_plan_cache"] = {}
+        self.__dict__["_class_plan_cache"] = {}
         r = super()._apply(fn, *a, **k)
         self.__dict__["_stamp_tensors"] = None      # buffers are re-created by _apply
         return r

@@ -43,7 +43,9 @@ class UNet3D(B200Module):
         if context_prior:
             self.CP_mega_voxels = CPMegaVoxels(f * 4, size_l3, bn_momentum=bn_momentum)
 
-    def emit(self, plan, x3d_l1):
+    def emit(self, plan, x3d_l1, classes=False, lut=None):
+        """-> the forward's output dict, or with `classes` only the uint16 class map [B, X, Y, Z] of the ssc head
+        (the occluded head, whose logits nothing then reads, is not planned)"""
         res = {}
         x3d_l2 = self.process_l1[1].emit(plan, self.process_l1[0].emit(plan, x3d_l1))
         x3d_l3 = self.process_l2[1].emit(plan, self.process_l2[0].emit(plan, x3d_l2))
@@ -55,6 +57,9 @@ class UNet3D(B200Module):
         x3d_up_l2 = self.up_13_l2.emit(plan, x3d_l3, skip=x3d_l2)
         x3d_up_l1 = self.up_12_l1.emit(plan, x3d_up_l2, skip=x3d_l1)
         x3d_up_lfull = self.up_l1_lfull.emit(plan, x3d_up_l1)
+        if classes:
+            out = self.ssc_head.emit(plan, x3d_up_lfull, classes=True, lut=lut)
+            return out[0] if self.cascade_cls else out
         if not self.infer_mode:
             res["x3d_l1"] = x3d_up_l1
             res["x3d_l2"] = x3d_up_l2

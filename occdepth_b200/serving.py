@@ -13,6 +13,9 @@ allocated per frame (a caching-allocator block that changes streams would serial
         if done is not None:
             logits = pipe.result(done)         # host tensor, valid until two more submits
     logits = pipe.result(pipe.flush())
+
+With `classes=True` every frame runs `model.predict_classes(batch, inv_map)` instead: the classifier writes the
+uint16 class map [B, X, Y, Z] (4 MB at config 2) and that is what is read back, not the 168 MB of logits.
 """
 import torch
 
@@ -20,12 +23,14 @@ from .engine import require_cuda
 
 
 class FramePipeline:
-    def __init__(self, model, img_shape, pix_shape, fov_shape, device=None, out_key="ssc_logit"):
+    def __init__(self, model, img_shape, pix_shape, fov_shape, device=None, out_key="ssc_logit", classes=False,
+                 inv_map=None):
         if not torch.cuda.is_available():
             raise RuntimeError("FramePipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         require_cuda(torch.empty(0, device=dev), "FramePipeline")
         self.model, self.dev, self.out_key = model, dev, out_key
+        self.classes, self.inv_map = classes, inv_map
         self.key = "%d" % model.project_scale
         self.main = torch.cuda.current_stream(dev)
         self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
@@ -53,9 +58,12 @@ class FramePipeline:
             buf["fov"].copy_(fov_h, non_blocking=True)
             self.in_ready[j].record(self.h2d)
         self.main.wait_event(self.in_ready[j])
+        batch = {"img": buf["img"], "projected_pix_" + self.key: [buf["pix"]], "fov_mask_" + self.key: [buf["fov"]]}
         with torch.no_grad():
-            res = self.model({"img": buf["img"], "projected_pix_" + self.key: [buf["pix"]],
-                              "fov_mask_" + self.key: [buf["fov"]]})[self.out_key]
+            if self.classes:
+                res = self.model.predict_classes(batch, self.inv_map)
+            else:
+                res = self.model(batch)[self.out_key]
         self.in_free[j].record(self.main)
         if self.dev_out[j] is None:
             self.dev_out[j] = torch.empty_like(res)
