@@ -130,7 +130,7 @@ extern "C" int occd_conv_debug_trace(long long* device_buf) {
   return OCCD_OK;
 }
 
-static int fill_epi(const occd_conv_desc* d, ConvEpi* e) {
+static void fill_epi(const occd_conv_desc* d, ConvEpi* e) {
   e->B = d->B; e->OD = d->OD; e->OH = d->OH; e->OW = d->OW;
   for (int i = 0; i < 3; ++i) { e->omul[i] = d->omul[i]; e->oadd[i] = d->oadd[i]; }
   e->ODf = d->ODf; e->OHf = d->OHf; e->OWf = d->OWf;
@@ -147,13 +147,36 @@ static int fill_epi(const occd_conv_desc* d, ConvEpi* e) {
   e->res2_cstride = d->res2_cstride; e->res2_coff = d->res2_coff; e->res2_post = d->res2_post;
   e->out1_mode = d->out1_mode; e->out1 = d->out1;
   e->out1_cstride = d->out1_cstride; e->out1_coff = d->out1_coff; e->out1_C = d->out1_C;
-  { const char* v = getenv("OCCD_DEBUG_EPI"); e->dbg = v ? atoi(v) : 0; }
-  return 0;
 }
 
-// Programmatic dependent launch (common.cuh): the conv kernels wait on griddepcontrol after their prologue (barrier
-// init, tensor-map prefetch overlap the tail of the previous grid); results are bit-identical either way.
-static int pdl_enabled() { return occd_pdl_enabled(); }
+static ConvEpi* plan_epi(occd_conv_plan* pl) {
+  switch (pl->impl) {
+    case OCCD_CONV_IMPL_SIMT: return &pl->simt.epi;
+    case OCCD_CONV_IMPL_HALO: return &pl->halo.epi;
+    case OCCD_CONV_IMPL_HALOX: return &pl->halox.epi;
+    default: return &pl->tc.epi;
+  }
+}
+
+static const char* impl_tag(int impl) {
+  switch (impl) {
+    case OCCD_CONV_IMPL_SIMT: return "simt";
+    case OCCD_CONV_IMPL_HALO: return "halo";
+    case OCCD_CONV_IMPL_HALOX: return "halox";
+    case OCCD_CONV_IMPL_TCX: return "tcx";
+    default: return "tc";
+  }
+}
+
+// plan creation refuses the descriptor: the message names the impl
+static int refuse(const occd_conv_plan* pl, int rc, const char* msg) {
+  char buf[256];
+  snprintf(buf, sizeof(buf), "occd_conv_plan_create(%s): %s", impl_tag(pl->impl), msg);
+  occd_set_last_error(buf);
+  return rc;
+}
+// a shape the impl's kernel cannot run
+#define PLAN_REQUIRE(cond, msg) do { if (!(cond)) return refuse(pl, OCCD_ERR_UNSUPPORTED, msg); } while (0)
 
 static int n_sms_current() {
   static int n_sms[64] = {0};
@@ -167,26 +190,49 @@ static int n_sms_current() {
   return n_sms[dev];
 }
 
-// Halo-tile plan: stride-1 "same" convolution whose taps are {-d,0,d} offsets, one source, one k-chunk, one N tile.
-// halo_geometry is pure host arithmetic; halo_encode builds the tensor maps.
-static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
-#define HALO_REQUIRE(cond, msg) do { if (!(cond)) { occd_set_last_error("occd_conv_plan_create(halo): " msg); return OCCD_ERR_UNSUPPORTED; } } while (0)
-  HALO_REQUIRE(d->n_src == 1, "one source only");
-  HALO_REQUIRE(d->stride[0] == 1 && d->stride[1] == 1 && d->stride[2] == 1, "stride must be 1");
-  HALO_REQUIRE(d->omul[0] == 1 && d->omul[1] == 1 && d->omul[2] == 1 && d->oadd[0] == 0 && d->oadd[1] == 0 &&
+// Persistent kernels: one CTA per SM, or one per tile when there are fewer tiles
+static int persistent_grid(occd_conv_plan* pl, long long num_tiles) {
+  PLAN_REQUIRE(num_tiles <= 2147483647LL, "too many tiles");
+  const int n_sms = n_sms_current();
+  pl->grid = dim3((unsigned)(num_tiles < n_sms ? num_tiles : n_sms));
+  return OCCD_OK;
+}
+
+// The K chunk (pl->kc channels, pl->rb bytes per swizzled smem row) for sources of at most C channels
+static int set_k_chunk(occd_conv_plan* pl, int C) {
+  pl->kc = chunk_channels(C, pl->esize);
+  pl->rb = pl->kc * pl->esize;
+  return pl->kc;
+}
+
+// The halo kernels' grid: a stride-1 "same" convolution, output grid = input grid less the source's halo margins
+static int same_grid(const occd_conv_desc* d, const occd_conv_plan* pl) {
+  PLAN_REQUIRE(d->stride[0] == 1 && d->stride[1] == 1 && d->stride[2] == 1, "stride must be 1");
+  PLAN_REQUIRE(d->omul[0] == 1 && d->omul[1] == 1 && d->omul[2] == 1 && d->oadd[0] == 0 && d->oadd[1] == 0 &&
                d->oadd[2] == 0, "identity output mapping only");
-  HALO_REQUIRE(d->OD + 2 * d->src_d0 == d->ID && d->OH == d->IH && d->OW == d->IW,
+  PLAN_REQUIRE(d->OD + 2 * d->src_d0 == d->ID && d->OH == d->IH && d->OW == d->IW,
                "output grid must equal the input grid (plus symmetric halo margins)");
-  HALO_REQUIRE(d->n_taps <= 27, "at most 27 taps");
-  HALO_REQUIRE(d->src_C[0] <= 128 / pl->esize && d->Cout_pad <= 128,
+  return OCCD_OK;
+}
+
+// Each tensor-core geometry below is pure host arithmetic.  Besides its parameter block it returns the activation
+// TMA box and traversal strides in (W, H, D) order and the weight box's rows (the N tile); occd_conv_plan_create
+// encodes the tensor maps from them once the geometry has accepted the descriptor.
+
+// Halo-tile plan: stride-1 "same" convolution whose taps are {-d,0,d} offsets, one source, one k-chunk, one N tile.
+static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3], int traversal[3], int* n_tile) {
+  PLAN_REQUIRE(d->n_src == 1, "one source only");
+  if (const int rc = same_grid(d, pl)) return rc;
+  PLAN_REQUIRE(d->n_taps <= 27, "at most 27 taps");
+  PLAN_REQUIRE(d->src_C[0] <= 128 / pl->esize && d->Cout_pad <= 128,
                "channel counts too large for the resident-weight scheme (one K chunk)");
   int dil = 0;
   for (int i = 0; i < d->n_taps; ++i) {
     const int o[3] = {abs(d->taps[i].dz), abs(d->taps[i].dy), abs(d->taps[i].dx)};
     for (int k = 0; k < 3; ++k)
-      if (o[k]) { if (!dil) dil = o[k]; HALO_REQUIRE(o[k] == dil, "taps must be {-d,0,d} offsets"); }
+      if (o[k]) { if (!dil) dil = o[k]; PLAN_REQUIRE(o[k] == dil, "taps must be {-d,0,d} offsets"); }
   }
-  HALO_REQUIRE(dil >= 1 && dil <= 8, "dilation must be 1..8");
+  PLAN_REQUIRE(dil >= 1 && dil <= 8, "dilation must be 1..8");
   int hal[3] = {0, 0, 0};
   for (int i = 0; i < d->n_taps; ++i) {
     if (d->taps[i].dz) hal[0] = 1;
@@ -194,21 +240,17 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
     if (d->taps[i].dx) hal[2] = 1;
   }
   HaloParams& h = pl->halo;
-  fill_epi(d, &h.epi);
-  const int KC = chunk_channels(d->src_C[0], pl->esize);
-  HALO_REQUIRE(d->Kpad == KC, "Kpad must equal the k-chunk");
-  pl->kc = KC;
-  pl->rb = KC * pl->esize;
+  PLAN_REQUIRE(d->Kpad == set_k_chunk(pl, d->src_C[0]), "Kpad must equal the k-chunk");
   const int row_bytes = pl->rb;
   h.d = dil; h.D = d->OD; h.H = d->IH; h.W = d->IW;
   h.src_d0 = d->src_d0;
   h.hd = hal[0]; h.hh = hal[1]; h.hw = hal[2];
   h.n_taps = d->n_taps;
   h.N_tile = d->Cout_pad;
-  HALO_REQUIRE(HaloTiles::has(h.N_tile), "no kernel compiled for this Cout_pad (16, 32, 48 or 64)");
+  PLAN_REQUIRE(HaloTiles::has(h.N_tile), "no kernel compiled for this Cout_pad (16, 32, 48 or 64)");
   h.b_stride = round_up(h.N_tile * row_bytes, 1024);
   h.w_bytes = h.n_taps * h.b_stride;
-  HALO_REQUIRE(h.w_bytes <= 112 * 1024, "weights do not fit in shared memory");
+  PLAN_REQUIRE(h.w_bytes <= 112 * 1024, "weights do not fit in shared memory");
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil, sW = (d->IW + dil - 1) / dil;
   const int smem_total = 227 * 1024 - staging_bytes(kStageHalo) - h.w_bytes - 2048;   // staging, barriers, slack
   // W extent of the box: the whole sub-sampled line when it fits, else equal splits of at most 62
@@ -236,7 +278,7 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
         h.R0 = R0; h.nM = nM; h.a_stage_bytes = stage;
       }
     }
-  HALO_REQUIRE(best_cost >= 0, "no tile shape fits");
+  PLAN_REQUIRE(best_cost >= 0, "no tile shape fits");
   h.tilesD = (sD + h.BD - 1) / h.BD; h.tilesH = (sH + h.BH - 1) / h.BH; h.tilesW = nW;
   h.box_bytes = h.PD * h.PH * h.PW * row_bytes;
   h.stages = smem_total / h.a_stage_bytes;
@@ -245,46 +287,34 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   for (int i = 0; i < d->n_taps; ++i)
     h.tap_off16[i] = (h.R0 + ((d->taps[i].dz / dil) * h.PH + d->taps[i].dy / dil) * h.PW + d->taps[i].dx / dil) *
                      row_bytes / 16;
-  h.pdl = pdl_enabled();
+  h.pdl = occd_pdl_enabled();
   pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(kStageHalo) + 128 + 1024;
-  const long long num_tiles = (long long)d->B * dil * dil * dil * h.tilesD * h.tilesH * h.tilesW;
-  HALO_REQUIRE(num_tiles < 2147483647LL, "too many tiles");
-  const int n_sms = n_sms_current();
-  pl->grid = dim3((unsigned)(num_tiles < n_sms ? num_tiles : n_sms));
-#undef HALO_REQUIRE
-  return OCCD_OK;
+  box[0] = (h.PW - 1) * dil + 1; box[1] = (h.PH - 1) * dil + 1; box[2] = (h.PD - 1) * dil + 1;
+  traversal[0] = traversal[1] = traversal[2] = dil;
+  *n_tile = h.N_tile;
+  return persistent_grid(pl, (long long)d->B * dil * dil * dil * h.tilesD * h.tilesH * h.tilesW);
 }
 
-
-// x-packed halo plan (conv_halox_kernel): host arithmetic
-static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
-#define HX_REQUIRE(cond, msg) do { if (!(cond)) { occd_set_last_error("occd_conv_plan_create(halox): " msg); return OCCD_ERR_UNSUPPORTED; } } while (0)
-  HX_REQUIRE(d->n_src == 1 && !d->weight_per_image, "one source, shared weights");
-  HX_REQUIRE(d->stride[0] == 1 && d->stride[1] == 1 && d->stride[2] == 1, "stride must be 1");
-  HX_REQUIRE(d->omul[0] == 1 && d->omul[1] == 1 && d->omul[2] == 1 && d->oadd[0] == 0 && d->oadd[1] == 0 &&
-             d->oadd[2] == 0, "identity output mapping only");
-  HX_REQUIRE(d->OD + 2 * d->src_d0 == d->ID && d->OH == d->IH && d->OW == d->IW,
-             "output grid must equal the input grid (plus symmetric halo margins)");
-  HX_REQUIRE(d->IW == 8 || d->IW == 16 || d->IW == 32, "innermost extent W must be 8, 16 or 32 (one warp row)");
-  HX_REQUIRE(d->n_taps % 3 == 0 && d->n_taps <= 27, "taps must come as W triples");
-  HX_REQUIRE(d->src_C[0] <= 128 / pl->esize && 3 * d->Cout_pad <= 256, "one K chunk, 3 * Cout_pad <= 256");
+// x-packed halo plan (conv_halox_kernel)
+static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3], int traversal[3], int* n_tile) {
+  PLAN_REQUIRE(d->n_src == 1 && !d->weight_per_image, "one source, shared weights");
+  if (const int rc = same_grid(d, pl)) return rc;
+  PLAN_REQUIRE(d->IW == 8 || d->IW == 16 || d->IW == 32, "innermost extent W must be 8, 16 or 32 (one warp row)");
+  PLAN_REQUIRE(d->n_taps % 3 == 0 && d->n_taps <= 27, "taps must come as W triples");
+  PLAN_REQUIRE(d->src_C[0] <= 128 / pl->esize && 3 * d->Cout_pad <= 256, "one K chunk, 3 * Cout_pad <= 256");
   const int dil = d->taps[2].dx;
-  HX_REQUIRE(dil >= 1 && dil <= 8 && dil < d->IW, "W dilation");
+  PLAN_REQUIRE(dil >= 1 && dil <= 8 && dil < d->IW, "W dilation");
   int hal[2] = {0, 0};
   for (int i = 0; i < d->n_taps; i += 3) {
     const occd_conv_tap &a = d->taps[i], &b = d->taps[i + 1], &c = d->taps[i + 2];
-    HX_REQUIRE(a.dx == -dil && b.dx == 0 && c.dx == dil && a.dz == b.dz && a.dz == c.dz && a.dy == b.dy &&
-               a.dy == c.dy, "taps must be ordered (dz, dy) groups of dx = -d, 0, +d");
-    HX_REQUIRE((a.dz == 0 || abs(a.dz) == dil) && (a.dy == 0 || abs(a.dy) == dil), "D / H taps must be {-d, 0, d}");
+    PLAN_REQUIRE(a.dx == -dil && b.dx == 0 && c.dx == dil && a.dz == b.dz && a.dz == c.dz && a.dy == b.dy &&
+                 a.dy == c.dy, "taps must be ordered (dz, dy) groups of dx = -d, 0, +d");
+    PLAN_REQUIRE((a.dz == 0 || abs(a.dz) == dil) && (a.dy == 0 || abs(a.dy) == dil), "D / H taps must be {-d, 0, d}");
     if (a.dz) hal[0] = 1;
     if (a.dy) hal[1] = 1;
   }
   HaloxParams& h = pl->halox;
-  fill_epi(d, &h.epi);
-  const int KC = chunk_channels(d->src_C[0], pl->esize);
-  HX_REQUIRE(d->Kpad == KC, "Kpad must equal the k-chunk");
-  pl->kc = KC;
-  pl->rb = KC * pl->esize;
+  PLAN_REQUIRE(d->Kpad == set_k_chunk(pl, d->src_C[0]), "Kpad must equal the k-chunk");
   const int RB = pl->rb, NMMA = RB / 32;
   h.d = dil; h.D = d->OD; h.H = d->IH;
   h.src_d0 = d->src_d0;
@@ -292,13 +322,13 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   h.n_groups = d->n_taps / 3;
   h.CP = d->Cout_pad;
   h.N_tile = 3 * d->Cout_pad;
-  HX_REQUIRE(HaloxTiles::has(h.N_tile), "no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)");
+  PLAN_REQUIRE(HaloxTiles::has(h.N_tile), "no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)");
   h.rb = RB;
   h.PW = d->IW;
   h.b_stride = round_up(h.N_tile * RB, 1024);
   h.w_bytes = h.n_groups * h.b_stride;
   const int smem_total = 227 * 1024 - staging_bytes(xp_stage_ld(h.N_tile)) - h.w_bytes - 2048;   // staging, barriers, slack
-  HX_REQUIRE(smem_total > 0, "weights do not fit in shared memory");
+  PLAN_REQUIRE(smem_total > 0, "weights do not fit in shared memory");
   const int HR = 128 / h.PW;                               // h-rows of one plane per M tile
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil;
   // CTA tile = BD planes x nB blocks of HR h-rows (<= 2 M tiles: two accumulator sets of nM x N_tile columns)
@@ -326,15 +356,13 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
       h.a_stage_bytes = stage; h.stages = stages > 4 ? 4 : stages;
     }
   }
-  HX_REQUIRE(best >= 0, "no tile shape fits");
+  PLAN_REQUIRE(best >= 0, "no tile shape fits");
   h.ring = 0;
   {
-    // plane ring instead of a single-stage box (see HaloxParams): needs D taps and four single-plane stages.
-    // OCCD_HALOX_RING=0 keeps the box (experiment hook)
-    static const bool ring_off = [] { const char* e = getenv("OCCD_HALOX_RING"); return e && atoi(e) == 0; }();
+    // plane ring instead of a single-stage box (see HaloxParams): needs D taps and four single-plane stages
     const int PHr = HR + 2 * hal[1];
     const int plane = round_up(PHr * h.PW * RB, 1024);
-    if (!ring_off && h.stages < 2 && hal[0] == 1 && 4 * plane <= smem_total && (PHr - 1) * dil + 1 <= 256) {
+    if (h.stages < 2 && hal[0] == 1 && 4 * plane <= smem_total && (PHr - 1) * dil + 1 <= 256) {
       h.ring = 1;
       h.BD = 1; h.BH = HR; h.PD = 3; h.PH = PHr; h.nM = 1;
       h.a_stage_bytes = plane; h.stages = 4;
@@ -359,111 +387,26 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   }
   h.sD = sD;
   h.n_cols = d->B * dil * dil * h.tilesH;
-  h.pdl = pdl_enabled();
+  h.pdl = occd_pdl_enabled();
   pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(xp_stage_ld(h.N_tile)) + 128 + 1024;
+  box[0] = h.PW; box[1] = (h.PH - 1) * dil + 1; box[2] = h.ring ? 1 : (h.PD - 1) * dil + 1;   // ring: one plane per load
+  traversal[0] = 1; traversal[1] = traversal[2] = dil;
+  *n_tile = h.N_tile;
   const long long num_tiles = h.ring ? (long long)h.n_cols * sD      // ring mode: M tiles; each CTA takes a contiguous share
                                      : (long long)d->B * dil * dil * h.tilesD * h.tilesH;
-  HX_REQUIRE(num_tiles < 2147483647LL, "too many tiles");
-  const int n_sms = n_sms_current();
-  pl->grid = dim3((unsigned)(num_tiles < n_sms ? num_tiles : n_sms));
+  if (const int rc = persistent_grid(pl, num_tiles)) return rc;
   h.pp = ping_pong(h.N_tile, h.ring ? num_tiles : num_tiles * h.nM, pl->grid.x);   // M tiles per CTA
-#undef HX_REQUIRE
   return OCCD_OK;
 }
 
-static CUtensorMapSwizzle swizzle_for(int rb) {
-  return rb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (rb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-}
-
-static CUtensorMapDataType tm_dtype(int dtype) {
-  return dtype == OCCD_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-}
-
-static int halo_encode(const occd_conv_desc* d, occd_conv_plan* pl) {
-  const HaloParams& h = pl->halo;
-  const int KC = pl->kc, C = d->src_C[0], dil = h.d, es = pl->esize;
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    occd_set_last_error("occd_conv_plan_create: cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
-    return OCCD_ERR_CUDA;
-  }
-  const CUtensorMapSwizzle sw = swizzle_for(pl->rb);
-  {
-    const cuuint64_t cs = (cuuint64_t)d->src_cstride[0] * es;
-    cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)d->IW, (cuuint64_t)d->IH, (cuuint64_t)d->ID, (cuuint64_t)d->B};
-    cuuint64_t gstr[4] = {cs, cs * d->IW, cs * d->IW * d->IH, cs * d->IW * d->IH * d->ID};
-    cuuint32_t box[5] = {(cuuint32_t)KC, (cuuint32_t)((h.PW - 1) * dil + 1), (cuuint32_t)((h.PH - 1) * dil + 1),
-                         (cuuint32_t)((h.PD - 1) * dil + 1), 1};
-    cuuint32_t estr[5] = {1, (cuuint32_t)dil, (cuuint32_t)dil, (cuuint32_t)dil, 1};
-    void* base = (void*)((const char*)d->src[0] + (size_t)d->src_coff[0] * es);
-    CUresult r = enc(&pl->tmA[0], tm_dtype(pl->dtype), 5, base, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { occd_set_last_error("occd_conv_plan_create(halo): cuTensorMapEncodeTiled(source) failed"); return OCCD_ERR_CUDA; }
-  }
-  {
-    cuuint64_t gdim[2] = {(cuuint64_t)d->Kpad, (cuuint64_t)d->n_taps * d->Cout_pad};
-    cuuint64_t gstr[1] = {(cuuint64_t)d->Kpad * es};
-    cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)h.N_tile};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&pl->tmW, tm_dtype(pl->dtype), 2, (void*)d->weight, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { occd_set_last_error("occd_conv_plan_create(halo): cuTensorMapEncodeTiled(weights) failed"); return OCCD_ERR_CUDA; }
-  }
-  return OCCD_OK;
-}
-
-
-static int halox_encode(const occd_conv_desc* d, occd_conv_plan* pl) {
-  const HaloxParams& h = pl->halox;
-  const int KC = pl->kc, C = d->src_C[0], dil = h.d, es = pl->esize;
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    occd_set_last_error("occd_conv_plan_create: cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
-    return OCCD_ERR_CUDA;
-  }
-  const CUtensorMapSwizzle sw = swizzle_for(pl->rb);
-  {
-    const cuuint64_t cs = (cuuint64_t)d->src_cstride[0] * es;
-    cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)d->IW, (cuuint64_t)d->IH, (cuuint64_t)d->ID, (cuuint64_t)d->B};
-    cuuint64_t gstr[4] = {cs, cs * d->IW, cs * d->IW * d->IH, cs * d->IW * d->IH * d->ID};
-    cuuint32_t box[5] = {(cuuint32_t)KC, (cuuint32_t)h.PW, (cuuint32_t)((h.PH - 1) * dil + 1),
-                         (cuuint32_t)(h.ring ? 1 : (h.PD - 1) * dil + 1), 1};   // ring mode: one plane per load
-    cuuint32_t estr[5] = {1, 1, (cuuint32_t)dil, (cuuint32_t)dil, 1};
-    void* base = (void*)((const char*)d->src[0] + (size_t)d->src_coff[0] * es);
-    CUresult r = enc(&pl->tmA[0], tm_dtype(pl->dtype), 5, base, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { occd_set_last_error("occd_conv_plan_create(halox): cuTensorMapEncodeTiled(source) failed"); return OCCD_ERR_CUDA; }
-  }
-  {
-    cuuint64_t gdim[2] = {(cuuint64_t)d->Kpad, (cuuint64_t)d->n_taps * d->Cout_pad};
-    cuuint64_t gstr[1] = {(cuuint64_t)d->Kpad * es};
-    cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)h.N_tile};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&pl->tmW, tm_dtype(pl->dtype), 2, (void*)d->weight, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { occd_set_last_error("occd_conv_plan_create(halox): cuTensorMapEncodeTiled(weights) failed"); return OCCD_ERR_CUDA; }
-  }
-  return OCCD_OK;
-}
-
-// Per-tap (TC) plan: host arithmetic only; tc_encode builds the tensor maps.  xp: x-packed variant (TCX)
-static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
+// Per-tap (TC) plan.  xp: x-packed variant (TCX)
+static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int box[3], int traversal[3],
+                       int* n_tile) {
   int maxC = 0;
   for (int s = 0; s < d->n_src; ++s) maxC = d->src_C[s] > maxC ? d->src_C[s] : maxC;
   TcParams& t = pl->tc;
-  fill_epi(d, &t.epi);
-  const int KC = chunk_channels(maxC, pl->esize);
-  pl->kc = KC;
-  pl->rb = KC * pl->esize;
-  const int RB = pl->rb;
-  if (d->Kpad % KC != 0) {
-    occd_set_last_error("occd_conv_plan_create: Kpad must be a multiple of the K chunk");
-    return OCCD_ERR_ARG;
-  }
+  const int KC = set_k_chunk(pl, maxC), RB = pl->rb;
+  if (d->Kpad % KC != 0) return refuse(pl, OCCD_ERR_ARG, "Kpad must be a multiple of the K chunk");
   t.n_taps = xp ? d->n_taps / 3 : d->n_taps;  // x-packed: one pipeline item per (source, dz, dy) group
   const int n_groups = d->n_groups > 1 ? d->n_groups : 1;
   if (n_groups > 1) {
@@ -474,11 +417,8 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
       ok = d->group_tap0[g + 1] > d->group_tap0[g];
       for (int i = 0; i < 3; ++i) ok = ok && d->group_oadd[g][i] >= 0 && d->group_oadd[g][i] < d->omul[i];
     }
-    if (!ok) {
-      occd_set_last_error("occd_conv_plan_create: tap groups need the per-tap TC kernel, ascending non-empty tap "
-                          "ranges covering all taps, 0 <= group_oadd < omul, no second output and at most one residual");
-      return OCCD_ERR_UNSUPPORTED;
-    }
+    PLAN_REQUIRE(ok, "tap groups need the per-tap TC kernel, ascending non-empty tap ranges covering all taps, "
+                     "0 <= group_oadd < omul, no second output and at most one residual");
   }
   t.n_groups = n_groups;
   t.src_d0 = d->src_d0;
@@ -493,17 +433,13 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
   if (xp) {
     // groups of three W taps -1, 0, +1 share one MMA with N = 3 * Cout_pad; the tile is 32 positions wide (30
     // outputs + one halo column each side) so that lane == column in the epilogue
-    if (d->n_taps % 3 || d->stride[2] != 1 || 3 * d->Cout_pad > 256) {
-      occd_set_last_error("occd_conv_plan_create(tcx): needs W-tap triples, W stride 1 and 3 * Cout_pad <= 256");
-      return OCCD_ERR_UNSUPPORTED;
-    }
+    PLAN_REQUIRE(d->n_taps % 3 == 0 && d->stride[2] == 1 && 3 * d->Cout_pad <= 256,
+                 "needs W-tap triples, W stride 1 and 3 * Cout_pad <= 256");
     for (int i = 0; i < d->n_taps; i += 3) {
       const occd_conv_tap &a = d->taps[i], &b = d->taps[i + 1], &c = d->taps[i + 2];
-      if (!(a.dx == -1 && b.dx == 0 && c.dx == 1 && a.src == b.src && a.src == c.src && a.dz == b.dz &&
-            a.dz == c.dz && a.dy == b.dy && a.dy == c.dy)) {
-        occd_set_last_error("occd_conv_plan_create(tcx): taps must be ordered (src, dz, dy) groups of dx = -1, 0, +1");
-        return OCCD_ERR_UNSUPPORTED;
-      }
+      PLAN_REQUIRE(a.dx == -1 && b.dx == 0 && c.dx == 1 && a.src == b.src && a.src == c.src && a.dz == b.dz &&
+                   a.dz == c.dz && a.dy == b.dy && a.dy == c.dy,
+                   "taps must be ordered (src, dz, dy) groups of dx = -1, 0, +1");
       t.tap_src[i / 3] = (signed char)b.src;
       t.tap_dz[i / 3] = (short)b.dz; t.tap_dy[i / 3] = (short)b.dy; t.tap_dx[i / 3] = 0;
     }
@@ -560,15 +496,12 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     const double out_bytes_per_col = 128.0 * ((d->out0 ? pl->esize : 0) + (d->out1_mode == OCCD_OUT1_CL ? pl->esize : 0) +
                                               (d->out1_mode == OCCD_OUT1_F32_PLANAR ||
                                                d->out1_mode == OCCD_OUT1_CLASS_U16 ? 4 : 0));
-    // experiment hook: OCCD_EPI_RATE overrides the model's epilogue drain rate
-    static const double epi_rate = [] { const char* e = getenv("OCCD_EPI_RATE"); const double v = e ? atof(e) : 0.0;
-                                        return v > 0.0 ? v : 12.0; }();
     // per-tile mainloop and epilogue of an n-column tile that stores out_cols channels
     auto estimate = [&](int n, int out_cols, double& mainloop, double& epi) {
       const double mma = (RB / 32) * mma_step_cycles(n);
       const double load = (128.0 + n) * RB / 44.0;
       mainloop = iters * (mma > load ? mma : load);
-      epi = out_bytes_per_col * out_cols / epi_rate;
+      epi = out_bytes_per_col * out_cols / 12.0;
     };
     double best = -1.0;
     for (int n = 16; !xp && n <= 256 && n <= d->Cout_pad; n += 16) {
@@ -585,17 +518,14 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
     }
     estimate(t.N_tile, xp ? d->Cout_pad : t.N_tile, est_mainloop, est_epi);
   }
-  if (d->out1_mode == OCCD_OUT1_CLASS_U16 && !xp && t.N_tile < d->Cout_pad) {
-    occd_set_last_error("occd_conv_plan_create: a class map needs every output channel in one N tile");
-    return OCCD_ERR_UNSUPPORTED;
-  }
-  if (!(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile))) {
-    occd_set_last_error(xp ? "occd_conv_plan_create(tcx): no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)"
-                           : "occd_conv_plan_create: no kernel compiled for this N tile");
-    return OCCD_ERR_UNSUPPORTED;
-  }
+  PLAN_REQUIRE(d->out1_mode != OCCD_OUT1_CLASS_U16 || xp || t.N_tile >= d->Cout_pad,
+               "a class map needs every output channel in one N tile");
+  PLAN_REQUIRE(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile),
+               xp ? "no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)" : "no kernel compiled for this N tile");
   t.rb = RB;
-  t.pdl = pdl_enabled();
+  // programmatic dependent launch (common.cuh): the conv kernels wait on griddepcontrol after their prologue (barrier
+  // init, tensor-map prefetch overlap the tail of the previous grid); results are bit-identical either way
+  t.pdl = occd_pdl_enabled();
   t.a_bytes = 128 * RB;
   t.b_bytes = t.N_tile * RB;
   t.b_stride = round_up(t.b_bytes, 1024);
@@ -633,68 +563,82 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp) {
   pl->smem = (size_t)stages * group * stage_bytes + st_bytes + 16 * kMaxStages + 64 + 1024;  // + staging, barriers, alignment slack
   const long long m_tiles = (long long)d->B * t.tiles_d * t.tiles_h * t.tiles_w;
   const long long all_tiles = m_tiles * (xp ? 1 : d->Cout_pad / t.N_tile) * n_groups;
-  if (all_tiles > 2147483647LL) {
-    occd_set_last_error("occd_conv_plan_create: too many tiles");
-    return OCCD_ERR_UNSUPPORTED;
-  }
+  if (const int rc = persistent_grid(pl, all_tiles)) return rc;
   t.num_m_tiles = (int)m_tiles;
-  {
-    const int n_sms = n_sms_current();
-    pl->grid = dim3((unsigned)(all_tiles < n_sms ? all_tiles : n_sms));
-  }
   // ping-pong hides a tile's epilogue under the next tile's mainloop, but one warpgroup then stores a whole tile
   // alone: a launch whose epilogue outweighs its mainloop (1x1 convs over few channels, store-bound) keeps both
   // warpgroups storing at once
   t.pp = ping_pong(t.N_tile, all_tiles, pl->grid.x) && est_mainloop >= est_epi;
+  box[0] = t.TW * d->stride[2]; box[1] = t.TH * d->stride[1]; box[2] = t.TD * d->stride[0];
+  traversal[0] = d->stride[2]; traversal[1] = d->stride[1]; traversal[2] = d->stride[0];
+  *n_tile = t.N_tile;
   return OCCD_OK;
 }
 
-static int tc_encode(const occd_conv_desc* d, occd_conv_plan* pl) {
-  const TcParams& t = pl->tc;
-  const int KC = pl->kc, es = pl->esize;
-  EncodeTiledFn enc = get_encode_fn();
+// SIMT plan: one thread per output position and group of 8 channels (per position with a class map)
+static int simt_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
+  SimtParams& s = pl->simt;
+  s.n_src = d->n_src; s.n_taps = d->n_taps;
+  for (int i = 0; i < d->n_src; ++i) {
+    s.src[i] = d->src[i];
+    s.src_C[i] = d->src_C[i]; s.src_cstride[i] = d->src_cstride[i]; s.src_coff[i] = d->src_coff[i];
+  }
+  s.ID = d->ID; s.IH = d->IH; s.IW = d->IW; s.src_d0 = d->src_d0;
+  for (int i = 0; i < 3; ++i) s.stride[i] = d->stride[i];
+  s.weight = d->weight;
+  s.Cout_pad = d->Cout_pad; s.Kpad = d->Kpad;
+  s.w_batch_rows = d->weight_per_image ? d->n_taps * d->Cout_pad : 0;
+  for (int i = 0; i < d->n_taps; ++i) {
+    s.tap_src[i] = (signed char)d->taps[i].src;
+    s.tap_dz[i] = (short)d->taps[i].dz; s.tap_dy[i] = (short)d->taps[i].dy; s.tap_dx[i] = (short)d->taps[i].dx;
+  }
+  const long long total = (long long)d->B * d->OD * d->OH * d->OW *
+                          (d->out1_mode == OCCD_OUT1_CLASS_U16 ? 1 : s.epi.Cout_store / 8);
+  pl->grid = dim3((unsigned)((total + 127) / 128));
+  return OCCD_OK;
+}
+
+// One tensor map of the plan's element type, swizzled to its K-chunk row; src: the source it maps, -1 for the weights
+static int encode_map(occd_conv_plan* pl, CUtensorMap* tm, int rank, const void* base, const cuuint64_t* gdim,
+                      const cuuint64_t* gstr, const cuuint32_t* box, const cuuint32_t* estr, int src) {
+  const EncodeTiledFn enc = get_encode_fn();
   if (!enc) {
     occd_set_last_error("occd_conv_plan_create: cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
     return OCCD_ERR_CUDA;
   }
-  const CUtensorMapSwizzle sw = swizzle_for(pl->rb);
-  for (int s = 0; s < d->n_src; ++s) {
-    const cuuint64_t cs = (cuuint64_t)d->src_cstride[s] * es;
-    cuuint64_t gdim[5] = {(cuuint64_t)d->src_C[s], (cuuint64_t)d->IW, (cuuint64_t)d->IH, (cuuint64_t)d->ID,
-                          (cuuint64_t)d->B};
-    cuuint64_t gstr[4] = {cs, cs * d->IW, cs * d->IW * d->IH, cs * d->IW * d->IH * d->ID};
-    cuuint32_t box[5] = {(cuuint32_t)KC, (cuuint32_t)(t.TW * d->stride[2]), (cuuint32_t)(t.TH * d->stride[1]),
-                         (cuuint32_t)(t.TD * d->stride[0]), 1};
-    cuuint32_t estr[5] = {1, (cuuint32_t)d->stride[2], (cuuint32_t)d->stride[1], (cuuint32_t)d->stride[0], 1};
-    void* base = (void*)((const char*)d->src[s] + (size_t)d->src_coff[s] * es);
-    CUresult r = enc(&pl->tmA[s], tm_dtype(pl->dtype), 5, base, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      char msg[160];
-      snprintf(msg, sizeof(msg), "occd_conv_plan_create: cuTensorMapEncodeTiled(source %d) failed with %d", s, (int)r);
-      occd_set_last_error(msg);
-      return OCCD_ERR_CUDA;
-    }
-  }
-  for (int s = d->n_src; s < OCCD_CONV_MAX_SRC; ++s) pl->tmA[s] = pl->tmA[0];
-  {
-    cuuint64_t gdim[2] = {(cuuint64_t)d->Kpad,
-                          (cuuint64_t)d->n_taps * d->Cout_pad * (d->weight_per_image ? d->B : 1)};
-    cuuint64_t gstr[1] = {(cuuint64_t)d->Kpad * es};
-    cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)t.N_tile};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&pl->tmW, tm_dtype(pl->dtype), 2, (void*)d->weight, gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      char msg[160];
-      snprintf(msg, sizeof(msg), "occd_conv_plan_create: cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
-      occd_set_last_error(msg);
-      return OCCD_ERR_CUDA;
-    }
-  }
-  return OCCD_OK;
+  const CUresult r = enc(tm, pl->dtype == OCCD_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                         rank, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         pl->rb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                       : (pl->rb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B),
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS) return OCCD_OK;
+  char msg[160];
+  if (src < 0) snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
+  else snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(source %d) failed with %d", src, (int)r);
+  return refuse(pl, OCCD_ERR_CUDA, msg);
+}
+
+// Source s, channels-last [B][ID][IH][IW] rows of src_cstride elements, channel window [src_coff, +src_C): one K
+// chunk by the box (W, H, D), taken at the traversal strides
+static int encode_activation(occd_conv_plan* pl, const occd_conv_desc* d, int s, const int box[3],
+                             const int traversal[3]) {
+  const cuuint64_t cs = (cuuint64_t)d->src_cstride[s] * pl->esize;
+  const cuuint64_t gdim[5] = {(cuuint64_t)d->src_C[s], (cuuint64_t)d->IW, (cuuint64_t)d->IH, (cuuint64_t)d->ID,
+                              (cuuint64_t)d->B};
+  const cuuint64_t gstr[4] = {cs, cs * d->IW, cs * d->IW * d->IH, cs * d->IW * d->IH * d->ID};
+  const cuuint32_t bx[5] = {(cuuint32_t)pl->kc, (cuuint32_t)box[0], (cuuint32_t)box[1], (cuuint32_t)box[2], 1};
+  const cuuint32_t estr[5] = {1, (cuuint32_t)traversal[0], (cuuint32_t)traversal[1], (cuuint32_t)traversal[2], 1};
+  return encode_map(pl, &pl->tmA[s], 5, (const char*)d->src[s] + (size_t)d->src_coff[s] * pl->esize, gdim, gstr, bx,
+                    estr, s);
+}
+
+// The weights, [rows][Kpad]: one K chunk by box_rows (the N tile)
+static int encode_weights(occd_conv_plan* pl, const occd_conv_desc* d, long long rows, int box_rows) {
+  const cuuint64_t gdim[2] = {(cuuint64_t)d->Kpad, (cuuint64_t)rows};
+  const cuuint64_t gstr[1] = {(cuuint64_t)d->Kpad * pl->esize};
+  const cuuint32_t box[2] = {(cuuint32_t)pl->kc, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return encode_map(pl, &pl->tmW, 2, d->weight, gdim, gstr, box, estr, -1);
 }
 
 extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** out) {
@@ -761,40 +705,17 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
   pl->dtype = d->dtype;
   pl->esize = es;
 
-  if (d->impl == OCCD_CONV_IMPL_SIMT) {
-    SimtParams& s = pl->simt;
-    fill_epi(d, &s.epi);
-    s.n_src = d->n_src; s.n_taps = d->n_taps;
-    for (int i = 0; i < d->n_src; ++i) {
-      s.src[i] = d->src[i];
-      s.src_C[i] = d->src_C[i]; s.src_cstride[i] = d->src_cstride[i]; s.src_coff[i] = d->src_coff[i];
-    }
-    s.ID = d->ID; s.IH = d->IH; s.IW = d->IW; s.src_d0 = d->src_d0;
-    for (int i = 0; i < 3; ++i) s.stride[i] = d->stride[i];
-    s.weight = d->weight;
-    s.Cout_pad = d->Cout_pad; s.Kpad = d->Kpad;
-    s.w_batch_rows = d->weight_per_image ? d->n_taps * d->Cout_pad : 0;
-    for (int i = 0; i < d->n_taps; ++i) {
-      s.tap_src[i] = (signed char)d->taps[i].src;
-      s.tap_dz[i] = (short)d->taps[i].dz; s.tap_dy[i] = (short)d->taps[i].dy; s.tap_dx[i] = (short)d->taps[i].dx;
-    }
-    const long long total = (long long)d->B * d->OD * d->OH * d->OW *
-                            (d->out1_mode == OCCD_OUT1_CLASS_U16 ? 1 : s.epi.Cout_store / 8);
-    pl->grid = dim3((unsigned)((total + 127) / 128));
-    *out = pl;
-    return OCCD_OK;
-  }
-
-  int rc;
-  if (d->impl == OCCD_CONV_IMPL_HALO) {
-    rc = halo_geometry(d, pl);
-    if (rc == OCCD_OK) rc = halo_encode(d, pl);
-  } else if (d->impl == OCCD_CONV_IMPL_HALOX) {
-    rc = halox_geometry(d, pl);
-    if (rc == OCCD_OK) rc = halox_encode(d, pl);
-  } else {
-    rc = tc_geometry(d, pl, d->impl == OCCD_CONV_IMPL_TCX);
-    if (rc == OCCD_OK) rc = tc_encode(d, pl);
+  fill_epi(d, plan_epi(pl));
+  int box[3], traversal[3], n_tile;   // the tensor-core geometries' TMA boxes
+  int rc = d->impl == OCCD_CONV_IMPL_SIMT    ? simt_geometry(d, pl)
+           : d->impl == OCCD_CONV_IMPL_HALO  ? halo_geometry(d, pl, box, traversal, &n_tile)
+           : d->impl == OCCD_CONV_IMPL_HALOX ? halox_geometry(d, pl, box, traversal, &n_tile)
+                                             : tc_geometry(d, pl, d->impl == OCCD_CONV_IMPL_TCX, box, traversal, &n_tile);
+  if (rc == OCCD_OK && d->impl != OCCD_CONV_IMPL_SIMT) {
+    for (int s = 0; rc == OCCD_OK && s < d->n_src; ++s) rc = encode_activation(pl, d, s, box, traversal);
+    for (int s = d->n_src; s < OCCD_CONV_MAX_SRC; ++s) pl->tmA[s] = pl->tmA[0];
+    const long long w_rows = (long long)d->n_taps * d->Cout_pad * (d->weight_per_image ? d->B : 1);
+    if (rc == OCCD_OK) rc = encode_weights(pl, d, w_rows, n_tile);
   }
   if (rc != OCCD_OK) { delete pl; return rc; }
   *out = pl;
@@ -808,9 +729,7 @@ extern "C" int occd_conv_plan_destroy(occd_conv_plan* plan) {
 
 extern "C" int occd_conv_plan_set_class_lut(occd_conv_plan* pl, const int* lut, int n) {
   OCCD_CHECK_ARG(pl != nullptr, "occd_conv_plan_set_class_lut: null plan");
-  ConvEpi* e = pl->impl == OCCD_CONV_IMPL_SIMT ? &pl->simt.epi
-               : pl->impl == OCCD_CONV_IMPL_HALO ? &pl->halo.epi
-               : pl->impl == OCCD_CONV_IMPL_HALOX ? &pl->halox.epi : &pl->tc.epi;
+  ConvEpi* e = plan_epi(pl);
   OCCD_CHECK_ARG(e->out1_mode == OCCD_OUT1_CLASS_U16, "occd_conv_plan_set_class_lut: the plan writes no class map");
   if (!lut) {
     e->class_lut_use = 0;

@@ -24,8 +24,6 @@ struct ConvEpi {
   int out1_cstride, out1_coff, out1_C;
   int class_lut_use;   // class-map output: store class_lut[class] instead of the class (occd_conv_plan_set_class_lut)
   unsigned short class_lut[OCCD_CLASS_LUT_MAX];
-  int dbg;   // experiment switch (OCCD_DEBUG_EPI, tools/conv_bench.py only): 1 = skip the out0 stores, 2 = skip the
-             // whole row epilogue (accumulators are read, nothing is stored)
 };
 
 __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, int oh, int ow, int oa0, int oa1,
@@ -125,17 +123,9 @@ __device__ __forceinline__ void conv_epilogue_compute(const ConvEpi& e, long lon
 template <typename T, int NV>
 __device__ __forceinline__ void conv_epilogue_row(const ConvEpi& e, int b, int od, int oh, int ow, int n0,
                                                   float* v) {
-  if (e.dbg == 2) return;
   const long long pos = epi_pos(e, b, od, oh, ow);
   conv_epilogue_compute<T, NV>(e, pos, b, n0, v);
   if (!e.out0) return;
-  if (e.dbg == 1) {   // keep the arithmetic alive without storing
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) s += v[i];
-    if (s == 123456.789f) reinterpret_cast<T*>(e.out0)[0] = Elem<T>::cvt(s);
-    return;
-  }
 #pragma unroll
   for (int g = 0; g < NV; g += 8) {
     const int n = n0 + g;
@@ -248,7 +238,7 @@ __device__ __forceinline__ void epi_finish(const EpiRow<T>& e, int c0, const uin
 
 // out0 only, and at most one residual: res1 (before the activation) or a post-activation res2
 __device__ __forceinline__ bool epi_fast_ok(const ConvEpi& e) {
-  return e.out1_mode == OCCD_OUT1_NONE && e.out0 != nullptr && e.dbg <= 1 &&
+  return e.out1_mode == OCCD_OUT1_NONE && e.out0 != nullptr &&
          (e.res2 == nullptr || (e.res2_post && e.res1 == nullptr));
 }
 
@@ -259,7 +249,7 @@ __device__ __forceinline__ EpiRow<T> epi_row(const ConvEpi& e, bool valid, int b
                                              int oa0, int oa1, int oa2) {
   EpiRow<T> er;
   const long long pos = valid ? epi_pos(e, b, od, oh, ow, oa0, oa1, oa2) : 0;
-  er.out = (valid && e.dbg == 0) ? reinterpret_cast<T*>(e.out0) + pos * e.out0_cstride + e.out0_coff + n0 : nullptr;
+  er.out = valid ? reinterpret_cast<T*>(e.out0) + pos * e.out0_cstride + e.out0_coff + n0 : nullptr;
   er.res = nullptr;
   er.res_post = 0;
   if (valid && e.res1) {
