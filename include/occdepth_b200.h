@@ -29,6 +29,10 @@ extern "C" {
 /* One channel "vector" is 8 consecutive channels (32 / 16 bytes): cstride, coff and C are multiples of 8.         */
 #define OCCD_DTYPE_F32 0
 #define OCCD_DTYPE_BF16 1
+/* Element types of class maps and labels (occd_ssc_confusion only); a float32 label is OCCD_DTYPE_F32.           */
+#define OCCD_DTYPE_U8 2
+#define OCCD_DTYPE_U16 3
+#define OCCD_DTYPE_I64 4
 
 /* -------------------------------------------------------------------------------------------- */
 /* library                                                                                      */
@@ -321,6 +325,19 @@ int occd_fc_fwd(const float* in, const float* w, const float* bias, float* out, 
 /* x[b][pos][c] *= gate[b][c] in place (SELayer: x * gate(x_se), flosp_depth.py:195-199)            */
 int occd_channel_scale(void* x, const float* gate, int dtype, long long B, long long S, int C, int cstride,
                        void* stream);
+
+/* -------------------------------------------------------------------------------------------- */
+/* Evaluation: the SSC metrics' confusion matrix (SSCMetrics.add_batch, loss/sscMetrics.py:70-91, as     */
+/* OccDepth.step calls it, OccDepth.py:526-529).  pred: class map of pred_dtype OCCD_DTYPE_U16 (what       */
+/* occd_argmax_classes and the class-map epilogue write) or OCCD_DTYPE_I64 (a torch argmax); label: of     */
+/* label_dtype OCCD_DTYPE_F32 (KITTI's float32 targets; a value that is not an integer is no class),       */
+/* OCCD_DTYPE_U8 (NYU) or OCCD_DTYPE_I64.  Both contiguous, n elements (B frames are one flat array).      */
+/* counts: n_classes^2 + 1 int64, ACCUMULATED (never cleared): counts[g*n_classes + p] += voxels with       */
+/* label g and prediction p; label 255 is skipped; counts[n_classes^2] += invalid voxels (a label outside  */
+/* [0, n_classes) that is not 255, or a prediction outside [0, n_classes) where the label is not 255).     */
+/* n_classes <= 64.                                                                                        */
+int occd_ssc_confusion(const void* pred, int pred_dtype, const void* label, int label_dtype, long long n,
+                       int n_classes, long long* counts, void* stream);
 
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */

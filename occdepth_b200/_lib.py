@@ -12,6 +12,7 @@ _LIB = None
 
 MAX_SCALES = 4
 DTYPE_F32, DTYPE_BF16 = 0, 1
+DTYPE_U8, DTYPE_U16, DTYPE_I64 = 2, 3, 4
 SFA_OUT_F32_PLANAR, SFA_OUT_BF16_CL, SFA_OUT_F32_CL, SFA_OUT_TF32_CL = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU, ACT_SIGMOID = 0, 1, 2, 3, 4
 
@@ -129,6 +130,7 @@ SYMBOLS = {
     "occd_virtual_view_fwd": (C.c_int, [_vp, _vp, _vp] + [_i] * 9 + [_f, _vp]),
     "occd_upsample_bilinear_ac": (C.c_int, [_vp, _vp] + [_i] * 11 + [_vp]),
     "occd_upsample_tapsum_ac": (C.c_int, [_vp, _vp, _vp] + [_i] * 15 + [_vp]),
+    "occd_ssc_confusion": (C.c_int, [_vp, _i, _vp, _i, _ll, _i, _vp, _vp]),
 }
 
 

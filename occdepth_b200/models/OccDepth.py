@@ -4,7 +4,8 @@ Same constructor, same `forward(batch) -> dict`, same state_dict keys.  The forw
 sm_90a launches: both stereo views go through the 2D UNet as one batch, the 4-scale / 2-view Stereo-SFA lift
 is a single fused kernel writing the channels-last voxel grid the 3D UNet consumes, and the logits are written
 in the reference's NCDHW fp32 layout by the last convolution's epilogue.
-Training (`step`, losses, optimisers; OccDepth.py:378-600) is out of scope of this package.
+Evaluation (`test_step` / `validation_step` and their epoch-end hooks) counts the SSC metrics of `predict_classes` on
+the device (occdepth_b200.metrics); training (`step`, losses, optimisers; OccDepth.py:378-538) is out of scope.
 """
 import os
 
@@ -13,6 +14,7 @@ import torch.nn as nn
 
 from .. import _lib
 from ..engine import CL, FnOp, Plan, _round_up, require_cuda
+from ..metrics import SSCMetrics
 from ._base import B200Module, _to_planar
 from .SFA import SFA, lift_multiscale
 from .unet2d import UNet2D
@@ -91,6 +93,10 @@ class OccDepth(_Base, B200Module):
                                     backbone_2d_name=config.backbone_2d_name,
                                     return_up_feats=config.return_up_feats)
         self.save_hyperparameters()
+        # counted on the device by test_step / validation_step; no state_dict entries (OccDepth.py:131-133)
+        self.train_metrics = SSCMetrics(self.n_classes)
+        self.val_metrics = SSCMetrics(self.n_classes)
+        self.test_metrics = SSCMetrics(self.n_classes)
         self.init_2d_to_3d_trans(config)
         if self.dataset not in ("kitti", "NYU"):
             raise NotImplementedError(self.dataset)
@@ -128,6 +134,7 @@ class OccDepth(_Base, B200Module):
         S = [int(s) // ps for s in self.full_scene_size]
         n_lo = 0
         window = None
+        plan.x_range = None
         if slab is not None:
             # one frame, X-slab partition: this rank lifts and decodes planes [x_lo, x_hi) of the voxel grid; the
             # 2D network is replicated (its receptive field is global: SE pooling) -- SURVEY.md section 8e.  Both
@@ -142,6 +149,7 @@ class OccDepth(_Base, B200Module):
             x_lo, x_hi = slab.partition(S[0], stages)
             n_lo, N = x_lo * S[1] * S[2], (x_hi - x_lo) * S[1] * S[2]
             window = (x_lo, x_hi - x_lo)
+            plan.x_range = (x_lo * ps, x_hi * ps)     # this rank's planes of the full-resolution outputs
             S = [x_hi - x_lo, S[1], S[2]]
         virtual = V == 1 and "gt_depth" in batch                          # process_rgbs, OccDepth.py:221-229
         VL = 2 if virtual else V                                           # views seen by the lift
@@ -389,4 +397,66 @@ class OccDepth(_Base, B200Module):
         return self.class_map(res["ssc_logit"], inv_map), res
 
     def step(self, *a, **k):
-        raise NotImplementedError("occdepth_b200 implements OccDepth.forward only (training is out of scope)")
+        raise NotImplementedError("occdepth_b200 implements the forward and the evaluation hooks only (training is "
+                                  "out of scope)")
+
+    # ---- evaluation: the metric side of the reference's test / validation steps (OccDepth.py:539-580) -----------
+    def slab_x_range(self):
+        """full-resolution X planes [lo, hi) of the class map predict_classes returned on this rank under
+        enable_slab_parallel, from its plan; None without the partition"""
+        if self.__dict__.get("slab_ctx") is None:
+            return None
+        (plan, *_), = self._class_plans().values()
+        return plan.x_range
+
+    def _count(self, metric, batch):
+        """the class map of `batch` (training class ids: no remap) counted against batch["target"] on the device;
+        under the slab partition, this rank's X-slab of both"""
+        y = self.predict_classes(batch)
+        target = batch["target"]
+        xr = self.slab_x_range()
+        if xr is not None:
+            target = target[:, xr[0]:xr[1]]
+        metric.add_batch(y, target.contiguous())
+
+    def test_step(self, batch, batch_idx):
+        self._count(self.test_metrics, batch)
+
+    def validation_step(self, batch, batch_idx):
+        self._count(self.val_metrics, batch)
+
+    @staticmethod
+    def _sum_over_ranks(*metrics):
+        """under a process group of several ranks, every rank's counters become the sum over ranks (the reference
+        reports each rank's own shard under DDP; here every rank reports the whole split)"""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            for m in metrics:
+                m.all_reduce()
+
+    def validation_epoch_end(self, outputs):
+        metric_list = [("train", self.train_metrics), ("val", self.val_metrics)]
+        self._sum_over_ranks(*(m for _, m in metric_list))
+        for prefix, metric in metric_list:
+            stats = metric.get_stats()
+            for i, class_name in enumerate(self.class_names):
+                self.log("{}_SemIoU/{}".format(prefix, class_name), stats["iou_ssc"][i], sync_dist=True)
+            self.log("{}/mIoU".format(prefix), stats["iou_ssc_mean"], sync_dist=True)
+            self.log("{}/IoU".format(prefix), stats["iou"], sync_dist=True)
+            self.log("{}/Precision".format(prefix), stats["precision"], sync_dist=True)
+            self.log("{}/Recall".format(prefix), stats["recall"], sync_dist=True)
+            metric.reset()
+
+    def test_epoch_end(self, outputs):
+        classes = self.class_names
+        metric_list = [("test", self.test_metrics)]
+        self._sum_over_ranks(*(m for _, m in metric_list))
+        for prefix, metric in metric_list:
+            print("{}======".format(prefix))
+            stats = metric.get_stats()
+            print("Precision={:.4f}, Recall={:.4f}, IoU={:.4f}".format(
+                stats["precision"] * 100, stats["recall"] * 100, stats["iou"] * 100))
+            print("class IoU: {}, ".format(classes))
+            print(" ".join(["{:.4f}, "] * len(classes)).format(*(stats["iou_ssc"] * 100).tolist()))
+            print("mIoU={:.4f}".format(stats["iou_ssc_mean"] * 100))
+            metric.reset()
