@@ -339,6 +339,49 @@ int occd_channel_scale(void* x, const float* gate, int dtype, long long B, long 
 int occd_ssc_confusion(const void* pred, int pred_dtype, const void* label, int label_dtype, long long n,
                        int n_classes, long long* counts, void* stream);
 
+/* -------------------------------------------------------------------------------------------- */
+/* Evaluation: the sums behind the losses of the reference's evaluation step (OccDepth.step,              */
+/* OccDepth.py:378-533).  Each entry point ADDS its sums (float64, never cleared) to `sums`, so frames,   */
+/* batches and later slabs compose by addition; occdepth_b200/losses.py forms the losses from them.       */
+/* Per-element math is fp32; each block writes one row of fp64 partials to `work` (work_len doubles, at   */
+/* least OCCD_LOSS_WORK_BLOCKS rows of the entry point's sum count), and the rows are added in block      */
+/* order: the same inputs give bit-identical sums.                                                        */
+#define OCCD_LOSS_WORK_BLOCKS 264
+#define OCCD_SSC_LOSS_MAX_CLASSES 64
+#define OCCD_SSC_LOSS_MAX_FRUSTUMS 64
+#define OCCD_SSC_LOSS_SUMS(C, F) (6 + 3 * (C) + (F) * (C))
+/* logits: fp32 [B][C][S] (channel-planar, the ssc_logit layout); label: [B][S] of label_dtype F32, U8 or */
+/* I64 (255 = ignore; decoded as occd_ssc_confusion does); weight: fp32 [C].  Over the voxels whose label */
+/* is not 255, with t the label and p = softmax(logits) (fp32, max-subtracted):                           */
+/*   sums[0] += sum w[t] * (logsumexp - x_t)   sums[1] += sum w[t]     (labels in [0, C) only)            */
+/*   sums[2] += #voxels                        sums[3] += #invalid (label outside [0, C) or not integer)  */
+/*   sums[6 + c] += sum p_c   sums[6 + C + c] += sum p_c [t == c]   sums[6 + 2C + c] += #[t == c]         */
+/* occ_logits / occ_weight (optional, together): fp32 [B][2][S] and [2] against the cascade target        */
+/* (labels other than 0 and 255 become 1): sums[4] += sum w_occ[t'] * (logsumexp - x_t'), sums[5] += sum */
+/* w_occ[t'].  frustum_masks (optional, n_frustums > 0): uint8 / bool [B][F][S]; over EVERY voxel,        */
+/* sums[6 + 3C + f*C + c] += sum mask_f * p_c.  C <= 64, F <= 64.                                         */
+int occd_ssc_loss_sums(const float* logits, const void* label, int label_dtype, int B, int n_classes, long long S,
+                       const float* weight, const float* occ_logits, const float* occ_weight,
+                       const uint8_t* frustum_masks, int n_frustums, double* sums, double* work, long long work_len,
+                       void* stream);
+/* CRP relation loss (compute_super_CP_multilabel_loss, loss/CRP_loss.py:4-25): P_logits fp32 [B][R][M][N] */
+/* against CP_mega_matrices uint8 [B][R][N][M] (note the transpose).  Per relation r, x a logit, y its     */
+/* entry:  sums[4r] += sum y softplus(-x)   sums[4r+1] += sum (1-y) softplus(x)   sums[4r+2] += sum y      */
+/*         sums[4r+3] += #[y == 0].   R <= 16.                                                             */
+#define OCCD_CRP_MAX_RELATIONS 16
+int occd_crp_relation_sums(const float* P_logits, const uint8_t* cp, int B, int R, int M, int N, double* sums,
+                           double* work, long long work_len, void* stream);
+/* Depth classification loss (DepthClsLoss.get_depth_loss, loss/depth_loss.py:14-87): gt fp32 [n][H][W],  */
+/* prob fp32 [n][D][h][w].  Per pixel of the (h, w) map: nearest resize of gt to (h*factor, w*factor)     */
+/* (PyTorch's index rule and float scale), smallest nonzero depth of the factor x factor patch (1e5 if    */
+/* none), bin = trunc((d - (d0 - step)) / step) kept if 0 <= bin < D + 1; the pixel is foreground when    */
+/* 1 <= bin <= D:  sums[0] += sum over foreground pixels of sum_d BCE(prob_d, [d == bin - 1]) (logs       */
+/* clamped at -100), sums[1] += #foreground.  D <= 1024, factor <= 64.                                    */
+#define OCCD_DEPTH_MAX_BINS 1024
+int occd_depth_cls_sums(const float* gt, int n_maps, int H, int W, const float* prob, int D, int h, int w,
+                        int factor, double d0, double step, double* sums, double* work, long long work_len,
+                        void* stream);
+
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,

@@ -131,7 +131,20 @@ SYMBOLS = {
     "occd_upsample_bilinear_ac": (C.c_int, [_vp, _vp] + [_i] * 11 + [_vp]),
     "occd_upsample_tapsum_ac": (C.c_int, [_vp, _vp, _vp] + [_i] * 15 + [_vp]),
     "occd_ssc_confusion": (C.c_int, [_vp, _i, _vp, _i, _ll, _i, _vp, _vp]),
+    "occd_ssc_loss_sums": (C.c_int, [_vp, _vp, _i, _i, _i, _ll, _vp, _vp, _vp, _vp, _i, _vp, _vp, _ll, _vp]),
+    "occd_crp_relation_sums": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _ll, _vp]),
+    "occd_depth_cls_sums": (C.c_int, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _vp, _ll,
+                                      _vp]),
 }
+LOSS_WORK_BLOCKS = 264
+SSC_LOSS_MAX_CLASSES = SSC_LOSS_MAX_FRUSTUMS = 64
+CRP_MAX_RELATIONS = 16
+DEPTH_MAX_BINS = 1024
+
+
+def ssc_loss_sums_len(C, F):
+    """length of occd_ssc_loss_sums' sums for C classes and F frustums (OCCD_SSC_LOSS_SUMS)"""
+    return 6 + 3 * C + F * C
 
 
 def lib():

@@ -5,23 +5,17 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "ssc_labels.cuh"
 #include "../../include/occdepth_b200.h"
 
 namespace {
 
+using namespace ssc_labels;
+
 constexpr int kMaxClasses = 64;          // the class-map remap's cap: (64*64 + 1) uint32 bins = 16 KB of shared memory
 constexpr int kGroup = 8;                // elements per thread and iteration: one 16-byte load of a uint16 map
 constexpr int kThreads = 256;
-constexpr int kIgnore = -1, kInvalid = -2;
 
-// label -> class in [0, C), kIgnore (255) or kInvalid (anything else, including a float that is not an integer)
-__device__ __forceinline__ int label_class(uint8_t v, int C) { return v == 255 ? kIgnore : (v < C ? (int)v : kInvalid); }
-__device__ __forceinline__ int label_class(long long v, int C) {
-  return v == 255 ? kIgnore : ((unsigned long long)v < (unsigned long long)C ? (int)v : kInvalid);
-}
-__device__ __forceinline__ int label_class(float v, int C) {
-  return v == 255.f ? kIgnore : ((v >= 0.f && v < (float)C && v == truncf(v)) ? (int)v : kInvalid);  // NaN: invalid
-}
 __device__ __forceinline__ int pred_class(unsigned short v, int C) { return v < C ? (int)v : kInvalid; }
 __device__ __forceinline__ int pred_class(long long v, int C) {
   return (unsigned long long)v < (unsigned long long)C ? (int)v : kInvalid;

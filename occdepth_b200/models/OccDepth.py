@@ -5,7 +5,9 @@ sm_90a launches: both stereo views go through the 2D UNet as one batch, the 4-sc
 is a single fused kernel writing the channels-last voxel grid the 3D UNet consumes, and the logits are written
 in the reference's NCDHW fp32 layout by the last convolution's epilogue.
 Evaluation (`test_step` / `validation_step` and their epoch-end hooks) counts the SSC metrics of `predict_classes` on
-the device (occdepth_b200.metrics); training (`step`, losses, optimisers; OccDepth.py:378-538) is out of scope.
+the device (occdepth_b200.metrics); with OCCDEPTH_EVAL_LOSSES=1 the steps also log the reference's losses, formed on
+the device (occdepth_b200.losses).  Training (`training_step`, backward, optimisers; OccDepth.py:535-538) is out of
+scope.
 """
 import os
 
@@ -14,6 +16,7 @@ import torch.nn as nn
 
 from .. import _lib
 from ..engine import CL, FnOp, Plan, _round_up, require_cuda
+from ..losses import step_losses
 from ..metrics import SSCMetrics
 from ._base import B200Module, _to_planar
 from .SFA import SFA, lift_multiscale
@@ -74,6 +77,19 @@ class OccDepth(_Base, B200Module):
         self.infer_mode = infer_mode
         if self.infer_mode:
             self.context_prior = False
+        # the loss switches of OccDepth.step (OccDepth.py:48-69, 96, 138-147); the losses run when
+        # OCCDEPTH_EVAL_LOSSES=1.  The drop-in never trains, so cur_batch stays 0 and the sem-scal decay factor is 1
+        self.relation_loss = _get(config, "relation_loss", False)
+        self.CE_ssc_loss = _get(config, "CE_ssc_loss", False)
+        self.sem_scal_loss = _get(config, "sem_scal_loss", False)
+        self.geo_scal_loss = _get(config, "geo_scal_loss", False)
+        self.fp_loss = _get(config, "fp_loss", False)
+        self.frustum_size = _get(config, "frustum_size", 4)
+        self.sem_step_decay_loss = _get(config, "sem_step_decay_loss", False)
+        self.depth_loss_w = _get(config, "depth_loss_weight", 1.0)
+        batch_size = _get(config, "batch_size_per_gpu", 1) * _get(config, "n_gpus", 1)
+        self.total_batch = ((3834 if config.dataset == "kitti" else 795) // batch_size) * 30
+        self.cur_batch = 0
         self.use_stereo_depth_gt = _get(config, "use_stereo_depth_gt", False)
         self.use_lidar_depth_gt = _get(config, "use_lidar_depth_gt", False)
         self.use_depth_gt = _get(config, "use_depth_gt", False)
@@ -121,6 +137,9 @@ class OccDepth(_Base, B200Module):
                     "infer_mode": self.infer_mode,
                 })
                 self.flosp_depth = FlospDepth(**self.flosp_depth_conf)
+                if self.with_depth_gt:                                  # DepthClsLoss (OccDepth.py:200-204)
+                    self.depth_downsample_factor = self.flosp_depth_conf["downsample_factor"]
+                    self.depth_d_bound = list(self.flosp_depth_conf["d_bound"])
         else:
             raise NotImplementedError(f"{self.trans_2d_to_3d} is not supported yet.")
 
@@ -419,11 +438,42 @@ class OccDepth(_Base, B200Module):
             target = target[:, xr[0]:xr[1]]
         metric.add_batch(y, target.contiguous())
 
+    def sem_decay_scale(self):
+        """the sem-scal loss factor of OccDepth.step (OccDepth.py:467-470)"""
+        if self.sem_step_decay_loss:
+            return max(0.1, (1 - self.cur_batch / self.total_batch))
+        return 1.0
+
+    @staticmethod
+    def eval_losses_enabled():
+        """OCCDEPTH_EVAL_LOSSES=1: test_step / validation_step also compute and log the reference's losses (read
+        when a step runs, so an unmodified evaluation script can switch it on)"""
+        v = os.environ.get("OCCDEPTH_EVAL_LOSSES", "0")
+        if v not in ("0", "1"):
+            raise ValueError("OCCDEPTH_EVAL_LOSSES must be '0' or '1'")
+        return v == "1"
+
+    def _eval_step(self, batch, step_type, metric):
+        if not self.eval_losses_enabled():
+            self._count(metric, batch)
+            return
+        if self.__dict__.get("slab_ctx") is not None:
+            raise NotImplementedError("OCCDEPTH_EVAL_LOSSES=1 under enable_slab_parallel: the losses of an X-slab "
+                                      "partition are not computed (unset OCCDEPTH_EVAL_LOSSES to count the metrics)")
+        # the reference's OccDepth.step: one forward, the losses in its order, the metrics, then the total
+        out = self(batch)
+        losses = step_losses(self, out, batch, step_type)
+        total = losses.pop(step_type + "/loss")
+        for key, value in losses.items():
+            self.log(key, value, on_epoch=True, sync_dist=True)
+        metric.add_batch(self.class_map(out["ssc_logit"]), batch["target"].contiguous())
+        self.log(step_type + "/loss", total, on_epoch=True, sync_dist=True)
+
     def test_step(self, batch, batch_idx):
-        self._count(self.test_metrics, batch)
+        self._eval_step(batch, "test", self.test_metrics)
 
     def validation_step(self, batch, batch_idx):
-        self._count(self.val_metrics, batch)
+        self._eval_step(batch, "val", self.val_metrics)
 
     @staticmethod
     def _sum_over_ranks(*metrics):
