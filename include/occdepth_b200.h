@@ -118,6 +118,10 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
 #define OCCD_CONV_IMPL_TCX 4  /* per-tap kernel, the three W taps of each (src,dz,dy) group packed into    */
                               /* ONE MMA (N = 3*Cout_pad <= 256): taps ordered as groups of dx = -1,0,+1,   */
                               /* W stride 1, tiles 32 wide (30 outputs), epilogue sums lane-shifted partials */
+#define OCCD_CONV_IMPL_AUTO 5 /* the library picks the kernel: the first of HALOX, then HALO (convs of 3..27 {-d,0,d}  */
+                              /* taps, Cout_pad <= 64, one K chunk) or else TCX (Cout_pad >= 48), then TC, whose    */
+                              /* plan accepts the shape; TC for tap groups and per-image weights.  When all refuse, */
+                              /* TC's refusal is returned.  occd_conv_plan_impl reports the kernel chosen           */
 #define OCCD_OUT1_NONE 0
 #define OCCD_OUT1_CL 1         /* pre-activation copy, channels-last in the plan's dtype            */
 #define OCCD_OUT1_BF16_CL OCCD_OUT1_CL
@@ -202,6 +206,8 @@ int occd_conv_run(const occd_conv_plan* plan, void* stream);
 int occd_conv_plan_set_class_lut(occd_conv_plan* plan, const int* lut, int n);
 /* introspection for tests / profiling: tile box (TD,TH,TW), N tile, K chunk, stages, grid          */
 int occd_conv_plan_info(const occd_conv_plan* plan, int* info8);
+/* the kernel (OCCD_CONV_IMPL_*, never _AUTO) the plan runs on                                      */
+int occd_conv_plan_impl(const occd_conv_plan* plan, int* impl);
 /* how the plan's tensor-core kernel shares M tiles between its two MMA warpgroups (fixed by the N tile):    */
 /* ping-pong (whole tiles, alternately: one tile's epilogue runs under the next tile's MMAs) or cooperative   */
 /* (both on every tile); OCCD_CONV_SCHED_NONE for the SIMT kernel                                            */

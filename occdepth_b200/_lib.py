@@ -44,7 +44,7 @@ class SfaParams(C.Structure):
 
 
 CONV_MAX_TAPS, CONV_MAX_SRC, CONV_MAX_GROUPS = 81, 3, 8
-CONV_IMPL_TC, CONV_IMPL_SIMT, CONV_IMPL_HALO, CONV_IMPL_HALOX, CONV_IMPL_TCX = 0, 1, 2, 3, 4
+CONV_IMPL_TC, CONV_IMPL_SIMT, CONV_IMPL_HALO, CONV_IMPL_HALOX, CONV_IMPL_TCX, CONV_IMPL_AUTO = 0, 1, 2, 3, 4, 5
 OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16 = 0, 1, 2, 3
 CLASS_LUT_MAX = 64
 ERR_ARG, ERR_CUDA, ERR_UNSUPPORTED = 1, 2, 3
@@ -106,6 +106,7 @@ SYMBOLS = {
     "occd_conv_plan_destroy": (C.c_int, [_vp]),
     "occd_conv_run": (C.c_int, [_vp, _vp]),
     "occd_conv_plan_info": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "occd_conv_plan_impl": (C.c_int, [_vp, C.POINTER(C.c_int)]),
     "occd_conv_plan_schedule": (C.c_int, [_vp, C.POINTER(C.c_int)]),
     "occd_conv_plan_set_class_lut": (C.c_int, [_vp, _vp, _i]),
     "occd_conv_debug_trace": (C.c_int, [_vp]),

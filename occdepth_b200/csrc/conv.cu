@@ -219,20 +219,36 @@ static int same_grid(const occd_conv_desc* d, const occd_conv_plan* pl) {
 // TMA box and traversal strides in (W, H, D) order and the weight box's rows (the N tile); occd_conv_plan_create
 // encodes the tensor maps from them once the geometry has accepted the descriptor.
 
-// Halo-tile plan: stride-1 "same" convolution whose taps are {-d,0,d} offsets, one source, one k-chunk, one N tile.
-static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3], int traversal[3], int* n_tile) {
+// The halo kernel's shapes: stride-1 "same" convolution of one source whose taps are {-d,0,d} offsets (*dil = d), one
+// k-chunk, one compiled N tile
+static int halo_shape(const occd_conv_desc* d, const occd_conv_plan* pl, int* dil) {
   PLAN_REQUIRE(d->n_src == 1, "one source only");
   if (const int rc = same_grid(d, pl)) return rc;
   PLAN_REQUIRE(d->n_taps <= 27, "at most 27 taps");
   PLAN_REQUIRE(d->src_C[0] <= 128 / pl->esize && d->Cout_pad <= 128,
                "channel counts too large for the resident-weight scheme (one K chunk)");
-  int dil = 0;
+  PLAN_REQUIRE(HaloTiles::has(d->Cout_pad), "no kernel compiled for this Cout_pad (16, 32, 48 or 64)");
+  *dil = 0;
   for (int i = 0; i < d->n_taps; ++i) {
     const int o[3] = {abs(d->taps[i].dz), abs(d->taps[i].dy), abs(d->taps[i].dx)};
     for (int k = 0; k < 3; ++k)
-      if (o[k]) { if (!dil) dil = o[k]; PLAN_REQUIRE(o[k] == dil, "taps must be {-d,0,d} offsets"); }
+      if (o[k]) { if (!*dil) *dil = o[k]; PLAN_REQUIRE(o[k] == *dil, "taps must be {-d,0,d} offsets"); }
   }
-  PLAN_REQUIRE(dil >= 1 && dil <= 8, "dilation must be 1..8");
+  PLAN_REQUIRE(*dil >= 1 && *dil <= 8, "dilation must be 1..8");
+  return OCCD_OK;
+}
+
+// OCCD_CONV_IMPL_AUTO plans a conv of three or more taps of the halo kernel's shapes on it, and on TC where the tile
+// search below refuses it
+static bool halo_eligible(const occd_conv_desc* d, const occd_conv_plan* pl) {
+  int dil;
+  return d->n_taps >= 3 && halo_shape(d, pl, &dil) == OCCD_OK;
+}
+
+// Halo-tile plan: a conv of halo_shape, resident weights, a box of at least 50 % useful MMA rows
+static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3], int traversal[3], int* n_tile) {
+  int dil;
+  if (const int rc = halo_shape(d, pl, &dil)) return rc;
   int hal[3] = {0, 0, 0};
   for (int i = 0; i < d->n_taps; ++i) {
     if (d->taps[i].dz) hal[0] = 1;
@@ -247,7 +263,6 @@ static int halo_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3]
   h.hd = hal[0]; h.hh = hal[1]; h.hw = hal[2];
   h.n_taps = d->n_taps;
   h.N_tile = d->Cout_pad;
-  PLAN_REQUIRE(HaloTiles::has(h.N_tile), "no kernel compiled for this Cout_pad (16, 32, 48 or 64)");
   h.b_stride = round_up(h.N_tile * row_bytes, 1024);
   h.w_bytes = h.n_taps * h.b_stride;
   PLAN_REQUIRE(h.w_bytes <= 112 * 1024, "weights do not fit in shared memory");
@@ -598,14 +613,42 @@ static int simt_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
   return OCCD_OK;
 }
 
+// A fresh plan on kernel `impl`, laid out by that kernel's geometry
+static int plan_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int impl, int box[3], int traversal[3],
+                         int* n_tile) {
+  const int dtype = pl->dtype, esize = pl->esize;
+  memset(pl, 0, sizeof(*pl));
+  pl->impl = impl;
+  pl->dtype = dtype;
+  pl->esize = esize;
+  fill_epi(d, plan_epi(pl));
+  return impl == OCCD_CONV_IMPL_SIMT    ? simt_geometry(d, pl)
+         : impl == OCCD_CONV_IMPL_HALO  ? halo_geometry(d, pl, box, traversal, n_tile)
+         : impl == OCCD_CONV_IMPL_HALOX ? halox_geometry(d, pl, box, traversal, n_tile)
+                                        : tc_geometry(d, pl, impl == OCCD_CONV_IMPL_TCX, box, traversal, n_tile);
+}
+
+// OCCD_CONV_IMPL_AUTO: the kernels to try, in order; the plan runs on the first whose geometry accepts the descriptor.
+// HALOX first: its geometry's checks are its whole rule.  Then HALO where halo_eligible holds, else TCX for 48 or more
+// output channels (narrower ones run best on the halo kernels; the TCX geometry checks the rest).  TC last.  Tap groups
+// and per-image weights run on TC only.
+static int auto_candidates(const occd_conv_desc* d, occd_conv_plan* pl, int impls[3]) {
+  int n = 0;
+  if (d->n_groups <= 1 && !d->weight_per_image) {
+    impls[n++] = OCCD_CONV_IMPL_HALOX;
+    pl->impl = OCCD_CONV_IMPL_HALO;   // (names the kernel in halo_eligible's refusals)
+    if (halo_eligible(d, pl)) impls[n++] = OCCD_CONV_IMPL_HALO;
+    else if (d->Cout_pad >= 48) impls[n++] = OCCD_CONV_IMPL_TCX;
+  }
+  impls[n++] = OCCD_CONV_IMPL_TC;
+  return n;
+}
+
 // One tensor map of the plan's element type, swizzled to its K-chunk row; src: the source it maps, -1 for the weights
 static int encode_map(occd_conv_plan* pl, CUtensorMap* tm, int rank, const void* base, const cuuint64_t* gdim,
                       const cuuint64_t* gstr, const cuuint32_t* box, const cuuint32_t* estr, int src) {
   const EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    occd_set_last_error("occd_conv_plan_create: cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
-    return OCCD_ERR_CUDA;
-  }
+  if (!enc) return refuse(pl, OCCD_ERR_CUDA, "cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
   const CUresult r = enc(tm, pl->dtype == OCCD_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
                          rank, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          pl->rb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -693,25 +736,26 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
                    "occd_conv_plan_create: tap offset");
   }
   OCCD_CHECK_ARG(d->impl == OCCD_CONV_IMPL_TC || d->impl == OCCD_CONV_IMPL_SIMT || d->impl == OCCD_CONV_IMPL_HALO ||
-                 d->impl == OCCD_CONV_IMPL_TCX || d->impl == OCCD_CONV_IMPL_HALOX, "occd_conv_plan_create: impl");
-  OCCD_CHECK_ARG(d->n_groups <= 1 || d->impl == OCCD_CONV_IMPL_TC, "occd_conv_plan_create: tap groups: TC impl only");
+                 d->impl == OCCD_CONV_IMPL_TCX || d->impl == OCCD_CONV_IMPL_HALOX || d->impl == OCCD_CONV_IMPL_AUTO,
+                 "occd_conv_plan_create: impl");
+  OCCD_CHECK_ARG(d->n_groups <= 1 || d->impl == OCCD_CONV_IMPL_TC || d->impl == OCCD_CONV_IMPL_AUTO,
+                 "occd_conv_plan_create: tap groups: TC impl only");
   OCCD_CHECK_ARG(!d->weight_per_image || (d->impl != OCCD_CONV_IMPL_HALO && d->impl != OCCD_CONV_IMPL_HALOX),
                  "occd_conv_plan_create: per-image weights: TC or SIMT impl");
 
   occd_conv_plan* pl = new (std::nothrow) occd_conv_plan;
   OCCD_CHECK_ARG(pl != nullptr, "occd_conv_plan_create: out of memory");
   memset(pl, 0, sizeof(*pl));
-  pl->impl = d->impl;
   pl->dtype = d->dtype;
   pl->esize = es;
 
-  fill_epi(d, plan_epi(pl));
+  int impls[3] = {d->impl};
+  const int n_impls = d->impl == OCCD_CONV_IMPL_AUTO ? auto_candidates(d, pl, impls) : 1;
   int box[3], traversal[3], n_tile;   // the tensor-core geometries' TMA boxes
-  int rc = d->impl == OCCD_CONV_IMPL_SIMT    ? simt_geometry(d, pl)
-           : d->impl == OCCD_CONV_IMPL_HALO  ? halo_geometry(d, pl, box, traversal, &n_tile)
-           : d->impl == OCCD_CONV_IMPL_HALOX ? halox_geometry(d, pl, box, traversal, &n_tile)
-                                             : tc_geometry(d, pl, d->impl == OCCD_CONV_IMPL_TCX, box, traversal, &n_tile);
-  if (rc == OCCD_OK && d->impl != OCCD_CONV_IMPL_SIMT) {
+  int rc = OCCD_OK;
+  for (int i = 0; i < n_impls; ++i)   // when every candidate refuses, the last (TC) refusal is returned
+    if ((rc = plan_geometry(d, pl, impls[i], box, traversal, &n_tile)) == OCCD_OK) break;
+  if (rc == OCCD_OK && pl->impl != OCCD_CONV_IMPL_SIMT) {
     for (int s = 0; rc == OCCD_OK && s < d->n_src; ++s) rc = encode_activation(pl, d, s, box, traversal);
     for (int s = d->n_src; s < OCCD_CONV_MAX_SRC; ++s) pl->tmA[s] = pl->tmA[0];
     const long long w_rows = (long long)d->n_taps * d->Cout_pad * (d->weight_per_image ? d->B : 1);
@@ -766,6 +810,12 @@ extern "C" int occd_conv_plan_info(const occd_conv_plan* pl, int* info) {
   info[0] = pl->tc.TD; info[1] = pl->tc.TH; info[2] = pl->tc.TW; info[3] = pl->tc.N_tile;
   info[4] = pl->kc; info[5] = pl->tc.stages * 100 + pl->tc.group; info[6] = (int)pl->grid.x;
   info[7] = pl->tc.num_m_tiles * (pl->impl == OCCD_CONV_IMPL_TCX ? 1 : pl->tc.Cout_pad / pl->tc.N_tile);
+  return OCCD_OK;
+}
+
+extern "C" int occd_conv_plan_impl(const occd_conv_plan* pl, int* impl) {
+  OCCD_CHECK_ARG(pl && impl, "occd_conv_plan_impl: null");
+  *impl = pl->impl;
   return OCCD_OK;
 }
 

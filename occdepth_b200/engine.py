@@ -58,60 +58,14 @@ def chunk_channels(C_, esize):
 
 
 def default_impl():
-    """'auto' (default): halo-tile wgmma kernel where the shape qualifies, the x-packed per-tap kernel for
-    narrow-output convs with W taps, else the per-tap wgmma kernel; 'tc' / 'tcx' / 'halo' / 'simt' force one
-    implementation (simt = CUDA-core cross-check)."""
+    """'auto' (default): None, the library picks the kernel per convolution (OCCD_CONV_IMPL_AUTO: the halo-tile
+    kernels where the shape qualifies, the x-packed per-tap kernel for wider outputs with W taps, else the per-tap
+    wgmma kernel); 'tc' / 'tcx' / 'halo' / 'halox' / 'simt' force one implementation (simt = CUDA-core cross-check)."""
     v = os.environ.get("OCCDEPTH_CONV_IMPL", "auto").lower()
     if v not in ("auto", "tc", "simt", "halo", "halox", "tcx"):
         raise ValueError("OCCDEPTH_CONV_IMPL must be 'auto', 'tc', 'tcx', 'halo', 'halox' or 'simt'")
     return {"auto": None, "tc": _lib.CONV_IMPL_TC, "simt": _lib.CONV_IMPL_SIMT, "halo": _lib.CONV_IMPL_HALO,
             "halox": _lib.CONV_IMPL_HALOX, "tcx": _lib.CONV_IMPL_TCX}[v]
-
-
-def halox_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf):
-    """shape test mirroring halox_geometry (csrc/conv.cu): stride-1 'same' conv on a grid whose innermost extent W is
-    8 / 16 / 32, taps = (dz, dy) groups of dx = -d, 0, +d with dz, dy in {-d, 0, d}, one K chunk, 3*Cout_pad <= 256"""
-    if len(srcs) != 1 or weight_buf is not None or len(taps) % 3 or not 3 <= len(taps) <= 27:
-        return False
-    if tuple(stride) != (1, 1, 1) or tuple(omul) != (1, 1, 1) or tuple(out_dims) != tuple(srcs[0].dims[1:]):
-        return False
-    if srcs[0].dims[3] not in (8, 16, 32) or srcs[0].C > 128 // srcs[0].esize or 3 * Cout_pad > 256:
-        return False
-    d = taps[2][3]
-    if d < 1 or d >= srcs[0].dims[3]:
-        return False
-    for i in range(0, len(taps), 3):
-        a, b, c = taps[i], taps[i + 1], taps[i + 2]
-        if not (a[:3] == b[:3] == c[:3] and (a[3], b[3], c[3]) == (-d, 0, d)):
-            return False
-        if a[1] not in (-d, 0, d) or a[2] not in (-d, 0, d):
-            return False
-    return True
-
-
-def tcx_eligible(taps, stride, Cout_pad):
-    """(src, dz, dy) groups of three W taps -1, 0, +1 (what conv_taps emits for a dense 3-wide kernel), W stride 1,
-    N = 3*Cout_pad <= 256, and enough output channels that the packed MMA beats three narrow ones (narrow outputs go
-    to the halo kernel)"""
-    if len(taps) % 3 or 3 * Cout_pad > 256 or Cout_pad < 48 or stride[2] != 1:
-        return False
-    for i in range(0, len(taps), 3):
-        a, b, c = taps[i], taps[i + 1], taps[i + 2]
-        if not (a[:3] == b[:3] == c[:3] and (a[3], b[3], c[3]) == (-1, 0, 1)):
-            return False
-    return True
-
-
-def halo_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf):
-    """shape test mirroring halo_geometry (csrc/conv.cu): stride-1 'same' conv, {-d,0,d} taps, one K chunk"""
-    if len(srcs) != 1 or weight_buf is not None or len(taps) < 3 or len(taps) > 27:
-        return False
-    if tuple(stride) != (1, 1, 1) or tuple(omul) != (1, 1, 1) or tuple(out_dims) != tuple(srcs[0].dims[1:]):
-        return False
-    if srcs[0].C > 128 // srcs[0].esize or Cout_pad > 64:
-        return False
-    offs = {abs(o) for t in taps for o in t[1:] if o}
-    return len(offs) == 1
 
 
 def require_cuda(t, what):
@@ -282,18 +236,9 @@ class ConvOp:
         d = _lib.ConvDesc()
         if impl is None:
             impl = default_impl()
-        auto = impl is None
         if groups:
-            auto, impl = False, _lib.CONV_IMPL_TC
-        if auto:
-            impl = (_lib.CONV_IMPL_HALO if halo_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf)
-                    else _lib.CONV_IMPL_TC)
-            if impl == _lib.CONV_IMPL_TC and tcx_eligible(taps, stride, Cout_pad):
-                impl = _lib.CONV_IMPL_TCX
-            if halox_eligible(srcs, taps, stride, omul, out_dims, Cout_pad, weight_buf):
-                self._fallback = impl
-                impl = _lib.CONV_IMPL_HALOX
-        d.impl = impl
+            impl = _lib.CONV_IMPL_TC
+        d.impl = _lib.CONV_IMPL_AUTO if impl is None else impl
         d.dtype = LIB_DTYPE[precision_of(adt)]
         d.n_src = len(srcs)
         for i, s in enumerate(srcs):
@@ -350,20 +295,13 @@ class ConvOp:
         self.flops = 2 * B * OD * OH * OW * Cout * sum(srcs[t[0]].C for t in taps)
         h = C.c_void_p()
         rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
-        if rc != 0 and auto and d.impl == _lib.CONV_IMPL_HALOX:
-            d.impl = self._fallback         # geometry declined (e.g. weights + one stage do not fit)
-            rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
-        if rc != 0 and auto and d.impl == _lib.CONV_IMPL_TCX:
-            d.impl = _lib.CONV_IMPL_TC
-            rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
-        if rc != 0 and auto and d.impl == _lib.CONV_IMPL_HALO:
-            d.impl = _lib.CONV_IMPL_TC      # shape did not fit the halo scheme: per-tap wgmma kernel
-            rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
         if rc == _lib.ERR_UNSUPPORTED and out1_mode == "classes":
             raise ClassMapUnsupported("occd_conv_plan_create(%s): %s" % (name, _lib.lib().occd_last_error().decode()))
         _lib.check(rc, "occd_conv_plan_create(%s)" % name)
         self.handle = h
-        self.impl = d.impl
+        impl = C.c_int()
+        _lib.check(_lib.lib().occd_conv_plan_impl(h, C.byref(impl)), "occd_conv_plan_impl")
+        self.impl = impl.value
         if lut is not None:
             self._lut = (C.c_int * len(lut))(*[int(v) for v in lut])
             _lib.check(_lib.lib().occd_conv_plan_set_class_lut(h, self._lut, len(lut)),
@@ -628,7 +566,3 @@ class FnOp:
 
     def run(self, stream):
         _lib.check(self.fn(stream), self.name)
-
-
-def kpad_for(C_, esize=2):
-    return _round_up(C_, chunk_channels(C_, esize))

@@ -8,7 +8,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..engine import CL, ConvOp, FnOp, fold_bn, kpad_for, out_size, _round_up
+from ..engine import CL, ConvOp, FnOp, fold_bn, out_size, _round_up
 from ._base import B200Module
 from .modules import ASPP, Process
 

@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..engine import ConvOp, FnOp, fold_bn, kpad_for, _round_up
+from ..engine import ConvOp, FnOp, fold_bn, _round_up
 
 ARCH = [("ds", 1, 3, 1, 1, 16), ("ir", 2, 3, 2, 6, 24), ("ir", 2, 5, 2, 6, 40), ("ir", 3, 3, 2, 6, 80),
         ("ir", 3, 5, 1, 6, 112), ("ir", 4, 5, 2, 6, 192), ("ir", 1, 3, 1, 6, 320)]

@@ -4,6 +4,7 @@ against the reference's published layer arithmetic (SURVEY.md section 0: 3-D UNe
 + 4.3 GMAC bmm) and the automatic halo-exchange insertion of the X-slab partition (24 exchanges, 1/8 of the work)."""
 import contextlib
 import io
+import re
 
 import pytest
 import torch
@@ -119,16 +120,40 @@ def test_occdepth_config2_slab_plan_shards_2d_net_by_view(simt, monkeypatch):
     assert full.flops > 2.5 * ents[1][0].flops
 
 
-def test_variant_eligibility_rules():
-    """host-side kernel selection rules (engine.py) on the shapes they were written for"""
+def _picked(build, precision="tf32"):
+    """the kernel occd_conv_plan_create plans build(plan)'s conv on: without a driver the tensor-map encode, the first
+    step after the choice, fails and names it"""
+    from occdepth_b200.engine import Plan
+    plan = Plan(torch.device("cpu"), precision=precision)
+    with pytest.raises(RuntimeError, match="cuTensorMapEncodeTiled unavailable") as ei:
+        build(plan)
+    return re.search(r"occd_conv_plan_create\((\w+)\): cuTensorMapEncodeTiled", str(ei.value)).group(1)
+
+
+def _conv(dims, ci, co, k, dilation=1, stride=1, impl=None):
+    """a 'same' conv of one image of grid dims"""
+    return lambda plan: plan.conv(plan.alloc(1, *dims, ci), torch.randn(co, ci, *k), torch.randn(co), stride=stride,
+                                  padding=tuple(dilation * (kk // 2) for kk in k), dilation=dilation, impl=impl)
+
+
+def test_auto_kernel_choice_rules(monkeypatch):
+    """the library's automatic kernel choice (OCCD_CONV_IMPL_AUTO) on the shapes its rules were written for"""
     from occdepth_b200 import engine as E
-    t333 = [(0, a, b, c) for a in (-1, 0, 1) for b in (-1, 0, 1) for c in (-1, 0, 1)]
-    t333_d2 = [(0, 2 * a, 2 * b, 2 * c) for a in (-1, 0, 1) for b in (-1, 0, 1) for c in (-1, 0, 1)]
-    two_src = [(s, 0, b, c) for s in (0, 1) for b in (-1, 0, 1) for c in (-1, 0, 1)]
-    assert E.tcx_eligible(t333, (1, 1, 1), 80) and E.tcx_eligible(two_src, (1, 1, 1), 80)
-    assert not E.tcx_eligible(t333_d2, (1, 1, 1), 64)        # W dilation 2: per-tap kernel has no sub-grids
-    assert not E.tcx_eligible(t333, (1, 1, 2), 64) and not E.tcx_eligible(t333, (1, 1, 1), 96)
-    assert not E.tcx_eligible(t333, (1, 1, 1), 32)           # narrow outputs: the halo kernel's shapes
+    monkeypatch.delenv("OCCDEPTH_CONV_IMPL", raising=False)
+    # (src, dz, dy) groups of W taps -1, 0, +1 and 48 <= Cout_pad <= 80: the x-packed per-tap kernel (W = 40 and 80
+    # output channels rule out both halo kernels)
+    assert _picked(_conv((4, 8, 40), 32, 80, (3, 3, 3))) == "tcx"
+
+    def two_src(plan):
+        xs = [plan.alloc(1, 4, 8, 40, 32) for _ in range(2)]
+        plan.conv_multi(xs, [torch.randn(80, 32, 1, 3, 3) for _ in xs], torch.randn(80), [(0, 1, 1)] * 2, [1, 1])
+    assert _picked(two_src) == "tcx"
+    # 64 tf32 source channels rule out the halo kernels: the per-tap kernel unless TCX applies
+    assert _picked(_conv((4, 8, 40), 64, 64, (3, 3, 3), dilation=2)) == "tc"     # W dilation 2: no sub-grids in TCX
+    assert _picked(_conv((4, 8, 40), 64, 64, (3, 3, 3), stride=(1, 1, 2))) == "tc"
+    assert _picked(_conv((4, 8, 40), 32, 96, (3, 3, 3))) == "tc"                 # N = 3 * 96 > 256
+    assert _picked(_conv((4, 8, 40), 64, 32, (3, 3, 3))) == "tc"                 # narrow outputs: not TCX ...
+    assert _picked(_conv((1, 24, 40), 32, 32, (1, 3, 3))) == "halo"              # ... but the halo kernel's shapes
     # K chunk = one swizzled smem row of 32 / 64 / 128 bytes
     assert [E.chunk_channels(c, 2) for c in (3, 16, 17, 32, 33, 64, 65, 2784)] == [16, 16, 32, 32, 64, 64, 64, 64]
     assert [E.chunk_channels(c, 4) for c in (3, 8, 9, 16, 17, 32, 33, 2784)] == [8, 8, 16, 16, 32, 32, 32, 32]
@@ -137,6 +162,45 @@ def test_variant_eligibility_rules():
     r = E.round_tf32_(t.clone())
     assert r.tolist()[:4] == [1.0, 1.0 + 2.0 ** -10, 1.0 + 2.0 ** -10, -(1.0 + 2.0 ** -10)]
     assert torch.equal(r.view(torch.int32) & 0x1FFF, torch.zeros(6, dtype=torch.int32))
+
+
+def test_auto_kernel_order(monkeypatch):
+    """OCCD_CONV_IMPL_AUTO tries HALOX, then HALO for the halo kernel's shapes or else TCX, then TC, and plans the first
+    whose geometry accepts; TC only for tap groups and per-image weights; an explicit kernel is kept"""
+    import ctypes as C
+    from occdepth_b200 import _lib
+    from occdepth_b200.engine import Plan
+    monkeypatch.delenv("OCCDEPTH_CONV_IMPL", raising=False)
+    assert _picked(_conv((8, 16, 32), 32, 32, (3, 3, 3))) == "halox"
+    # tf32: HALOX cannot hold nine resident 240-row weight slices, HALO has no 80-channel tile: TCX
+    assert _picked(_conv((8, 16, 32), 32, 80, (3, 3, 3))) == "tcx"
+    # a halo-kernel shape whose tile search finds no box (a 2^3 grid fills < 50 % of the MMA rows): TC, not TCX
+    assert _picked(_conv((2, 2, 2), 16, 64, (3, 3, 3))) == "tc"
+    assert _picked(_conv((8, 16, 32), 32, 32, (3, 3, 3), impl=_lib.CONV_IMPL_TC)) == "tc"
+    plan = Plan(torch.device("cpu"), precision="tf32")
+    _conv((8, 16, 32), 32, 32, (3, 3, 3), impl=_lib.CONV_IMPL_SIMT)(plan)
+    assert plan.ops[0].impl == _lib.CONV_IMPL_SIMT
+    L = _lib.lib()
+
+    def auto(d):
+        """the kernel AUTO picks for descriptor d"""
+        d.impl = _lib.CONV_IMPL_AUTO
+        assert L.occd_conv_plan_create(C.byref(d), C.byref(C.c_void_p())) == _lib.ERR_CUDA
+        return re.search(r"occd_conv_plan_create\((\w+)\)", L.occd_last_error().decode()).group(1)
+
+    def desc():
+        return _lib.ConvDesc.from_buffer_copy(plan.ops[0].desc)
+    assert auto(desc()) == "halox"
+    d = desc()
+    d.weight_per_image = 1
+    assert auto(d) == "tc"
+    d = desc()                  # two tap groups, written to the even and the odd positions of a twice finer grid
+    d.n_groups = 2
+    d.group_tap0[:3] = [0, 9, 27]
+    d.group_oadd[1][:] = [1, 1, 1]
+    d.omul[:] = [2, 2, 2]
+    d.ODf, d.OHf, d.OWf = 16, 32, 64
+    assert auto(d) == "tc"
 
 
 @pytest.mark.parametrize("precision", ["tf32", "bf16"])
