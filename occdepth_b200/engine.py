@@ -270,6 +270,11 @@ class ConvOp:
         d.res2_post = 1 if res2_post else 0
         d.out0_exact = 1 if out0_exact else 0
         self._keep = [srcs, out0, res1, res2, out1]
+        # the tensors behind the descriptor's pointers, by role: a planned launch can be inspected and replayed alone
+        self.srcs, self.out0, self.res1, self.res2 = list(srcs), out0, res1, res2
+        self.out1, self.out1_mode = out1, out1_mode
+        self.weight_runtime = weight_buf is not None      # `weight` is written by another launch of the plan
+        self.lut = None if lut is None else tuple(int(v) for v in lut)
         if out0 is not None:
             assert out0.dims == (B,) + fd and out0.C >= Cout and out0.buf.dtype == adt, (out0.dims, fd, out0.C, Cout)
             d.out0, d.out0_cstride, d.out0_coff = out0.ptr, out0.cstride, out0.coff
