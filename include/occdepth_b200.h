@@ -257,6 +257,17 @@ int occd_vox2pix_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, con
 /* Normalize of the datasets (data/semantic_kitti/kitti_dataset.py:164-171,376-402); mean/std: HOST    */
 int occd_normalize_rgb_u8(const void* in, float* out, int H0, int W0, int H, int W, const float* mean,
                           const float* stdv, void* stream);
+/* the same pre-processing written straight into the forward's channels-last image buffer: n uint8 RGB images     */
+/* (device; image i, row y starts at in + i*img_stride + y*row_stride bytes, pixels are 3 contiguous bytes) of     */
+/* raw size H0 x W0 -> out [n][H][W][cstride] of out_dtype (OCCD_DTYPE_F32: TF32 values, OCCD_DTYPE_BF16), the top- */
+/* left H x W crop.  Bit for bit occd_planar_to_cl(occd_normalize_rgb_u8(image i)) for every image; channels        */
+/* [3, cstride) are written as zeros.  cstride: multiple of 8; out 16-byte aligned; mean/std: HOST                  */
+int occd_stage_rgb_u8_cl(const void* in, long long img_stride, long long row_stride, int n, int H0, int W0, int H,
+                         int W, const float* mean, const float* stdv, void* out, int out_dtype, int cstride,
+                         void* stream);
+/* NYU's depth map (data/NYU/nyu_dataset.py:42-48 load_depth): out[i] = float32(in[i] / divisor) (the division in   */
+/* float64), clamped to [0, max_depth] in float32; in: n uint16 (device), out: n float32 (device)                  */
+int occd_depth_u16_to_f32(const void* in, float* out, long long n, double divisor, float max_depth, void* stream);
 
 /* -------------------------------------------------------------------------------------------- */
 /* EfficientNet / decoder bandwidth kernels (channels-last 2-D maps of element type `dtype`)       */

@@ -56,3 +56,41 @@ extern "C" int occd_normalize_rgb_u8(const void* in, float* out, int H0, int W0,
   OCCD_CHECK_LAUNCH();
   return OCCD_OK;
 }
+
+// occd_stage_rgb_u8_cl: n uint8 HWC images -> the forward's channels-last input [n][H][W][cstride], equal to
+// occd_planar_to_cl(occd_normalize_rgb_u8(image)) in one pass
+extern "C" int occd_stage_rgb_u8_cl(const void* in, long long img_stride, long long row_stride, int n, int H0, int W0,
+                                    int H, int W, const float* mean, const float* stdv, void* out, int out_dtype,
+                                    int cstride, void* stream) {
+  OCCD_CHECK_ARG(in && out && mean && stdv, "occd_stage_rgb_u8_cl: null argument");
+  OCCD_CHECK_ARG(n > 0 && H > 0 && W > 0 && H <= H0 && W <= W0,
+                 "occd_stage_rgb_u8_cl: the crop must lie inside the image");
+  OCCD_CHECK_ARG(row_stride >= 3LL * W0 && (n == 1 || img_stride >= (long long)(H0 - 1) * row_stride + 3LL * W0),
+                 "occd_stage_rgb_u8_cl: strides overlap the rows / images");
+  OCCD_CHECK_ARG(cstride >= 8 && cstride % 8 == 0, "occd_stage_rgb_u8_cl: cstride must be a multiple of 8");
+  OCCD_CHECK_ARG(reinterpret_cast<uintptr_t>(out) % 16 == 0, "occd_stage_rgb_u8_cl: out must be 16-byte aligned");
+  nrm::StageArgs a;
+  a.in = (const unsigned char*)in; a.img_stride = img_stride; a.row_stride = row_stride;
+  a.out = out; a.H = H; a.W = W; a.cstride = cstride;
+  for (int c = 0; c < 3; ++c) { a.mean[c] = mean[c]; a.stdv[c] = stdv[c]; }
+  const long long total = (long long)n * H * W;
+  OCCD_CHECK_ARG((total + 255) / 256 <= 2147483647LL, "occd_stage_rgb_u8_cl: too many pixels");
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (out_dtype == OCCD_DTYPE_BF16) nrm::stage_rgb_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(a, total);
+  else if (out_dtype == OCCD_DTYPE_F32) nrm::stage_rgb_kernel<float><<<grid, 256, 0, st>>>(a, total);
+  else { occd_set_last_error("occd_stage_rgb_u8_cl: dtype"); return OCCD_ERR_ARG; }
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+
+// occd_depth_u16_to_f32: NYU's load_depth (data/NYU/nyu_dataset.py:42-48) of a decoded uint16 depth PNG
+extern "C" int occd_depth_u16_to_f32(const void* in, float* out, long long n, double divisor, float max_depth,
+                                     void* stream) {
+  OCCD_CHECK_ARG(in && out && n > 0 && divisor > 0, "occd_depth_u16_to_f32: bad args");
+  OCCD_CHECK_ARG((n + 255) / 256 <= 2147483647LL, "occd_depth_u16_to_f32: too many pixels");
+  nrm::depth_u16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      (const unsigned short*)in, out, n, divisor, max_depth);
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}

@@ -36,33 +36,56 @@ def volume_dims(vox_origin, voxel_size, scene_size):
     return np.ceil((vol_bnds[:, 1] - vol_bnds[:, 0]) / voxel_size).copy(order="C").astype(int)
 
 
-def vox2pix(cam_E, cam_k, vox_origin, voxel_size, img_W, img_H, scene_size, pattern_id, device=None):
-    """occdepth.data.utils.helpers.vox2pix on the GPU (see module docstring).  Raises if no CUDA device."""
-    dev = torch.device("cuda" if device is None else device)
+def _require_cuda(dev, what):
     if dev.type != "cuda" or not torch.cuda.is_available():
-        raise RuntimeError("occdepth_b200.data.vox2pix runs on CUDA (sm_90a) only -- there is no CPU fallback")
+        raise RuntimeError("occdepth_b200.data.%s runs on CUDA (sm_90a) only -- there is no CPU fallback" % what)
+
+
+def pose_is_f32(cam_E):
+    """np.dot(cam_E, [pts 1]) stays in float32 for a float32 pose; every other pose is applied in float64"""
+    return np.asarray(cam_E).dtype == np.float32
+
+
+def vox2pix_into(pix, fov, pix_z, cam_E, cam_k, vox_origin, voxel_size, img_W, img_H, scene_size, pattern_id):
+    """vox2pix into caller-owned CUDA buffers (no allocation): pix int64 (N, P, 2), fov bool (N, P), pix_z: N values
+    of the pose's precision (float32 for a float32 pose, else float64; any buffer of that many bytes).  Enqueued on
+    the current stream of pix's device."""
     if not 0 <= int(pattern_id) < len(PIXEL_PATTERNS):
         raise IndexError("pattern_id out of range")        # the reference indexes the same 9-entry list
     X, Y, Z = (int(v) for v in volume_dims(vox_origin, voxel_size, scene_size))
-    E = np.asarray(cam_E)
-    f32_pose = E.dtype == np.float32          # np.dot(cam_E, [pts 1]) stays in float32 for a float32 pose
-    E = np.ascontiguousarray(E.astype(np.float32 if f32_pose else np.float64))
+    f32_pose = pose_is_f32(cam_E)
+    E = np.ascontiguousarray(np.asarray(cam_E).astype(np.float32 if f32_pose else np.float64))
     k32 = np.ascontiguousarray(np.asarray(cam_k).astype(np.float32))         # fusion.py:331 intr.astype(float32)
     o32 = np.ascontiguousarray(np.asarray(vox_origin).astype(np.float32))    # fusion.py:205
     if E.shape != (4, 4) or k32.shape != (3, 3) or o32.shape != (3,):
         raise ValueError("vox2pix: cam_E must be 4x4, cam_k 3x3, vox_origin (3,)")
     pat = np.ascontiguousarray(np.asarray(PIXEL_PATTERNS[int(pattern_id)], dtype=np.int32))
     P, N = len(pat), X * Y * Z
+    if (tuple(pix.shape) != (N, P, 2) or pix.dtype != torch.int64 or tuple(fov.shape) != (N, P)
+            or fov.dtype != torch.bool or not (pix.is_contiguous() and fov.is_contiguous())
+            or pix_z.numel() * pix_z.element_size() < N * (4 if f32_pose else 8)):
+        raise ValueError("vox2pix_into: the buffers do not hold a (%d, %d) index grid" % (N, P))
+    rc = _lib.lib().occd_vox2pix_fwd(E.ctypes.data_as(C.c_void_p), 1 if f32_pose else 0,
+                                     k32.ctypes.data_as(C.c_void_p),
+                                     o32.ctypes.data_as(C.c_void_p), float(voxel_size), X, Y, Z, int(img_W),
+                                     int(img_H), pat.ctypes.data_as(C.c_void_p), P, pix.data_ptr(),
+                                     fov.data_ptr(), pix_z.data_ptr(), _lib.stream_ptr())
+    _lib.check(rc, "occd_vox2pix_fwd")
+
+
+def vox2pix(cam_E, cam_k, vox_origin, voxel_size, img_W, img_H, scene_size, pattern_id, device=None):
+    """occdepth.data.utils.helpers.vox2pix on the GPU (see module docstring).  Raises if no CUDA device."""
+    dev = torch.device("cuda" if device is None else device)
+    _require_cuda(dev, "vox2pix")
+    if not 0 <= int(pattern_id) < len(PIXEL_PATTERNS):
+        raise IndexError("pattern_id out of range")
+    X, Y, Z = (int(v) for v in volume_dims(vox_origin, voxel_size, scene_size))
+    P, N = len(PIXEL_PATTERNS[int(pattern_id)]), X * Y * Z
     with torch.cuda.device(dev):
         pix = torch.empty(N, P, 2, dtype=torch.int64, device=dev)
         fov = torch.empty(N, P, dtype=torch.bool, device=dev)
-        pix_z = torch.empty(N, dtype=torch.float32 if f32_pose else torch.float64, device=dev)
-        rc = _lib.lib().occd_vox2pix_fwd(E.ctypes.data_as(C.c_void_p), 1 if f32_pose else 0,
-                                         k32.ctypes.data_as(C.c_void_p),
-                                         o32.ctypes.data_as(C.c_void_p), float(voxel_size), X, Y, Z, int(img_W),
-                                         int(img_H), pat.ctypes.data_as(C.c_void_p), P, pix.data_ptr(),
-                                         fov.data_ptr(), pix_z.data_ptr(), _lib.stream_ptr())
-        _lib.check(rc, "occd_vox2pix_fwd")
+        pix_z = torch.empty(N, dtype=torch.float32 if pose_is_f32(cam_E) else torch.float64, device=dev)
+        vox2pix_into(pix, fov, pix_z, cam_E, cam_k, vox_origin, voxel_size, img_W, img_H, scene_size, pattern_id)
     return pix, fov, pix_z
 
 
@@ -75,8 +98,7 @@ def normalize_rgb(img_u8, img_H, img_W, mean=IMAGENET_MEAN, std=IMAGENET_STD, de
     `normalize_rgb((np.array(img, np.float32) / 255.0)[:img_H, :img_W])` of kitti_dataset.py:376-402
     (ToTensor + Normalize).  The host->device copy is the uint8 image (4x smaller than the float tensor)."""
     dev = torch.device("cuda" if device is None else device)
-    if dev.type != "cuda" or not torch.cuda.is_available():
-        raise RuntimeError("occdepth_b200.data.normalize_rgb runs on CUDA (sm_90a) only -- there is no CPU fallback")
+    _require_cuda(dev, "normalize_rgb")
     t = torch.as_tensor(np.asarray(img_u8) if not isinstance(img_u8, torch.Tensor) else img_u8)
     if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
         raise ValueError("normalize_rgb: expected a uint8 (H, W, 3) RGB image")
@@ -91,3 +113,42 @@ def normalize_rgb(img_u8, img_H, img_W, mean=IMAGENET_MEAN, std=IMAGENET_STD, de
                                               _lib.stream_ptr())
         _lib.check(rc, "occd_normalize_rgb_u8")
     return out
+
+
+def stage_rgb_u8(imgs_u8, out, out_dtype, img_H, img_W, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """`normalize_rgb` of n images written straight into a channels-last buffer: imgs_u8 a CUDA uint8 (n, H0, W0, 3)
+    tensor (any image / row strides, pixels 3 contiguous bytes), out a CUDA tensor [n, ..., img_H, img_W, cstride] of
+    the activation type `out_dtype` (_lib.DTYPE_F32: TF32 values, _lib.DTYPE_BF16).  Bit for bit
+    `occd_planar_to_cl(normalize_rgb(image))`, pad channels zero (`occd_stage_rgb_u8_cl`); enqueued on the current
+    stream, no allocation."""
+    if not (imgs_u8.is_cuda and imgs_u8.dtype == torch.uint8 and imgs_u8.dim() == 4 and imgs_u8.shape[3] == 3
+            and imgs_u8.stride(3) == 1 and imgs_u8.stride(2) == 3):
+        raise ValueError("stage_rgb_u8: expected a CUDA uint8 (n, H, W, 3) tensor with 3-byte pixels")
+    n, H0, W0 = (int(v) for v in imgs_u8.shape[:3])
+    want_dt = {_lib.DTYPE_F32: torch.float32, _lib.DTYPE_BF16: torch.bfloat16}.get(int(out_dtype))
+    if not (out.is_cuda and out.dtype == want_dt and out.is_contiguous()
+            and out.numel() == n * img_H * img_W * out.shape[-1]):
+        raise ValueError("stage_rgb_u8: out must be a contiguous CUDA tensor [n, ..., H, W, cstride]")
+    m32 = np.ascontiguousarray(np.asarray(mean, dtype=np.float32))
+    s32 = np.ascontiguousarray(np.asarray(std, dtype=np.float32))
+    rc = _lib.lib().occd_stage_rgb_u8_cl(imgs_u8.data_ptr(), imgs_u8.stride(0), imgs_u8.stride(1), n, H0, W0,
+                                         int(img_H), int(img_W), m32.ctypes.data_as(C.c_void_p),
+                                         s32.ctypes.data_as(C.c_void_p), out.data_ptr(), int(out_dtype),
+                                         int(out.shape[-1]), _lib.stream_ptr())
+    _lib.check(rc, "occd_stage_rgb_u8_cl")
+
+
+NYU_DEPTH_SCALE, NYU_MAX_DEPTH = 8000.0, 10.0     # nyu_dataset.py:42-48
+
+
+def depth_u16_to_f32(depth_u16, out, divisor=NYU_DEPTH_SCALE, max_depth=NYU_MAX_DEPTH):
+    """NYU's `load_depth` of a decoded uint16 depth PNG into a CUDA float32 tensor of the same element count:
+    float32(depth / divisor) (float64 division), clamped to [0, max_depth] (`occd_depth_u16_to_f32`); enqueued on the
+    current stream, no allocation."""
+    if not (depth_u16.is_cuda and depth_u16.dtype == torch.uint16 and depth_u16.is_contiguous()):
+        raise ValueError("depth_u16_to_f32: expected a contiguous CUDA uint16 tensor")
+    if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == depth_u16.numel()):
+        raise ValueError("depth_u16_to_f32: out must be a contiguous CUDA float32 tensor of the same size")
+    rc = _lib.lib().occd_depth_u16_to_f32(depth_u16.data_ptr(), out.data_ptr(), depth_u16.numel(), float(divisor),
+                                          float(max_depth), _lib.stream_ptr())
+    _lib.check(rc, "occd_depth_u16_to_f32")

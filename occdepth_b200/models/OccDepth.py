@@ -288,13 +288,22 @@ class OccDepth(_Base, B200Module):
         converted or copied.  inv_map: one label id per class (at most 64), the submission writer's remap.  Its plan is
         cached apart from the forward's (alternating both rebuilds neither); under enable_slab_parallel this rank's
         X-slab."""
-        lut = None
-        if inv_map is not None:
-            import numpy as np
-            lut = tuple(int(v) for v in np.asarray(inv_map).astype(np.int64).reshape(-1))
-            if len(lut) != self.n_classes:
-                raise ValueError("OccDepth.predict_classes: inv_map must hold one label id per class")
-        return self._run(batch, ("classes", lut))
+        return self._run(batch, ("classes", self._class_lut(inv_map)))
+
+    def _class_lut(self, inv_map):
+        if inv_map is None:
+            return None
+        import numpy as np
+        lut = tuple(int(v) for v in np.asarray(inv_map).astype(np.int64).reshape(-1))
+        if len(lut) != self.n_classes:
+            raise ValueError("OccDepth.predict_classes: inv_map must hold one label id per class")
+        return lut
+
+    def _plan_key(self, B, V, H, W, N, P, dev, virtual, virtual_bf):
+        """cache key of the launch plan of one batch shape (shared by tensor batches and camera frames)"""
+        slab = self.__dict__.get("slab_ctx")
+        return (B, V, H, W, N, P, str(dev), virtual, virtual_bf if virtual else 0.0,
+                None if slab is None else (slab.rank, slab.world), self.precision, self.param_stamp())
 
     def _run(self, batch, classes):
         img = batch["img"]
@@ -312,13 +321,12 @@ class OccDepth(_Base, B200Module):
         fm = batch["fov_mask_{}".format(ps)]
         N, P = pp[0].shape[1], pp[0].shape[2]
         virtual = V == 1 and "gt_depth" in batch
-        slab = self.__dict__.get("slab_ctx")
-        key = (B, V, H, W, N, P, str(dev), virtual, float(batch["virtual_bf"][0]) if virtual else 0.0,
-               None if slab is None else (slab.rank, slab.world), self.precision, self.param_stamp())
+        key = self._plan_key(B, V, H, W, N, P, dev, virtual, float(batch["virtual_bf"][0]) if virtual else 0.0)
+        stage = lambda ent: self._stage(ent, batch, img, pp, fm, dev)    # noqa: E731
         with torch.cuda.device(dev):           # launches, tensor maps and function attributes follow the tensors
             if classes is not None:
-                return self._classes_on(batch, key + classes, img, pp, fm, B, V, H, W, N, P, dev, classes)
-            return self._forward_on(batch, key, img, pp, fm, B, V, H, W, N, P, dev)
+                return self._classes_on(batch, key + classes, B, V, H, W, N, P, dev, classes, stage)
+            return self._forward_on(batch, key, B, V, H, W, N, P, dev, stage)
 
     def prepare(self, batch):
         """build and cache the launch plan (weight snapshot, buffers, tensor maps, CUDA graph) for this batch's
@@ -331,7 +339,8 @@ class OccDepth(_Base, B200Module):
             self.__dict__.pop("_build_only", None)
         return self
 
-    def _forward_on(self, batch, key, img, pp, fm, B, V, H, W, N, P, dev):
+    def _forward_on(self, batch, key, B, V, H, W, N, P, dev, stage):
+        """batch: what _build reads (shapes, the virtual view, vox_origin); stage(ent) fills the plan's inputs"""
         ent = self._plans().get(key)
         if ent is None:
             self._plans().clear()              # weights changed / new shape: drop the stale snapshot
@@ -340,11 +349,11 @@ class OccDepth(_Base, B200Module):
             self._plans()[key] = ent
         if self.__dict__.get("_build_only"):
             return None
-        self._stage(ent, batch, img, pp, fm, dev)
+        stage(ent)
         ent[0].run()
         return self._outputs(ent)
 
-    def _classes_on(self, batch, key, img, pp, fm, B, V, H, W, N, P, dev, classes):
+    def _classes_on(self, batch, key, B, V, H, W, N, P, dev, classes, stage):
         cache = self._class_plans()
         ent = cache.get(key)
         if ent is None:
@@ -354,13 +363,14 @@ class OccDepth(_Base, B200Module):
             cache[key] = ent
         if self.__dict__.get("_build_only"):
             return None
-        self._stage(ent, batch, img, pp, fm, dev)
+        stage(ent)
         ent[0].run()
         return ent[4].clone()                  # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
         """copy this batch's inputs into the static input buffers of plan entry `ent`"""
         plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
+        plan.calib_mark = None                 # the index buffers no longer hold a camera frame's calibration
         B, V, _, H, W = img.shape
         CL.from_planar(img.reshape(B * V, 3, H, W) if view_sel is None else img[:, view_sel].reshape(B, 3, H, W),
                        out=img_cl)
@@ -372,6 +382,137 @@ class OccDepth(_Base, B200Module):
             fov[b].copy_(fm[b][:, n_lo:n_lo + nl], non_blocking=True)
         if self.trans_2d_to_3d == "flosp_depth":
             self.flosp_depth.stage_inputs(batch, dev, plan.flosp_state)
+
+    # ---- camera frames: uint8 images and calibration in, the datasets' pre-processing on the device -------------
+    def predict_frame(self, frame, classes=True, inv_map=None):
+        """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map` as in predict_classes) or
+        the forward's output dict (classes=False), through the same cached plan a tensor batch of the same shapes
+        uses.  Only the staging differs: the datasets' pre-processing (eval split, no augmentation) runs on the device
+        and writes the plan's input buffers -- the images through `occd_stage_rgb_u8_cl`, the indices through
+        `occd_vox2pix_fwd`, NYU's depth map through `occd_depth_u16_to_f32`.
+
+        frame (host arrays or tensors; the images and depth map may already be on the device):
+          "img": uint8 RGB (V, H0, W0, 3), or (H0, W0, 3) for one view: the decoded camera images, cropped to
+                 `img_hw` on the device (kitti_dataset.py:376-402)
+          KITTI: "cam_k" (V, 3, 3) and "T_velo_2_cam" (V, 4, 4) (kitti_dataset.py:196-290)
+          NYU:   "cam_pose" (4, 4), "vox_origin" (3,), "cam_k" (3, 3) (default: the dataset's), "depth": the uint16
+                 depth PNG (H, W) when the model runs the virtual right view (nyu_dataset.py:116-200)
+          optional geometry, fixed per dataset: "img_hw" (KITTI (370, 1220), NYU (480, 640)), "vox_origin" (KITTI
+          (0, -25.6, -2)), "voxel_size" (KITTI 0.2 * project_scale, NYU 0.08), "scene_size", "pattern_id" (0)
+        The indices are recomputed only when the calibration differs from what the plan's index buffers hold (a KITTI
+        sequence keeps one); NYU poses change every frame.  One frame per call; not under enable_slab_parallel."""
+        if self.__dict__.get("slab_ctx") is not None:
+            raise NotImplementedError("OccDepth.predict_frame: not under enable_slab_parallel (a camera frame is staged "
+                                      "whole on one device); use forward / predict_classes with a tensor batch")
+        if self.infer_mode and self.trans_2d_to_3d == "flosp_depth":
+            raise NotImplementedError("OccDepth.predict_frame: infer_mode with flosp_depth takes the caller's sampling "
+                                      "grids, not camera matrices; use forward / predict_classes with a tensor batch")
+        dev = next(self.parameters()).device
+        self._check_mode(torch.empty(0, device=dev))
+        f = self._frame_inputs(frame, dev)
+        key = self._plan_key(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"])
+        stage = lambda ent: self._stage_frame(ent, f)     # noqa: E731
+        with torch.cuda.device(dev):
+            if classes:
+                cls = ("classes", self._class_lut(inv_map))
+                return self._classes_on(f["batch"], key + cls, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
+                                        stage)
+            return self._forward_on(f["batch"], key, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage)
+
+    def _frame_inputs(self, frame, dev):
+        """host side of predict_frame: the views' poses, the geometry, the stand-in batch _build and FlospDepth read"""
+        import numpy as np
+        from .. import data as D
+        img = frame["img"]
+        if not isinstance(img, torch.Tensor):
+            img = torch.from_numpy(np.ascontiguousarray(img))
+        if img.dim() == 5:
+            if img.shape[0] != 1:
+                raise NotImplementedError("OccDepth.predict_frame: one frame per call (batch size %d)" % img.shape[0])
+            img = img[0]
+        if img.dim() == 3:
+            img = img.unsqueeze(0)
+        if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] != 3:
+            raise ValueError("OccDepth.predict_frame: frame['img'] must be uint8 RGB (V, H, W, 3)")
+        if img.stride(3) != 1 or img.stride(2) != 3:
+            img = img.contiguous()
+        img = img.to(dev, non_blocking=True)
+        V = int(img.shape[0])
+        nyu = self.dataset == "NYU"
+        H, W = (int(v) for v in frame.get("img_hw", (480, 640) if nyu else (370, 1220)))
+        g = dict(voxel_size=frame.get("voxel_size", 0.08 if nyu else 0.2 * self.project_scale),
+                 scene_size=tuple(frame.get("scene_size", (4.8, 4.8, 2.88) if nyu else (51.2, 51.2, 6.4))),
+                 pattern_id=int(frame.get("pattern_id", 0)))
+        depth, bf = None, 0.0
+        if nyu:                                                   # nyu_dataset.py:126-190, collate.py:31-41
+            if V != 1:
+                raise ValueError("OccDepth.predict_frame: an NYU frame holds one image")
+            cam_k = np.asarray(frame.get("cam_k", [[518.8579, 0, 320], [0, 518.8579, 240], [0, 0, 1]]))
+            cam_k = cam_k.reshape(3, 3)
+            vox_origin = np.asarray(frame["vox_origin"])
+            T_world_2_cam = np.linalg.inv(np.asarray(frame["cam_pose"]))
+            poses = [(T_world_2_cam, cam_k)]
+            depth = frame.get("depth")
+            batch = {"cam_k": [torch.from_numpy(np.array([cam_k])).double()],
+                     "T_velo_2_cam": [torch.from_numpy(T_world_2_cam[np.newaxis, ...]).float()],
+                     "ida_mats": [torch.eye(4).unsqueeze(0)], "vox_origin": torch.from_numpy(vox_origin[None]).double()}
+            if depth is not None:
+                virtual_baseline = 0.1
+                T_cam0_2_cam1 = np.array([[1, 0, 0, -virtual_baseline], [0, 1, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]])
+                poses.append((T_cam0_2_cam1 @ T_world_2_cam, cam_k))
+                bf = float(np.array(virtual_baseline * 518.8579))
+                if not isinstance(depth, torch.Tensor):
+                    depth = torch.from_numpy(np.ascontiguousarray(depth))
+                if depth.dtype != torch.uint16 or depth.dim() != 2:
+                    raise ValueError("OccDepth.predict_frame: frame['depth'] must be the uint16 depth PNG (H, W)")
+                depth = depth.contiguous().to(dev, non_blocking=True)
+                batch.update(gt_depth=torch.empty((1, 1) + tuple(depth.shape), device="meta"), virtual_bf=[bf])
+            calib = None                                          # a new pose every frame
+        else:                                                     # kitti_dataset.py:196-290, collate.py:26-28
+            cam_k = np.asarray(frame["cam_k"])
+            T = np.asarray(frame["T_velo_2_cam"])
+            if cam_k.shape != (V, 3, 3) or T.shape != (V, 4, 4):
+                raise ValueError("OccDepth.predict_frame: a KITTI frame of %d images needs cam_k (%d, 3, 3) and "
+                                 "T_velo_2_cam (%d, 4, 4)" % (V, V, V))
+            vox_origin = np.asarray(frame.get("vox_origin", np.array([0, -25.6, -2])))
+            poses = [(T[v], cam_k[v]) for v in range(V)]
+            # img_transform((0, 0, W, H), False) is the identity (kitti_dataset.py:380-390)
+            batch = {"cam_k": [torch.from_numpy(cam_k).double()], "T_velo_2_cam": [torch.from_numpy(T).float()],
+                     "ida_mats": [torch.eye(4).unsqueeze(0).repeat(V, 1, 1)]}
+            calib = tuple((a.dtype.str, a.shape, a.tobytes()) for a in (T, cam_k, vox_origin)) + \
+                (float(g["voxel_size"]), g["scene_size"], g["pattern_id"], H, W)
+        X, Y, Z = (int(v) for v in D.volume_dims(vox_origin, g["voxel_size"], g["scene_size"]))
+        S = [int(s) // self.project_scale for s in self.full_scene_size]
+        if X * Y * Z != S[0] * S[1] * S[2]:
+            raise ValueError("OccDepth.predict_frame: the geometry gives a %dx%dx%d voxel grid, the model lifts into "
+                             "%dx%dx%d" % (X, Y, Z, S[0], S[1], S[2]))
+        if not 0 <= g["pattern_id"] < len(D.PIXEL_PATTERNS):
+            raise IndexError("pattern_id out of range")
+        return dict(g, imgs=img, V=V, H=H, W=W, N=X * Y * Z, P=len(D.PIXEL_PATTERNS[g["pattern_id"]]), poses=poses,
+                    vox_origin=vox_origin, depth=depth, virtual=depth is not None, virtual_bf=bf, batch=batch,
+                    calib=calib)
+
+    def _stage_frame(self, ent, f):
+        """the device side of predict_frame: stage frame `f` into the static input buffers of plan entry `ent`"""
+        from .. import data as D
+        plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
+        imgs = f["imgs"] if view_sel is None else f["imgs"][view_sel:view_sel + 1]
+        D.stage_rgb_u8(imgs, img_cl.buf, img_cl.lib_dtype, f["H"], f["W"])
+        if depth0 is not None:
+            if tuple(f["depth"].shape) != tuple(depth0.shape):
+                raise ValueError("OccDepth.predict_frame: depth map %r, the plan holds %r"
+                                 % (tuple(f["depth"].shape), tuple(depth0.shape)))
+            D.depth_u16_to_f32(f["depth"], depth0)
+        if f["calib"] is not None and f["calib"] == getattr(plan, "calib_mark", None):
+            return                              # same calibration: the indices and camera tables are in place
+        if getattr(plan, "pix_z", None) is None:
+            plan.pix_z = torch.empty(pix.shape[2], dtype=torch.float64, device=pix.device)   # vox2pix's depth output
+        for v, (E, K) in enumerate(f["poses"]):
+            D.vox2pix_into(pix[0, v], fov[0, v], plan.pix_z, E, K, f["vox_origin"], f["voxel_size"], f["W"], f["H"],
+                           f["scene_size"], f["pattern_id"])
+        if self.trans_2d_to_3d == "flosp_depth":
+            self.flosp_depth.stage_inputs(f["batch"], pix.device, plan.flosp_state)
+        plan.calib_mark = f["calib"]
 
     def _outputs(self, ent):
         """the forward's output dict from plan entry `ent` after it ran (under the slab partition: this rank's

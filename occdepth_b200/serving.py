@@ -94,3 +94,139 @@ class FramePipeline:
     def join(self):
         """make the compute stream wait for every outstanding read-back (for timing with CUDA events)"""
         self.main.wait_stream(self.d2h)
+
+
+class CameraPipeline:
+    """`OccDepth.predict_frame` for a stream of camera frames in host memory, with FramePipeline's overlap: the H2D
+    copy of frame i+1's uint8 images (and NYU depth map) and the D2H read of frame i-1's class map (or logits) run on
+    their own streams while frame i computes.  Per frame only the raw images (3 MB for a KITTI stereo pair), the depth
+    PNG and a few matrices leave the host; normalisation, cropping and the projection indices are computed on the
+    device, straight into the plan's input buffers.
+
+        pipe = CameraPipeline(model, img_hw=(370, 1220))          # KITTI; geometry fixed per pipeline
+        for frame in frames:            # {"img": uint8 (V, H0, W0, 3), "cam_k": (V, 3, 3), "T_velo_2_cam": (V, 4, 4)}
+            done = pipe.submit(frame)   # returns the PREVIOUS frame's ticket (or None)
+            if done is not None:
+                y_pred = pipe.result(done)             # pinned host tensor, valid until two more submits
+        y_pred = pipe.result(pipe.flush())
+
+    `frame` is what predict_frame takes (NYU: "img", "cam_pose", "vox_origin", "cam_k", "depth"); the constructor's
+    geometry (img_hw, vox_origin, voxel_size, scene_size, pattern_id) fills the keys a frame leaves out.  Two pinned
+    and two device image / depth buffers, sized from the first frame and regrown only when a larger raw image arrives;
+    nothing else is allocated per frame.  One frame per submit; not under enable_slab_parallel, nor for infer_mode with
+    flosp_depth (that route takes sampling grids, not camera matrices)."""
+
+    def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
+                 inv_map=None, device=None, out_key="ssc_logit"):
+        if not torch.cuda.is_available():
+            raise RuntimeError("CameraPipeline: occdepth_b200 needs a CUDA (sm_90a) device")
+        if model.__dict__.get("slab_ctx") is not None:
+            raise NotImplementedError("CameraPipeline: not under enable_slab_parallel (a camera frame is staged whole "
+                                      "on one device)")
+        if model.infer_mode and model.trans_2d_to_3d == "flosp_depth":
+            raise NotImplementedError("CameraPipeline: infer_mode with flosp_depth takes the caller's sampling grids, "
+                                      "not camera matrices")
+        dev = torch.device(device) if device is not None else next(model.parameters()).device
+        require_cuda(torch.empty(0, device=dev), "CameraPipeline")
+        self.model, self.dev, self.out_key = model, dev, out_key
+        self.classes, self.inv_map = classes, inv_map
+        self.geometry = {"img_hw": tuple(img_hw), "pattern_id": int(pattern_id)}
+        for k, v in (("vox_origin", vox_origin), ("voxel_size", voxel_size), ("scene_size", scene_size)):
+            if v is not None:
+                self.geometry[k] = v
+        self.main = torch.cuda.current_stream(dev)
+        self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
+        self.bufs = {"img": [None, None], "depth": [None, None]}     # (pinned host, device) flat byte buffers
+        self.dev_out, self.host_out = [None, None], [None, None]
+        self.in_ready, self.in_free, self.host_free, self.out_ready, self.out_free = (
+            [torch.cuda.Event(), torch.cuda.Event()] for _ in range(5))
+        for j in range(2):
+            self.in_free[j].record(self.main)
+            self.host_free[j].record(self.h2d)
+            self.out_free[j].record(self.main)
+        self.n = 0
+        self.h2d_bytes = 0            # bytes copied host -> device by the last submit
+
+    @staticmethod
+    def _host(x, what):
+        if isinstance(x, torch.Tensor):
+            if x.is_cuda:
+                raise ValueError("CameraPipeline.submit: frame[%r] must be in host memory" % what)
+            return x
+        import numpy as np
+        return torch.from_numpy(np.ascontiguousarray(x))
+
+    def _stage_h2d(self, name, j, x):
+        """copy host tensor x into pinned buffer j (once its previous H2D has finished), enqueue the H2D copy into
+        device buffer j; returns the device view of x's shape"""
+        nb = x.numel() * x.element_size()
+        buf = self.bufs[name][j]
+        if buf is None or buf[0].numel() < nb:
+            torch.cuda.synchronize(self.dev)      # a larger raw image: nothing may still read the old buffers
+            buf = (torch.empty(nb, dtype=torch.uint8).pin_memory(), torch.empty(nb, dtype=torch.uint8, device=self.dev))
+            self.bufs[name][j] = buf
+        host = buf[0][:nb].view(x.dtype).view(x.shape)
+        host.copy_(x)
+        dev = buf[1][:nb].view(x.dtype).view(x.shape)
+        dev.copy_(host, non_blocking=True)        # on the h2d stream (the caller's context)
+        self.h2d_bytes += nb
+        return dev
+
+    def submit(self, frame):
+        """enqueue one camera frame (host arrays / tensors, see the class docstring).  Returns the ticket of the frame
+        submitted before this one -- its read-back overlaps this frame's forward -- or None."""
+        img = self._host(frame["img"], "img")
+        if img.dim() == 5:
+            if img.shape[0] != 1:
+                raise NotImplementedError("CameraPipeline.submit: one frame per submit (batch size %d)" % img.shape[0])
+            img = img[0]
+        depth = frame.get("depth")
+        depth = None if depth is None else self._host(depth, "depth")
+        j = self.n & 1
+        self.host_free[j].synchronize()           # pinned buffer j: its previous H2D copy has been read
+        self.h2d_bytes = 0
+        f = dict(self.geometry)
+        f.update(frame)
+        with torch.cuda.stream(self.h2d):
+            self.h2d.wait_event(self.in_free[j])
+            f["img"] = self._stage_h2d("img", j, img)
+            if depth is not None:
+                f["depth"] = self._stage_h2d("depth", j, depth)
+            self.in_ready[j].record(self.h2d)
+            self.host_free[j].record(self.h2d)
+        self.main.wait_event(self.in_ready[j])
+        with torch.no_grad():
+            res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map)
+        if not self.classes:
+            res = res[self.out_key]
+        self.in_free[j].record(self.main)
+        if self.dev_out[j] is None or self.dev_out[j].shape != res.shape:
+            self.out_free[j].synchronize()
+            self.dev_out[j] = torch.empty_like(res)
+            self.host_out[j] = torch.empty(res.shape, dtype=res.dtype).pin_memory()
+        self.main.wait_event(self.out_free[j])
+        self.dev_out[j].copy_(res)           # the result leaves the allocator-owned tensor on the compute stream
+        self.out_ready[j].record(self.main)
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(self.out_ready[j])
+            self.host_out[j].copy_(self.dev_out[j], non_blocking=True)
+            self.out_free[j].record(self.d2h)
+        self.n += 1
+        return self.n - 2 if self.n >= 2 else None
+
+    def flush(self):
+        """ticket of the last submitted frame (nothing further overlaps its read-back)"""
+        return self.n - 1 if self.n else None
+
+    def result(self, ticket):
+        """host tensor (pinned) of a submitted frame; blocks until its D2H read has finished.  The buffer is reused by
+        the second submit after the one that produced it."""
+        if ticket is None or ticket < self.n - 2 or ticket >= self.n:
+            raise ValueError("CameraPipeline.result: ticket %r is not one of the two frames in flight" % (ticket,))
+        j = ticket & 1
+        self.out_free[j].synchronize()
+        return self.host_out[j]
+
+    def join(self):
+        """make the compute stream wait for every outstanding read-back (for timing with CUDA events)"""
+        self.main.wait_stream(self.d2h)
