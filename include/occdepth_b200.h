@@ -399,6 +399,31 @@ int occd_depth_cls_sums(const float* gt, int n_maps, int H, int W, const float* 
                         int factor, double d0, double step, double* sums, double* work, long long work_len,
                         void* stream);
 
+/* -------------------------------------------------------------------------------------------- */
+/* Occupied-voxel list of a class map: what the visualisation scripts build on the host from `y_pred` and     */
+/* `fov_mask_1` (scripts/visualization/kitti_vis_pred.py:9-32, 69-89; kitti_vis_pred_batch.py, NYU_vis_pred.py). */
+/* class_map: uint16 [B][N], N = X*Y*Z in C order (what the class-map epilogue / occd_argmax_classes write, with */
+/* or without a remap); fov_mask: numpy bool bytes [B][N] or NULL (then every voxel counts as inside).  A voxel is */
+/* occupied when empty < class < ignore (the scripts' 0 < class < 255).  Per frame b:                            */
+/*   count[b][2]        occupied voxels inside / outside the FOV (the true counts, whatever cap is)               */
+/*   hist[b][n_classes] occupied voxels per class id below n_classes (<= 64); larger ids are listed, not counted  */
+/*   index[b][cap], cls[b][cap], xyz[b][cap][3] (xyz may be NULL): one row per occupied voxel, the voxels inside   */
+/*     the FOV first, then the others, each group in ascending flat index -- the order of numpy's boolean        */
+/*     indexing.  Only the first min(cap, total) rows are written; nothing else of the three arrays is touched.   */
+/* index = index0 + the voxel's flat index in its frame (index0: the flat index of this map's first voxel in a    */
+/* larger grid, e.g. x_lo*Y*Z for an X-slab; 0 otherwise).  xyz = the centre of voxel (x, y, z) = the unravelled  */
+/* index: float32(((double)x * voxel_size + voxel_size / 2) + origin[0]) and likewise y, z -- a float64 product    */
+/* and sums, rounded once; without `origin` (HOST pointer to 3 doubles, or NULL) these are the rows of            */
+/* get_grid_coords([X, Y, Z], voxel_size) cast to float32, for the X == Y grids the scripts call it with.         */
+/* work: OCCD_VOXEL_WORK_LEN(B, N) uint32, 8-byte aligned, contents irrelevant before and after.  hist is cleared */
+/* by the call.  Three launches on `stream`; the same inputs give the same bytes.                                 */
+#define OCCD_VOXEL_TILE 2048
+#define OCCD_VOXEL_WORK_LEN(B, N) (2LL * (B) * (((N) + OCCD_VOXEL_TILE - 1) / OCCD_VOXEL_TILE))
+int occd_occupied_voxels(const uint16_t* class_map, const uint8_t* fov_mask, int B, int X, int Y, int Z, int index0,
+                         int empty, int ignore, int n_classes, int cap, uint32_t* count, uint32_t* hist,
+                         int32_t* index, uint16_t* cls, float* xyz, double voxel_size, const double* origin,
+                         uint32_t* work, long long work_len, void* stream);
+
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,

@@ -138,7 +138,16 @@ SYMBOLS = {
     "occd_crp_relation_sums": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _ll, _vp]),
     "occd_depth_cls_sums": (C.c_int, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _vp, _ll,
                                       _vp]),
+    "occd_occupied_voxels": (C.c_int, [_vp, _vp] + [_i] * 9 + [_vp] * 5 + [C.c_double, _vp, _vp, _ll, _vp]),
 }
+VOXEL_TILE = 2048
+
+
+def voxel_work_len(B, N):
+    """uint32 elements of occd_occupied_voxels' workspace (OCCD_VOXEL_WORK_LEN)"""
+    return 2 * B * ((N + VOXEL_TILE - 1) // VOXEL_TILE)
+
+
 LOSS_WORK_BLOCKS = 264
 SSC_LOSS_MAX_CLASSES = SSC_LOSS_MAX_FRUSTUMS = 64
 CRP_MAX_RELATIONS = 16

@@ -401,6 +401,10 @@ class OccDepth(_Base, B200Module):
           (0, -25.6, -2)), "voxel_size" (KITTI 0.2 * project_scale, NYU 0.08), "scene_size", "pattern_id" (0)
         The indices are recomputed only when the calibration differs from what the plan's index buffers hold (a KITTI
         sequence keeps one); NYU poses change every frame.  One frame per call; not under enable_slab_parallel."""
+        return self._run_frame(self._frame_checked(frame), classes, inv_map)
+
+    def _frame_checked(self, frame):
+        """the refusals of the camera route, then `_frame_inputs`"""
         if self.__dict__.get("slab_ctx") is not None:
             raise NotImplementedError("OccDepth.predict_frame: not under enable_slab_parallel (a camera frame is staged "
                                       "whole on one device); use forward / predict_classes with a tensor batch")
@@ -409,7 +413,10 @@ class OccDepth(_Base, B200Module):
                                       "grids, not camera matrices; use forward / predict_classes with a tensor batch")
         dev = next(self.parameters()).device
         self._check_mode(torch.empty(0, device=dev))
-        f = self._frame_inputs(frame, dev)
+        return self._frame_inputs(frame, dev)
+
+    def _run_frame(self, f, classes, inv_map):
+        dev = f["imgs"].device
         key = self._plan_key(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"])
         stage = lambda ent: self._stage_frame(ent, f)     # noqa: E731
         with torch.cuda.device(dev):
@@ -513,6 +520,92 @@ class OccDepth(_Base, B200Module):
         if self.trans_2d_to_3d == "flosp_depth":
             self.flosp_depth.stage_inputs(f["batch"], pix.device, plan.flosp_state)
         plan.calib_mark = f["calib"]
+
+    # ---- the occupied-voxel list: what every consumer of a class map builds from it first ----------------------
+    def predict_voxels(self, batch_or_frame, inv_map=None, fov_mask=None, capacity=None, voxel_size=None,
+                       vox_origin=None, out=None):
+        """`predict_classes` (a tensor batch: it carries "projected_pix_<project_scale>") or `predict_frame` (a camera
+        frame), then `voxels.occupied_voxels` of the class map on the same stream -> VoxelList: per frame the counts,
+        the class histogram and the rows (flat index, class, voxel centre) of the occupied voxels, inside the FOV
+        first, in numpy's order; nothing is read back until the caller asks the list for counts or rows.
+
+        fov_mask: None takes the frame's `fov_mask_1` -- batch["fov_mask_1"] when the batch has it (what
+                  generate_output.py saves for the visualisation scripts), and for a camera frame the mask `vox2pix`
+                  gives at the output resolution, computed on the device and kept while the calibration stays the same
+                  (once for a KITTI sequence).  A per-frame mask of the datasets' shape (V, N, P) stands for its first
+                  view's centre pixel, `[0, :, 0]`, as in kitti_vis_pred_batch.py:92-93.  False: no mask.  NYU has no
+                  default mask: its `fov_mask_1` follows vox2pix's (x, y, z) voxel order, not the prediction's
+                  (x, z, y), and NYU_vis_pred.py keeps one list.
+        voxel_size: of the output grid (default 0.2 for KITTI, 0.08 for NYU); vox_origin: added to the centres.
+        inv_map, capacity, out: as in predict_classes / occupied_voxels.
+        Under enable_slab_parallel (tensor batches) the list holds this rank's X-slab with the whole grid's flat
+        indices and coordinates: the ranks' in-FOV rows concatenated in rank order, then their out-of-FOV rows, are
+        the unpartitioned list."""
+        if "projected_pix_%d" % self.project_scale in batch_or_frame:
+            y = self.predict_classes(batch_or_frame, inv_map)
+            x_range = self.slab_x_range()
+            if fov_mask is None:
+                fov_mask = False if self.dataset == "NYU" else batch_or_frame.get("fov_mask_1", False)
+        else:
+            f = self._frame_checked(batch_or_frame)
+            y = self._run_frame(f, True, inv_map)
+            x_range = None
+            if fov_mask is None and y is not None:
+                fov_mask = False if self.dataset == "NYU" else self._frame_fov_mask_1(f)
+        if y is None:                          # prepare(): the plan was built, nothing ran
+            return None
+        return self._list_voxels(y, x_range, fov_mask, capacity, voxel_size, vox_origin, out)
+
+    def _list_voxels(self, y, x_range, fov_mask, capacity, voxel_size, vox_origin, out):
+        """the list of class map `y` [B, Xl, Y, Z]: the whole grid, or planes x_range = [lo, hi) of it"""
+        from ..voxels import occupied_voxels
+        B, _, Y, Z = y.shape
+        lo, hi = (0, y.shape[1]) if x_range is None else x_range
+        n_full = int(self.full_scene_size[0]) * Y * Z
+        mask = None
+        if fov_mask is not None and fov_mask is not False:
+            frames = [fov_mask] if getattr(fov_mask, "ndim", 0) == 1 else list(fov_mask)
+            rows = []
+            for m in frames:
+                m = torch.as_tensor(m)
+                if m.dim() == 3:               # the datasets' (V, N, P)
+                    m = m[0, :, 0]
+                if m.numel() != n_full:
+                    raise ValueError("OccDepth.predict_voxels: a frame's fov_mask holds %d values, the output grid %d "
+                                     "voxels" % (m.numel(), n_full))
+                rows.append(m.reshape(-1)[lo * Y * Z:hi * Y * Z].to(y.device, non_blocking=True))
+            if len(rows) != B:
+                raise ValueError("OccDepth.predict_voxels: %d masks for %d frames" % (len(rows), B))
+            mask = torch.stack(rows)
+        if voxel_size is None:
+            voxel_size = 0.08 if self.dataset == "NYU" else 0.2
+        return occupied_voxels(y, mask, voxel_size=voxel_size, vox_origin=vox_origin, capacity=capacity,
+                               index0=lo * Y * Z, out=out)
+
+    def _frame_fov_mask_1(self, f):
+        """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
+        resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only.  Kept with the calibration it was
+        computed from."""
+        import numpy as np
+        from .. import data as D
+        held = self.__dict__.get("_fov_mask_1")
+        if f["calib"] is not None and held is not None and held[0] == f["calib"] and held[1].device == f["imgs"].device:
+            return held[1]
+        voxel = f["voxel_size"] / self.project_scale
+        n1 = int(np.prod(D.volume_dims(f["vox_origin"], voxel, f["scene_size"])))
+        if n1 != int(np.prod([int(s) for s in self.full_scene_size])):
+            raise ValueError("OccDepth.predict_voxels: the geometry gives %d voxels at the output resolution, the model "
+                             "predicts %d" % (n1, int(np.prod([int(s) for s in self.full_scene_size]))))
+        dev = f["imgs"].device
+        E, K = f["poses"][0]
+        with torch.cuda.device(dev):
+            pix = torch.empty(n1, 1, 2, dtype=torch.int64, device=dev)
+            fov = torch.empty(n1, 1, dtype=torch.bool, device=dev)
+            pix_z = torch.empty(n1, dtype=torch.float64, device=dev)
+            D.vox2pix_into(pix, fov, pix_z, E, K, f["vox_origin"], voxel, f["W"], f["H"], f["scene_size"], 0)
+        mask = fov.view(-1)
+        self.__dict__["_fov_mask_1"] = (f["calib"], mask)
+        return mask
 
     def _outputs(self, ent):
         """the forward's output dict from plan entry `ent` after it ran (under the slab partition: this rank's

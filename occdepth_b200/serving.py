@@ -114,12 +114,20 @@ class CameraPipeline:
     geometry (img_hw, vox_origin, voxel_size, scene_size, pattern_id) fills the keys a frame leaves out.  Two pinned
     and two device image / depth buffers, sized from the first frame and regrown only when a larger raw image arrives;
     nothing else is allocated per frame.  One frame per submit; not under enable_slab_parallel, nor for infer_mode with
-    flosp_depth (that route takes sampling grids, not camera matrices)."""
+    flosp_depth (that route takes sampling grids, not camera matrices).
+
+    `output="voxels"` lists every frame's occupied voxels on the device (`OccDepth.predict_voxels`) and reads back the
+    counts, the class histogram and the first `capacity` rows (flat index, class, voxel centre: 18 bytes a row; default
+    capacity an eighth of the output grid) instead of the class map; `result(ticket)` trims them to the rows written
+    and says whether the frame held more (`truncated`).  `d2h_bytes` is what a frame reads back."""
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
-                 inv_map=None, device=None, out_key="ssc_logit"):
+                 inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None):
         if not torch.cuda.is_available():
             raise RuntimeError("CameraPipeline: occdepth_b200 needs a CUDA (sm_90a) device")
+        if output not in (None, "voxels"):
+            raise ValueError("CameraPipeline: output must be None (the class map or logits, as `classes` says) or "
+                             "'voxels', got %r" % (output,))
         if model.__dict__.get("slab_ctx") is not None:
             raise NotImplementedError("CameraPipeline: not under enable_slab_parallel (a camera frame is staged whole "
                                       "on one device)")
@@ -146,6 +154,14 @@ class CameraPipeline:
             self.out_free[j].record(self.main)
         self.n = 0
         self.h2d_bytes = 0            # bytes copied host -> device by the last submit
+        self.output = output
+        if output == "voxels":
+            n_out = 1
+            for s in model.full_scene_size:
+                n_out *= int(s)
+            self.capacity = n_out // 8 if capacity is None else int(capacity)
+            self.vox = [None, None]       # the two device lists, overwritten in place
+            self.d2h_bytes = 0            # bytes read back per frame
 
     @staticmethod
     def _host(x, what):
@@ -195,6 +211,8 @@ class CameraPipeline:
             self.in_ready[j].record(self.h2d)
             self.host_free[j].record(self.h2d)
         self.main.wait_event(self.in_ready[j])
+        if self.output == "voxels":
+            return self._submit_voxels(f, j)
         with torch.no_grad():
             res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map)
         if not self.classes:
@@ -214,17 +232,48 @@ class CameraPipeline:
         self.n += 1
         return self.n - 2 if self.n >= 2 else None
 
+    def _submit_voxels(self, f, j):
+        """the tail of submit for output="voxels": list the frame into device list j, then read back the counts, the
+        histogram and the first `capacity` rows in one batch of copies -- the host learns the count from that same
+        batch, so no second round trip decides how much to copy"""
+        self.main.wait_event(self.out_free[j])        # list j is overwritten in place: its last read-back is done
+        with torch.no_grad():
+            vl = self.model.predict_voxels(f, inv_map=self.inv_map, capacity=self.capacity, out=self.vox[j])
+        self.in_free[j].record(self.main)
+        if self.vox[j] is None:
+            self.vox[j] = vl
+            self.host_out[j] = {k: torch.empty(getattr(vl, k)[0].shape, dtype=getattr(vl, k).dtype).pin_memory()
+                                for k in ("count", "hist", "index", "cls", "xyz")}
+            self.d2h_bytes = sum(t.numel() * t.element_size() for t in self.host_out[j].values())
+        self.out_ready[j].record(self.main)
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(self.out_ready[j])
+            for k, host in self.host_out[j].items():
+                host.copy_(getattr(vl, k)[0], non_blocking=True)
+            self.out_free[j].record(self.d2h)
+        self.n += 1
+        return self.n - 2 if self.n >= 2 else None
+
     def flush(self):
         """ticket of the last submitted frame (nothing further overlaps its read-back)"""
         return self.n - 1 if self.n else None
 
     def result(self, ticket):
         """host tensor (pinned) of a submitted frame; blocks until its D2H read has finished.  The buffer is reused by
-        the second submit after the one that produced it."""
+        the second submit after the one that produced it.  With output="voxels": a dict of numpy views of the pinned
+        buffers, trimmed to the rows that were written -- "count" (inside, outside the FOV; the true counts), "hist",
+        "index", "cls", "xyz" (the in-FOV rows first, "n_in" of them) and "truncated"."""
         if ticket is None or ticket < self.n - 2 or ticket >= self.n:
             raise ValueError("CameraPipeline.result: ticket %r is not one of the two frames in flight" % (ticket,))
         j = ticket & 1
         self.out_free[j].synchronize()
+        if self.output == "voxels":
+            h = {k: v.numpy() for k, v in self.host_out[j].items()}
+            count = h["count"].astype("int64")
+            total = int(count.sum())
+            n = min(total, self.capacity)
+            return dict(count=count, hist=h["hist"], index=h["index"][:n], cls=h["cls"][:n], xyz=h["xyz"][:n],
+                        n_in=min(int(count[0]), n), truncated=total > self.capacity)
         return self.host_out[j]
 
     def join(self):
