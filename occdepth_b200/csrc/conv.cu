@@ -342,7 +342,7 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3
   h.PW = d->IW;
   h.b_stride = round_up(h.N_tile * RB, 1024);
   h.w_bytes = h.n_groups * h.b_stride;
-  const int smem_total = 227 * 1024 - staging_bytes(xp_stage_ld(h.N_tile)) - h.w_bytes - 2048;   // staging, barriers, slack
+  const int smem_total = 227 * 1024 - xp_xchg_bytes(dil) - h.w_bytes - 2048;   // neighbour exchange, barriers, slack
   PLAN_REQUIRE(smem_total > 0, "weights do not fit in shared memory");
   const int HR = 128 / h.PW;                               // h-rows of one plane per M tile
   const int sD = (d->OD + dil - 1) / dil, sH = (d->IH + dil - 1) / dil;
@@ -403,7 +403,7 @@ static int halox_geometry(const occd_conv_desc* d, occd_conv_plan* pl, int box[3
   h.sD = sD;
   h.n_cols = d->B * dil * dil * h.tilesH;
   h.pdl = occd_pdl_enabled();
-  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + staging_bytes(xp_stage_ld(h.N_tile)) + 128 + 1024;
+  pl->smem = (size_t)h.w_bytes + (size_t)h.stages * h.a_stage_bytes + xp_xchg_bytes(dil) + 128 + 1024;
   box[0] = h.PW; box[1] = (h.PH - 1) * dil + 1; box[2] = h.ring ? 1 : (h.PD - 1) * dil + 1;   // ring: one plane per load
   traversal[0] = 1; traversal[1] = traversal[2] = dil;
   *n_tile = h.N_tile;
@@ -553,7 +553,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int
     if (it > total_iters) total_iters = it;
   }
   // persistent kernel: one CTA per SM owns the shared memory (227 KB less the epilogue staging and barriers)
-  const int st_bytes = staging_bytes(xp ? xp_stage_ld(t.N_tile) : kStageWide);
+  const int st_bytes = xp ? xp_xchg_bytes(1) : staging_bytes(kStageWide);
   const int budget = 227 * 1024 - st_bytes - 16 * kMaxStages - 64 - 1024;
   // (tap, k-chunk) items per pipeline stage: the single-thread producer/MMA hand-off costs ~0.25 us, so a stage
   // must carry >= ~512 tensor-pipe cycles of work (or up to 9 items) while leaving >= 3 stages in flight

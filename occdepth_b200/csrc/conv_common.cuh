@@ -69,6 +69,30 @@ __device__ __forceinline__ float class_value(const ConvEpi& e, long long pos, in
   if (e.res2 && !e.res2_post) v += Elem<T>::up(reinterpret_cast<const T*>(e.res2)[pos * e.res2_cstride + e.res2_coff + n]);
   return v;
 }
+// class_value of the 8 channels [n0, n0 + 8) (n0 < Cout_store, a multiple of 8) with vector loads, taken into the
+// arg-max in ascending channel order
+template <typename T>
+__device__ __forceinline__ void class_take8(const ConvEpi& e, long long pos, int n0, const float* v, ClassArg& a) {
+  float x[8];
+  const float4 b0 = __ldg(reinterpret_cast<const float4*>(e.bias + n0));
+  const float4 b1 = __ldg(reinterpret_cast<const float4*>(e.bias + n0 + 4));
+  x[0] = v[0] + b0.x; x[1] = v[1] + b0.y; x[2] = v[2] + b0.z; x[3] = v[3] + b0.w;
+  x[4] = v[4] + b1.x; x[5] = v[5] + b1.y; x[6] = v[6] + b1.z; x[7] = v[7] + b1.w;
+  float r[8];
+  if (e.res1) {
+    Elem<T>::ld8(reinterpret_cast<const T*>(e.res1) + pos * e.res1_cstride + e.res1_coff + n0, r);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] += r[i];
+  }
+  if (e.res2 && !e.res2_post) {
+    Elem<T>::ld8(reinterpret_cast<const T*>(e.res2) + pos * e.res2_cstride + e.res2_coff + n0, r);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] += r[i];
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (n0 + i < e.Cout) class_arg_take(a, x[i], n0 + i);
+}
 
 // Epilogue arithmetic for one output position `pos` and NV consecutive channels [n0, n0+NV) held in v[] (fp32
 // accumulators): v = acc + bias + res1 (+ res2); the optional second output (pre-activation value: channels-last or

@@ -4,6 +4,7 @@
 #pragma once
 #include "conv_common.cuh"
 #include "conv_tc.cuh"
+#include <type_traits>
 #include <utility>
 
 namespace occd_conv {
@@ -31,18 +32,20 @@ __host__ __device__ constexpr bool ping_pong(int n, long long tiles, long long c
 // arrivals that free a stage: one per MMA warp that reads it (4 per warpgroup)
 __host__ __device__ constexpr int empty_arrivals(bool pp) { return pp ? 4 : 8; }
 constexpr int kEmptyArrivals = 8;   // the halo kernels: both warpgroups read every stage
-// named barriers: 1 + wg: a warpgroup's epilogue staging; kTurnBar + wg: warpgroup wg may issue wgmma (ping-pong)
+// named barriers: 1 + wg: a warpgroup's epilogue staging / neighbour exchange; kTurnBar + wg: warpgroup wg may issue
+// wgmma (ping-pong)
 constexpr int kTurnBar = 3;
 // accumulator staging for the epilogue: [2 warpgroups][64 rows][LD floats].  The per-tap kernel stages rounds of
-// 32 columns (LD = kStageWide); the x-packed kernels rounds of 8 channels (xp_stage_ld); the halo kernel, whose
-// resident weights leave less shared memory, rounds of 8 columns (LD = kStageHalo)
+// 32 columns (LD = kStageWide); the halo kernel, whose resident weights leave less shared memory, rounds of 8 columns
+// (LD = kStageHalo)
 constexpr int kStageWide = 36;
 constexpr int kStageHalo = 10;
 __host__ __device__ constexpr int staging_bytes(int ld) { return 2 * 64 * ld * 4; }
-// x-packed staging: the 8-column blocks of all three column groups side by side (two barriers per round) for
-// N <= kPingPongMaxN; the wider tiles, whose resident weights in the halo kernel leave 4 KB less room, stage two
-// blocks and then the third (four barriers per round)
-__host__ __device__ constexpr int xp_stage_ld(int n) { return ping_pong(n) ? 26 : 18; }
+// The x-packed kernels keep the accumulator in registers and exchange only the W neighbours that cross a warp's 16
+// rows: per 16-channel chunk, every warp leaves the Q_0 of its last d rows and the Q_2 of its first d rows
+// ([4 warps][2][d][16] floats per warpgroup; d <= 8, the W dilation)
+__host__ __device__ constexpr int xp_xchg_floats(int d) { return 4 * 2 * d * 16; }
+__host__ __device__ constexpr int xp_xchg_bytes(int d) { return 2 * xp_xchg_floats(d) * 4; }
 
 struct TcParams {
   ConvEpi epi;
@@ -190,82 +193,114 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
   }
 }
 
-// Epilogue of the x-packed kernels: the accumulator holds three column groups Q_c (c = 0, 1, 2: the W taps -d, 0,
-// +d) of CP = N / 3 columns each and out[r] = Q_0[r - d] + Q_1[r] + Q_2[r + d], where r -+ d stays inside the line of PW
-// rows (lo_ok / hi_ok false: the neighbour is the conv's zero padding).  Rounds of 8 channels: the 8-column blocks of
-// Q_0, Q_1 and Q_2 are staged (xp_stage_ld) and threads 0..63 (one per row) form the sums.
-// The sums of up to 32 channels stay in registers and go through the row epilogue together, so that its bias and
-// residual loads are issued once per chunk rather than behind every round's barriers.  A class map instead feeds each
-// round's 8 sums straight into the row's running arg-max (one thread sees every channel of its row).
+// __shfl_sync of an accumulator value on an f32 register: with the intrinsic the compiler keeps the accumulator in
+// integer registers (shfl is a .b32 operation) and copies it into f32 registers around every wgmma, which breaks the
+// wgmma pipeline (ptxas injects warpgroup.arrive / wait and serialises)
+__device__ __forceinline__ float shfl_acc(float x, int src) {
+  float r;
+  asm volatile("shfl.sync.idx.b32 %0, %1, %2, 0x1f, 0xffffffff;" : "=f"(r) : "f"(x), "r"(src));
+  return r;
+}
+
+// The x-packed epilogue's view of a thread's two rows 16 w + l / 4 + {0, 8} (lane l of warp w): lo_ok / hi_ok
+// false where the W neighbour r - d / r + d falls outside the line, i.e. onto the conv's zero padding; and the
+// output position of the row whose channels the thread stores, 16 w + l / 4 + 8 ((l % 4) >> 1)
+struct XpRows {
+  bool lo_ok[2], hi_ok[2];
+  bool valid;
+  int od, oh, ow;
+};
+
+// Epilogue of the x-packed kernels, straight from the accumulator registers: the accumulator holds three column
+// groups Q_c (c = 0, 1, 2: the W taps -d, 0, +d) of CP = N / 3 columns each and out[r] = (Q_1[r] + Q_0[r - d]) +
+// Q_2[r + d], where r -+ d stays inside the line of rows.  In the m64nN fragment lane l of warp w holds rows
+// 16 w + l / 4 and + 8, columns 2 (l % 4) + {0, 1} of every 8-column block, so every thread
+// holds the same channels of Q_0, Q_1 and Q_2: a neighbour inside the warp's 16 rows is a shuffle from lane l -+ 4 d,
+// one in the next or previous warp comes through the exchange buffer xb (xp_xchg_floats(d) floats, this
+// warpgroup's).  Chunks of 16 channels: two barriers each.  The sums of a row's 8-channel block are then gathered
+// into one lane of the quad (a 4 x 4 transpose of channel pairs by shuffle), which runs the row epilogue on them;
+// a class map instead takes them into the row's running arg-max, and the two lanes of a row merge theirs.
 template <typename T, int N>
-__device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
-                                            int warp4, int lane, int t, int d, bool lo_ok, bool hi_ok, bool valid,
-                                            int b, int od, int oh, int ow) {
-  constexpr int LD = xp_stage_ld(N);
-  constexpr int Q2COL = LD >= 24 ? 16 : 0;   // column of Q_2's block: beside the others, or in Q_0's place later
+__device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* xb, int bar_id,
+                                            int warp4, int lane, int d, const XpRows& rows, int b) {
   constexpr int CP = N / 3;
-  constexpr int CH = CP < 32 ? CP : 32;   // channels per chunk
-  const bool mine = t < 64 && valid;
-  if (e.out1_mode == OCCD_OUT1_CLASS_U16) {
+  constexpr unsigned FULL = 0xffffffffu;
+  const int g = lane >> 2, q = lane & 3;
+  const int lo_src = (lane - 4 * d) & 31, hi_src = (lane + 4 * d) & 31;
+  const int wfl = 2 * d * 16;   // exchange floats per warp: [Q_0 of the last d rows, Q_2 of the first d rows][16]
+  float* const mine = xb + warp4 * wfl;
+  const bool my_valid = rows.valid;   // after the transpose this lane holds 8 channels of row 16 w + g + 8 (q >> 1)
+  // one copy of the chunk loop per output kind (CLS: class map), so that neither carries the other's registers
+  auto chunks = [&](auto cls) {
+    constexpr bool CLS = decltype(cls)::value;
     ClassArg ca = class_arg_init();
-    const long long pos = mine ? epi_pos(e, b, od, oh, ow) : 0;
+    const long long pos = CLS && my_valid ? epi_pos(e, b, rows.od, rows.oh, rows.ow) : 0;
 #pragma unroll
-    for (int c0 = 0; c0 < CP; c0 += 8) {
-      tc::wg_sync(bar_id);
-      stage8<LD, N>(st, acc, c0 >> 3, 0, warp4, lane);
-      stage8<LD, N>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
-      if constexpr (Q2COL != 0) stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, Q2COL, warp4, lane);
-      tc::wg_sync(bar_id);
-      // Q_1 + Q_0 goes back into this row's own Q_1 block, which no other thread reads, instead of staying in
-      // registers across the next staging
-      if (mine) {
+    for (int c0 = 0; c0 < CP; c0 += 16) {
+      tc::wg_sync(bar_id);   // the previous chunk's exchange reads are done
 #pragma unroll
-        for (int i = 0; i < 8; ++i) st[t * LD + 8 + i] += lo_ok ? st[(t - d) * LD + i] : 0.f;
-      }
-      if constexpr (Q2COL == 0) {
-        tc::wg_sync(bar_id);
-        stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
-        tc::wg_sync(bar_id);
-      }
-      if (mine) {
-#pragma unroll 1
-        for (int i = 0; i < 8 && c0 + i < e.Cout; ++i) {
-          const float x = st[t * LD + 8 + i] + (hi_ok ? st[(t + d) * LD + Q2COL + i] : 0.f);
-          class_arg_take(ca, class_value<T>(e, pos, c0 + i, x), c0 + i);
+      for (int jb = 0; jb < 2; ++jb)
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int c = 8 * jb + 2 * q + k;
+          const int j0 = 4 * ((c0 >> 3) + jb) + k, j2 = 4 * ((2 * CP + c0) >> 3) + 4 * jb + k;
+          if (g >= 8 - d) mine[(g - (8 - d)) * 16 + c] = acc[j0 + 2];
+          if (g < d) mine[(d + g) * 16 + c] = acc[j2];
         }
-      }
-    }
-    if (mine) class_store(e, pos, ca);
-    return;
-  }
-#pragma unroll
-  for (int c1 = 0; c1 < CP; c1 += CH) {
-    float v[CH];
-#pragma unroll
-    for (int j = 0; j < CH; j += 8) {
-      const int c0 = c1 + j;
-      if (c0 >= CP) break;
-      tc::wg_sync(bar_id);   // the previous round's reads are done
-      stage8<LD, N>(st, acc, c0 >> 3, 0, warp4, lane);
-      stage8<LD, N>(st, acc, (CP + c0) >> 3, 8, warp4, lane);
-      if constexpr (Q2COL != 0) stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, Q2COL, warp4, lane);
       tc::wg_sync(bar_id);
-      if (mine) {
+      float v[2][2][2];   // [row][8-channel block][channel of the pair]
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[j + i] = st[t * LD + 8 + i] + (lo_ok ? st[(t - d) * LD + i] : 0.f);
-      }
-      if constexpr (Q2COL == 0) {
-        tc::wg_sync(bar_id);
-        stage8<LD, N>(st, acc, (2 * CP + c0) >> 3, 0, warp4, lane);
-        tc::wg_sync(bar_id);
-      }
-      if (mine) {
+      for (int jb = 0; jb < 2; ++jb)
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[j + i] += hi_ok ? st[(t + d) * LD + Q2COL + i] : 0.f;
+        for (int k = 0; k < 2; ++k) {
+          const int c = 8 * jb + 2 * q + k;
+          const int j0 = 4 * ((c0 >> 3) + jb) + k, j1 = 4 * ((CP + c0) >> 3) + 4 * jb + k,
+                    j2 = 4 * ((2 * CP + c0) >> 3) + 4 * jb + k;
+          const float q0a = shfl_acc(acc[j0], lo_src), q0b = shfl_acc(acc[j0 + 2], lo_src);
+          const float q2a = shfl_acc(acc[j2], hi_src), q2b = shfl_acc(acc[j2 + 2], hi_src);
+          // row 16 w + g: Q_0 of row g - d (the previous warp's when g < d), Q_2 of row g + d
+          const float lo0 = g >= d ? q0a : (warp4 > 0 ? mine[g * 16 + c - wfl] : 0.f);
+          const float hi0 = g + d < 8 ? q2a : q2b;
+          // row 16 w + g + 8: Q_0 of row g + 8 - d, Q_2 of row g + 8 + d (the next warp's when g + d >= 8)
+          const float lo1 = g >= d ? q0b : q0a;
+          const float hi1 = g + d < 8 ? q2b : (warp4 < 3 ? mine[wfl + (2 * d + g - 8) * 16 + c] : 0.f);
+          v[0][jb][k] = acc[j1] + (rows.lo_ok[0] ? lo0 : 0.f);
+          v[0][jb][k] += rows.hi_ok[0] ? hi0 : 0.f;
+          v[1][jb][k] = acc[j1 + 2] + (rows.lo_ok[1] ? lo1 : 0.f);
+          v[1][jb][k] += rows.hi_ok[1] ? hi1 : 0.f;
+        }
+      // unit u = 2 * row + block: this lane holds its channel pair q; after the transpose o[p] is pair p of unit q
+      float2 u[4], o[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) o[i] = u[i] = make_float2(v[i >> 1][i & 1][0], v[i >> 1][i & 1][1]);
+#pragma unroll
+      for (int k = 1; k < 4; ++k) {
+        // lane q ^ k sends its pair of unit q while this lane sends its pair of unit q ^ k
+        const int pk = q ^ k;
+        float2 snd = u[0];
+#pragma unroll
+        for (int i = 1; i < 4; ++i) snd = pk == i ? u[i] : snd;
+        const float2 r = make_float2(__shfl_xor_sync(FULL, snd.x, k), __shfl_xor_sync(FULL, snd.y, k));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o[i] = pk == i ? r : o[i];
+      }
+      float w8[8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { w8[2 * i] = o[i].x; w8[2 * i + 1] = o[i].y; }
+      const int n0 = c0 + 8 * (q & 1);
+      if constexpr (CLS) {
+        if (my_valid && n0 < e.Cout) class_take8<T>(e, pos, n0, w8, ca);
+      } else {
+        if (my_valid) conv_epilogue_row<T, 8>(e, b, rows.od, rows.oh, rows.ow, n0, w8);
       }
     }
-    if (mine) conv_epilogue_row<T, CH>(e, b, od, oh, ow, c1, v);
-  }
+    if constexpr (CLS) {
+      class_arg_merge_xor(ca, 1);   // lanes q and q ^ 1 hold the two blocks of each chunk of one row
+      if ((q & 1) == 0 && my_valid) class_store(e, pos, ca);
+    }
+  };
+  if (e.out1_mode == OCCD_OUT1_CLASS_U16) chunks(std::true_type{});
+  else chunks(std::false_type{});
 }
 
 __device__ __forceinline__ void pdl_prologue_done(int pdl) {
@@ -295,11 +330,11 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_a + (uint32_t)(p.stages * p.group) * p.a_bytes;
-  constexpr int LD = XP ? xp_stage_ld(N) : kStageWide;
+  constexpr int LD = kStageWide;
   static_assert(!PP || ping_pong(N), "ping-pong holds N accumulator registers per thread");
   constexpr int NH = PP ? 2 : 1;   // 64-row halves of the M tile in one warpgroup's accumulator
   const uint32_t smem_st = smem_b + (uint32_t)(p.stages * p.group) * p.b_stride;
-  const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
+  const uint32_t bar_base = smem_st + (uint32_t)(XP ? xp_xchg_bytes(1) : staging_bytes(LD));
   const uint32_t full_bar = bar_base;
   const uint32_t empty_bar = bar_base + 8u * kMaxStages;
 
@@ -377,7 +412,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
   const int wg = (warp >> 2) - 1;
   const int warp4 = warp & 3;
   const int t = threadIdx.x & 127;
-  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
+  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) +
+              wg * (XP ? xp_xchg_floats(1) : 64 * LD);
   const int nmma = RB / 32;
   const uint64_t a_half = (uint64_t)(64 * RB / 16);
   const uint64_t da0 = tc::make_sdesc(smem_a, RB) + (PP ? 0 : wg * a_half);
@@ -427,13 +463,15 @@ conv_tc_kernel(const __grid_constant__ TcParams p, const __grid_constant__ CUten
       const int r64 = 64 * (PP ? h : wg);   // first row of this 64-row half of the M tile
       if constexpr (XP) {
         // TW == 32: row == tile column inside each 32-row line, so the W neighbours' partial sums are rows r -+ 1
-        const int row = r64 + t;
+        // (the line's first and last rows are halo columns, never stored)
+        const int row = r64 + 16 * warp4 + (lane >> 2) + 8 * ((lane & 3) >> 1);
         const int rw = row % 32;
         const int rh = (row / 32) % p.TH;
         const int rd = row / (32 * p.TH);
         const int od = td * p.TD + rd, oh = th * p.TH + rh, ow = tw * 30 + rw - 1;
-        const bool valid = t < 64 && od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && rw >= 1 && rw <= 30;
-        epilogue_xp<T, N>(p.epi, acc[h], st, 1 + wg, warp4, lane, t, 1, true, true, valid, b, od, oh, ow);
+        const XpRows rows{{true, true}, {true, true},
+                          od < p.epi.OD && oh < p.epi.OH && ow < p.epi.OW && rw >= 1 && rw <= 30, od, oh, ow};
+        epilogue_xp<T, N>(p.epi, acc[h], st, 1 + wg, warp4, lane, 1, rows, b);
       } else {
         const int row = r64 + (t >> 1);
         const int rw = row % p.TW;
@@ -639,11 +677,10 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_w = smem_base;                                   // [n_groups][b_stride] resident weights
   const uint32_t smem_a = smem_w + (uint32_t)p.w_bytes;                 // [stages][a_stage_bytes]
-  constexpr int LD = xp_stage_ld(N);
   static_assert(!PP || ping_pong(N), "ping-pong holds N accumulator registers per thread");
   constexpr int NH = PP ? 2 : 1;
-  const uint32_t smem_st = smem_a + (uint32_t)p.stages * p.a_stage_bytes;
-  const uint32_t bar_base = smem_st + (uint32_t)staging_bytes(LD);
+  const uint32_t smem_st = smem_a + (uint32_t)p.stages * p.a_stage_bytes;   // neighbour exchange (xp_xchg_bytes)
+  const uint32_t bar_base = smem_st + (uint32_t)xp_xchg_bytes(p.d);
   const uint32_t full_bar = bar_base;            // [4]
   const uint32_t empty_bar = bar_base + 32u;     // [4]
   const uint32_t w_bar = bar_base + 64u;
@@ -684,8 +721,9 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   // ring mode: position in the plane sequence -> (batch, residue class, H tile) and the run of planes [z0, z1) this CTA
   // takes from that column
   auto decode_ring = [&](long long pos, int& b, int& ra, int& rb, int& th, int& z0, int& z1) {
-    int t = (int)(pos / p.sD);
-    z0 = (int)(pos - (long long)t * p.sD);
+    const int ip = (int)pos;   // < n_cols * sD, an M-tile count (int, like num_tiles): a 32-bit division
+    int t = ip / p.sD;
+    z0 = ip - t * p.sD;
     const long long left = ring_hi - pos;
     z1 = (long long)(p.sD - z0) < left ? p.sD : z0 + (int)left;
     th = t % p.tilesH; t /= p.tilesH;
@@ -738,8 +776,7 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   tc::reg_alloc<232>();
   const int wg = (warp >> 2) - 1;
   const int warp4 = warp & 3;
-  const int t = threadIdx.x & 127;
-  float* st = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * 64 * LD;
+  float* xb = reinterpret_cast<float*>(smem_raw + (smem_st - tc::smem_u32(smem_raw))) + wg * xp_xchg_floats(d);
   const int nmma = RB / 32;
   const uint64_t db_w = tc::make_sdesc(smem_w, RB);
   const int w_step16 = p.b_stride / 16;
@@ -750,12 +787,14 @@ conv_halox_kernel(const __grid_constant__ HaloxParams p, const __grid_constant__
   auto tile_epilogue = [&](int b, int ra, int rb, int od, int oh_base) {
 #pragma unroll
     for (int h = 0; h < NH; ++h) {
-      const int rr = 64 * (PP ? h : wg) + t;   // row inside the M tile (epilogue threads t < 64)
+      const int r0 = 64 * (PP ? h : wg) + 16 * warp4 + (lane >> 2);   // the thread's first row inside the M tile
+      const int pw0 = r0 % p.PW, pw1 = (r0 + 8) % p.PW;                // == output w
+      const int rr = r0 + 8 * ((lane & 3) >> 1);                         // the row it stores
       const int hr = rr / p.PW;                // h-row inside the M tile
-      const int pw = rr - hr * p.PW;           // == output w
       const int oh = (oh_base + hr) * d + rb;
-      const bool valid = t < 64 && od < p.D && oh < p.H;
-      epilogue_xp<T, N>(p.epi, acc[h], st, 1 + wg, warp4, lane, t, d, pw >= d, pw + d < p.PW, valid, b, od, oh, pw);
+      const XpRows rows{{pw0 >= d, pw1 >= d}, {pw0 + d < p.PW, pw1 + d < p.PW}, od < p.D && oh < p.H, od, oh,
+                        rr - hr * p.PW};
+      epilogue_xp<T, N>(p.epi, acc[h], xb, 1 + wg, warp4, lane, d, rows, b);
     }
   };
   tc::mbar_wait(w_bar, 0);
