@@ -429,6 +429,78 @@ int occd_occupied_voxels(const uint16_t* class_map, const uint8_t* fov_mask, int
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,
                           int cs_in, int cs_out, int dh, int dw, float bf_scale, void* stream);
 
+/* -------------------------------------------------------------------------------------------- */
+/* Model files: one camera frame in, the class map out, without Python.  occdepth_b200.deploy.export writes the   */
+/* launch list of a model's class-map plan (OccDepth.predict_frame) with its weights and constant tables; the      */
+/* calls below load it and replay it (file layout: DESIGN.md section 9).                                          */
+#define OCCD_OK 0
+#define OCCD_ERR_ARG 1         /* bad argument                                                    */
+#define OCCD_ERR_CUDA 2        /* CUDA runtime / driver error                                     */
+#define OCCD_ERR_UNSUPPORTED 3 /* e.g. a model file of another format or ABI version              */
+#define OCCD_ERR_FORMAT 4      /* not a model file: bad magic, truncated, unknown entry point,    */
+                               /* an index or pointer fix-up outside its table or buffer          */
+#define OCCD_ERR_IO 5          /* the file cannot be opened or read                              */
+#define OCCD_MODEL_FORMAT_VERSION 1
+#define OCCD_FRAME_NO_GRAPH 1  /* occd_frame.flags: launch the records one by one, no CUDA graph  */
+
+typedef struct occd_model occd_model;
+
+typedef struct {
+  int precision;          /* OCCD_DTYPE_F32 (tf32 plan) or OCCD_DTYPE_BF16                             */
+  int dataset;            /* 0 KITTI, 1 NYU                                                            */
+  int V;                  /* images per frame                                                          */
+  int img_h, img_w;       /* the crop the network sees (raw images may be larger)                     */
+  int project_scale;
+  int X, Y, Z;            /* the output class map: uint16 [X][Y][Z]                                   */
+  int n_classes;
+  int has_depth;          /* NYU virtual right view: occd_frame.depth is required                     */
+  int depth_h, depth_w;
+  int flosp_depth;        /* the FlospDepth prior: camera tables are rebuilt with the calibration     */
+  int graph;              /* 1 once the replay has been captured into a CUDA graph                    */
+  long long device_bytes; /* device memory the model holds                                            */
+  double voxel_size, vox_origin[3], scene_size[3]; /* the default geometry (vox_origin: KITTI's)     */
+} occd_model_geom;
+
+typedef struct {
+  const void* images;           /* DEVICE uint8 RGB (V, H0, W0, 3); image i, row y at images + i*img_stride + */
+  long long img_stride;         /* y*row_stride bytes; pixels are 3 contiguous bytes                         */
+  long long row_stride;
+  int H0, W0;                   /* raw size, >= the model's img_h x img_w                                   */
+  const void* cam_k;            /* HOST: KITTI (V, 3, 3); NYU (3, 3) or NULL for the dataset's default      */
+  const void* pose;             /* HOST: KITTI T_velo_2_cam (V, 4, 4); NYU T_world_2_cam (4, 4), the inverse */
+                                /* of the camera pose (the dataset's np.linalg.inv(cam_pose))               */
+  int calib_f32;                /* cam_k and pose are float32 (1) or float64 (0)                            */
+  const double* vox_origin;     /* HOST 3 doubles; required for NYU; NULL: the model's default             */
+  const double* scene_size;     /* HOST 3 doubles or NULL: the model's                                      */
+  double voxel_size;            /* 0: the model's                                                           */
+  const uint16_t* depth;        /* DEVICE uint16 depth PNG (depth_h, depth_w), when geom.has_depth          */
+  int depth_h, depth_w;
+  int flags;                    /* OCCD_FRAME_*                                                             */
+} occd_frame;
+
+/* Reads and validates the whole file before touching a device, then allocates and uploads on the current device   */
+/* and creates the convolution plans.  On failure *m is NULL and nothing is left allocated.                          */
+int occd_model_load(const char* path, occd_model** m);
+int occd_model_info(const occd_model* m, occd_model_geom* geom);
+/* One frame -> class_map (DEVICE uint16 [X][Y][Z], the caller's) on `stream`: the images are cropped and normalised */
+/* into the plan's input buffer, NYU's depth map converted, and -- when the calibration differs from the last       */
+/* frame's, and for every NYU frame -- the projection indices and FlospDepth camera tables are rebuilt.  Then the   */
+/* records are replayed: the first run launches them one by one and captures them into a CUDA graph, later runs     */
+/* launch the graph (OCCD_FRAME_NO_GRAPH: always one by one).  Allocates nothing per frame; calls on one model must  */
+/* not overlap.                                                                                                    */
+int occd_model_run_frame(occd_model* m, const occd_frame* frame, uint16_t* class_map, void* stream);
+int occd_model_destroy(occd_model* m);
+
+/* FlospDepth's per-camera tables on the host (FlospDepth.camera_tables of occdepth_b200, flosp_depth.py:466-541),  */
+/* bit for bit: cams[v] = {rows 0..2 of T[v] @ grid_to_lidar, rows 0..2 of K4[v], identity ida} (40 floats) and      */
+/* scaled_pixel_size[v] = |(1/fx, 1/fy)| * 1000, all float32 after casting cam_k (n_cams 3x3) and T (n_cams 4x4)     */
+/* from float64, or float32 when inputs_f32.  grid_to_lidar: 16 floats, or NULL with nyu_vox_origin (3 doubles):     */
+/* NYU's grid from that origin (extent 4.8 x 4.8 x 2.88 m, 0.08 m voxels / project_scale).  voxel_num (3 ints, or   */
+/* NULL) receives the NYU grid's dimensions.  HOST pointers only.                                                    */
+int occd_flosp_camera_tables(int n_cams, const void* cam_k, const void* T, int inputs_f32, const float* grid_to_lidar,
+                             const double* nyu_vox_origin, int project_scale, float* cams, float* scaled_pixel_size,
+                             int* voxel_num);
+
 #ifdef __cplusplus
 }
 #endif

@@ -96,7 +96,33 @@ def build(verbose=False, force=False):
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
+    build_occd_run(nvcc, force=jobs or force)
     return out
+
+
+def occd_run_path():
+    return os.path.join(LIBDIR, "occd_run")
+
+
+def build_occd_run(nvcc, force=False):
+    """tools/occd_run.c: a plain C program linked against libocc_b200.so (found next to it) and the CUDA runtime"""
+    src = os.path.join(HERE, "..", "tools", "occd_run.c")
+    hdr = os.path.join(HERE, "..", "include", "occdepth_b200.h")
+    h = hashlib.sha1()
+    for p in (src, hdr):
+        with open(p, "rb") as f:
+            h.update(f.read())
+    exe, stamp = occd_run_path(), occd_run_path() + ".sha1"
+    if not force and os.path.exists(exe) and os.path.exists(stamp) and open(stamp).read().strip() == h.hexdigest():
+        return exe
+    cmd = [nvcc, "-O2", "-x", "c", src, "-I", os.path.dirname(hdr), "-L", LIBDIR, "-locc_b200",
+           "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN", "-o", exe]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("occd_run build failed:\n" + r.stdout + r.stderr)
+    with open(stamp, "w") as f:
+        f.write(h.hexdigest())
+    return exe
 
 
 if __name__ == "__main__":

@@ -5,6 +5,7 @@ libocc_b200.so has not been built (python -m occdepth_b200._build / __graft_entr
 """
 import ctypes as C
 import os
+import threading
 
 from . import _build
 
@@ -47,7 +48,27 @@ CONV_MAX_TAPS, CONV_MAX_SRC, CONV_MAX_GROUPS = 81, 3, 8
 CONV_IMPL_TC, CONV_IMPL_SIMT, CONV_IMPL_HALO, CONV_IMPL_HALOX, CONV_IMPL_TCX, CONV_IMPL_AUTO = 0, 1, 2, 3, 4, 5
 OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16 = 0, 1, 2, 3
 CLASS_LUT_MAX = 64
-ERR_ARG, ERR_CUDA, ERR_UNSUPPORTED = 1, 2, 3
+ERR_ARG, ERR_CUDA, ERR_UNSUPPORTED, ERR_FORMAT, ERR_IO = 1, 2, 3, 4, 5
+MODEL_FORMAT_VERSION = 1
+FRAME_NO_GRAPH = 1
+
+
+class ModelGeom(C.Structure):
+    """occd_model_geom"""
+    _fields_ = [("precision", C.c_int), ("dataset", C.c_int), ("V", C.c_int), ("img_h", C.c_int),
+                ("img_w", C.c_int), ("project_scale", C.c_int), ("X", C.c_int), ("Y", C.c_int), ("Z", C.c_int),
+                ("n_classes", C.c_int), ("has_depth", C.c_int), ("depth_h", C.c_int), ("depth_w", C.c_int),
+                ("flosp_depth", C.c_int), ("graph", C.c_int), ("device_bytes", C.c_longlong),
+                ("voxel_size", C.c_double), ("vox_origin", C.c_double * 3), ("scene_size", C.c_double * 3)]
+
+
+class Frame(C.Structure):
+    """occd_frame"""
+    _fields_ = [("images", C.c_void_p), ("img_stride", C.c_longlong), ("row_stride", C.c_longlong),
+                ("H0", C.c_int), ("W0", C.c_int), ("cam_k", C.c_void_p), ("pose", C.c_void_p),
+                ("calib_f32", C.c_int), ("vox_origin", C.c_void_p), ("scene_size", C.c_void_p),
+                ("voxel_size", C.c_double), ("depth", C.c_void_p), ("depth_h", C.c_int), ("depth_w", C.c_int),
+                ("flags", C.c_int)]
 
 
 class ConvTap(C.Structure):
@@ -139,6 +160,11 @@ SYMBOLS = {
     "occd_depth_cls_sums": (C.c_int, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, C.c_double, C.c_double, _vp, _vp, _ll,
                                       _vp]),
     "occd_occupied_voxels": (C.c_int, [_vp, _vp] + [_i] * 9 + [_vp] * 5 + [C.c_double, _vp, _vp, _ll, _vp]),
+    "occd_model_load": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
+    "occd_model_info": (C.c_int, [_vp, C.POINTER(ModelGeom)]),
+    "occd_model_run_frame": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp]),
+    "occd_model_destroy": (C.c_int, [_vp]),
+    "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
 }
 VOXEL_TILE = 2048
 
@@ -159,9 +185,17 @@ def ssc_loss_sums_len(C, F):
     return 6 + 3 * C + F * C
 
 
+# deploy.export: while its thread has `recorder` set, lib() returns that stand-in there (which records the calls it
+# forwards); other threads keep the library
+_RECORDING = threading.local()
+
+
 def lib():
     """Load libocc_b200.so (once).  Fails loudly when it is missing -- never falls back."""
     global _LIB
+    rec = getattr(_RECORDING, "recorder", None)
+    if rec is not None:
+        return rec
     if _LIB is None:
         path = _build.lib_path()
         if not os.path.exists(path):

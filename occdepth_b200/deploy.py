@@ -1,0 +1,385 @@
+"""Python-free deployment: export a model's camera-frame class-map plan to one self-contained model file, which
+libocc_b200.so loads and replays from C (`occd_model_load` / `occd_model_run_frame`, include/occdepth_b200.h;
+tools/occd_run.c is a standalone consumer).  The file layout is documented in DESIGN.md section 9.
+
+The export records, it does not re-describe: the plan is built by the same `OccDepth._build` that
+`predict_frame` uses, while `_lib.lib()` returns a recording stand-in, and then run once through it.  Every call the
+run makes becomes a record (entry point name + arguments typed by `_lib.SYMBOLS`); device pointers become
+(buffer, offset) pairs into the storages the plan holds, host structs and arrays become byte blobs with pointer
+fix-ups, and convolution plans are stored as the descriptors they were created from.  No model code knows about
+export, so a launch a model adds later is exported as it is.
+"""
+import bisect
+import ctypes as C
+import os
+import struct
+
+import numpy as np
+import torch
+
+from . import _lib
+from .engine import CL, ConvOp
+
+MAGIC = b"OCCDMODL"
+ROLES = ("img", "pix", "fov", "pix_z", "depth", "cams", "sps", "classes")
+FLAG_FLOSP_DEPTH, FLAG_VIRTUAL = 1, 2
+PATTERN_MAX = 64
+
+_STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
+_PASS_THROUGH = {"occd_last_error", "occd_abi_version", "occd_conv_plan_info", "occd_conv_plan_impl",
+                 "occd_conv_plan_schedule"}
+
+
+class ExportError(RuntimeError):
+    """the plan holds something a model file cannot carry (a pointer outside every buffer the plan holds, an
+    argument of unknown kind)"""
+
+
+def _ptr_offsets(t, base=0):
+    """byte offsets of the c_void_p fields of ctypes type `t` (structs and arrays, recursively)"""
+    if t is C.c_void_p:
+        return [base]
+    if isinstance(t, type) and issubclass(t, C.Array):
+        step = C.sizeof(t._type_)
+        return [o for i in range(t._length_) for o in _ptr_offsets(t._type_, base + i * step)]
+    if isinstance(t, type) and issubclass(t, C.Structure):
+        return [o for f in t._fields_ for o in _ptr_offsets(f[1], base + getattr(t, f[0]).offset)]
+    return []
+
+
+def _host_blob(obj):
+    """ctypes object -> (bytes, [(offset, pointer value)]) of its host memory and the device pointers inside it"""
+    raw = bytearray(C.string_at(C.addressof(obj), C.sizeof(obj)))
+    ptrs = []
+    for off in _ptr_offsets(type(obj)):
+        v = int.from_bytes(raw[off:off + 8], "little")
+        if v:
+            ptrs.append((off, v))
+            raw[off:off + 8] = bytes(8)
+    return bytes(raw), ptrs
+
+
+class _Recorder:
+    """stands in for the loaded library: forwards every call while the plan is built (recording the convolution
+    plans created and their class LUTs), then records without executing while the plan runs"""
+
+    def __init__(self, real):
+        self._real = real
+        self.recording = False
+        self.plans = {}            # handle value -> [descriptor blob, (lut bytes, n) or None]
+        self.calls = []            # (entry point, [raw argument])
+
+    def __getattr__(self, name):
+        fn = getattr(self._real, name)
+        if name not in _lib.SYMBOLS:
+            return fn
+        argtypes = _lib.SYMBOLS[name][1]
+
+        def call(*args):
+            if not self.recording or name in _PASS_THROUGH:
+                rc = fn(*args)
+                if rc == 0 and name == "occd_conv_plan_create":
+                    self.plans[args[1]._obj.value] = [_host_blob(args[0]._obj), None]
+                elif rc == 0 and name == "occd_conv_plan_set_class_lut":
+                    lut = None if args[1] is None else (bytes(args[1]), int(args[2]))
+                    self.plans[_handle(args[0])][1] = lut
+                return rc
+            self.calls.append((name, [self._arg(name, i, a, t) for i, (a, t) in enumerate(zip(args, argtypes))]))
+            return 0
+        return call
+
+    def _arg(self, name, i, a, t):
+        if t is C.c_int or t is C.c_longlong:
+            return ("i" if t is C.c_int else "l", int(getattr(a, "value", a)))
+        if t is C.c_float or t is C.c_double:
+            return ("f" if t is C.c_float else "d", float(getattr(a, "value", a)))
+        if a is _STREAM:
+            return ("s",)
+        if name == "occd_conv_run" and i == 0:
+            h = _handle(a)
+            if h not in self.plans:
+                raise ExportError("export: occd_conv_run argument 0: a convolution plan created outside the build")
+            return ("c", h)
+        if a is None:
+            return ("n",)
+        if type(a).__name__ == "CArgObject":               # C.byref(struct)
+            return ("h", _host_blob(a._obj))
+        if isinstance(a, (C.Array, C.Structure)):
+            return ("h", _host_blob(a))
+        v = a.value if isinstance(a, C.c_void_p) else a
+        if v is None or (isinstance(v, (int, np.integer)) and int(v) == 0):
+            return ("n",)
+        if isinstance(v, (int, np.integer)):
+            return ("p", int(v))
+        raise ExportError("export: %s argument %d: cannot record a %s" % (name, i, type(a).__name__))
+
+
+def _handle(h):
+    return h.value if isinstance(h, C.c_void_p) else int(h)
+
+
+def _collect(obj, out):
+    if isinstance(obj, torch.Tensor):
+        out.append(obj)
+    elif isinstance(obj, CL):
+        out.append(obj.buf)
+    elif isinstance(obj, (list, tuple)):
+        for x in obj:
+            _collect(x, out)
+    elif isinstance(obj, dict):
+        for x in obj.values():
+            _collect(x, out)
+
+
+class _Buffers:
+    """the device storages a plan holds, overlapping ones merged, with their contents"""
+
+    def __init__(self, tensors):
+        spans = {}
+        for t in tensors:
+            if t.is_cuda:
+                s = t.untyped_storage()
+                spans[s.data_ptr()] = s
+        iv = []                                         # [base, end, [storages]]
+        for base in sorted(spans):
+            s = spans[base]
+            end = base + s.nbytes()
+            if iv and base < iv[-1][1]:
+                iv[-1][1] = max(iv[-1][1], end)
+                iv[-1][2].append(s)
+            else:
+                iv.append([base, end, [s]])
+        self.iv = iv
+        self.bases = [b for b, _, _ in iv]
+
+    def place(self, p, what):
+        k = bisect.bisect_right(self.bases, p) - 1
+        if k < 0 or not p < self.iv[k][1]:
+            raise ExportError("export: %s: pointer 0x%x lands in no buffer the plan holds" % (what, p))
+        return k, p - self.iv[k][0]
+
+    def contents(self, k):
+        """bytes of buffer k, or None when it is all zeros"""
+        base, end, storages = self.iv[k]
+        out = np.zeros(end - base, dtype=np.uint8)
+        for s in storages:
+            u8 = torch.empty(0, dtype=torch.uint8, device=s.device).set_(s, 0, (s.nbytes(),), (1,))
+            o = s.data_ptr() - base
+            out[o:o + s.nbytes()] = u8.cpu().numpy()
+        return out.tobytes() if out.any() else None
+
+
+def export(model, path, frame, inv_map=None):
+    """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map)` for frames of this
+    frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame refuses, with the
+    same messages.  Returns a dict of what was written (records, buffers, bytes).
+
+    The recording stand-in replaces the library for the calling thread only, so other threads may keep serving
+    through the library meanwhile; `model` itself must not run elsewhere during the export (as for predict_frame)."""
+    from . import data as D
+    f = model._frame_checked(frame)
+    lut = model._class_lut(inv_map)
+    dev = f["imgs"].device
+    rec = _Recorder(_lib.lib())
+    with torch.cuda.device(dev), torch.no_grad():
+        _lib._RECORDING.recorder = rec
+        try:
+            ent = model._build(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"], classes=("classes", lut),
+                               capture=False)
+            plan, img_cl, pix, fov, out, depth0 = ent[:6]
+            plan.pix_z = torch.zeros(pix.shape[2], dtype=torch.float64, device=dev)
+            state = getattr(plan, "flosp_state", None)
+            tensors = []
+            for op in plan.ops:
+                _collect(getattr(op, "_keep", ()), tensors)
+                if isinstance(op, ConvOp):
+                    tensors += [op.weight, op.bias]
+            _collect([img_cl, pix, fov, out, depth0, plan.pix_z, state], tensors)
+            torch.cuda.synchronize()
+            bufs = _Buffers(tensors)
+            contents = [bufs.contents(k) for k in range(len(bufs.iv))]     # before the run: activations are zero
+            rec.recording = True
+            plan.run(_STREAM)
+        finally:
+            rec.recording = False
+            _lib._RECORDING.recorder = None
+
+    blobs, plan_ids = [], {}
+
+    def blob(b, what):
+        data, ptrs = b
+        blobs.append((data, [(o,) + bufs.place(v, what) for o, v in ptrs]))
+        return len(blobs) - 1
+
+    records = []
+    for name, args in rec.calls:
+        enc = []
+        for i, a in enumerate(args):
+            what = "%s argument %d" % (name, i)
+            if a[0] == "p":
+                enc.append(("p",) + bufs.place(a[1], what))
+            elif a[0] == "h":
+                enc.append(("h", blob(a[1], what)))
+            elif a[0] == "c":
+                if a[1] not in plan_ids:
+                    plan_ids[a[1]] = len(plan_ids)
+                enc.append(("c", plan_ids[a[1]]))
+            else:
+                enc.append(a)
+        records.append((name, enc))
+    plans = []
+    for h, pid in sorted(plan_ids.items(), key=lambda kv: kv[1]):
+        desc, lut_rec = rec.plans[h]
+        d = blob(desc, "occd_conv_plan_create descriptor")
+        if lut_rec is None:
+            plans.append((d, -1, 0))
+        else:
+            blobs.append((lut_rec[0], []))
+            plans.append((d, len(blobs) - 1, lut_rec[1]))
+
+    def role(t):
+        if t is None:
+            return (-1, 0, 0)
+        assert t.is_contiguous()
+        k, off = bufs.place(t.data_ptr(), "role buffer")
+        return (k, off, t.numel() * t.element_size())
+
+    roles = [role(img_cl.buf), role(pix), role(fov), role(plan.pix_z), role(depth0),
+             role(state["cams"] if state else None), role(state["sps"] if state else None), role(out)]
+    flosp = model.trans_2d_to_3d == "flosp_depth"
+    nyu = model.dataset == "NYU"
+    G = np.zeros(16, np.float32)
+    n_cams, vn = 0, (0, 0, 0)
+    if flosp:
+        n_cams, vn = int(state["n_cams"]), tuple(int(v) for v in state["vn"])
+        if not nyu:
+            G = model.flosp_depth._grid_to_lidar(None)[0].numpy().reshape(-1)
+    pattern = np.zeros((PATTERN_MAX, 2), np.int32)
+    pattern[:f["P"]] = np.asarray(D.PIXEL_PATTERNS[f["pattern_id"]], np.int32)
+    lut_arr = np.zeros(_lib.CLASS_LUT_MAX, np.int32)
+    if lut is not None:
+        lut_arr[:len(lut)] = lut
+    S = [int(s) // model.project_scale for s in model.full_scene_size]
+    hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
+                              1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0),
+                              f["V"], f["H"], f["W"], model.project_scale),
+           struct.pack("<7I", *S, *out.shape[1:], f["P"]), pattern.astype("<i4").tobytes(),
+           struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
+                       *[float(v) for v in f["scene_size"]]),
+           struct.pack("<2I", model.n_classes, 0 if lut is None else 1), lut_arr.astype("<i4").tobytes(),
+           struct.pack("<d3I", float(f["virtual_bf"]), *(depth0.shape if depth0 is not None else (0, 0)), n_cams),
+           struct.pack("<3I", *vn),
+           G.astype("<f4").tobytes(), struct.pack("<I", img_cl.cstride)]
+    hdr += [struct.pack("<iQQ", *r) for r in roles]
+    hdr.append(struct.pack("<4I", len(bufs.iv), len(blobs), len(plans), len(records)))
+    n_bytes = 0
+    with open(path, "wb") as fh:
+        def w(b):
+            nonlocal n_bytes
+            fh.write(b)
+            n_bytes += len(b)
+        for b in hdr:
+            w(b)
+        for k, (base, end, _) in enumerate(bufs.iv):
+            w(struct.pack("<QI", end - base, 0 if contents[k] is None else 1))
+            if contents[k] is not None:
+                w(contents[k])
+        for data, fix in blobs:
+            w(struct.pack("<Q", len(data)) + data + struct.pack("<I", len(fix)))
+            for o, k, off in fix:
+                w(struct.pack("<QIQ", o, k, off))
+        for p in plans:
+            w(struct.pack("<IiI", *p))
+        for name, enc in records:
+            nm = name.encode()
+            w(struct.pack("<H", len(nm)) + nm + struct.pack("<I", len(enc)))
+            for a in enc:
+                tag = a[0].encode()
+                if a[0] == "p":
+                    w(tag + struct.pack("<IQ", a[1], a[2]))
+                elif a[0] in "hc":
+                    w(tag + struct.pack("<I", a[1]))
+                elif a[0] in "ilfd":
+                    w(tag + struct.pack("<" + {"i": "i", "l": "q", "f": "f", "d": "d"}[a[0]], a[1]))
+                else:
+                    w(tag)
+    return dict(records=len(records), buffers=len(bufs.iv), plans=len(plans), bytes=n_bytes,
+                data_buffers=sum(c is not None for c in contents))
+
+
+class LoadedModel:
+    """ctypes handle of a model file loaded by the C runtime (occd_model_load), for Python callers that want the
+    Python-free route's results: `run_frame` takes the frame dict of OccDepth.predict_frame."""
+
+    def __init__(self, path):
+        L = _lib.lib()
+        h = C.c_void_p()
+        _lib.check(L.occd_model_load(os.fsencode(path), C.byref(h)), "occd_model_load(%s)" % path)
+        self.handle = h
+        self.geom = self.info()
+
+    def info(self):
+        g = _lib.ModelGeom()
+        _lib.check(_lib.lib().occd_model_info(self.handle, C.byref(g)), "occd_model_info")
+        return g
+
+    def run_frame(self, frame, out=None, stream=None, graph=True):
+        """frame: as OccDepth.predict_frame takes it (the uint8 images may be on the host or the device) -> the
+        uint16 class map [1, X, Y, Z] on the current device, enqueued on `stream` (default: the current stream)"""
+        g = self.geom
+        img = torch.as_tensor(frame["img"])
+        if img.dim() == 3:
+            img = img.unsqueeze(0)
+        img = img.contiguous().cuda()
+        keep = [img]
+
+        def host(a, dt=np.float64):
+            a = np.ascontiguousarray(np.asarray(a, dt))
+            keep.append(a)
+            return a.ctypes.data
+
+        f = _lib.Frame()
+        f.images, f.H0, f.W0 = img.data_ptr(), img.shape[1], img.shape[2]
+        f.img_stride, f.row_stride = img.stride(0), img.stride(1)
+        # a float32 pose is applied in float32, as predict_frame does; cam_k then goes in the same type
+        pose = np.asarray(frame["cam_pose"] if g.dataset == 1 else frame["T_velo_2_cam"])
+        f.calib_f32 = 1 if pose.dtype == np.float32 else 0
+        cdt = np.float32 if f.calib_f32 else np.float64
+        if g.dataset == 1:
+            f.pose = host(np.linalg.inv(pose), cdt)
+            f.cam_k = host(frame["cam_k"], cdt) if "cam_k" in frame else None
+            f.vox_origin = host(frame["vox_origin"])
+            if g.has_depth:
+                d = torch.as_tensor(frame["depth"]).contiguous().cuda()
+                keep.append(d)
+                f.depth, f.depth_h, f.depth_w = d.data_ptr(), d.shape[0], d.shape[1]
+        else:
+            f.cam_k, f.pose = host(frame["cam_k"], cdt), host(pose, cdt)
+            if "vox_origin" in frame:
+                f.vox_origin = host(frame["vox_origin"])
+        if "scene_size" in frame:
+            f.scene_size = host(frame["scene_size"])
+        f.voxel_size = float(frame.get("voxel_size", 0.0))
+        f.flags = 0 if graph else _lib.FRAME_NO_GRAPH
+        if out is None:
+            out = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.uint16, device=img.device)
+        if stream is not None:
+            # the inputs were copied and `out` allocated on the current stream; they must live until `stream` is done
+            stream.wait_stream(torch.cuda.current_stream())
+            for t in [k for k in keep if isinstance(k, torch.Tensor)] + [out]:
+                t.record_stream(stream)
+        st = (stream or torch.cuda.current_stream()).cuda_stream
+        _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), out.data_ptr(), C.c_void_p(st)),
+                   "occd_model_run_frame")
+        return out
+
+    def close(self):
+        if self.handle:
+            _lib.lib().occd_model_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass

@@ -144,9 +144,10 @@ class OccDepth(_Base, B200Module):
             raise NotImplementedError(f"{self.trans_2d_to_3d} is not supported yet.")
 
     # ------------------------------------------------------------------------------------------
-    def _build(self, B, V, H, W, N, P, dev, batch, classes=None):
+    def _build(self, B, V, H, W, N, P, dev, batch, classes=None, capture=True):
         """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut): the plan of
-        predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor)"""
+        predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor).  capture=False: no
+        CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says"""
         slab = self.__dict__.get("slab_ctx")
         plan = Plan(dev, slab=slab, precision=self.precision)
         ps = self.project_scale
@@ -271,7 +272,7 @@ class OccDepth(_Base, B200Module):
             out = self.net_3d_decoder.emit(plan, x3d)
         else:
             out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1])
-        if os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
+        if capture and os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
             try:
                 plan.capture()
             except Exception as e:  # noqa: BLE001 -- same kernels either way; only the launch mechanism differs

@@ -1,0 +1,161 @@
+/*
+ * occd_run -- run an exported OccDepth model (occdepth_b200.deploy.export) on camera frames, without Python.
+ * Linked only against libocc_b200.so and the CUDA runtime; `python -m occdepth_b200._build` builds it next to
+ * the library (occdepth_b200/lib/occd_run).
+ *
+ *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]
+ *
+ * Inputs are raw little-endian files, one record per frame, frames back to back (no image decoder):
+ *   IMAGES  N x V x H0 x W0 x 3 uint8, RGB, row-major (H0 x W0 default to the model's crop; --raw gives larger
+ *           images, cropped to the top-left corner as the datasets do)
+ *   CALIB   N records of float64: KITTI  V x 9 cam_k, then V x 16 T_velo_2_cam (row-major)
+ *                                  NYU    9 cam_k, 16 T_world_2_cam (the inverse of the camera pose), 3 vox_origin
+ *   DEPTH   (NYU models with the virtual view) N x depth_h x depth_w uint16, the depth PNGs' values
+ * Output: OUT_DIR/NNNNNN.label per frame, the uint16 class map (X x Y x Z, C order) as the KITTI submission writer
+ * stores it; the labels are remapped when the model was exported with inv_map.  Prints ms per frame (device time
+ * of occd_model_run_frame, from CUDA events) and the mean over the frames after the first.
+ */
+#include <cuda_runtime.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "occdepth_b200.h"
+
+#define CK(x)                                                                          \
+  do {                                                                                 \
+    cudaError_t e_ = (x);                                                              \
+    if (e_ != cudaSuccess) {                                                           \
+      fprintf(stderr, "occd_run: %s: %s\n", #x, cudaGetErrorString(e_));              \
+      return 1;                                                                        \
+    }                                                                                  \
+  } while (0)
+#define OK(x)                                                                          \
+  do {                                                                                 \
+    if ((x) != OCCD_OK) {                                                              \
+      fprintf(stderr, "occd_run: %s: %s\n", #x, occd_last_error());                    \
+      return 1;                                                                        \
+    }                                                                                  \
+  } while (0)
+
+static int read_exact(FILE* f, void* dst, size_t n, const char* what) {
+  if (fread(dst, 1, n, f) != n) {
+    fprintf(stderr, "occd_run: %s is shorter than the frames asked for\n", what);
+    return 0;
+  }
+  return 1;
+}
+
+int main(int argc, char** argv) {
+  if (argc < 6) {
+    fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]\n");
+    return 2;
+  }
+  const char *model_path = argv[1], *img_path = argv[2], *calib_path = argv[3], *out_dir = argv[5];
+  const char* depth_path = NULL;
+  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0;
+  for (int i = 6; i < argc; ++i) {
+    if (!strcmp(argv[i], "--raw") && i + 2 < argc) {
+      H0 = atoi(argv[++i]);
+      W0 = atoi(argv[++i]);
+    } else if (!strcmp(argv[i], "--depth") && i + 1 < argc) {
+      depth_path = argv[++i];
+    } else if (!strcmp(argv[i], "--no-graph")) {
+      flags |= OCCD_FRAME_NO_GRAPH;
+    } else {
+      fprintf(stderr, "occd_run: unknown option %s\n", argv[i]);
+      return 2;
+    }
+  }
+  occd_model* m = NULL;
+  OK(occd_model_load(model_path, &m));
+  occd_model_geom g;
+  OK(occd_model_info(m, &g));
+  if (!H0) {
+    H0 = g.img_h;
+    W0 = g.img_w;
+  }
+  const int nyu = g.dataset == 1;
+  const size_t img_bytes = (size_t)g.V * H0 * W0 * 3;
+  const size_t n_calib = nyu ? 9 + 16 + 3 : (size_t)g.V * 25;
+  const size_t map_bytes = (size_t)g.X * g.Y * g.Z * 2;
+  const size_t depth_bytes = (size_t)g.depth_h * g.depth_w * 2;
+  if (g.has_depth && !depth_path) {
+    fprintf(stderr, "occd_run: this model takes a depth map per frame (--depth)\n");
+    return 2;
+  }
+  FILE* fi = fopen(img_path, "rb");
+  FILE* fc = fopen(calib_path, "rb");
+  FILE* fd = depth_path ? fopen(depth_path, "rb") : NULL;
+  if (!fi || !fc || (depth_path && !fd)) {
+    fprintf(stderr, "occd_run: cannot open the input files\n");
+    return 1;
+  }
+  unsigned char* h_img = (unsigned char*)malloc(img_bytes);
+  unsigned short* h_depth = (unsigned short*)malloc(depth_bytes ? depth_bytes : 1);
+  unsigned short* h_map = (unsigned short*)malloc(map_bytes);
+  double* calib = (double*)malloc(n_calib * sizeof(double));
+  void *d_img, *d_depth = NULL, *d_map;
+  cudaStream_t st;
+  cudaEvent_t e0, e1;
+  CK(cudaMalloc(&d_img, img_bytes));
+  CK(cudaMalloc(&d_map, map_bytes));
+  if (g.has_depth) CK(cudaMalloc(&d_depth, depth_bytes));
+  CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  CK(cudaEventCreate(&e0));
+  CK(cudaEventCreate(&e1));
+  double total = 0;
+  for (int i = 0; i < n; ++i) {
+    if (!read_exact(fi, h_img, img_bytes, "IMAGES") || !read_exact(fc, calib, n_calib * 8, "CALIB") ||
+        (fd && !read_exact(fd, h_depth, depth_bytes, "DEPTH")))
+      return 1;
+    CK(cudaMemcpyAsync(d_img, h_img, img_bytes, cudaMemcpyHostToDevice, st));
+    if (fd) CK(cudaMemcpyAsync(d_depth, h_depth, depth_bytes, cudaMemcpyHostToDevice, st));
+    occd_frame f;
+    memset(&f, 0, sizeof(f));
+    f.images = d_img;
+    f.img_stride = (long long)H0 * W0 * 3;
+    f.row_stride = (long long)W0 * 3;
+    f.H0 = H0;
+    f.W0 = W0;
+    f.cam_k = calib;
+    f.pose = nyu ? calib + 9 : calib + 9 * g.V;
+    f.calib_f32 = 0;
+    f.vox_origin = nyu ? calib + 25 : NULL;
+    f.depth = (const uint16_t*)d_depth;
+    f.depth_h = g.depth_h;
+    f.depth_w = g.depth_w;
+    f.flags = flags;
+    CK(cudaEventRecord(e0, st));
+    OK(occd_model_run_frame(m, &f, (uint16_t*)d_map, st));
+    CK(cudaEventRecord(e1, st));
+    CK(cudaMemcpyAsync(h_map, d_map, map_bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    if (i > 0) total += ms;
+    char path[4096];
+    snprintf(path, sizeof(path), "%s/%06d.label", out_dir, i);
+    FILE* fo = fopen(path, "wb");
+    if (!fo || fwrite(h_map, 1, map_bytes, fo) != map_bytes) {
+      fprintf(stderr, "occd_run: cannot write %s\n", path);
+      return 1;
+    }
+    fclose(fo);
+    printf("frame %d: %.3f ms\n", i, ms);
+  }
+  if (n > 1) printf("mean over frames 1..%d: %.3f ms per frame\n", n - 1, total / (n - 1));
+  OK(occd_model_destroy(m));
+  fclose(fi);
+  fclose(fc);
+  if (fd) fclose(fd);
+  free(h_img);
+  free(h_depth);
+  free(h_map);
+  free(calib);
+  cudaFree(d_img);
+  cudaFree(d_map);
+  if (d_depth) cudaFree(d_depth);
+  cudaStreamDestroy(st);
+  return 0;
+}
