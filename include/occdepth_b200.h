@@ -251,6 +251,12 @@ int occd_copy_channels(const void* in, void* out, int dtype, long long positions
 int occd_vox2pix_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
                      double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern, int P,
                      long long* pix, unsigned char* fov, void* pix_z, void* stream);
+/* the same for voxels [v0, v0 + n) of that C order only (0 <= v0, 1 <= n, v0 + n <= X*Y*Z), written to pix [n][P][2], */
+/* fov [n][P], pix_z [n]: bit for bit that slice of occd_vox2pix_fwd's outputs.  An X-slab [x0, x1) of the grid is  */
+/* v0 = x0*Y*Z, n = (x1 - x0)*Y*Z.                                                                                  */
+int occd_vox2pix_range_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
+                           double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern, int P,
+                           long long* pix, unsigned char* fov, void* pix_z, long long v0, long long n, void* stream);
 
 /* uint8 RGB HWC image [H0][W0][3] (device) -> float32 CHW [3][H][W] of the top-left H x W crop:     */
 /* ((u8 / 255) - mean[c]) / std[c] in float32 = np.array(img, float32) / 255.0, crop, ToTensor,        */

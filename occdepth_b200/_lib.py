@@ -137,6 +137,8 @@ SYMBOLS = {
     "occd_stage_rgb_u8_cl": (C.c_int, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "occd_depth_u16_to_f32": (C.c_int, [_vp, _vp, _ll, C.c_double, _f, _vp]),
     "occd_vox2pix_fwd": (C.c_int, [_vp, _i, _vp, _vp, C.c_double, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
+    "occd_vox2pix_range_fwd": (C.c_int, [_vp, _i, _vp, _vp, C.c_double, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp,
+                                         _ll, _ll, _vp]),
     "occd_cl_transpose": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _ll, _vp]),
     "occd_copy_channels": (C.c_int, [_vp, _vp, _i, _ll, _i, _i, _i, _i, _i, _vp]),
     "occd_dwconv2d_fwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp] + [_i] * 14 + [_vp]),

@@ -104,6 +104,7 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_ssc_confusion),         OCCD_ENTRY(occd_ssc_loss_sums),
     OCCD_ENTRY(occd_crp_relation_sums),     OCCD_ENTRY(occd_depth_cls_sums),
     OCCD_ENTRY(occd_occupied_voxels),       OCCD_ENTRY(occd_virtual_view_fwd),
+    OCCD_ENTRY(occd_vox2pix_range_fwd),
 };
 
 const Entry* find_entry(const std::string& name) {

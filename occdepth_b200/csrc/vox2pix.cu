@@ -1,7 +1,9 @@
 // Data-pipeline kernels (SURVEY 8f row 2).
-// occd_vox2pix_fwd: the data pipeline's voxel -> pixel index generation on the device (SURVEY 8f row 2).
+// occd_vox2pix_fwd: the data pipeline's voxel -> pixel index generation on the device (SURVEY 8f row 2);
+// occd_vox2pix_range_fwd: one window of the same voxel order (a rank's X-slab under the slab partition).
 // replaces occdepth/data/utils/helpers.py:94-169 (vox2pix) as called per view and per scale by the datasets
 // (data/semantic_kitti/kitti_dataset.py, data/NYU/nyu_dataset.py).
+#include <stdio.h>
 #include "vox2pix.cuh"
 #include "normalize_rgb.cuh"
 #include "../../include/occdepth_b200.h"
@@ -11,7 +13,7 @@ namespace {
 template <typename T>
 int run(const void* cam_E, const float* cam_k, const float* vox_origin, double voxel_size, int X, int Y, int Z,
         int img_W, int img_H, const int* pattern, int P, long long* pix, unsigned char* fov, void* pix_z,
-        cudaStream_t st) {
+        long long v0, long long n, cudaStream_t st) {
   v2p::Args<T> a;
   for (int i = 0; i < 12; ++i) a.E[i] = static_cast<const T*>(cam_E)[i];
   a.fx = cam_k[0]; a.fy = cam_k[4]; a.cx = cam_k[2]; a.cy = cam_k[5];
@@ -20,10 +22,33 @@ int run(const void* cam_E, const float* cam_k, const float* vox_origin, double v
   a.X = X; a.Y = Y; a.Z = Z; a.W = img_W; a.H = img_H; a.P = P;
   for (int p = 0; p < P; ++p) { a.pat[p][0] = pattern[2 * p]; a.pat[p][1] = pattern[2 * p + 1]; }
   a.pix = pix; a.fov = fov; a.pix_z = static_cast<T*>(pix_z);
-  const long long N = (long long)X * Y * Z;
-  v2p::vox2pix_kernel<T><<<(unsigned)((N + 255) / 256), 256, 0, st>>>(a, N);
+  a.v0 = v0;
+  v2p::vox2pix_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, n);
   OCCD_CHECK_LAUNCH();
   return OCCD_OK;
+}
+
+// voxels [v0, v0 + n) of the X*Y*Z grid; `who` names the entry point in the refusals
+int vox2pix_window(const char* who, const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
+                   double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern, int P,
+                   long long* pix, unsigned char* fov, void* pix_z, long long v0, long long n, void* stream) {
+  auto refuse = [&](const char* what) {
+    char msg[160];                        // occd_set_last_error keeps a copy
+    snprintf(msg, sizeof msg, "%s: %s", who, what);
+    occd_set_last_error(msg);
+    return OCCD_ERR_ARG;
+  };
+  if (!(cam_E && cam_k && vox_origin && pattern && pix && fov)) return refuse("null argument");
+  if (!(X > 0 && Y > 0 && Z > 0 && img_W > 0 && img_H > 0 && voxel_size > 0)) return refuse("dims");
+  if (!(P >= 1 && P <= v2p::kMaxPattern)) return refuse("pattern size must be 1..25");
+  const long long N = (long long)X * Y * Z;
+  if (!(v0 >= 0 && n >= 1 && v0 <= N - n)) return refuse("the window [v0, v0 + n) must lie inside the X*Y*Z grid");
+  if ((n + 255) / 256 > 2147483647LL) return refuse("too many voxels");
+  cudaStream_t st = (cudaStream_t)stream;
+  return pose_is_f32 ? run<float>(cam_E, cam_k, vox_origin, voxel_size, X, Y, Z, img_W, img_H, pattern, P, pix, fov,
+                                  pix_z, v0, n, st)
+                     : run<double>(cam_E, cam_k, vox_origin, voxel_size, X, Y, Z, img_W, img_H, pattern, P, pix, fov,
+                                   pix_z, v0, n, st);
 }
 
 }  // namespace
@@ -31,15 +56,17 @@ int run(const void* cam_E, const float* cam_k, const float* vox_origin, double v
 extern "C" int occd_vox2pix_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
                                 double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern,
                                 int P, long long* pix, unsigned char* fov, void* pix_z, void* stream) {
-  OCCD_CHECK_ARG(cam_E && cam_k && vox_origin && pattern && pix && fov, "occd_vox2pix_fwd: null argument");
-  OCCD_CHECK_ARG(X > 0 && Y > 0 && Z > 0 && img_W > 0 && img_H > 0 && voxel_size > 0, "occd_vox2pix_fwd: dims");
-  OCCD_CHECK_ARG(P >= 1 && P <= v2p::kMaxPattern, "occd_vox2pix_fwd: pattern size must be 1..25");
-  OCCD_CHECK_ARG(((long long)X * Y * Z + 255) / 256 <= 2147483647LL, "occd_vox2pix_fwd: too many voxels");
-  cudaStream_t st = (cudaStream_t)stream;
-  return pose_is_f32 ? run<float>(cam_E, cam_k, vox_origin, voxel_size, X, Y, Z, img_W, img_H, pattern, P, pix, fov,
-                                  pix_z, st)
-                     : run<double>(cam_E, cam_k, vox_origin, voxel_size, X, Y, Z, img_W, img_H, pattern, P, pix, fov,
-                                   pix_z, st);
+  const long long N = X > 0 && Y > 0 && Z > 0 ? (long long)X * Y * Z : 1;
+  return vox2pix_window("occd_vox2pix_fwd", cam_E, pose_is_f32, cam_k, vox_origin, voxel_size, X, Y, Z, img_W, img_H,
+                        pattern, P, pix, fov, pix_z, 0, N, stream);
+}
+
+extern "C" int occd_vox2pix_range_fwd(const void* cam_E, int pose_is_f32, const float* cam_k,
+                                      const float* vox_origin, double voxel_size, int X, int Y, int Z, int img_W,
+                                      int img_H, const int* pattern, int P, long long* pix, unsigned char* fov,
+                                      void* pix_z, long long v0, long long n, void* stream) {
+  return vox2pix_window("occd_vox2pix_range_fwd", cam_E, pose_is_f32, cam_k, vox_origin, voxel_size, X, Y, Z, img_W,
+                        img_H, pattern, P, pix, fov, pix_z, v0, n, stream);
 }
 
 // occd_normalize_rgb_u8: uint8 HWC image -> cropped, normalised float32 CHW (the datasets' `normalize_rgb`,

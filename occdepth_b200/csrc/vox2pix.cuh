@@ -7,7 +7,8 @@
 //   xc       = int64(rint(cam_0 * fx32 / cam_2 + cx32)), yc likewise                   (same precision; np.round =
 //              half to even)
 //   pix[p]   = (xc + pattern[p].x, yc + pattern[p].y);  fov[p] = 0 <= x < W && 0 <= y < H && cam_2 > 0
-// Voxel order: C order over (X, Y, Z) (np.meshgrid(..., indexing="ij") flattened).  One thread per voxel.
+// Voxel order: C order over (X, Y, Z) (np.meshgrid(..., indexing="ij") flattened).  One thread per voxel.  A window
+// [v0, v0 + n) of that order (an X-slab of the grid) writes its voxels to outputs [0, n); the whole grid is v0 = 0.
 // __host__ __device__ body: tests/host_emul/ runs it on the CPU against the reference itself.
 #pragma once
 #include <math.h>
@@ -26,9 +27,10 @@ struct Args {
   double voxel_size;
   int X, Y, Z, W, H, P;
   int pat[kMaxPattern][2];
-  long long* pix;        // [N][P][2] (x, y)
-  unsigned char* fov;    // [N][P] (numpy bool)
-  T* pix_z;              // [N] or null
+  long long* pix;        // [n][P][2] (x, y)
+  unsigned char* fov;    // [n][P] (numpy bool)
+  T* pix_z;              // [n] or null
+  long long v0 = 0;      // flat index of the window's first voxel; output i holds voxel v0 + i
 };
 
 V2P_HD double mul_rn(double a, double b) {
@@ -97,11 +99,13 @@ V2P_HD long long to_pix(double v) {
 }
 V2P_HD long long to_pix(float v) { return to_pix((double)rintf(v)); }
 
+// output n of the window: voxel a.v0 + n
 template <typename T>
 V2P_HD void body(const Args<T>& a, long long n) {
-  const int k = (int)(n % a.Z);
-  const int j = (int)((n / a.Z) % a.Y);
-  const int i = (int)(n / ((long long)a.Z * a.Y));
+  const long long v = a.v0 + n;
+  const int k = (int)(v % a.Z);
+  const int j = (int)((v / a.Z) % a.Y);
+  const int i = (int)(v / ((long long)a.Z * a.Y));
   const int idx[3] = {i, j, k};
   T c[3];
 #pragma unroll

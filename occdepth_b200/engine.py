@@ -526,12 +526,13 @@ class Plan:
 
     def capture(self):
         """Capture the launch sequence into a CUDA graph (buffers are static, so replay is valid).  Communication
-        ops (NCCL halo exchange / all-gather of the slab partition) are not captured: the graph covers the ops
-        before the first of them (the replicated 2D network and the lift), the rest is launched eagerly."""
+        ops (NCCL halo exchange / all-gather / class-map gather of the slab partition) are not captured: the graph
+        covers the ops before the first of them (the replicated 2D network and the lift), the rest is launched
+        eagerly."""
         self.graph = None
         n = len(self.ops)
         for i, op in enumerate(self.ops):
-            if getattr(op, "name", "") in ("halo_exchange", "all_gather"):
+            if getattr(op, "name", "") in ("halo_exchange", "all_gather", "gather_root"):
                 n = i
                 break
         self.run()                      # warm-up outside capture (lazy module loading, func attributes)

@@ -173,12 +173,8 @@ class OccDepth(_Base, B200Module):
             S = [x_hi - x_lo, S[1], S[2]]
         virtual = V == 1 and "gt_depth" in batch                          # process_rgbs, OccDepth.py:221-229
         VL = 2 if virtual else V                                           # views seen by the lift
-        # slab partition over an even number of ranks: the 2D network is sharded BY VIEW (its receptive field is
-        # global inside a view -- SE pooling -- but the two views are independent, process_rgbs OccDepth.py:208-219):
-        # ranks [0, R/2) run view 0, ranks [R/2, R) view 1, and one all-gather hands every rank both views' maps
-        view_shard = (slab is not None and V == 2 and not virtual and slab.world % 2 == 0
-                      and os.environ.get("OCCDEPTH_SLAB_VIEW_SHARD", "1") == "1")
-        view_sel = (slab.rank // (slab.world // 2)) if view_shard else None
+        view_sel = self.slab_view(V, virtual)
+        view_shard = view_sel is not None
         img = plan.alloc(B * (1 if view_shard else V), 1, H, W, 3)
         Cf = self.feature_2d_oc
         assert Cf == self.feature, "feature_2d_oc must equal feature (the lift feeds the 3D net directly)"
@@ -272,6 +268,15 @@ class OccDepth(_Base, B200Module):
             out = self.net_3d_decoder.emit(plan, x3d)
         else:
             out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1])
+            if classes[2:] == ("root",):
+                # predict_frame(slab_output="root"): rank 0 gathers the ranks' slabs into the whole map, which is then
+                # this plan's output there; the other ranks' plans output nothing
+                bounds = [(lo * ps, hi * ps) for lo, hi in slab.bounds]       # every rank's plan.x_range
+                whole = None
+                if slab.rank == 0:
+                    whole = torch.empty((1, bounds[-1][1]) + tuple(out.shape[2:]), dtype=out.dtype, device=dev)
+                plan.add(slab.gather_root_op(out, whole, bounds))
+                out = whole
         if capture and os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
             try:
                 plan.capture()
@@ -299,6 +304,18 @@ class OccDepth(_Base, B200Module):
         if len(lut) != self.n_classes:
             raise ValueError("OccDepth.predict_classes: inv_map must hold one label id per class")
         return lut
+
+    def slab_view(self, V, virtual=False):
+        """the one view of a V-view frame this rank's plan stages under enable_slab_parallel, or None (every view).
+        Over an even number of ranks a stereo frame's 2D network is sharded BY VIEW (its receptive field is global
+        inside a view -- SE pooling -- but the two views are independent, process_rgbs OccDepth.py:208-219): ranks
+        [0, R/2) run view 0, ranks [R/2, R) view 1, and one all-gather hands every rank both views' maps.  `virtual`:
+        the frame's second view is NYU's virtual one, computed from the first."""
+        slab = self.__dict__.get("slab_ctx")
+        if (slab is None or V != 2 or virtual or slab.world % 2
+                or os.environ.get("OCCDEPTH_SLAB_VIEW_SHARD", "1") != "1"):
+            return None
+        return slab.rank // (slab.world // 2)
 
     def _plan_key(self, B, V, H, W, N, P, dev, virtual, virtual_bf):
         """cache key of the launch plan of one batch shape (shared by tensor batches and camera frames)"""
@@ -366,6 +383,8 @@ class OccDepth(_Base, B200Module):
             return None
         stage(ent)
         ent[0].run()
+        if ent[4] is None:                     # slab_output="root" on a rank other than 0
+            return None
         return ent[4].clone()                  # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
@@ -385,7 +404,7 @@ class OccDepth(_Base, B200Module):
             self.flosp_depth.stage_inputs(batch, dev, plan.flosp_state)
 
     # ---- camera frames: uint8 images and calibration in, the datasets' pre-processing on the device -------------
-    def predict_frame(self, frame, classes=True, inv_map=None):
+    def predict_frame(self, frame, classes=True, inv_map=None, slab_output=None):
         """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map` as in predict_classes) or
         the forward's output dict (classes=False), through the same cached plan a tensor batch of the same shapes
         uses.  Only the staging differs: the datasets' pre-processing (eval split, no augmentation) runs on the device
@@ -401,14 +420,31 @@ class OccDepth(_Base, B200Module):
           optional geometry, fixed per dataset: "img_hw" (KITTI (370, 1220), NYU (480, 640)), "vox_origin" (KITTI
           (0, -25.6, -2)), "voxel_size" (KITTI 0.2 * project_scale, NYU 0.08), "scene_size", "pattern_id" (0)
         The indices are recomputed only when the calibration differs from what the plan's index buffers hold (a KITTI
-        sequence keeps one); NYU poses change every frame.  One frame per call; not under enable_slab_parallel."""
-        return self._run_frame(self._frame_checked(frame), classes, inv_map)
+        sequence keeps one); NYU poses change every frame.  One frame per call.
 
-    def _frame_checked(self, frame):
+        Under enable_slab_parallel every rank is handed the same frame and `slab_output` says which result it wants:
+          "slab": this rank's X-slab, as predict_classes returns it (classes=False: the forward's per-rank dict);
+          "root": (classes=True only) rank 0 returns the whole [1, X, Y, Z] map, bit for bit the unpartitioned one,
+                  gathered from the ranks' slabs; the other ranks return None.
+        Each rank stages its own view under view sharding (else every view), the whole depth map, and the indices of
+        its X-slab only (`occd_vox2pix_range_fwd`).  Without slab_output the partition is refused; without the
+        partition slab_output must be None."""
+        return self._run_frame(self._frame_checked(frame, slab_output, classes), classes, inv_map, slab_output)
+
+    def _frame_checked(self, frame, slab_output=None, classes=True):
         """the refusals of the camera route, then `_frame_inputs`"""
-        if self.__dict__.get("slab_ctx") is not None:
-            raise NotImplementedError("OccDepth.predict_frame: not under enable_slab_parallel (a camera frame is staged "
-                                      "whole on one device); use forward / predict_classes with a tensor batch")
+        if slab_output not in (None, "slab", "root"):
+            raise ValueError("OccDepth.predict_frame: slab_output must be None, 'slab' or 'root', got %r"
+                             % (slab_output,))
+        if self.__dict__.get("slab_ctx") is None:
+            if slab_output is not None:
+                raise ValueError("OccDepth.predict_frame: slab_output=%r needs enable_slab_parallel" % (slab_output,))
+        elif slab_output is None:
+            raise NotImplementedError("OccDepth.predict_frame: under enable_slab_parallel a camera frame needs "
+                                      "slab_output='slab' (every rank's X-slab) or 'root' (the whole map on rank 0)")
+        if slab_output == "root" and not classes:
+            raise ValueError("OccDepth.predict_frame: slab_output='root' gathers the class map (classes=True); the "
+                             "logits stay on their ranks (slab_output='slab')")
         if self.infer_mode and self.trans_2d_to_3d == "flosp_depth":
             raise NotImplementedError("OccDepth.predict_frame: infer_mode with flosp_depth takes the caller's sampling "
                                       "grids, not camera matrices; use forward / predict_classes with a tensor batch")
@@ -416,13 +452,13 @@ class OccDepth(_Base, B200Module):
         self._check_mode(torch.empty(0, device=dev))
         return self._frame_inputs(frame, dev)
 
-    def _run_frame(self, f, classes, inv_map):
+    def _run_frame(self, f, classes, inv_map, slab_output=None):
         dev = f["imgs"].device
         key = self._plan_key(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"])
         stage = lambda ent: self._stage_frame(ent, f)     # noqa: E731
         with torch.cuda.device(dev):
             if classes:
-                cls = ("classes", self._class_lut(inv_map))
+                cls = ("classes", self._class_lut(inv_map)) + (("root",) if slab_output == "root" else ())
                 return self._classes_on(f["batch"], key + cls, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
                                         stage)
             return self._forward_on(f["batch"], key, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage)
@@ -515,16 +551,19 @@ class OccDepth(_Base, B200Module):
             return                              # same calibration: the indices and camera tables are in place
         if getattr(plan, "pix_z", None) is None:
             plan.pix_z = torch.empty(pix.shape[2], dtype=torch.float64, device=pix.device)   # vox2pix's depth output
+        # under the slab partition the index buffers hold this rank's window [n_lo, n_lo + N) of the lift's X-major
+        # voxel order: the rank computes that window only, for every pose (NYU's virtual view too)
+        window = None if plan.x_range is None else (n_lo, pix.shape[2])
         for v, (E, K) in enumerate(f["poses"]):
             D.vox2pix_into(pix[0, v], fov[0, v], plan.pix_z, E, K, f["vox_origin"], f["voxel_size"], f["W"], f["H"],
-                           f["scene_size"], f["pattern_id"])
+                           f["scene_size"], f["pattern_id"], voxel_range=window)
         if self.trans_2d_to_3d == "flosp_depth":
             self.flosp_depth.stage_inputs(f["batch"], pix.device, plan.flosp_state)
         plan.calib_mark = f["calib"]
 
     # ---- the occupied-voxel list: what every consumer of a class map builds from it first ----------------------
     def predict_voxels(self, batch_or_frame, inv_map=None, fov_mask=None, capacity=None, voxel_size=None,
-                       vox_origin=None, out=None):
+                       vox_origin=None, out=None, slab_output=None):
         """`predict_classes` (a tensor batch: it carries "projected_pix_<project_scale>") or `predict_frame` (a camera
         frame), then `voxels.occupied_voxels` of the class map on the same stream -> VoxelList: per frame the counts,
         the class histogram and the rows (flat index, class, voxel centre) of the occupied voxels, inside the FOV
@@ -539,32 +578,41 @@ class OccDepth(_Base, B200Module):
                   (x, z, y), and NYU_vis_pred.py keeps one list.
         voxel_size: of the output grid (default 0.2 for KITTI, 0.08 for NYU); vox_origin: added to the centres.
         inv_map, capacity, out: as in predict_classes / occupied_voxels.
-        Under enable_slab_parallel (tensor batches) the list holds this rank's X-slab with the whole grid's flat
-        indices and coordinates: the ranks' in-FOV rows concatenated in rank order, then their out-of-FOV rows, are
-        the unpartitioned list."""
+        Under enable_slab_parallel (tensor batches, and camera frames with slab_output="slab") the list holds this
+        rank's X-slab with the whole grid's flat indices and coordinates: the ranks' in-FOV rows concatenated in rank
+        order, then their out-of-FOV rows, are the unpartitioned list.  A camera frame's default mask is then this
+        rank's window of it, from `occd_vox2pix_range_fwd`.  slab_output="root": rank 0 lists the gathered whole map
+        (the unpartitioned list exactly), the other ranks return None."""
+        window_mask = None
         if "projected_pix_%d" % self.project_scale in batch_or_frame:
             y = self.predict_classes(batch_or_frame, inv_map)
             x_range = self.slab_x_range()
             if fov_mask is None:
                 fov_mask = False if self.dataset == "NYU" else batch_or_frame.get("fov_mask_1", False)
         else:
-            f = self._frame_checked(batch_or_frame)
-            y = self._run_frame(f, True, inv_map)
-            x_range = None
+            f = self._frame_checked(batch_or_frame, slab_output)
+            y = self._run_frame(f, True, inv_map, slab_output)
+            x_range = self.slab_x_range() if slab_output == "slab" else None
             if fov_mask is None and y is not None:
-                fov_mask = False if self.dataset == "NYU" else self._frame_fov_mask_1(f)
-        if y is None:                          # prepare(): the plan was built, nothing ran
+                if self.dataset == "NYU":
+                    fov_mask = False
+                else:
+                    window_mask = self._frame_fov_mask_1(f, x_range)
+        if y is None:                          # prepare(): the plan was built, nothing ran (or "root" off rank 0)
             return None
-        return self._list_voxels(y, x_range, fov_mask, capacity, voxel_size, vox_origin, out)
+        return self._list_voxels(y, x_range, fov_mask, capacity, voxel_size, vox_origin, out, window_mask)
 
-    def _list_voxels(self, y, x_range, fov_mask, capacity, voxel_size, vox_origin, out):
-        """the list of class map `y` [B, Xl, Y, Z]: the whole grid, or planes x_range = [lo, hi) of it"""
+    def _list_voxels(self, y, x_range, fov_mask, capacity, voxel_size, vox_origin, out, window_mask=None):
+        """the list of class map `y` [B, Xl, Y, Z]: the whole grid, or planes x_range = [lo, hi) of it.  fov_mask holds
+        the whole grid per frame; window_mask (one frame) only y's planes of it"""
         from ..voxels import occupied_voxels
         B, _, Y, Z = y.shape
         lo, hi = (0, y.shape[1]) if x_range is None else x_range
         n_full = int(self.full_scene_size[0]) * Y * Z
         mask = None
-        if fov_mask is not None and fov_mask is not False:
+        if window_mask is not None:
+            mask = window_mask.view(1, -1)
+        elif fov_mask is not None and fov_mask is not False:
             frames = [fov_mask] if getattr(fov_mask, "ndim", 0) == 1 else list(fov_mask)
             rows = []
             for m in frames:
@@ -583,29 +631,36 @@ class OccDepth(_Base, B200Module):
         return occupied_voxels(y, mask, voxel_size=voxel_size, vox_origin=vox_origin, capacity=capacity,
                                index0=lo * Y * Z, out=out)
 
-    def _frame_fov_mask_1(self, f):
+    def _frame_fov_mask_1(self, f, x_range=None):
         """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
-        resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only.  Kept with the calibration it was
-        computed from."""
+        resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only; x_range = [lo, hi): only those X
+        planes of it.  Kept with the calibration and window it was computed from."""
         import numpy as np
         from .. import data as D
         held = self.__dict__.get("_fov_mask_1")
-        if f["calib"] is not None and held is not None and held[0] == f["calib"] and held[1].device == f["imgs"].device:
+        key = (f["calib"], x_range)
+        if f["calib"] is not None and held is not None and held[0] == key and held[1].device == f["imgs"].device:
             return held[1]
         voxel = f["voxel_size"] / self.project_scale
         n1 = int(np.prod(D.volume_dims(f["vox_origin"], voxel, f["scene_size"])))
         if n1 != int(np.prod([int(s) for s in self.full_scene_size])):
             raise ValueError("OccDepth.predict_voxels: the geometry gives %d voxels at the output resolution, the model "
                              "predicts %d" % (n1, int(np.prod([int(s) for s in self.full_scene_size]))))
+        window, n = None, n1
+        if x_range is not None:
+            plane = n1 // int(self.full_scene_size[0])
+            window = (x_range[0] * plane, (x_range[1] - x_range[0]) * plane)
+            n = window[1]
         dev = f["imgs"].device
         E, K = f["poses"][0]
         with torch.cuda.device(dev):
-            pix = torch.empty(n1, 1, 2, dtype=torch.int64, device=dev)
-            fov = torch.empty(n1, 1, dtype=torch.bool, device=dev)
-            pix_z = torch.empty(n1, dtype=torch.float64, device=dev)
-            D.vox2pix_into(pix, fov, pix_z, E, K, f["vox_origin"], voxel, f["W"], f["H"], f["scene_size"], 0)
+            pix = torch.empty(n, 1, 2, dtype=torch.int64, device=dev)
+            fov = torch.empty(n, 1, dtype=torch.bool, device=dev)
+            pix_z = torch.empty(n, dtype=torch.float64, device=dev)
+            D.vox2pix_into(pix, fov, pix_z, E, K, f["vox_origin"], voxel, f["W"], f["H"], f["scene_size"], 0,
+                           voxel_range=window)
         mask = fov.view(-1)
-        self.__dict__["_fov_mask_1"] = (f["calib"], mask)
+        self.__dict__["_fov_mask_1"] = (key, mask)
         return mask
 
     def _outputs(self, ent):

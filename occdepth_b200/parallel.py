@@ -148,6 +148,38 @@ class AllGatherOp:
         dist.all_gather_into_tensor(self.dst, self.src)
 
 
+class GatherRootOp:
+    """Plan op: rank 0 assembles the whole uint16 class map [1, X, Y, Z] from every rank's full-resolution X-slab
+    src [1, hi - lo, Y, Z]; bounds[r] = (lo, hi) of rank r.  Rank 0 copies its own slab and receives the others straight
+    into their planes of dst (one grouped send/recv); the other ranks send and take dst=None.  The bytes move as uint8,
+    whatever the map's element type."""
+
+    def __init__(self, ctx, src, dst, bounds):
+        self.ctx, self.name, self.flops = ctx, "gather_root", 0
+        if not src.is_contiguous() or src.shape[1] != bounds[ctx.rank][1] - bounds[ctx.rank][0]:
+            raise RuntimeError("gather_root: rank %d's slab %r does not hold planes %r" % (ctx.rank, tuple(src.shape),
+                                                                                       bounds[ctx.rank]))
+        self.src, self.dst, self.bounds = src, dst, bounds
+        self.parts = None
+        if ctx.rank == 0:
+            self.parts = [dst[:, lo:hi] for lo, hi in bounds]          # contiguous: one frame, planes are outermost
+        self.bytes = src.numel() * src.element_size()
+
+    @staticmethod
+    def _u8(t):
+        return t.reshape(-1).view(torch.uint8)
+
+    def run(self, stream=None):
+        c = self.ctx
+        if c.rank == 0:
+            self.parts[0].copy_(self.src)
+            ops = [dist.P2POp(dist.irecv, self._u8(self.parts[r]), r) for r in range(1, c.world)]
+        else:
+            ops = [dist.P2POp(dist.isend, self._u8(self.src), 0)]
+        for req in dist.batch_isend_irecv(ops):
+            req.wait()
+
+
 class SlabContext:
     def __init__(self, rank=None, world=None, halo=3):
         w, r, _ = env_world()
@@ -163,6 +195,9 @@ class SlabContext:
 
     def all_gather_op(self, src, dst):
         return AllGatherOp(self, src, dst)
+
+    def gather_root_op(self, src, dst, bounds):
+        return GatherRootOp(self, src, dst, bounds)
 
     def slab(self, n):
         """planes [lo, hi) of an extent-n axis owned by this rank (n must divide evenly)"""
@@ -194,7 +229,7 @@ class SlabContext:
 # the R plans are executed in lock-step and the exchange ops copy directly between the plans' buffers.
 class SimSlabGroup:
     def __init__(self, world, halo=3):
-        self.world, self.ex, self.ag = world, {}, {}
+        self.world, self.ex, self.ag, self.gr = world, {}, {}, {}
         self.ctxs = [SimSlabContext(self, r, world, halo) for r in range(world)]
 
     @staticmethod
@@ -234,10 +269,29 @@ class _SimAllGatherOp(AllGatherOp):
             flat[r].copy_(peers[r].src.reshape(-1))
 
 
+class _SimGatherRootOp(GatherRootOp):
+    def __init__(self, ctx, src, dst, bounds, idx):
+        super().__init__(ctx, src, dst, bounds)
+        self.idx = idx
+
+    def run(self, stream=None):
+        if self.ctx.rank != 0:
+            return
+        peers = self.ctx.group.gr[self.idx]
+        for r in range(self.ctx.world):
+            self.parts[r].copy_(peers[r].src)
+
+
 class SimSlabContext(SlabContext):
     def __init__(self, group, rank, world, halo):
         super().__init__(rank, world, halo)
-        self.group, self.n_gathers = group, 0
+        self.group, self.n_gathers, self.n_root_gathers = group, 0, 0
+
+    def gather_root_op(self, src, dst, bounds):
+        op = _SimGatherRootOp(self, src, dst, bounds, self.n_root_gathers)
+        self.group.gr.setdefault(self.n_root_gathers, {})[self.rank] = op
+        self.n_root_gathers += 1
+        return op
 
     def exchange_op(self, cl):
         op = _SimExchangeOp(self, cl, self.n_exchanges)

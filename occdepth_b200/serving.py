@@ -113,8 +113,13 @@ class CameraPipeline:
     `frame` is what predict_frame takes (NYU: "img", "cam_pose", "vox_origin", "cam_k", "depth"); the constructor's
     geometry (img_hw, vox_origin, voxel_size, scene_size, pattern_id) fills the keys a frame leaves out.  Two pinned
     and two device image / depth buffers, sized from the first frame and regrown only when a larger raw image arrives;
-    nothing else is allocated per frame.  One frame per submit; not under enable_slab_parallel, nor for infer_mode with
-    flosp_depth (that route takes sampling grids, not camera matrices).
+    nothing else is allocated per frame.  One frame per submit; not for infer_mode with flosp_depth (that route takes
+    sampling grids, not camera matrices).
+
+    Under enable_slab_parallel (one pipeline per rank, every rank submitting the same frames) `slab_output` is
+    required and means what it does for predict_frame: "slab" reads back this rank's X-slab, "root" the whole class
+    map (or voxel list) on rank 0 -- the other ranks read nothing back and their `result()` is None.  Under the
+    partition's view sharding a rank copies only the view its plan stages (`OccDepth.slab_view`).
 
     `output="voxels"` lists every frame's occupied voxels on the device (`OccDepth.predict_voxels`) and reads back the
     counts, the class histogram and the first `capacity` rows (flat index, class, voxel centre: 18 bytes a row; default
@@ -122,15 +127,23 @@ class CameraPipeline:
     and says whether the frame held more (`truncated`).  `d2h_bytes` is what a frame reads back."""
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
-                 inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None):
+                 inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None):
         if not torch.cuda.is_available():
             raise RuntimeError("CameraPipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         if output not in (None, "voxels"):
             raise ValueError("CameraPipeline: output must be None (the class map or logits, as `classes` says) or "
                              "'voxels', got %r" % (output,))
-        if model.__dict__.get("slab_ctx") is not None:
-            raise NotImplementedError("CameraPipeline: not under enable_slab_parallel (a camera frame is staged whole "
-                                      "on one device)")
+        if slab_output not in (None, "slab", "root"):
+            raise ValueError("CameraPipeline: slab_output must be None, 'slab' or 'root', got %r" % (slab_output,))
+        slab = model.__dict__.get("slab_ctx")
+        if slab is None:
+            if slab_output is not None:
+                raise ValueError("CameraPipeline: slab_output=%r needs enable_slab_parallel" % (slab_output,))
+        elif slab_output is None:
+            raise NotImplementedError("CameraPipeline: under enable_slab_parallel a pipeline needs slab_output='slab' "
+                                      "(every rank's X-slab) or 'root' (the whole map on rank 0)")
+        if slab_output == "root" and not classes and output is None:
+            raise ValueError("CameraPipeline: slab_output='root' gathers the class map (classes=True)")
         if model.infer_mode and model.trans_2d_to_3d == "flosp_depth":
             raise NotImplementedError("CameraPipeline: infer_mode with flosp_depth takes the caller's sampling grids, "
                                       "not camera matrices")
@@ -155,6 +168,8 @@ class CameraPipeline:
         self.n = 0
         self.h2d_bytes = 0            # bytes copied host -> device by the last submit
         self.output = output
+        self.slab_output = slab_output
+        self.reads_back = slab_output != "root" or slab.rank == 0     # "root": only rank 0 has a result
         if output == "voxels":
             n_out = 1
             for s in model.full_scene_size:
@@ -198,6 +213,8 @@ class CameraPipeline:
             img = img[0]
         depth = frame.get("depth")
         depth = None if depth is None else self._host(depth, "depth")
+        V = int(img.shape[0]) if img.dim() == 4 else 1
+        sel = self.model.slab_view(V, virtual=depth is not None)
         j = self.n & 1
         self.host_free[j].synchronize()           # pinned buffer j: its previous H2D copy has been read
         self.h2d_bytes = 0
@@ -205,7 +222,11 @@ class CameraPipeline:
         f.update(frame)
         with torch.cuda.stream(self.h2d):
             self.h2d.wait_event(self.in_free[j])
-            f["img"] = self._stage_h2d("img", j, img)
+            if sel is None:
+                f["img"] = self._stage_h2d("img", j, img)
+            else:
+                # this rank's plan stages view `sel` only: copy that one, and let every view of the frame read it
+                f["img"] = self._stage_h2d("img", j, img[sel:sel + 1]).expand(V, -1, -1, -1)
             if depth is not None:
                 f["depth"] = self._stage_h2d("depth", j, depth)
             self.in_ready[j].record(self.h2d)
@@ -214,10 +235,14 @@ class CameraPipeline:
         if self.output == "voxels":
             return self._submit_voxels(f, j)
         with torch.no_grad():
-            res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map)
+            res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map,
+                                           slab_output=self.slab_output)
+        self.in_free[j].record(self.main)
+        if not self.reads_back:
+            self.n += 1
+            return self.n - 2 if self.n >= 2 else None
         if not self.classes:
             res = res[self.out_key]
-        self.in_free[j].record(self.main)
         if self.dev_out[j] is None or self.dev_out[j].shape != res.shape:
             self.out_free[j].synchronize()
             self.dev_out[j] = torch.empty_like(res)
@@ -238,8 +263,12 @@ class CameraPipeline:
         batch, so no second round trip decides how much to copy"""
         self.main.wait_event(self.out_free[j])        # list j is overwritten in place: its last read-back is done
         with torch.no_grad():
-            vl = self.model.predict_voxels(f, inv_map=self.inv_map, capacity=self.capacity, out=self.vox[j])
+            vl = self.model.predict_voxels(f, inv_map=self.inv_map, capacity=self.capacity, out=self.vox[j],
+                                           slab_output=self.slab_output)
         self.in_free[j].record(self.main)
+        if not self.reads_back:
+            self.n += 1
+            return self.n - 2 if self.n >= 2 else None
         if self.vox[j] is None:
             self.vox[j] = vl
             self.host_out[j] = {k: torch.empty(getattr(vl, k)[0].shape, dtype=getattr(vl, k).dtype).pin_memory()
@@ -262,9 +291,12 @@ class CameraPipeline:
         """host tensor (pinned) of a submitted frame; blocks until its D2H read has finished.  The buffer is reused by
         the second submit after the one that produced it.  With output="voxels": a dict of numpy views of the pinned
         buffers, trimmed to the rows that were written -- "count" (inside, outside the FOV; the true counts), "hist",
-        "index", "cls", "xyz" (the in-FOV rows first, "n_in" of them) and "truncated"."""
+        "index", "cls", "xyz" (the in-FOV rows first, "n_in" of them) and "truncated".  None on a rank other than 0
+        with slab_output="root"."""
         if ticket is None or ticket < self.n - 2 or ticket >= self.n:
             raise ValueError("CameraPipeline.result: ticket %r is not one of the two frames in flight" % (ticket,))
+        if not self.reads_back:
+            return None
         j = ticket & 1
         self.out_free[j].synchronize()
         if self.output == "voxels":
