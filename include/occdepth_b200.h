@@ -132,6 +132,11 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
                                /* occd_argmax_classes returns for the OCCD_OUT1_F32_PLANAR logits of the same       */
                                /* descriptor; optional label remap: occd_conv_plan_set_class_lut.  Needs every     */
                                /* channel in one N tile and no tap groups (else OCCD_ERR_UNSUPPORTED)               */
+#define OCCD_OUT1_CLASS_U16_CONF 4 /* class map and its confidence, uint16 [2][B][positions]: [0] the map of      */
+                                   /* OCCD_OUT1_CLASS_U16, [1] the float16 bits of the top class's softmax          */
+                                   /* probability, 1 / sum_c exp(l_c - max l), computed in fp32 and rounded once;   */
+                                   /* NaN where a value is NaN or +inf.  The map is bit-identical to mode 3's, the   */
+                                   /* lut does not touch the confidence, and the same refusals apply                */
 #define OCCD_CLASS_LUT_MAX 64
 
 typedef struct {
@@ -235,6 +240,11 @@ int occd_cl_transpose(const void* in, void* out, int dtype, int B, int P, int C,
 /* pointer, C ints, C <= 64) or NULL: out = uint16(lut[class]), the inv_map remap of                  */
 /* scripts/generate_kitti_submission.py:79 (data/semantic_kitti/io_data.py:99-113)                    */
 int occd_argmax_classes(const float* in, void* out, long long B, int C, long long S, const int* lut, void* stream);
+/* occd_argmax_classes plus the top class's softmax probability: conf (2-byte aligned) gets the float16 bits of   */
+/* max_c softmax(in[b][:][s]) as OCCD_OUT1_CLASS_U16_CONF's second half holds them (NaN where a logit is NaN or  */
+/* +inf); out as occd_argmax_classes writes it, lut applied to the class only                                   */
+int occd_argmax_classes_conf(const float* in, void* out, void* conf, long long B, int C, long long S, const int* lut,
+                             void* stream);
 /* copy a channel window (C % 8 == 0) between channels-last buffers (torch.cat of CRP3D.py:90)    */
 int occd_copy_channels(const void* in, void* out, int dtype, long long positions, int C, int in_cstride,
                        int in_coff, int out_cstride, int out_coff, void* stream);
@@ -495,6 +505,10 @@ int occd_model_info(const occd_model* m, occd_model_geom* geom);
 /* launch the graph (OCCD_FRAME_NO_GRAPH: always one by one).  Allocates nothing per frame; calls on one model must  */
 /* not overlap.                                                                                                    */
 int occd_model_run_frame(occd_model* m, const occd_frame* frame, uint16_t* class_map, void* stream);
+/* occd_model_run_frame plus the class map's confidence: conf (DEVICE float16 [X][Y][Z], 2-byte aligned) gets the  */
+/* top class's softmax probability of every voxel (OCCD_OUT1_CLASS_U16_CONF).  OCCD_ERR_UNSUPPORTED for a model    */
+/* exported without confidence; occd_model_run_frame on a model exported with it writes the map only.              */
+int occd_model_run_frame_conf(occd_model* m, const occd_frame* frame, uint16_t* class_map, void* conf, void* stream);
 int occd_model_destroy(occd_model* m);
 
 /* FlospDepth's per-camera tables on the host (FlospDepth.camera_tables of occdepth_b200, flosp_depth.py:466-541),  */

@@ -46,7 +46,7 @@ class SfaParams(C.Structure):
 
 CONV_MAX_TAPS, CONV_MAX_SRC, CONV_MAX_GROUPS = 81, 3, 8
 CONV_IMPL_TC, CONV_IMPL_SIMT, CONV_IMPL_HALO, CONV_IMPL_HALOX, CONV_IMPL_TCX, CONV_IMPL_AUTO = 0, 1, 2, 3, 4, 5
-OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16 = 0, 1, 2, 3
+OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16, OUT1_CLASS_U16_CONF = 0, 1, 2, 3, 4
 CLASS_LUT_MAX = 64
 ERR_ARG, ERR_CUDA, ERR_UNSUPPORTED, ERR_FORMAT, ERR_IO = 1, 2, 3, 4, 5
 MODEL_FORMAT_VERSION = 1
@@ -133,6 +133,7 @@ SYMBOLS = {
     "occd_conv_debug_trace": (C.c_int, [_vp]),
     "occd_softmax_planar_to_cl": (C.c_int, [_vp, _vp, _i, _ll, _i, _ll, _i, _i, _vp]),
     "occd_argmax_classes": (C.c_int, [_vp, _vp, _ll, _i, _ll, _vp, _vp]),
+    "occd_argmax_classes_conf": (C.c_int, [_vp, _vp, _vp, _ll, _i, _ll, _vp, _vp]),
     "occd_normalize_rgb_u8": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "occd_stage_rgb_u8_cl": (C.c_int, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "occd_depth_u16_to_f32": (C.c_int, [_vp, _vp, _ll, C.c_double, _f, _vp]),
@@ -165,6 +166,7 @@ SYMBOLS = {
     "occd_model_load": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
     "occd_model_info": (C.c_int, [_vp, C.POINTER(ModelGeom)]),
     "occd_model_run_frame": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp]),
+    "occd_model_run_frame_conf": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp, _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
 }

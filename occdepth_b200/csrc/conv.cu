@@ -26,7 +26,7 @@ using namespace occd_conv;
 // channel group, so that one thread holds the position's arg-max
 template <typename T>
 __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ SimtParams p) {
-  const bool cls = p.epi.out1_mode == OCCD_OUT1_CLASS_U16;
+  const bool cls = class_mode(p.epi.out1_mode), conf = p.epi.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
   const int ngroups = cls ? 1 : p.epi.Cout_store / 8;
   const long long total = (long long)p.epi.B * p.epi.OD * p.epi.OH * p.epi.OW * ngroups;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ 
 #pragma unroll
     for (int i = 0; i < 8; ++i)
       if (g * 8 + i < p.epi.Cout)
-        class_arg_take(ca, class_value<T>(p.epi, epi_pos(p.epi, b, od, oh, ow), g * 8 + i, acc[i]), g * 8 + i);
+        class_arg_take(ca, class_value<T>(p.epi, epi_pos(p.epi, b, od, oh, ow), g * 8 + i, acc[i]), g * 8 + i, conf);
   }
   if (cls) class_store(p.epi, epi_pos(p.epi, b, od, oh, ow), ca);
 }
@@ -506,11 +506,10 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int
     iters = (iters + n_groups - 1) / n_groups;   // tap groups: the mean group; every CTA gets its share of each
     const long long m_tiles0 = (long long)d->B * t.tiles_d * t.tiles_h * t.tiles_w * n_groups;
     const int n_sms = n_sms_current();
-    // (a class map is costed as the planar logits it stands in for: both plans of one descriptor get the same tiles,
-    // so the map equals the arg-max of the logits bit for bit)
+    // (a class map, with or without its confidence, is costed as the planar logits it stands in for: every plan of
+    // one descriptor gets the same tiles, so the map equals the arg-max of the logits bit for bit)
     const double out_bytes_per_col = 128.0 * ((d->out0 ? pl->esize : 0) + (d->out1_mode == OCCD_OUT1_CL ? pl->esize : 0) +
-                                              (d->out1_mode == OCCD_OUT1_F32_PLANAR ||
-                                               d->out1_mode == OCCD_OUT1_CLASS_U16 ? 4 : 0));
+                                              (d->out1_mode == OCCD_OUT1_F32_PLANAR || class_mode(d->out1_mode) ? 4 : 0));
     // per-tile mainloop and epilogue of an n-column tile that stores out_cols channels
     auto estimate = [&](int n, int out_cols, double& mainloop, double& epi) {
       const double mma = (RB / 32) * mma_step_cycles(n);
@@ -533,7 +532,7 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int
     }
     estimate(t.N_tile, xp ? d->Cout_pad : t.N_tile, est_mainloop, est_epi);
   }
-  PLAN_REQUIRE(d->out1_mode != OCCD_OUT1_CLASS_U16 || xp || t.N_tile >= d->Cout_pad,
+  PLAN_REQUIRE(!class_mode(d->out1_mode) || xp || t.N_tile >= d->Cout_pad,
                "a class map needs every output channel in one N tile");
   PLAN_REQUIRE(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile),
                xp ? "no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)" : "no kernel compiled for this N tile");
@@ -608,7 +607,7 @@ static int simt_geometry(const occd_conv_desc* d, occd_conv_plan* pl) {
     s.tap_dz[i] = (short)d->taps[i].dz; s.tap_dy[i] = (short)d->taps[i].dy; s.tap_dx[i] = (short)d->taps[i].dx;
   }
   const long long total = (long long)d->B * d->OD * d->OH * d->OW *
-                          (d->out1_mode == OCCD_OUT1_CLASS_U16 ? 1 : s.epi.Cout_store / 8);
+                          (class_mode(d->out1_mode) ? 1 : s.epi.Cout_store / 8);
   pl->grid = dim3((unsigned)((total + 127) / 128));
   return OCCD_OK;
 }
@@ -710,7 +709,7 @@ extern "C" int occd_conv_plan_create(const occd_conv_desc* d, occd_conv_plan** o
                    aligned(d->out1), "occd_conv_plan_create: out1 channel window");
   if (d->out1_mode == OCCD_OUT1_F32_PLANAR)
     OCCD_CHECK_ARG(d->out1 && d->out1_coff + d->Cout <= d->out1_C, "occd_conv_plan_create: out1 planar window");
-  if (d->out1_mode == OCCD_OUT1_CLASS_U16) {
+  if (class_mode(d->out1_mode)) {
     OCCD_CHECK_ARG(d->out1 && reinterpret_cast<uintptr_t>(d->out1) % 2 == 0 && d->Cout <= 65535,
                    "occd_conv_plan_create: a class map needs an aligned uint16 out1 and at most 65535 classes");
     if (d->out0) {
@@ -774,7 +773,7 @@ extern "C" int occd_conv_plan_destroy(occd_conv_plan* plan) {
 extern "C" int occd_conv_plan_set_class_lut(occd_conv_plan* pl, const int* lut, int n) {
   OCCD_CHECK_ARG(pl != nullptr, "occd_conv_plan_set_class_lut: null plan");
   ConvEpi* e = plan_epi(pl);
-  OCCD_CHECK_ARG(e->out1_mode == OCCD_OUT1_CLASS_U16, "occd_conv_plan_set_class_lut: the plan writes no class map");
+  OCCD_CHECK_ARG(class_mode(e->out1_mode), "occd_conv_plan_set_class_lut: the plan writes no class map");
   if (!lut) {
     e->class_lut_use = 0;
     return OCCD_OK;

@@ -1,6 +1,7 @@
 // Device-side parameter block + shared epilogue for the implicit-GEMM convolution kernels.
 #pragma once
 #include "common.cuh"
+#include <cuda_fp16.h>
 #include "../../include/occdepth_b200.h"
 
 struct ConvEpi {
@@ -36,28 +37,70 @@ __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, in
   return epi_pos(e, b, od, oh, ow, e.oadd[0], e.oadd[1], e.oadd[2]);
 }
 
-// Running arg-max of the class-map output (OCCD_OUT1_CLASS_U16) over the channels one thread has seen, taken in
-// ascending channel order.  The rule is argmax_classes_kernel's (elementwise.cu): the first index of the largest value;
-// a NaN in channel 0 wins, a NaN anywhere else is skipped.  A NaN channel 0 is held as +inf, which no later value beats
-// and which wins every tie by its index, so two threads' partial results merge with the same take().
+// Running arg-max of the class-map output (OCCD_OUT1_CLASS_U16[_CONF]) over the channels one thread has seen, taken
+// in ascending channel order.  The rule is argmax_classes_kernel's (elementwise.cu): the first index of the largest
+// value; a NaN in channel 0 wins, a NaN anywhere else is skipped.  A NaN channel 0 is held as +inf, which no later
+// value beats and which wins every tie by its index, so two threads' partial results merge with the same rule.
+// With a confidence (conf == true) the same pass keeps a running softmax of the raw values: m, their largest value
+// (NaN never becomes it), and s = sum exp(v - m).  The top-class probability is then 1 / s, and NaN where a value
+// is NaN (s is NaN) or +inf (m == +inf), or where every value is -inf (m == -inf): torch.softmax's NaN cases.
+// Host and device share the helpers, so that a CPU build can replay the epilogues' merge orders.
 struct ClassArg {
   float v;
   int c;
+  float m, s;
 };
-__device__ __forceinline__ ClassArg class_arg_init() { return ClassArg{-INFINITY, 0x7fffffff}; }
-__device__ __forceinline__ void class_arg_take(ClassArg& a, float v, int c) {
+__host__ __device__ __forceinline__ bool class_mode(int out1_mode) {
+  return out1_mode == OCCD_OUT1_CLASS_U16 || out1_mode == OCCD_OUT1_CLASS_U16_CONF;
+}
+__host__ __device__ __forceinline__ ClassArg class_arg_init() { return ClassArg{-INFINITY, 0x7fffffff, -INFINITY, 0.f}; }
+__host__ __device__ __forceinline__ void class_arg_take(ClassArg& a, float v, int c, bool conf) {
+  if (conf) {
+    // v == a.m adds exp(0) without forming -inf - -inf; a NaN v adds NaN
+    if (v > a.m) {
+      a.s = a.s * expf(a.m - v) + 1.f;
+      a.m = v;
+    } else {
+      a.s += v == a.m ? 1.f : expf(v - a.m);
+    }
+  }
   if (c == 0 && v != v) v = INFINITY;
   if (v > a.v || (v == a.v && c < a.c)) { a.v = v; a.c = c; }
 }
-// the partial result of lane ^ mask joins this lane's (every lane of the warp calls it)
-__device__ __forceinline__ void class_arg_merge_xor(ClassArg& a, int mask) {
-  const float v = __shfl_xor_sync(0xffffffffu, a.v, mask);
-  const int c = __shfl_xor_sync(0xffffffffu, a.c, mask);
-  class_arg_take(a, v, c);
+// partial result b (channels disjoint from a's) joins a: the arg-max by take()'s rule, the softmax sums rescaled to
+// the larger maximum (a partial that has seen nothing, m == -inf and s == 0, is the identity)
+__host__ __device__ __forceinline__ void class_arg_join(ClassArg& a, const ClassArg& b, bool conf) {
+  if (conf) {
+    const float m = fmaxf(a.m, b.m);
+    a.s = (a.m == m ? a.s : a.s * expf(a.m - m)) + (b.m == m ? b.s : b.s * expf(b.m - m));
+    a.m = m;
+  }
+  if (b.v > a.v || (b.v == a.v && b.c < a.c)) { a.v = b.v; a.c = b.c; }
 }
-// out1[pos]: the class map has the planar logits' spatial index, one uint16 per position
+// the top-class probability of a complete result (see ClassArg), in fp32
+__host__ __device__ __forceinline__ float class_arg_conf(const ClassArg& a) {
+  return (a.m == INFINITY || a.m == -INFINITY) ? NAN : 1.f / a.s;
+}
+// the partial result of lane ^ mask joins this lane's (every lane of the warp calls it)
+__device__ __forceinline__ void class_arg_merge_xor(ClassArg& a, int mask, bool conf) {
+  ClassArg b;
+  b.v = __shfl_xor_sync(0xffffffffu, a.v, mask);
+  b.c = __shfl_xor_sync(0xffffffffu, a.c, mask);
+  if (conf) {
+    b.m = __shfl_xor_sync(0xffffffffu, a.m, mask);
+    b.s = __shfl_xor_sync(0xffffffffu, a.s, mask);
+  }
+  class_arg_join(a, b, conf);
+}
+// out1[pos]: the class map has the planar logits' spatial index, one uint16 per position; in OCCD_OUT1_CLASS_U16_CONF
+// the float16 confidence follows the whole map, at out1[B * positions + pos]
 __device__ __forceinline__ void class_store(const ConvEpi& e, long long pos, const ClassArg& a) {
-  reinterpret_cast<unsigned short*>(e.out1)[pos] = e.class_lut_use ? e.class_lut[a.c] : (unsigned short)a.c;
+  unsigned short* o = reinterpret_cast<unsigned short*>(e.out1);
+  o[pos] = e.class_lut_use ? e.class_lut[a.c] : (unsigned short)a.c;
+  if (e.out1_mode == OCCD_OUT1_CLASS_U16_CONF) {
+    const __half_raw h = __float2half_rn(class_arg_conf(a));
+    o[(long long)e.B * e.ODf * e.OHf * e.OWf + pos] = h.x;
+  }
 }
 // Pre-activation value of channel n at position pos from its accumulator sum: acc + bias + res1 (+ res2), the additions
 // of conv_epilogue_compute in its order, one channel at a time.  The class-map epilogues feed the arg-max with it
@@ -89,9 +132,10 @@ __device__ __forceinline__ void class_take8(const ConvEpi& e, long long pos, int
 #pragma unroll
     for (int i = 0; i < 8; ++i) x[i] += r[i];
   }
+  const bool conf = e.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
 #pragma unroll
   for (int i = 0; i < 8; ++i)
-    if (n0 + i < e.Cout) class_arg_take(a, x[i], n0 + i);
+    if (n0 + i < e.Cout) class_arg_take(a, x[i], n0 + i, conf);
 }
 
 // Epilogue arithmetic for one output position `pos` and NV consecutive channels [n0, n0+NV) held in v[] (fp32

@@ -137,8 +137,9 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
   constexpr int ROUND = LD == kStageWide ? 32 : 8;
   constexpr int TPR = ROUND == 8 ? 1 : 2, VW = ROUND / TPR;   // threads per row, channels per thread
   const int row = t / TPR, h = t % TPR;
-  if (e.out1_mode == OCCD_OUT1_CLASS_U16) {
-    // class map: every value joins the row's running arg-max as it leaves the staging buffer
+  if (class_mode(e.out1_mode)) {
+    // class map: every value joins the row's running arg-max (and softmax) as it leaves the staging buffer
+    const bool conf = e.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
     ClassArg ca = class_arg_init();
     const long long pos = valid ? epi_pos(e, b, od, oh, ow) : 0;
 #pragma unroll
@@ -152,10 +153,10 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
       if (valid && row < 64 && cc < N) {
 #pragma unroll 1
         for (int i = 0; i < VW && n0 + cc + i < e.Cout; ++i)
-          class_arg_take(ca, class_value<T>(e, pos, n0 + cc + i, st[row * LD + VW * h + i]), n0 + cc + i);
+          class_arg_take(ca, class_value<T>(e, pos, n0 + cc + i, st[row * LD + VW * h + i]), n0 + cc + i, conf);
       }
     }
-    if constexpr (TPR == 2) class_arg_merge_xor(ca, 1);
+    if constexpr (TPR == 2) class_arg_merge_xor(ca, 1, conf);
     if (valid && row < 64 && h == 0) class_store(e, pos, ca);
     return;
   }
@@ -219,7 +220,7 @@ struct XpRows {
 // one in the next or previous warp comes through the exchange buffer xb (xp_xchg_floats(d) floats, this
 // warpgroup's).  Chunks of 16 channels: two barriers each.  The sums of a row's 8-channel block are then gathered
 // into one lane of the quad (a 4 x 4 transpose of channel pairs by shuffle), which runs the row epilogue on them;
-// a class map instead takes them into the row's running arg-max, and the two lanes of a row merge theirs.
+// a class map instead takes them into the row's running arg-max (and softmax), and the two lanes of a row merge theirs.
 template <typename T, int N>
 __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* xb, int bar_id,
                                             int warp4, int lane, int d, const XpRows& rows, int b) {
@@ -295,11 +296,12 @@ __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)
       }
     }
     if constexpr (CLS) {
-      class_arg_merge_xor(ca, 1);   // lanes q and q ^ 1 hold the two blocks of each chunk of one row
+      // lanes q and q ^ 1 hold the two blocks of each chunk of one row
+      class_arg_merge_xor(ca, 1, e.out1_mode == OCCD_OUT1_CLASS_U16_CONF);
       if ((q & 1) == 0 && my_valid) class_store(e, pos, ca);
     }
   };
-  if (e.out1_mode == OCCD_OUT1_CLASS_U16) chunks(std::true_type{});
+  if (class_mode(e.out1_mode)) chunks(std::true_type{});
   else chunks(std::false_type{});
 }
 

@@ -1,7 +1,6 @@
 // Small bandwidth-bound helpers around the implicit-GEMM convolutions (channels-last activations, bf16 or
 // TF32-valued fp32: see Elem<T> in common.cuh).
-#include "common.cuh"
-#include "../../include/occdepth_b200.h"
+#include "conv_common.cuh"
 
 namespace {
 
@@ -85,6 +84,28 @@ __global__ void argmax_classes_kernel(const float* __restrict__ in, unsigned sho
   out[i] = lut.use ? lut.v[arg] : (unsigned short)arg;
 }
 
+// argmax_classes_kernel plus the top class's softmax probability (OCCD_OUT1_CLASS_U16_CONF's confidence): the same
+// running arg-max and softmax as the class-map epilogues (conv_common.cuh), over the channels in ascending order
+__global__ void argmax_classes_conf_kernel(const float* __restrict__ in, unsigned short* __restrict__ out,
+                                           unsigned short* __restrict__ conf, int C, long long S, long long total,
+                                           const ClassLut lut) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const long long b = i / S, s = i - b * S;
+  const float* p = in + b * C * S + s;
+  ClassArg a = class_arg_init();
+  for (int c = 0; c < C; ++c) class_arg_take(a, p[(long long)c * S], c, true);
+  out[i] = lut.use ? lut.v[a.c] : (unsigned short)a.c;
+  const __half_raw h = __float2half_rn(class_arg_conf(a));
+  conf[i] = h.x;
+}
+
+int class_lut_of(const int* lut, int C, ClassLut* l) {
+  l->use = lut ? 1 : 0;
+  for (int c = 0; c < kMaxLut; ++c) l->v[c] = (lut && c < C) ? (unsigned short)lut[c] : 0;  // .astype(np.uint16)
+  return OCCD_OK;
+}
+
 }  // namespace
 
 extern "C" int occd_argmax_classes(const float* in, void* out, long long B, int C, long long S, const int* lut,
@@ -94,10 +115,25 @@ extern "C" int occd_argmax_classes(const float* in, void* out, long long B, int 
   const long long total = B * S;
   OCCD_CHECK_ARG((total + 255) / 256 <= 2147483647LL, "occd_argmax_classes: too many positions");
   ClassLut l;
-  l.use = lut ? 1 : 0;
-  for (int c = 0; c < kMaxLut; ++c) l.v[c] = (lut && c < C) ? (unsigned short)lut[c] : 0;  // .astype(np.uint16)
+  class_lut_of(lut, C, &l);
   argmax_classes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       in, (unsigned short*)out, C, S, total, l);
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+
+extern "C" int occd_argmax_classes_conf(const float* in, void* out, void* conf, long long B, int C, long long S,
+                                        const int* lut, void* stream) {
+  OCCD_CHECK_ARG(in && out && conf && B > 0 && C > 0 && C <= 65535 && S > 0, "occd_argmax_classes_conf: args");
+  OCCD_CHECK_ARG(reinterpret_cast<uintptr_t>(out) % 2 == 0 && reinterpret_cast<uintptr_t>(conf) % 2 == 0,
+                 "occd_argmax_classes_conf: out and conf must be 2-byte aligned");
+  OCCD_CHECK_ARG(!lut || C <= kMaxLut, "occd_argmax_classes_conf: a label remap supports at most 64 classes");
+  const long long total = B * S;
+  OCCD_CHECK_ARG((total + 255) / 256 <= 2147483647LL, "occd_argmax_classes_conf: too many positions");
+  ClassLut l;
+  class_lut_of(lut, C, &l);
+  argmax_classes_conf_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      in, (unsigned short*)out, (unsigned short*)conf, C, S, total, l);
   OCCD_CHECK_LAUNCH();
   return OCCD_OK;
 }

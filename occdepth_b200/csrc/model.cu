@@ -35,6 +35,11 @@ struct ArgOf {  // pointer parameters
   static T get(const Arg& a) { return static_cast<T>(a.p); }
 };
 template <>
+struct ArgOf<occd_model*> {  // a model handle cannot be stored in a file: only NULL is recorded (the call then refuses)
+  static constexpr char tag = 'n';
+  static occd_model* get(const Arg&) { return nullptr; }
+};
+template <>
 struct ArgOf<int> {
   static constexpr char tag = 'i';
   static int get(const Arg& a) { return a.i; }
@@ -104,7 +109,9 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_ssc_confusion),         OCCD_ENTRY(occd_ssc_loss_sums),
     OCCD_ENTRY(occd_crp_relation_sums),     OCCD_ENTRY(occd_depth_cls_sums),
     OCCD_ENTRY(occd_occupied_voxels),       OCCD_ENTRY(occd_virtual_view_fwd),
-    OCCD_ENTRY(occd_vox2pix_range_fwd),
+    OCCD_ENTRY(occd_vox2pix_range_fwd),     OCCD_ENTRY(occd_argmax_classes_conf),
+    // takes a stream like the launches, so it has a signature here; its model handle can only be NULL
+    OCCD_ENTRY(occd_model_run_frame_conf),
 };
 
 const Entry* find_entry(const std::string& name) {
@@ -118,7 +125,8 @@ const char kMagic[8] = {'O', 'C', 'C', 'D', 'M', 'O', 'D', 'L'};
 enum Role { ROLE_IMG, ROLE_PIX, ROLE_FOV, ROLE_PIX_Z, ROLE_DEPTH, ROLE_CAMS, ROLE_SPS, ROLE_CLASSES, N_ROLES };
 const char* kRoleNames[N_ROLES] = {"image", "pix", "fov", "pix_z", "depth", "camera tables", "scaled_pixel_size",
                                    "class map"};
-enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2 };
+enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4 };   // FLAG_CONF: the class-map role holds the map, then its
+                                                                   // float16 confidence (OCCD_OUT1_CLASS_U16_CONF)
 const size_t kArenaAlign = 512;  // the caching allocator's block alignment, which the plans were built with
 
 struct Reader {
@@ -205,6 +213,7 @@ struct occd_model {
   float cams[4 * 40], sps[4];
 
   void* dev(int role) const { return arena + buf_off[roles[role].buffer] + roles[role].off; }
+  uint64_t map_bytes() const { return (uint64_t)out[0] * out[1] * out[2] * 2; }   // one uint16 class map
 };
 
 namespace {
@@ -269,6 +278,8 @@ int parse(occd_model* m) {
   if ((m->precision != OCCD_DTYPE_F32 && m->precision != OCCD_DTYPE_BF16) || m->dataset > 1 || m->V < 1 ||
       m->V > 4 || m->P < 1 || m->P > 64 || m->n_cams > 4 || m->img_cstride % 8 != 0)
     return fail(OCCD_ERR_FORMAT, "occd_model_load: header field out of range");
+  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF))
+    return fail(OCCD_ERR_FORMAT, "occd_model_load: unknown header flag bits");
   // counts are bounded by what the file can hold before anything is sized from them
   const size_t left = r.n - r.pos;
   if (n_buf > left / 12 || n_blob > left / 12 || n_plan > left / 12 || n_rec > left / 6)
@@ -380,7 +391,7 @@ int parse(occd_model* m) {
   const uint64_t want_len[N_ROLES] = {
       (uint64_t)m->V * m->img_h * m->img_w * m->img_cstride * (m->precision == OCCD_DTYPE_F32 ? 4 : 2),
       (uint64_t)VL * N * m->P * 16, (uint64_t)VL * N * m->P, N * 8, (uint64_t)m->depth_h * m->depth_w * 4,
-      (uint64_t)m->n_cams * 160, (uint64_t)m->n_cams * 4, (uint64_t)m->out[0] * m->out[1] * m->out[2] * 2};
+      (uint64_t)m->n_cams * 160, (uint64_t)m->n_cams * 4, m->map_bytes() * ((m->flags & FLAG_CONF) ? 2 : 1)};
   for (int k = 0; k < N_ROLES; ++k) {
     const RoleRef& ro = m->roles[k];
     if (!need[k]) continue;
@@ -705,9 +716,10 @@ extern "C" int occd_model_info(const occd_model* m, occd_model_geom* g) {
   return OCCD_OK;
 }
 
-extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t* class_map, void* stream) {
-  OCCD_CHECK_ARG(m && f && f->images && class_map, "occd_model_run_frame: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+namespace {
+
+// stages the frame and replays the records (through the graph when there is one) on `stream`
+int run_records(occd_model* m, const occd_frame* f, cudaStream_t st) {
   int rc = stage(m, f, st);
   if (rc != OCCD_OK) return rc;
   cudaError_t e;
@@ -733,9 +745,39 @@ extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t
   } else if ((e = cudaGraphLaunch(m->graph_exec, st)) != cudaSuccess) {
     return cuda_fail(e, "occd_model_run_frame: cudaGraphLaunch");
   }
-  if ((e = cudaMemcpyAsync(class_map, m->dev(ROLE_CLASSES), m->roles[ROLE_CLASSES].len, cudaMemcpyDeviceToDevice,
-                           st)) != cudaSuccess)
+  return OCCD_OK;
+}
+
+}  // namespace
+
+extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t* class_map, void* stream) {
+  OCCD_CHECK_ARG(m && f && f->images && class_map, "occd_model_run_frame: null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = run_records(m, f, st);
+  if (rc != OCCD_OK) return rc;
+  cudaError_t e;
+  if ((e = cudaMemcpyAsync(class_map, m->dev(ROLE_CLASSES), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) !=
+      cudaSuccess)
     return cuda_fail(e, "occd_model_run_frame: class map copy");
+  return OCCD_OK;
+}
+
+extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uint16_t* class_map, void* conf,
+                                         void* stream) {
+  OCCD_CHECK_ARG(m && f && f->images && class_map && conf, "occd_model_run_frame_conf: null argument");
+  if (!(m->flags & FLAG_CONF)) {
+    occd_set_last_error("occd_model_run_frame_conf: the model was exported without confidence");
+    return OCCD_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = run_records(m, f, st);
+  if (rc != OCCD_OK) return rc;
+  const char* roles = static_cast<const char*>(m->dev(ROLE_CLASSES));
+  cudaError_t e;
+  if ((e = cudaMemcpyAsync(class_map, roles, m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+    return cuda_fail(e, "occd_model_run_frame_conf: class map copy");
+  if ((e = cudaMemcpyAsync(conf, roles + m->map_bytes(), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+    return cuda_fail(e, "occd_model_run_frame_conf: confidence copy");
   return OCCD_OK;
 }
 

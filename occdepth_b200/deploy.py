@@ -22,7 +22,8 @@ from .engine import CL, ConvOp
 
 MAGIC = b"OCCDMODL"
 ROLES = ("img", "pix", "fov", "pix_z", "depth", "cams", "sps", "classes")
-FLAG_FLOSP_DEPTH, FLAG_VIRTUAL = 1, 2
+FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF = 1, 2, 4    # FLAG_CONF: the class-map role holds the map, then its
+                                                       # float16 confidence
 PATTERN_MAX = 64
 
 _STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
@@ -169,10 +170,12 @@ class _Buffers:
         return out.tobytes() if out.any() else None
 
 
-def export(model, path, frame, inv_map=None):
-    """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map)` for frames of this
-    frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame refuses, with the
-    same messages.  Returns a dict of what was written (records, buffers, bytes).
+def export(model, path, frame, inv_map=None, confidence=False):
+    """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map, confidence=confidence)`
+    for frames of this frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame
+    refuses, with the same messages.  Returns a dict of what was written (records, buffers, bytes).  With
+    `confidence` the file's class-map role holds the map and then its confidence (header flag FLAG_CONF), which
+    `occd_model_run_frame_conf` reads; without it the file is what it always was.
 
     The recording stand-in replaces the library for the calling thread only, so other threads may keep serving
     through the library meanwhile; `model` itself must not run elsewhere during the export (as for predict_frame)."""
@@ -184,8 +187,8 @@ def export(model, path, frame, inv_map=None):
     with torch.cuda.device(dev), torch.no_grad():
         _lib._RECORDING.recorder = rec
         try:
-            ent = model._build(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"], classes=("classes", lut),
-                               capture=False)
+            ent = model._build(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"],
+                               classes=model._class_key(inv_map, confidence), capture=False)
             plan, img_cl, pix, fov, out, depth0 = ent[:6]
             plan.pix_z = torch.zeros(pix.shape[2], dtype=torch.float64, device=dev)
             state = getattr(plan, "flosp_state", None)
@@ -261,9 +264,9 @@ def export(model, path, frame, inv_map=None):
         lut_arr[:len(lut)] = lut
     S = [int(s) // model.project_scale for s in model.full_scene_size]
     hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
-                              1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0),
-                              f["V"], f["H"], f["W"], model.project_scale),
-           struct.pack("<7I", *S, *out.shape[1:], f["P"]), pattern.astype("<i4").tobytes(),
+                              1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0)
+                              | (FLAG_CONF if confidence else 0), f["V"], f["H"], f["W"], model.project_scale),
+           struct.pack("<7I", *S, *out.shape[-3:], f["P"]), pattern.astype("<i4").tobytes(),
            struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
                        *[float(v) for v in f["scene_size"]]),
            struct.pack("<2I", model.n_classes, 0 if lut is None else 1), lut_arr.astype("<i4").tobytes(),
@@ -323,9 +326,11 @@ class LoadedModel:
         _lib.check(_lib.lib().occd_model_info(self.handle, C.byref(g)), "occd_model_info")
         return g
 
-    def run_frame(self, frame, out=None, stream=None, graph=True):
+    def run_frame(self, frame, out=None, stream=None, graph=True, conf=None):
         """frame: as OccDepth.predict_frame takes it (the uint8 images may be on the host or the device) -> the
-        uint16 class map [1, X, Y, Z] on the current device, enqueued on `stream` (default: the current stream)"""
+        uint16 class map [1, X, Y, Z] on the current device, enqueued on `stream` (default: the current stream).
+        `conf`: a float16 [1, X, Y, Z] device tensor (or True: allocate one) that gets the map's confidence through
+        occd_model_run_frame_conf; the result is then (map, conf)."""
         g = self.geom
         img = torch.as_tensor(frame["img"])
         if img.dim() == 3:
@@ -363,15 +368,23 @@ class LoadedModel:
         f.flags = 0 if graph else _lib.FRAME_NO_GRAPH
         if out is None:
             out = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.uint16, device=img.device)
+        if conf is True:
+            conf = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.float16, device=img.device)
+        if conf is not None:
+            assert conf.dtype == torch.float16 and conf.is_cuda and conf.is_contiguous() and conf.numel() == out.numel()
         if stream is not None:
             # the inputs were copied and `out` allocated on the current stream; they must live until `stream` is done
             stream.wait_stream(torch.cuda.current_stream())
-            for t in [k for k in keep if isinstance(k, torch.Tensor)] + [out]:
+            for t in [k for k in keep if isinstance(k, torch.Tensor)] + [out] + ([] if conf is None else [conf]):
                 t.record_stream(stream)
         st = (stream or torch.cuda.current_stream()).cuda_stream
-        _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), out.data_ptr(), C.c_void_p(st)),
-                   "occd_model_run_frame")
-        return out
+        if conf is None:
+            _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), out.data_ptr(), C.c_void_p(st)),
+                       "occd_model_run_frame")
+            return out
+        _lib.check(_lib.lib().occd_model_run_frame_conf(self.handle, C.byref(f), out.data_ptr(), conf.data_ptr(),
+                                                        C.c_void_p(st)), "occd_model_run_frame_conf")
+        return out, conf
 
     def close(self):
         if self.handle:

@@ -190,6 +190,9 @@ class ClassMapUnsupported(RuntimeError):
     """occd_conv_plan_create refused a class-map output (OCCD_ERR_UNSUPPORTED) for the kernel this launch runs on"""
 
 
+CLASS_MODES = ("classes", "classes_conf")     # ConvOp / Plan.conv out1 modes that write a class map
+
+
 class ConvOp:
     """One planned implicit-GEMM launch (occd_conv_plan_create / occd_conv_run)."""
 
@@ -201,7 +204,8 @@ class ConvOp:
         bias: fp32 [Cout];  out0/res1/res2: CL on the full output grid;  out1: CL (pre-activation bf16 copy) or
         fp32 planar tensor [B, C1, D, H, W] (mode "planar", written at channel out1_coff), or the uint16 class map
         [B, D, H, W] of the pre-activation values (mode "classes", no out0; lut: Cout label ids or None, the remap of
-        occd_argmax_classes).  Raises ClassMapUnsupported when the chosen kernel cannot write a class map.
+        occd_argmax_classes), or that map followed by the float16 bits of its confidence, uint16 [2, B, D, H, W]
+        (mode "classes_conf").  Raises ClassMapUnsupported when the chosen kernel cannot write a class map.
         groups: [(n_taps_of_group, (oadd_d, oadd_h, oadd_w))] -- several convolutions over the same sources in one
         launch, each with its own slice of `taps` and output offset (occd_conv_desc.n_groups; per-tap TC kernel)."""
         self.name = name
@@ -296,11 +300,15 @@ class ConvOp:
             assert out0 is None and out1.dtype == torch.uint16 and out1.is_contiguous()
             assert tuple(out1.shape) == (B,) + fd
             d.out1_mode, d.out1 = _lib.OUT1_CLASS_U16, out1.data_ptr()
+        elif out1_mode == "classes_conf":
+            assert out0 is None and out1.dtype == torch.uint16 and out1.is_contiguous()
+            assert tuple(out1.shape) == (2, B) + fd
+            d.out1_mode, d.out1 = _lib.OUT1_CLASS_U16_CONF, out1.data_ptr()
         self.desc = d
         self.flops = 2 * B * OD * OH * OW * Cout * sum(srcs[t[0]].C for t in taps)
         h = C.c_void_p()
         rc = _lib.lib().occd_conv_plan_create(C.byref(d), C.byref(h))
-        if rc == _lib.ERR_UNSUPPORTED and out1_mode == "classes":
+        if rc == _lib.ERR_UNSUPPORTED and out1_mode in CLASS_MODES:
             raise ClassMapUnsupported("occd_conv_plan_create(%s): %s" % (name, _lib.lib().occd_last_error().decode()))
         _lib.check(rc, "occd_conv_plan_create(%s)" % name)
         self.handle = h
@@ -413,7 +421,9 @@ class Plan:
              out0_exact=False, lut=None):
         """x: CL; weight fp32 [Cout,Cin,kd,kh,kw] (BN already folded); returns the output CL.
         out1_mode="classes": out1 is a uint16 [B, D, H, W] class map (no out0), written by the conv's epilogue; where
-        the kernel cannot do that, the logits go to a plan-owned fp32 buffer and occd_argmax_classes maps them."""
+        the kernel cannot do that, the logits go to a plan-owned fp32 buffer and occd_argmax_classes maps them.
+        out1_mode="classes_conf": out1 is uint16 [2, B, D, H, W], the map and then the float16 bits of each position's
+        top-class softmax probability (the fallback: occd_argmax_classes_conf)."""
         s, p, d = _t3(stride), _t3(padding), _t3(dilation)
         B, ID, IH, IW = x.dims
         co, ci, kd, kh, kw = weight.shape
@@ -431,18 +441,19 @@ class Plan:
         self.need_halo(x, taps, s[0], od[0])
         kw = dict(out0=out, act=act, res1=res1, res2=res2, stride=s, name=name, impl=impl, res2_post=res2_post,
                   out0_exact=out0_exact)
-        if out1_mode == "classes":
+        if out1_mode in CLASS_MODES:
             try:
-                self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode="classes", lut=lut, **kw))
+                self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode=out1_mode, lut=lut, **kw))
             except ClassMapUnsupported:
-                self._class_map_fallback(x, taps, ws, bias, od, out1, lut, kw)
+                self._class_map_fallback(x, taps, ws, bias, od, out1, lut, kw, out1_mode == "classes_conf")
             return out
         self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode=out1_mode, out1_coff=out1_coff, **kw))
         return out
 
-    def _class_map_fallback(self, x, taps, ws, bias, od, classes, lut, kw):
+    def _class_map_fallback(self, x, taps, ws, bias, od, classes, lut, kw, conf=False):
         """the class map of a conv whose kernel cannot write one: planar fp32 logits into a plan-owned buffer, then
-        occd_argmax_classes (the same values and rule, so the same map)"""
+        occd_argmax_classes (the same values and rule, so the same map); with `conf` occd_argmax_classes_conf, which
+        writes classes[0] and the confidence bits classes[1]"""
         B = x.dims[0]
         co = int(bias.numel())
         logits = torch.empty((B, co) + tuple(od), dtype=torch.float32, device=self.device)
@@ -450,6 +461,11 @@ class Plan:
         L = _lib.lib()
         S = od[0] * od[1] * od[2]
         lut_c = None if lut is None else (C.c_int * len(lut))(*[int(v) for v in lut])
+        if conf:
+            self.add(FnOp(lambda st: L.occd_argmax_classes_conf(logits.data_ptr(), classes[0].data_ptr(),
+                                                                classes[1].data_ptr(), B, co, S, lut_c, st),
+                          "occd_argmax_classes_conf", keep=(logits, classes, lut_c)))
+            return
         self.add(FnOp(lambda st: L.occd_argmax_classes(logits.data_ptr(), classes.data_ptr(), B, co, S, lut_c, st),
                       "occd_argmax_classes", keep=(logits, classes, lut_c)))
 

@@ -145,9 +145,10 @@ class OccDepth(_Base, B200Module):
 
     # ------------------------------------------------------------------------------------------
     def _build(self, B, V, H, W, N, P, dev, batch, classes=None, capture=True):
-        """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut): the plan of
-        predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor).  capture=False: no
-        CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says"""
+        """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut, *options): the
+        plan of predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor).  Options:
+        "conf" -- `out` is uint16 [2, B, X, Y, Z], the map then the float16 bits of its confidence; "root" -- see
+        below.  capture=False: no CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says"""
         slab = self.__dict__.get("slab_ctx")
         plan = Plan(dev, slab=slab, precision=self.precision)
         ps = self.project_scale
@@ -267,15 +268,21 @@ class OccDepth(_Base, B200Module):
         if classes is None:
             out = self.net_3d_decoder.emit(plan, x3d)
         else:
-            out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1])
-            if classes[2:] == ("root",):
-                # predict_frame(slab_output="root"): rank 0 gathers the ranks' slabs into the whole map, which is then
-                # this plan's output there; the other ranks' plans output nothing
+            conf = "conf" in classes[2:]
+            out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1], confidence=conf)
+            if "root" in classes[2:]:
+                # predict_frame(slab_output="root"): rank 0 gathers the ranks' slabs into the whole map (and its
+                # confidence: a second gather of the same shape), which is then this plan's output there; the other
+                # ranks' plans output nothing
                 bounds = [(lo * ps, hi * ps) for lo, hi in slab.bounds]       # every rank's plan.x_range
+                parts = [out[0], out[1]] if conf else [out]
                 whole = None
                 if slab.rank == 0:
-                    whole = torch.empty((1, bounds[-1][1]) + tuple(out.shape[2:]), dtype=out.dtype, device=dev)
-                plan.add(slab.gather_root_op(out, whole, bounds))
+                    whole = torch.empty(((2,) if conf else ()) + (1, bounds[-1][1]) + tuple(out.shape[-2:]),
+                                        dtype=out.dtype, device=dev)
+                for k, part in enumerate(parts):
+                    plan.add(slab.gather_root_op(part, None if whole is None else (whole[k] if conf else whole),
+                                                 bounds))
                 out = whole
         if capture and os.environ.get("OCCDEPTH_CUDA_GRAPH", "1") == "1":
             try:
@@ -288,13 +295,20 @@ class OccDepth(_Base, B200Module):
     def forward(self, batch):
         return self._run(batch, None)
 
-    def predict_classes(self, batch, inv_map=None):
+    def predict_classes(self, batch, inv_map=None, confidence=False):
         """uint16 class per voxel [B, X, Y, Z]: bit for bit `class_map(self(batch)["ssc_logit"], inv_map)`, but the
         classifier's epilogue writes the map, so no logits (and none of the forward's other outputs) are stored,
         converted or copied.  inv_map: one label id per class (at most 64), the submission writer's remap.  Its plan is
         cached apart from the forward's (alternating both rebuilds neither); under enable_slab_parallel this rank's
-        X-slab."""
-        return self._run(batch, ("classes", self._class_lut(inv_map)))
+        X-slab.  confidence=True: returns (map, conf), conf float16 [B, X, Y, Z] each voxel's top-class softmax
+        probability, max softmax(ssc_logit), computed by the same epilogue in fp32 and rounded once (NaN where a logit
+        is NaN or +inf; inv_map does not touch it).  The map is the same either way."""
+        return self._run(batch, self._class_key(inv_map, confidence))
+
+    def _class_key(self, inv_map, confidence=False, root=False):
+        """the `classes` argument of _build (and part of the class-map plan's cache key)"""
+        return (("classes", self._class_lut(inv_map)) + (("conf",) if confidence else ())
+                + (("root",) if root else ()))
 
     def _class_lut(self, inv_map):
         if inv_map is None:
@@ -385,6 +399,8 @@ class OccDepth(_Base, B200Module):
         ent[0].run()
         if ent[4] is None:                     # slab_output="root" on a rank other than 0
             return None
+        if "conf" in classes[2:]:              # uint16 [2, ...]: the map, then the confidence's float16 bits
+            return ent[4][0].clone(), ent[4][1].clone().view(torch.float16)
         return ent[4].clone()                  # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
@@ -404,9 +420,9 @@ class OccDepth(_Base, B200Module):
             self.flosp_depth.stage_inputs(batch, dev, plan.flosp_state)
 
     # ---- camera frames: uint8 images and calibration in, the datasets' pre-processing on the device -------------
-    def predict_frame(self, frame, classes=True, inv_map=None, slab_output=None):
-        """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map` as in predict_classes) or
-        the forward's output dict (classes=False), through the same cached plan a tensor batch of the same shapes
+    def predict_frame(self, frame, classes=True, inv_map=None, slab_output=None, confidence=False):
+        """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map` and `confidence` as in
+        predict_classes) or the forward's output dict (classes=False), through the same cached plan a tensor batch of the same shapes
         uses.  Only the staging differs: the datasets' pre-processing (eval split, no augmentation) runs on the device
         and writes the plan's input buffers -- the images through `occd_stage_rgb_u8_cl`, the indices through
         `occd_vox2pix_fwd`, NYU's depth map through `occd_depth_u16_to_f32`.
@@ -424,12 +440,16 @@ class OccDepth(_Base, B200Module):
 
         Under enable_slab_parallel every rank is handed the same frame and `slab_output` says which result it wants:
           "slab": this rank's X-slab, as predict_classes returns it (classes=False: the forward's per-rank dict);
-          "root": (classes=True only) rank 0 returns the whole [1, X, Y, Z] map, bit for bit the unpartitioned one,
-                  gathered from the ranks' slabs; the other ranks return None.
+          "root": (classes=True only) rank 0 returns the whole [1, X, Y, Z] map (with `confidence` the whole (map,
+                  conf)), bit for bit the unpartitioned one, gathered from the ranks' slabs; the other ranks return
+                  None.
         Each rank stages its own view under view sharding (else every view), the whole depth map, and the indices of
         its X-slab only (`occd_vox2pix_range_fwd`).  Without slab_output the partition is refused; without the
         partition slab_output must be None."""
-        return self._run_frame(self._frame_checked(frame, slab_output, classes), classes, inv_map, slab_output)
+        if confidence and not classes:
+            raise ValueError("OccDepth.predict_frame: confidence=True is the class map's confidence (classes=True)")
+        return self._run_frame(self._frame_checked(frame, slab_output, classes), classes, inv_map, slab_output,
+                               confidence)
 
     def _frame_checked(self, frame, slab_output=None, classes=True):
         """the refusals of the camera route, then `_frame_inputs`"""
@@ -452,13 +472,13 @@ class OccDepth(_Base, B200Module):
         self._check_mode(torch.empty(0, device=dev))
         return self._frame_inputs(frame, dev)
 
-    def _run_frame(self, f, classes, inv_map, slab_output=None):
+    def _run_frame(self, f, classes, inv_map, slab_output=None, confidence=False):
         dev = f["imgs"].device
         key = self._plan_key(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"])
         stage = lambda ent: self._stage_frame(ent, f)     # noqa: E731
         with torch.cuda.device(dev):
             if classes:
-                cls = ("classes", self._class_lut(inv_map)) + (("root",) if slab_output == "root" else ())
+                cls = self._class_key(inv_map, confidence, slab_output == "root")
                 return self._classes_on(f["batch"], key + cls, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
                                         stage)
             return self._forward_on(f["batch"], key, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage)
@@ -675,13 +695,14 @@ class OccDepth(_Base, B200Module):
         return res
 
     @staticmethod
-    def class_map(ssc_logit, inv_map=None):
+    def class_map(ssc_logit, inv_map=None, confidence=False):
         """uint16 class per voxel from the fp32 logits [B, C, X, Y, Z] on the GPU -- what the reference's callers
         compute on the host after copying all logits back (`np.argmax(torch.softmax(pred["ssc_logit"], 1).cpu(),
         1).astype(np.uint16)`, scripts/generate_output.py:94-97; eval.py does the same).  168 MB of logits shrink to
         a 4 MB map before the device->host read.  `inv_map` (int array of C label ids, io_data.get_inv_map) applies the
         submission writer's remap `inv_map[y_pred].astype(np.uint16)` (generate_kitti_submission.py:79) in the same
-        launch."""
+        launch.  confidence=True: returns (map, conf), conf float16 [B, X, Y, Z] the top class's softmax probability
+        (occd_argmax_classes_conf; NaN where a logit is NaN or +inf; the remap does not touch it)."""
         from .. import _lib
         if not (ssc_logit.is_cuda and ssc_logit.dtype == torch.float32 and ssc_logit.dim() == 5):
             raise RuntimeError("OccDepth.class_map: expected CUDA fp32 logits [B, C, X, Y, Z]")
@@ -695,8 +716,13 @@ class OccDepth(_Base, B200Module):
             lut = np.ascontiguousarray(np.asarray(inv_map).astype(np.int32))
             if lut.shape != (Cn,):
                 raise ValueError("OccDepth.class_map: inv_map must hold one label id per class")
-        _lib.check(_lib.lib().occd_argmax_classes(x.data_ptr(), out.data_ptr(), B, Cn, S,
-                                                  None if lut is None else lut.ctypes.data, _lib.stream_ptr()),
+        lut_p = None if lut is None else lut.ctypes.data
+        if confidence:
+            conf = torch.empty(out.shape, dtype=torch.float16, device=x.device)
+            _lib.check(_lib.lib().occd_argmax_classes_conf(x.data_ptr(), out.data_ptr(), conf.data_ptr(), B, Cn, S,
+                                                           lut_p, _lib.stream_ptr()), "occd_argmax_classes_conf")
+            return out, conf
+        _lib.check(_lib.lib().occd_argmax_classes(x.data_ptr(), out.data_ptr(), B, Cn, S, lut_p, _lib.stream_ptr()),
                    "occd_argmax_classes")
         return out
 

@@ -56,13 +56,15 @@ def _planar_out(plan, x, C_):
     return torch.empty(B, C_, D, H, W, dtype=torch.float32, device=plan.device)
 
 
-def _classifier(plan, x, w, b, name, classes, lut, res1=None):
+def _classifier(plan, x, w, b, name, classes, lut, res1=None, confidence=False):
     """the head's last conv: fp32 planar logits [B, n_classes, D, H, W], or (classes) their uint16 arg-max map
-    [B, D, H, W] (label ids lut[class] when lut is given) written by the same epilogue instead"""
+    [B, D, H, W] (label ids lut[class] when lut is given) written by the same epilogue instead; with `confidence`
+    uint16 [2, B, D, H, W]: that map, then the float16 bits of each voxel's top-class softmax probability"""
     if classes:
         B, D, H, W = x.dims
-        out = torch.empty(B, D, H, W, dtype=torch.uint16, device=plan.device)
-        plan.conv(x, w, b, padding=1, res1=res1, out1=out, out1_mode="classes", lut=lut, no_out0=True, name=name)
+        shape, mode = ((2, B, D, H, W), "classes_conf") if confidence else ((B, D, H, W), "classes")
+        out = torch.empty(shape, dtype=torch.uint16, device=plan.device)
+        plan.conv(x, w, b, padding=1, res1=res1, out1=out, out1_mode=mode, lut=lut, no_out0=True, name=name)
         return out
     out = _planar_out(plan, x, w.shape[0])
     plan.conv(x, w, b, padding=1, res1=res1, out1=out, out1_mode="planar", no_out0=True, name=name)
@@ -88,14 +90,14 @@ class SegmentationHead(B200Module):
         _aspp_params(self, planes, dilations_conv_list)
         self.conv_classes = nn.Conv3d(planes, nbr_classes, kernel_size=3, padding=1, stride=1)
 
-    def emit(self, plan, x, classes=False, lut=None):
+    def emit(self, plan, x, classes=False, lut=None, confidence=False):
         """-> fp32 planar logits [B, n_classes, X, Y, Z] (written directly by the last conv's epilogue), or with
-        `classes` their uint16 class map [B, X, Y, Z]"""
+        `classes` their uint16 class map [B, X, Y, Z] (`confidence`: see _classifier)"""
         w, b = fold_bn(self.conv0.weight, self.conv0.bias, None)
         x0 = plan.conv(x, w, b, padding=1, act="relu", name="head.conv0")
         x1 = _emit_aspp(plan, self, x0, name="head.aspp")
         w, b = fold_bn(self.conv_classes.weight, self.conv_classes.bias, None)
-        return _classifier(plan, x1, w, b, "head.conv_classes", classes, lut)
+        return _classifier(plan, x1, w, b, "head.conv_classes", classes, lut, confidence=confidence)
 
     def forward(self, x_in):
         return self._run_planar(x_in)
@@ -111,9 +113,9 @@ class SegmentationHeadCascadeCLS(B200Module):
         self.occ_classes = nn.Conv3d(planes, occ_classes, kernel_size=3, padding=1, stride=1)
         self.softmax = nn.Softmax(dim=1)
 
-    def emit(self, plan, x, classes=False, lut=None):
+    def emit(self, plan, x, classes=False, lut=None, confidence=False):
         """-> (ssc logits, occupancy logits), fp32 planar; with `classes` the ssc output is the uint16 class map
-        [B, X, Y, Z] (the occupancy logits still feed the softmax)"""
+        [B, X, Y, Z] (the occupancy logits still feed the softmax; `confidence`: see _classifier)"""
         planes = self.conv0.out_channels
         w, b = fold_bn(self.conv0.weight, self.conv0.bias, None)
         x0 = plan.conv(x, w, b, padding=1, act="relu", name="head.conv0")
@@ -135,7 +137,7 @@ class SegmentationHeadCascadeCLS(B200Module):
         # `part` only feeds the second launch's epilogue add (never an MMA operand): stored unrounded in tf32 mode
         part = plan.conv(x1, w[:, :planes].contiguous(), b, padding=1, name="head.conv_classes.a", out0_exact=True)
         logits = _classifier(plan, sm, w[:, planes:].contiguous(), torch.zeros_like(b), "head.conv_classes.b", classes,
-                             lut, res1=part)
+                             lut, res1=part, confidence=confidence)
         return logits, x_occ
 
     def forward(self, x_in):

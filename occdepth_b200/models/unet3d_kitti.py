@@ -43,8 +43,9 @@ class UNet3D(B200Module):
         if context_prior:
             self.CP_mega_voxels = CPMegaVoxels(f * 4, size_l3, bn_momentum=bn_momentum)
 
-    def emit(self, plan, x3d_l1, classes=False, lut=None):
+    def emit(self, plan, x3d_l1, classes=False, lut=None, confidence=False):
         """-> the forward's output dict, or with `classes` only the uint16 class map [B, X, Y, Z] of the ssc head
+        (`confidence`: uint16 [2, B, X, Y, Z], the map and its float16 confidence bits, modules._classifier)
         (the occluded head, whose logits nothing then reads, is not planned)"""
         res = {}
         x3d_l2 = self.process_l1[1].emit(plan, self.process_l1[0].emit(plan, x3d_l1))
@@ -58,7 +59,7 @@ class UNet3D(B200Module):
         x3d_up_l1 = self.up_12_l1.emit(plan, x3d_up_l2, skip=x3d_l1)
         x3d_up_lfull = self.up_l1_lfull.emit(plan, x3d_up_l1)
         if classes:
-            out = self.ssc_head.emit(plan, x3d_up_lfull, classes=True, lut=lut)
+            out = self.ssc_head.emit(plan, x3d_up_lfull, classes=True, lut=lut, confidence=confidence)
             return out[0] if self.cascade_cls else out
         if not self.infer_mode:
             res["x3d_l1"] = x3d_up_l1

@@ -35,8 +35,9 @@ class UNet3D(B200Module):
             size_1_16 = tuple(int(np.ceil(i / 4)) for i in full_scene_size)
             self.CP_mega_voxels = CPMegaVoxels(f16, size_1_16, n_relations=n_relations, bn_momentum=bn_momentum)
 
-    def emit(self, plan, x3d_1_4, classes=False, lut=None):
-        """-> the forward's output dict, or with `classes` only the uint16 class map [B, X, Y, Z] of the ssc head"""
+    def emit(self, plan, x3d_1_4, classes=False, lut=None, confidence=False):
+        """-> the forward's output dict, or with `classes` only the uint16 class map [B, X, Y, Z] of the ssc head
+        (`confidence`: uint16 [2, B, X, Y, Z], the map and its float16 confidence bits, modules._classifier)"""
         res = {}
         x3d_1_8 = self.process_1_4[1].emit(plan, self.process_1_4[0].emit(plan, x3d_1_4))
         x3d_1_16 = self.process_1_8[1].emit(plan, self.process_1_8[0].emit(plan, x3d_1_8))
@@ -48,7 +49,7 @@ class UNet3D(B200Module):
         x3d_up_1_8 = self.up_1_16_1_8.emit(plan, x3d_1_16, skip=x3d_1_8)
         x3d_up_1_4 = self.up_1_8_1_4.emit(plan, x3d_up_1_8, skip=x3d_1_4)
         if classes:
-            out = self.ssc_head_1_4.emit(plan, x3d_up_1_4, classes=True, lut=lut)
+            out = self.ssc_head_1_4.emit(plan, x3d_up_1_4, classes=True, lut=lut, confidence=confidence)
             return out[0] if self.cascade_cls else out
         if not self.infer_mode:
             res["x3d_l1"] = x3d_up_1_4

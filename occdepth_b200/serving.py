@@ -15,22 +15,48 @@ allocated per frame (a caching-allocator block that changes streams would serial
     logits = pipe.result(pipe.flush())
 
 With `classes=True` every frame runs `model.predict_classes(batch, inv_map)` instead: the classifier writes the
-uint16 class map [B, X, Y, Z] (4 MB at config 2) and that is what is read back, not the 168 MB of logits.
+uint16 class map [B, X, Y, Z] (4 MB at config 2) and that is what is read back, not the 168 MB of logits.  With
+`confidence=True` as well, the float16 top-class probability of every voxel is read back beside it and `result` returns
+(map, conf).
 """
 import torch
 
 from .engine import require_cuda
 
 
+def _result_buffers(res):
+    """the device and pinned host buffers of one read-back slot: the result's shape, or for a (map, conf) pair one
+    uint16 [2, ...] buffer that holds the map and then the confidence's float16 bits"""
+    if isinstance(res, tuple):
+        dev = torch.empty((2,) + tuple(res[0].shape), dtype=torch.uint16, device=res[0].device)
+    else:
+        dev = torch.empty_like(res)
+    return dev, torch.empty(dev.shape, dtype=dev.dtype).pin_memory()
+
+
+def _copy_result(dst, res):
+    if isinstance(res, tuple):
+        dst[0].copy_(res[0])
+        dst[1].copy_(res[1].view(torch.uint16))
+    else:
+        dst.copy_(res)
+
+
+def _host_result(host, confidence):
+    return (host[0], host[1].view(torch.float16)) if confidence else host
+
+
 class FramePipeline:
     def __init__(self, model, img_shape, pix_shape, fov_shape, device=None, out_key="ssc_logit", classes=False,
-                 inv_map=None):
+                 inv_map=None, confidence=False):
         if not torch.cuda.is_available():
             raise RuntimeError("FramePipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         require_cuda(torch.empty(0, device=dev), "FramePipeline")
+        if confidence and not classes:
+            raise ValueError("FramePipeline: confidence=True is the class map's confidence (classes=True)")
         self.model, self.dev, self.out_key = model, dev, out_key
-        self.classes, self.inv_map = classes, inv_map
+        self.classes, self.inv_map, self.confidence = classes, inv_map, confidence
         self.key = "%d" % model.project_scale
         self.main = torch.cuda.current_stream(dev)
         self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
@@ -61,15 +87,14 @@ class FramePipeline:
         batch = {"img": buf["img"], "projected_pix_" + self.key: [buf["pix"]], "fov_mask_" + self.key: [buf["fov"]]}
         with torch.no_grad():
             if self.classes:
-                res = self.model.predict_classes(batch, self.inv_map)
+                res = self.model.predict_classes(batch, self.inv_map, confidence=self.confidence)
             else:
                 res = self.model(batch)[self.out_key]
         self.in_free[j].record(self.main)
         if self.dev_out[j] is None:
-            self.dev_out[j] = torch.empty_like(res)
-            self.host_out[j] = torch.empty(res.shape, dtype=res.dtype).pin_memory()
+            self.dev_out[j], self.host_out[j] = _result_buffers(res)
         self.main.wait_event(self.out_free[j])
-        self.dev_out[j].copy_(res)           # the result leaves the allocator-owned tensor on the compute stream
+        _copy_result(self.dev_out[j], res)   # the result leaves the allocator-owned tensor on the compute stream
         self.out_ready[j].record(self.main)
         with torch.cuda.stream(self.d2h):
             self.d2h.wait_event(self.out_ready[j])
@@ -83,13 +108,13 @@ class FramePipeline:
         return self.n - 1 if self.n else None
 
     def result(self, ticket):
-        """host tensor of a submitted frame; blocks until its D2H read has finished.  The buffer is reused by the
-        second submit after the one that produced it."""
+        """host tensor of a submitted frame (with `confidence`: (map, conf) views of one pinned buffer); blocks until
+        its D2H read has finished.  The buffer is reused by the second submit after the one that produced it."""
         if ticket is None or ticket < self.n - 2 or ticket >= self.n:
             raise ValueError("FramePipeline.result: ticket %r is not one of the two frames in flight" % (ticket,))
         j = ticket & 1
         self.out_free[j].synchronize()
-        return self.host_out[j]
+        return _host_result(self.host_out[j], self.confidence)
 
     def join(self):
         """make the compute stream wait for every outstanding read-back (for timing with CUDA events)"""
@@ -116,6 +141,9 @@ class CameraPipeline:
     nothing else is allocated per frame.  One frame per submit; not for infer_mode with flosp_depth (that route takes
     sampling grids, not camera matrices).
 
+    `confidence=True` (with classes=True) reads back each voxel's float16 top-class probability beside the map into the
+    same pinned buffer; `result(ticket)` then returns (map, conf).
+
     Under enable_slab_parallel (one pipeline per rank, every rank submitting the same frames) `slab_output` is
     required and means what it does for predict_frame: "slab" reads back this rank's X-slab, "root" the whole class
     map (or voxel list) on rank 0 -- the other ranks read nothing back and their `result()` is None.  Under the
@@ -127,12 +155,16 @@ class CameraPipeline:
     and says whether the frame held more (`truncated`).  `d2h_bytes` is what a frame reads back."""
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
-                 inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None):
+                 inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None,
+                 confidence=False):
         if not torch.cuda.is_available():
             raise RuntimeError("CameraPipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         if output not in (None, "voxels"):
             raise ValueError("CameraPipeline: output must be None (the class map or logits, as `classes` says) or "
                              "'voxels', got %r" % (output,))
+        if confidence and (output is not None or not classes):
+            raise ValueError("CameraPipeline: confidence=True is the class map's confidence (classes=True, "
+                             "output=None); the voxel list has no confidence column")
         if slab_output not in (None, "slab", "root"):
             raise ValueError("CameraPipeline: slab_output must be None, 'slab' or 'root', got %r" % (slab_output,))
         slab = model.__dict__.get("slab_ctx")
@@ -150,7 +182,7 @@ class CameraPipeline:
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         require_cuda(torch.empty(0, device=dev), "CameraPipeline")
         self.model, self.dev, self.out_key = model, dev, out_key
-        self.classes, self.inv_map = classes, inv_map
+        self.classes, self.inv_map, self.confidence = classes, inv_map, confidence
         self.geometry = {"img_hw": tuple(img_hw), "pattern_id": int(pattern_id)}
         for k, v in (("vox_origin", vox_origin), ("voxel_size", voxel_size), ("scene_size", scene_size)):
             if v is not None:
@@ -236,19 +268,19 @@ class CameraPipeline:
             return self._submit_voxels(f, j)
         with torch.no_grad():
             res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map,
-                                           slab_output=self.slab_output)
+                                           slab_output=self.slab_output, confidence=self.confidence)
         self.in_free[j].record(self.main)
         if not self.reads_back:
             self.n += 1
             return self.n - 2 if self.n >= 2 else None
         if not self.classes:
             res = res[self.out_key]
-        if self.dev_out[j] is None or self.dev_out[j].shape != res.shape:
+        shape = (2,) + tuple(res[0].shape) if self.confidence else res.shape
+        if self.dev_out[j] is None or self.dev_out[j].shape != shape:
             self.out_free[j].synchronize()
-            self.dev_out[j] = torch.empty_like(res)
-            self.host_out[j] = torch.empty(res.shape, dtype=res.dtype).pin_memory()
+            self.dev_out[j], self.host_out[j] = _result_buffers(res)
         self.main.wait_event(self.out_free[j])
-        self.dev_out[j].copy_(res)           # the result leaves the allocator-owned tensor on the compute stream
+        _copy_result(self.dev_out[j], res)   # the result leaves the allocator-owned tensor on the compute stream
         self.out_ready[j].record(self.main)
         with torch.cuda.stream(self.d2h):
             self.d2h.wait_event(self.out_ready[j])
@@ -288,7 +320,8 @@ class CameraPipeline:
         return self.n - 1 if self.n else None
 
     def result(self, ticket):
-        """host tensor (pinned) of a submitted frame; blocks until its D2H read has finished.  The buffer is reused by
+        """host tensor (pinned) of a submitted frame, or with `confidence` (map, conf) views of one pinned buffer;
+        blocks until its D2H read has finished.  The buffer is reused by
         the second submit after the one that produced it.  With output="voxels": a dict of numpy views of the pinned
         buffers, trimmed to the rows that were written -- "count" (inside, outside the FOV; the true counts), "hist",
         "index", "cls", "xyz" (the in-FOV rows first, "n_in" of them) and "truncated".  None on a rank other than 0
@@ -306,7 +339,7 @@ class CameraPipeline:
             n = min(total, self.capacity)
             return dict(count=count, hist=h["hist"], index=h["index"][:n], cls=h["cls"][:n], xyz=h["xyz"][:n],
                         n_in=min(int(count[0]), n), truncated=total > self.capacity)
-        return self.host_out[j]
+        return _host_result(self.host_out[j], self.confidence)
 
     def join(self):
         """make the compute stream wait for every outstanding read-back (for timing with CUDA events)"""
