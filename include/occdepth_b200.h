@@ -511,6 +511,22 @@ int occd_model_run_frame(occd_model* m, const occd_frame* frame, uint16_t* class
 int occd_model_run_frame_conf(occd_model* m, const occd_frame* frame, uint16_t* class_map, void* conf, void* stream);
 int occd_model_destroy(occd_model* m);
 
+/* Model files under the X-slab partition (DESIGN.md section 9): one file per rank, each holding that rank's plan of */
+/* predict_frame(slab_output="root").  The ranks' collectives are launches on an occd_comm, created and destroyed   */
+/* through include/occdepth_b200_comm.h (NCCL, one rank per process and device; or `world` local ranks on one       */
+/* device).  Each is enqueued on `stream` only, so it replays inside a CUDA graph.  A NULL communicator is refused.  */
+typedef struct occd_comm occd_comm;
+/* halo exchange of one halo-carrying activation: planes [halo, halo + planes) of `base` (plane_bytes each) are      */
+/* this rank's; min(halo, planes) planes go to each X-neighbour, and the neighbours' come back into the margins      */
+/* [halo - min(halo, planes), halo) and [halo + planes, halo + planes + min(halo, planes))                           */
+int occd_comm_halo_exchange(occd_comm* comm, void* base, long long plane_bytes, int halo, int planes, void* stream);
+/* dst (world * bytes) = every rank's src (bytes), in rank order                                                     */
+int occd_comm_all_gather(occd_comm* comm, const void* src, void* dst, long long bytes, void* stream);
+/* rank 0's dst gets every rank's planes: bounds (HOST, 2 * world ints) holds rank r's [lo, hi) at bounds[2r],       */
+/* bounds[2r + 1]; src holds this rank's hi - lo planes of plane_bytes each.  dst is ignored on the other ranks.     */
+int occd_comm_gather_root(occd_comm* comm, const void* src, void* dst, const int* bounds, long long plane_bytes,
+                          void* stream);
+
 /* FlospDepth's per-camera tables on the host (FlospDepth.camera_tables of occdepth_b200, flosp_depth.py:466-541),  */
 /* bit for bit: cams[v] = {rows 0..2 of T[v] @ grid_to_lidar, rows 0..2 of K4[v], identity ida} (40 floats) and      */
 /* scaled_pixel_size[v] = |(1/fx, 1/fy)| * 1000, all float32 after casting cam_k (n_cams 3x3) and T (n_cams 4x4)     */

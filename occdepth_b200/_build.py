@@ -15,6 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIBNAME = "libocc_b200.so"
+HEADERS = ("occdepth_b200.h", "occdepth_b200_comm.h")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -44,8 +45,9 @@ def _digest(path):
         if hdr.endswith((".cuh", ".h")):
             with open(os.path.join(CSRC, hdr), "rb") as f:
                 h.update(f.read())
-    with open(os.path.join(HERE, "..", "include", "occdepth_b200.h"), "rb") as f:
-        h.update(f.read())
+    for hdr in HEADERS:
+        with open(os.path.join(HERE, "..", "include", hdr), "rb") as f:
+            h.update(f.read())
     h.update(" ".join(NVCC_FLAGS).encode())
     return h.hexdigest()
 
@@ -92,7 +94,7 @@ def build(verbose=False, force=False):
             list(ex.map(compile_one, jobs))
     out = lib_path()
     if jobs or not os.path.exists(out):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out] + objs
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out] + objs + ["-ldl"]   # NCCL is loaded at run time (csrc/comm.cu)
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
@@ -109,7 +111,7 @@ def build_occd_run(nvcc, force=False):
     src = os.path.join(HERE, "..", "tools", "occd_run.c")
     hdr = os.path.join(HERE, "..", "include", "occdepth_b200.h")
     h = hashlib.sha1()
-    for p in (src, hdr):
+    for p in [src] + [os.path.join(HERE, "..", "include", x) for x in HEADERS]:
         with open(p, "rb") as f:
             h.update(f.read())
     exe, stamp = occd_run_path(), occd_run_path() + ".sha1"

@@ -169,7 +169,20 @@ SYMBOLS = {
     "occd_model_run_frame_conf": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp, _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "occd_comm_halo_exchange": (C.c_int, [_vp, _vp, _ll, _i, _i, _vp]),
+    "occd_comm_all_gather": (C.c_int, [_vp, _vp, _vp, _ll, _vp]),
+    "occd_comm_gather_root": (C.c_int, [_vp, _vp, _vp, _vp, _ll, _vp]),
 }
+# include/occdepth_b200_comm.h: communicators and slab model files; none of these is a launch a model file records
+COMM_SYMBOLS = {
+    "occd_comm_unique_id": (C.c_int, [C.c_char_p, _vp]),
+    "occd_comm_create": (C.c_int, [C.c_char_p, _vp, _i, _i, C.POINTER(C.c_void_p)]),
+    "occd_comm_create_local": (C.c_int, [_i, C.POINTER(C.c_void_p)]),
+    "occd_comm_destroy": (C.c_int, [_vp]),
+    "occd_model_load_slab": (C.c_int, [C.c_char_p, _vp, C.POINTER(C.c_void_p)]),
+    "occd_model_run_frame_group": (C.c_int, [C.POINTER(C.c_void_p), _i, C.POINTER(Frame), _vp, _vp, _vp]),
+}
+COMM_ID_BYTES = 128
 VOXEL_TILE = 2048
 
 
@@ -192,6 +205,15 @@ def ssc_loss_sums_len(C, F):
 # deploy.export: while its thread has `recorder` set, lib() returns that stand-in there (which records the calls it
 # forwards); other threads keep the library
 _RECORDING = threading.local()
+# the communicator argument of a recorded collective: the model file's communicator slot, which the loader fills
+MODEL_COMM = object()
+
+
+def recording():
+    """True while deploy.export records a plan's run on this thread: the collective ops then emit the library's
+    collective launches (on MODEL_COMM) instead of running"""
+    rec = getattr(_RECORDING, "recorder", None)
+    return rec is not None and rec.recording
 
 
 def lib():
@@ -207,7 +229,7 @@ def lib():
                 "occdepth_b200: %s is missing -- build it with `python -m occdepth_b200._build` "
                 "(or __graft_entry__.build()); there is no CPU fallback" % path)
         L = C.CDLL(path)
-        for name, (res, args) in SYMBOLS.items():
+        for name, (res, args) in list(SYMBOLS.items()) + list(COMM_SYMBOLS.items()):
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args

@@ -5,7 +5,9 @@
 // one device arena, host structs are byte blobs with pointer fix-ups, convolution plans are created at load.  The
 // layout is documented field by field in DESIGN.md section 9; the Python writer is the only producer.
 #include "common.cuh"
+#include "comm.cuh"
 #include "../../include/occdepth_b200.h"
+#include "../../include/occdepth_b200_comm.h"
 
 #include <math.h>
 #include <stdio.h>
@@ -38,6 +40,11 @@ template <>
 struct ArgOf<occd_model*> {  // a model handle cannot be stored in a file: only NULL is recorded (the call then refuses)
   static constexpr char tag = 'n';
   static occd_model* get(const Arg&) { return nullptr; }
+};
+template <>
+struct ArgOf<occd_comm*> {  // the model's communicator (tag 'm'), filled in by occd_model_load_slab; or NULL ('n')
+  static constexpr char tag = 'm';
+  static occd_comm* get(const Arg& a) { return static_cast<occd_comm*>(a.p); }
 };
 template <>
 struct ArgOf<int> {
@@ -80,7 +87,7 @@ struct Sig {
 
 struct Entry {
   const char* name;
-  const char* sig;  // one tag per parameter: p i l f d
+  const char* sig;  // one tag per parameter: p i l f d, m (a communicator)
   AnyFn fn;
   Invoke call;
 };
@@ -112,7 +119,12 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_vox2pix_range_fwd),     OCCD_ENTRY(occd_argmax_classes_conf),
     // takes a stream like the launches, so it has a signature here; its model handle can only be NULL
     OCCD_ENTRY(occd_model_run_frame_conf),
+    // the X-slab partition's collectives: the lock-step runner of a local group stops after each
+    OCCD_ENTRY(occd_comm_halo_exchange),    OCCD_ENTRY(occd_comm_all_gather),
+    OCCD_ENTRY(occd_comm_gather_root),
 };
+
+bool is_collective(const Entry* e) { return strncmp(e->name, "occd_comm_", 10) == 0; }
 
 const Entry* find_entry(const std::string& name) {
   for (const Entry& e : kEntries)
@@ -125,8 +137,11 @@ const char kMagic[8] = {'O', 'C', 'C', 'D', 'M', 'O', 'D', 'L'};
 enum Role { ROLE_IMG, ROLE_PIX, ROLE_FOV, ROLE_PIX_Z, ROLE_DEPTH, ROLE_CAMS, ROLE_SPS, ROLE_CLASSES, N_ROLES };
 const char* kRoleNames[N_ROLES] = {"image", "pix", "fov", "pix_z", "depth", "camera tables", "scaled_pixel_size",
                                    "class map"};
-enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4 };   // FLAG_CONF: the class-map role holds the map, then its
-                                                                   // float16 confidence (OCCD_OUT1_CLASS_U16_CONF)
+enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4,   // FLAG_CONF: the class-map role holds the map, then its
+       FLAG_SLAB = 16 };                                         // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
+                                                                 // FLAG_SLAB: one rank's plan, a slab block follows
+                                                                 // (bit 3 stays unassigned)
+const uint32_t kMaxWorld = 64;
 const size_t kArenaAlign = 512;  // the caching allocator's block alignment, which the plans were built with
 
 struct Reader {
@@ -211,7 +226,16 @@ struct occd_model {
   std::vector<uint8_t> calib;  // the calibration the index buffers hold (KITTI)
   bool calib_valid = false;
   float cams[4 * 40], sps[4];
+  // the X-slab partition (FLAG_SLAB): this rank, every rank's [lo, hi) planes of the lift grid, this rank's window of
+  // the lift's voxel order, the one view it stages (-1: every view) and the whole map's X extent (rank 0's output)
+  uint32_t rank = 0, world = 1, map_x = 0;
+  std::vector<uint32_t> bounds;
+  uint64_t n_lo = 0, n_len = 0;
+  int32_t view_sel = -1;
+  occd_comm* comm = nullptr;                 // not owned
+  std::vector<occd_model*> graph_ranks;      // a local group's graph (held by rank 0): the models it was captured over
 
+  bool slab() const { return (flags & FLAG_SLAB) != 0; }
   void* dev(int role) const { return arena + buf_off[roles[role].buffer] + roles[role].off; }
   uint64_t map_bytes() const { return (uint64_t)out[0] * out[1] * out[2] * 2; }   // one uint16 class map
 };
@@ -272,14 +296,49 @@ int parse(occd_model* m) {
     m->roles[k].off = r.get<uint64_t>();
     m->roles[k].len = r.get<uint64_t>();
   }
+  if (m->flags & FLAG_SLAB) {
+    m->rank = r.get<uint32_t>();
+    m->world = r.get<uint32_t>();
+    if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (slab block)");
+    if (m->world < 1 || m->world > kMaxWorld || m->rank >= m->world)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: slab rank " + std::to_string(m->rank) + " of " +
+                                       std::to_string(m->world) + " out of range");
+    m->bounds.resize(2 * m->world);
+    for (uint32_t& b : m->bounds) b = r.get<uint32_t>();
+    m->n_lo = r.get<uint64_t>();
+    m->n_len = r.get<uint64_t>();
+    m->view_sel = r.get<int32_t>();
+    m->map_x = r.get<uint32_t>();
+    if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (slab block)");
+  }
   uint32_t n_buf = r.get<uint32_t>(), n_blob = r.get<uint32_t>(), n_plan = r.get<uint32_t>(),
            n_rec = r.get<uint32_t>();
   if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (header)");
   if ((m->precision != OCCD_DTYPE_F32 && m->precision != OCCD_DTYPE_BF16) || m->dataset > 1 || m->V < 1 ||
       m->V > 4 || m->P < 1 || m->P > 64 || m->n_cams > 4 || m->img_cstride % 8 != 0)
     return fail(OCCD_ERR_FORMAT, "occd_model_load: header field out of range");
-  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF))
+  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB))
     return fail(OCCD_ERR_FORMAT, "occd_model_load: unknown header flag bits");
+  if (m->slab()) {
+    // every rank's slab, in rank order, tiles the lift grid's X planes; this rank's window is its slab's voxels
+    const uint64_t plane = (uint64_t)m->grid[1] * m->grid[2];
+    bool tiles = m->bounds[0] == 0 && m->bounds[2 * m->world - 1] == m->grid[0];
+    for (uint32_t k = 0; k < m->world; ++k)
+      tiles = tiles && m->bounds[2 * k + 1] > m->bounds[2 * k] && (k == 0 || m->bounds[2 * k] == m->bounds[2 * k - 1]);
+    if (!tiles)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: the slab bounds do not tile the " + std::to_string(m->grid[0]) +
+                                       " X planes of the grid");
+    if (m->n_lo != m->bounds[2 * m->rank] * plane || m->n_len != (m->bounds[2 * m->rank + 1] - m->bounds[2 * m->rank]) * plane)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: the index window is not rank " + std::to_string(m->rank) +
+                                       "'s slab");
+    if (m->view_sel < -1 || m->view_sel >= (int32_t)m->V || (m->view_sel >= 0 && (m->flags & FLAG_VIRTUAL)))
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: staged view " + std::to_string(m->view_sel) + " outside [-1, " +
+                                       std::to_string(m->V) + ")");
+    if (m->map_x != m->out[0])
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: the slab block's map extent is not the header's");
+    if (m->dataset == 1 && (m->flags & FLAG_FLOSP_DEPTH))
+      return fail(OCCD_ERR_UNSUPPORTED, "occd_model_load: NYU with the FlospDepth prior has no X-slab partition");
+  }
   // counts are bounded by what the file can hold before anything is sized from them
   const size_t left = r.n - r.pos;
   if (n_buf > left / 12 || n_blob > left / 12 || n_plan > left / 12 || n_rec > left / 6)
@@ -364,13 +423,13 @@ int parse(occd_model* m) {
         case 'l': a.v.l = r.get<int64_t>(); break;
         case 'f': a.v.f = r.get<float>(); break;
         case 'd': a.v.d = r.get<double>(); break;
-        case 'n': case 's': break;
+        case 'n': case 's': case 'm': break;
         default: return fail(OCCD_ERR_FORMAT, "occd_model_load: record " + std::to_string(i) + ": bad argument tag");
       }
       if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (record " + std::to_string(i) + ")");
       const char want = rec.e->sig[k];
       const bool ptr_tag = a.tag == 'p' || a.tag == 'h' || a.tag == 'c' || a.tag == 'n' || a.tag == 's';
-      if (want == 'p' ? !ptr_tag : a.tag != want)
+      if (want == 'p' ? !ptr_tag : want == 'm' ? (a.tag != 'm' && a.tag != 'n') : a.tag != want)
         return fail(OCCD_ERR_FORMAT, "occd_model_load: record " + std::to_string(i) + " (" + name + "): argument " +
                                          std::to_string(k) + " has the wrong type");
       const std::string where = "occd_model_load: record " + std::to_string(i) + " (" + name + ") argument " +
@@ -380,16 +439,19 @@ int parse(occd_model* m) {
       if (a.tag == 'h' && a.id >= n_blob) return fail(OCCD_ERR_FORMAT, where + "host blob id out of range");
       if (a.tag == 'c' && a.id >= n_plan) return fail(OCCD_ERR_FORMAT, where + "convolution plan id out of range");
       if (a.tag == 's') rec.streams.push_back((int)k);
+      if (a.tag == 'm' && !m->slab()) return fail(OCCD_ERR_FORMAT, where + "a communicator in a file without the slab partition");
     }
   }
   if (r.pos != r.n) return fail(OCCD_ERR_FORMAT, "occd_model_load: trailing bytes after the records");
 
+  // under the slab partition: the staged view only, this rank's window of the indices, the whole map on rank 0 only
   const bool need[N_ROLES] = {true, true, true, true, (m->flags & FLAG_VIRTUAL) != 0,
-                              (m->flags & FLAG_FLOSP_DEPTH) != 0, (m->flags & FLAG_FLOSP_DEPTH) != 0, true};
-  const uint64_t N = (uint64_t)m->grid[0] * m->grid[1] * m->grid[2];
+                              (m->flags & FLAG_FLOSP_DEPTH) != 0, (m->flags & FLAG_FLOSP_DEPTH) != 0, m->rank == 0};
+  const uint64_t N = m->slab() ? m->n_len : (uint64_t)m->grid[0] * m->grid[1] * m->grid[2];
   const uint32_t VL = (m->flags & FLAG_VIRTUAL) ? 2 : m->V;
   const uint64_t want_len[N_ROLES] = {
-      (uint64_t)m->V * m->img_h * m->img_w * m->img_cstride * (m->precision == OCCD_DTYPE_F32 ? 4 : 2),
+      (uint64_t)(m->view_sel >= 0 ? 1 : m->V) * m->img_h * m->img_w * m->img_cstride *
+          (m->precision == OCCD_DTYPE_F32 ? 4 : 2),
       (uint64_t)VL * N * m->P * 16, (uint64_t)VL * N * m->P, N * 8, (uint64_t)m->depth_h * m->depth_w * 4,
       (uint64_t)m->n_cams * 160, (uint64_t)m->n_cams * 4, m->map_bytes() * ((m->flags & FLAG_CONF) ? 2 : 1)};
   for (int k = 0; k < N_ROLES; ++k) {
@@ -457,6 +519,7 @@ int upload(occd_model* m) {
       if (a.tag == 'h') v.p = m->blobs[a.id].bytes.data();
       if (a.tag == 'c') v.p = m->plans[a.id];
       if (a.tag == 'n' || a.tag == 's') v.p = nullptr;
+      if (a.tag == 'm') v.p = m->comm;
     }
   }
   if ((e = cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking)) != cudaSuccess) {
@@ -466,13 +529,46 @@ int upload(occd_model* m) {
   return OCCD_OK;
 }
 
+int call(Record& rec, cudaStream_t st) {
+  for (int k : rec.streams) rec.args[k].p = st;
+  return rec.e->call(rec.e->fn, rec.args.data());
+}
+
 int replay(occd_model* m, cudaStream_t st) {
   for (Record& rec : m->recs) {
-    for (int k : rec.streams) rec.args[k].p = st;
-    int rc = rec.e->call(rec.e->fn, rec.args.data());
+    int rc = call(rec, st);
     if (rc != OCCD_OK) return rc;
   }
   return OCCD_OK;
+}
+
+// the ranks of a local group on one stream, as parallel.SimSlabGroup.run_lockstep runs them: each rank up to and
+// including its next collective (a local collective only posts its arguments), the last rank's post then enqueues that
+// collective's copies for all ranks
+int replay_lockstep(occd_model* const* ms, int world, cudaStream_t st) {
+  std::vector<size_t> pos(world, 0);
+  for (;;) {
+    int ended = 0;
+    for (int r = 0; r < world; ++r) {
+      std::vector<Record>& recs = ms[r]->recs;
+      bool at_collective = false;
+      while (pos[r] < recs.size() && !at_collective) {
+        Record& rec = recs[pos[r]++];
+        int rc = call(rec, st);
+        if (rc != OCCD_OK) {
+          occd_comm_reset(ms[0]->comm);
+          return rc;
+        }
+        at_collective = is_collective(rec.e);
+      }
+      ended += at_collective ? 0 : 1;
+    }
+    if (ended == world) return OCCD_OK;
+    if (ended) {
+      occd_comm_reset(ms[0]->comm);
+      return fail(OCCD_ERR_ARG, "occd_model_run_frame_group: the ranks' files hold different numbers of collectives");
+    }
+  }
 }
 
 template <typename T>
@@ -486,8 +582,11 @@ void load_as_f32(const void* src, int n, float* dst) {
 int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
   static const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
   const bool nyu = m->dataset == 1;
-  int rc = occd_stage_rgb_u8_cl(f->images, f->img_stride, f->row_stride, (int)m->V, f->H0, f->W0, (int)m->img_h,
-                                (int)m->img_w, mean, stdv, m->dev(ROLE_IMG), (int)m->precision, (int)m->img_cstride, st);
+  // under the partition's view sharding the rank stages its one view
+  const void* images = static_cast<const uint8_t*>(f->images) + (m->view_sel > 0 ? m->view_sel * f->img_stride : 0);
+  int rc = occd_stage_rgb_u8_cl(images, f->img_stride, f->row_stride, m->view_sel >= 0 ? 1 : (int)m->V, f->H0, f->W0,
+                                (int)m->img_h, (int)m->img_w, mean, stdv, m->dev(ROLE_IMG), (int)m->precision,
+                                (int)m->img_cstride, st);
   if (rc != OCCD_OK) return rc;
   if (m->flags & FLAG_VIRTUAL) {
     OCCD_CHECK_ARG(f->depth != nullptr && f->depth_h == (int)m->depth_h && f->depth_w == (int)m->depth_w,
@@ -556,14 +655,19 @@ int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
   float k32[4][9];
   for (int v = 0; v < n_views; ++v)
     for (int i = 0; i < 9; ++i) k32[v][i] = (float)K[nyu ? 0 : v][i];
-  const long long N = (long long)m->grid[0] * m->grid[1] * m->grid[2];
+  // under the slab partition every pose's indices of this rank's window [n_lo, n_lo + n_len) only
+  const long long N = m->slab() ? (long long)m->n_len : (long long)m->grid[0] * m->grid[1] * m->grid[2];
   for (int v = 0; v < n_views; ++v) {
     const void* pose = f32_pose[v] ? (const void*)Ef[v] : (const void*)E[v];
-    rc = occd_vox2pix_fwd(pose, f32_pose[v], k32[v], o32, voxel, dims[0], dims[1], dims[2], (int)m->img_w,
-                          (int)m->img_h, &m->pattern[0][0], (int)m->P,
-                          static_cast<long long*>(m->dev(ROLE_PIX)) + (long long)v * N * m->P * 2,
-                          static_cast<unsigned char*>(m->dev(ROLE_FOV)) + (long long)v * N * m->P, m->dev(ROLE_PIX_Z),
-                          st);
+    long long* pix = static_cast<long long*>(m->dev(ROLE_PIX)) + (long long)v * N * m->P * 2;
+    unsigned char* fov = static_cast<unsigned char*>(m->dev(ROLE_FOV)) + (long long)v * N * m->P;
+    if (m->slab())
+      rc = occd_vox2pix_range_fwd(pose, f32_pose[v], k32[v], o32, voxel, dims[0], dims[1], dims[2], (int)m->img_w,
+                                  (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z),
+                                  (long long)m->n_lo, N, st);
+    else
+      rc = occd_vox2pix_fwd(pose, f32_pose[v], k32[v], o32, voxel, dims[0], dims[1], dims[2], (int)m->img_w,
+                            (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z), st);
     if (rc != OCCD_OK) return rc;
   }
   if (m->flags & FLAG_FLOSP_DEPTH) {
@@ -657,8 +761,10 @@ extern "C" int occd_flosp_camera_tables(int n_cams, const void* cam_k, const voi
   return OCCD_OK;
 }
 
-extern "C" int occd_model_load(const char* path, occd_model** out) {
-  OCCD_CHECK_ARG(path && out, "occd_model_load: null argument");
+namespace {
+
+// reads and validates the file (no device touched), then -- when `accept` agrees -- uploads it
+int load(const char* path, occd_comm* comm, occd_model** out, int (*accept)(const occd_model*, const occd_comm*)) {
   *out = nullptr;
   FILE* fp = fopen(path, "rb");
   if (!fp) return fail(OCCD_ERR_IO, std::string("occd_model_load: cannot open ") + path);
@@ -675,7 +781,9 @@ extern "C" int occd_model_load(const char* path, occd_model** out) {
     delete m;
     return fail(OCCD_ERR_IO, std::string("occd_model_load: cannot read ") + path);
   }
+  m->comm = comm;
   int rc = parse(m);
+  if (rc == OCCD_OK) rc = accept(m, comm);
   if (rc == OCCD_OK) rc = upload(m);
   m->buf_data.clear();
   std::vector<uint8_t>().swap(m->file);
@@ -687,6 +795,39 @@ extern "C" int occd_model_load(const char* path, occd_model** out) {
   }
   *out = m;
   return OCCD_OK;
+}
+
+int accept_plain(const occd_model* m, const occd_comm*) {
+  if (m->slab())
+    return fail(OCCD_ERR_UNSUPPORTED, "occd_model_load: the file is rank " + std::to_string(m->rank) + " of an X-slab "
+                                      "partition over " + std::to_string(m->world) + " ranks; load it with "
+                                      "occd_model_load_slab");
+  return OCCD_OK;
+}
+
+int accept_slab(const occd_model* m, const occd_comm* c) {
+  if (!m->slab())
+    return fail(OCCD_ERR_UNSUPPORTED, "occd_model_load_slab: the file holds no X-slab partition; load it with "
+                                      "occd_model_load");
+  int rank, world, kind;
+  occd_comm_describe(c, &rank, &world, &kind);
+  if ((uint32_t)rank != m->rank || (uint32_t)world != m->world)
+    return fail(OCCD_ERR_ARG, "occd_model_load_slab: the file is rank " + std::to_string(m->rank) + " of " +
+                                  std::to_string(m->world) + ", the communicator rank " + std::to_string(rank) +
+                                  " of " + std::to_string(world));
+  return OCCD_OK;
+}
+
+}  // namespace
+
+extern "C" int occd_model_load(const char* path, occd_model** out) {
+  OCCD_CHECK_ARG(path && out, "occd_model_load: null argument");
+  return load(path, nullptr, out, accept_plain);
+}
+
+extern "C" int occd_model_load_slab(const char* path, occd_comm* comm, occd_model** out) {
+  OCCD_CHECK_ARG(path && comm && out, "occd_model_load_slab: null argument");
+  return load(path, comm, out, accept_slab);
 }
 
 extern "C" int occd_model_info(const occd_model* m, occd_model_geom* g) {
@@ -718,53 +859,84 @@ extern "C" int occd_model_info(const occd_model* m, occd_model_geom* g) {
 
 namespace {
 
-// stages the frame and replays the records (through the graph when there is one) on `stream`
-int run_records(occd_model* m, const occd_frame* f, cudaStream_t st) {
-  int rc = stage(m, f, st);
-  if (rc != OCCD_OK) return rc;
+void drop_graph(occd_model* m) {
+  if (m->graph_exec) cudaGraphExecDestroy(m->graph_exec);
+  if (m->graph) cudaGraphDestroy(m->graph);
+  m->graph_exec = nullptr;
+  m->graph = nullptr;
+}
+
+// replays the records (through `owner`'s graph when there is one) on `stream`: rep(stream) launches them one by one
+template <typename Replay>
+int execute(occd_model* owner, int flags, cudaStream_t st, Replay rep) {
+  int rc;
   cudaError_t e;
-  if ((f->flags & OCCD_FRAME_NO_GRAPH) || m->graph_exec == nullptr) {
-    if ((rc = replay(m, st)) != OCCD_OK) return rc;
-    if (!(f->flags & OCCD_FRAME_NO_GRAPH)) {
+  if ((flags & OCCD_FRAME_NO_GRAPH) || owner->graph_exec == nullptr) {
+    if ((rc = rep(st)) != OCCD_OK) return rc;
+    if (!(flags & OCCD_FRAME_NO_GRAPH)) {
       // the first run is also the warm-up (module loading, function attributes); the graph is captured after it
-      if ((e = cudaStreamBeginCapture(m->capture_stream, cudaStreamCaptureModeThreadLocal)) != cudaSuccess)
+      if ((e = cudaStreamBeginCapture(owner->capture_stream, cudaStreamCaptureModeThreadLocal)) != cudaSuccess)
         return cuda_fail(e, "occd_model_run_frame: cudaStreamBeginCapture");
       cudaGraph_t graph = nullptr;
-      rc = replay(m, m->capture_stream);
-      e = cudaStreamEndCapture(m->capture_stream, &graph);
-      if (rc == OCCD_OK && e == cudaSuccess && (e = cudaGraphInstantiate(&m->graph_exec, graph, 0)) == cudaSuccess) {
-        m->graph = graph;
+      rc = rep(owner->capture_stream);
+      e = cudaStreamEndCapture(owner->capture_stream, &graph);
+      if (rc == OCCD_OK && e == cudaSuccess && (e = cudaGraphInstantiate(&owner->graph_exec, graph, 0)) == cudaSuccess) {
+        owner->graph = graph;
       } else {
         // nothing half-made stays behind: a later run captures afresh
-        m->graph_exec = nullptr;
+        owner->graph_exec = nullptr;
         if (graph) cudaGraphDestroy(graph);
         if (rc != OCCD_OK) return rc;
         return cuda_fail(e, "occd_model_run_frame: graph capture");
       }
     }
-  } else if ((e = cudaGraphLaunch(m->graph_exec, st)) != cudaSuccess) {
+  } else if ((e = cudaGraphLaunch(owner->graph_exec, st)) != cudaSuccess) {
     return cuda_fail(e, "occd_model_run_frame: cudaGraphLaunch");
   }
+  return OCCD_OK;
+}
+
+// stages the frame and replays the records (through the graph when there is one) on `stream`
+int run_records(occd_model* m, const occd_frame* f, cudaStream_t st) {
+  if (m->comm) {
+    int rank, world, kind;
+    occd_comm_describe(m->comm, &rank, &world, &kind);
+    if (kind == OCCD_COMM_LOCAL)
+      return fail(OCCD_ERR_UNSUPPORTED, "occd_model_run_frame: a model on a local communicator runs with its group "
+                                        "through occd_model_run_frame_group");
+  }
+  int rc = stage(m, f, st);
+  if (rc != OCCD_OK) return rc;
+  return execute(m, f->flags, st, [m](cudaStream_t s) { return replay(m, s); });
+}
+
+// the whole map (and its confidence) of a model whose plan outputs one: every unpartitioned model, rank 0 of a slab
+int copy_out(const occd_model* m, uint16_t* class_map, void* conf, cudaStream_t st, const char* what) {
+  if (m->rank != 0) return OCCD_OK;
+  const char* roles = static_cast<const char*>(m->dev(ROLE_CLASSES));
+  cudaError_t e;
+  if ((e = cudaMemcpyAsync(class_map, roles, m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+    return cuda_fail(e, (std::string(what) + ": class map copy").c_str());
+  if (conf &&
+      (e = cudaMemcpyAsync(conf, roles + m->map_bytes(), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+    return cuda_fail(e, (std::string(what) + ": confidence copy").c_str());
   return OCCD_OK;
 }
 
 }  // namespace
 
 extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t* class_map, void* stream) {
-  OCCD_CHECK_ARG(m && f && f->images && class_map, "occd_model_run_frame: null argument");
+  OCCD_CHECK_ARG(m && f && f->images && (class_map || m->rank != 0), "occd_model_run_frame: null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int rc = run_records(m, f, st);
   if (rc != OCCD_OK) return rc;
-  cudaError_t e;
-  if ((e = cudaMemcpyAsync(class_map, m->dev(ROLE_CLASSES), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) !=
-      cudaSuccess)
-    return cuda_fail(e, "occd_model_run_frame: class map copy");
-  return OCCD_OK;
+  return copy_out(m, class_map, nullptr, st, "occd_model_run_frame");
 }
 
 extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uint16_t* class_map, void* conf,
                                          void* stream) {
-  OCCD_CHECK_ARG(m && f && f->images && class_map && conf, "occd_model_run_frame_conf: null argument");
+  OCCD_CHECK_ARG(m && f && f->images && ((class_map && conf) || m->rank != 0),
+                 "occd_model_run_frame_conf: null argument");
   if (!(m->flags & FLAG_CONF)) {
     occd_set_last_error("occd_model_run_frame_conf: the model was exported without confidence");
     return OCCD_ERR_UNSUPPORTED;
@@ -772,13 +944,38 @@ extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uin
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int rc = run_records(m, f, st);
   if (rc != OCCD_OK) return rc;
-  const char* roles = static_cast<const char*>(m->dev(ROLE_CLASSES));
-  cudaError_t e;
-  if ((e = cudaMemcpyAsync(class_map, roles, m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-    return cuda_fail(e, "occd_model_run_frame_conf: class map copy");
-  if ((e = cudaMemcpyAsync(conf, roles + m->map_bytes(), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-    return cuda_fail(e, "occd_model_run_frame_conf: confidence copy");
-  return OCCD_OK;
+  return copy_out(m, class_map, conf, st, "occd_model_run_frame_conf");
+}
+
+extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
+                                          void* conf, void* stream) {
+  OCCD_CHECK_ARG(ms && world >= 1 && f && f->images && class_map, "occd_model_run_frame_group: null argument");
+  for (int r = 0; r < world; ++r) {
+    OCCD_CHECK_ARG(ms[r] && ms[r]->comm, "occd_model_run_frame_group: every rank's model, loaded with a local "
+                                         "communicator, is needed");
+    int rank, w, kind;
+    occd_comm_describe(ms[r]->comm, &rank, &w, &kind);
+    OCCD_CHECK_ARG(kind == OCCD_COMM_LOCAL && rank == r && w == world &&
+                       occd_comm_group(ms[r]->comm) == occd_comm_group(ms[0]->comm),
+                   "occd_model_run_frame_group: models[r] must be rank r of one local group of `world` ranks");
+  }
+  if (conf && !(ms[0]->flags & FLAG_CONF)) {
+    occd_set_last_error("occd_model_run_frame_group: the model was exported without confidence");
+    return OCCD_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  for (int r = 0; r < world; ++r) {
+    int rc = stage(ms[r], f, st);
+    if (rc != OCCD_OK) return rc;
+  }
+  // rank 0 holds the group's graph; it is captured afresh when the group's models change
+  occd_model* owner = ms[0];
+  if (owner->graph_exec && owner->graph_ranks != std::vector<occd_model*>(ms, ms + world)) drop_graph(owner);
+  const bool capture = !(f->flags & OCCD_FRAME_NO_GRAPH) && owner->graph_exec == nullptr;
+  int rc = execute(owner, f->flags, st, [ms, world](cudaStream_t s) { return replay_lockstep(ms, world, s); });
+  if (rc != OCCD_OK) return rc;
+  if (capture && owner->graph_exec) owner->graph_ranks.assign(ms, ms + world);
+  return copy_out(owner, class_map, conf, st, "occd_model_run_frame_group");
 }
 
 extern "C" int occd_model_destroy(occd_model* m) {

@@ -22,8 +22,9 @@ from .engine import CL, ConvOp
 
 MAGIC = b"OCCDMODL"
 ROLES = ("img", "pix", "fov", "pix_z", "depth", "cams", "sps", "classes")
-FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF = 1, 2, 4    # FLAG_CONF: the class-map role holds the map, then its
-                                                       # float16 confidence
+FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF, FLAG_SLAB = 1, 2, 4, 16  # FLAG_CONF: the class-map role holds the map,
+                                                                   # then its float16 confidence; FLAG_SLAB: one
+                                                                   # rank's plan of the X-slab partition
 PATTERN_MAX = 64
 
 _STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
@@ -96,6 +97,8 @@ class _Recorder:
             return ("f" if t is C.c_float else "d", float(getattr(a, "value", a)))
         if a is _STREAM:
             return ("s",)
+        if a is _lib.MODEL_COMM:
+            return ("m",)
         if name == "occd_conv_run" and i == 0:
             h = _handle(a)
             if h not in self.plans:
@@ -170,17 +173,27 @@ class _Buffers:
         return out.tobytes() if out.any() else None
 
 
-def export(model, path, frame, inv_map=None, confidence=False):
+def export(model, path, frame, inv_map=None, confidence=False, slab_output=None):
     """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map, confidence=confidence)`
     for frames of this frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame
     refuses, with the same messages.  Returns a dict of what was written (records, buffers, bytes).  With
     `confidence` the file's class-map role holds the map and then its confidence (header flag FLAG_CONF), which
     `occd_model_run_frame_conf` reads; without it the file is what it always was.
 
+    Under enable_slab_parallel, slab_output="root" (the only value a file carries) writes this rank's plan of
+    `predict_frame(frame, slab_output="root", ...)`: every rank exports the same frame to its own path, and the
+    files are loaded by `occd_model_load_slab` on each rank's communicator (header flag FLAG_SLAB and a slab block).
+    The recording runs no collective: the plan's communication ops emit the library's collective launches instead,
+    so the ranks' plans may also be built one after another on one device (parallel.SimSlabGroup contexts).
+
     The recording stand-in replaces the library for the calling thread only, so other threads may keep serving
     through the library meanwhile; `model` itself must not run elsewhere during the export (as for predict_frame)."""
     from . import data as D
-    f = model._frame_checked(frame)
+    f = model._frame_checked(frame, slab_output)
+    slab = model.__dict__.get("slab_ctx")
+    if slab_output == "slab":
+        raise NotImplementedError("deploy.export: a model file holds the whole map on rank 0 (slab_output='root'); "
+                                  "per-rank slabs are not exported")
     lut = model._class_lut(inv_map)
     dev = f["imgs"].device
     rec = _Recorder(_lib.lib())
@@ -188,8 +201,8 @@ def export(model, path, frame, inv_map=None, confidence=False):
         _lib._RECORDING.recorder = rec
         try:
             ent = model._build(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"],
-                               classes=model._class_key(inv_map, confidence), capture=False)
-            plan, img_cl, pix, fov, out, depth0 = ent[:6]
+                               classes=model._class_key(inv_map, confidence, slab is not None), capture=False)
+            plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
             plan.pix_z = torch.zeros(pix.shape[2], dtype=torch.float64, device=dev)
             state = getattr(plan, "flosp_state", None)
             tensors = []
@@ -263,10 +276,13 @@ def export(model, path, frame, inv_map=None, confidence=False):
     if lut is not None:
         lut_arr[:len(lut)] = lut
     S = [int(s) // model.project_scale for s in model.full_scene_size]
+    # the whole map on every rank's header (rank 0's output; the other ranks' plans output nothing)
+    out_dims = tuple(out.shape[-3:]) if out is not None else tuple(int(s) for s in model.full_scene_size)
     hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
                               1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0)
-                              | (FLAG_CONF if confidence else 0), f["V"], f["H"], f["W"], model.project_scale),
-           struct.pack("<7I", *S, *out.shape[-3:], f["P"]), pattern.astype("<i4").tobytes(),
+                              | (FLAG_CONF if confidence else 0) | (FLAG_SLAB if slab is not None else 0),
+                              f["V"], f["H"], f["W"], model.project_scale),
+           struct.pack("<7I", *S, *out_dims, f["P"]), pattern.astype("<i4").tobytes(),
            struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
                        *[float(v) for v in f["scene_size"]]),
            struct.pack("<2I", model.n_classes, 0 if lut is None else 1), lut_arr.astype("<i4").tobytes(),
@@ -274,6 +290,12 @@ def export(model, path, frame, inv_map=None, confidence=False):
            struct.pack("<3I", *vn),
            G.astype("<f4").tobytes(), struct.pack("<I", img_cl.cstride)]
     hdr += [struct.pack("<iQQ", *r) for r in roles]
+    if slab is not None:
+        # rank, world, every rank's [lo, hi) of the lift grid, this rank's index window, its staged view, the whole
+        # map's X extent
+        hdr.append(struct.pack("<2I", slab.rank, slab.world)
+                   + struct.pack("<%dI" % (2 * slab.world), *[b for lo_hi in slab.bounds for b in lo_hi])
+                   + struct.pack("<2QiI", n_lo, pix.shape[2], -1 if view_sel is None else view_sel, out_dims[0]))
     hdr.append(struct.pack("<4I", len(bufs.iv), len(blobs), len(plans), len(records)))
     n_bytes = 0
     with open(path, "wb") as fh:
@@ -310,15 +332,66 @@ def export(model, path, frame, inv_map=None, confidence=False):
                 data_buffers=sum(c is not None for c in contents))
 
 
+class Comm:
+    """a communicator of the library (occd_comm, include/occdepth_b200_comm.h) for slab-partition model files.
+    Comm(id, rank, world): NCCL, one rank per process on the current device, collective over the ranks; `id` is
+    Comm.unique_id() of rank 0, shipped to the others by the caller.  Comm.local(world): `world` ranks in this process
+    on the current device, run together by run_frame_group.  `nccl_lib`: the path of libnccl.so.2 (None: the soname,
+    which torch has usually loaded already)."""
+
+    def __init__(self, id=None, rank=0, world=1, nccl_lib=None, _handle=None):
+        self.rank, self.world = rank, world
+        if _handle is not None:
+            self.handle = _handle
+            return
+        h = C.c_void_p()
+        _lib.check(_lib.lib().occd_comm_create(_path(nccl_lib), bytes(id), rank, world, C.byref(h)),
+                   "occd_comm_create")
+        self.handle = h
+
+    @staticmethod
+    def unique_id(nccl_lib=None):
+        buf = C.create_string_buffer(_lib.COMM_ID_BYTES)
+        _lib.check(_lib.lib().occd_comm_unique_id(_path(nccl_lib), buf), "occd_comm_unique_id")
+        return buf.raw
+
+    @classmethod
+    def local(cls, world):
+        hs = (C.c_void_p * world)()
+        _lib.check(_lib.lib().occd_comm_create_local(world, hs), "occd_comm_create_local")
+        return [cls(rank=r, world=world, _handle=C.c_void_p(hs[r])) for r in range(world)]
+
+    def close(self):
+        if self.handle:
+            _lib.lib().occd_comm_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
+
+
+def _path(p):
+    return None if p is None else os.fsencode(p)
+
+
 class LoadedModel:
     """ctypes handle of a model file loaded by the C runtime (occd_model_load), for Python callers that want the
-    Python-free route's results: `run_frame` takes the frame dict of OccDepth.predict_frame."""
+    Python-free route's results: `run_frame` takes the frame dict of OccDepth.predict_frame.  With `comm` (a Comm)
+    the file is one rank's of the X-slab partition (occd_model_load_slab); the model keeps the communicator alive."""
 
-    def __init__(self, path):
+    def __init__(self, path, comm=None):
         L = _lib.lib()
         h = C.c_void_p()
-        _lib.check(L.occd_model_load(os.fsencode(path), C.byref(h)), "occd_model_load(%s)" % path)
+        if comm is None:
+            _lib.check(L.occd_model_load(os.fsencode(path), C.byref(h)), "occd_model_load(%s)" % path)
+        else:
+            _lib.check(L.occd_model_load_slab(os.fsencode(path), comm.handle, C.byref(h)),
+                       "occd_model_load_slab(%s)" % path)
         self.handle = h
+        self.comm = comm
         self.geom = self.info()
 
     def info(self):
@@ -330,61 +403,16 @@ class LoadedModel:
         """frame: as OccDepth.predict_frame takes it (the uint8 images may be on the host or the device) -> the
         uint16 class map [1, X, Y, Z] on the current device, enqueued on `stream` (default: the current stream).
         `conf`: a float16 [1, X, Y, Z] device tensor (or True: allocate one) that gets the map's confidence through
-        occd_model_run_frame_conf; the result is then (map, conf)."""
-        g = self.geom
-        img = torch.as_tensor(frame["img"])
-        if img.dim() == 3:
-            img = img.unsqueeze(0)
-        img = img.contiguous().cuda()
-        keep = [img]
-
-        def host(a, dt=np.float64):
-            a = np.ascontiguousarray(np.asarray(a, dt))
-            keep.append(a)
-            return a.ctypes.data
-
-        f = _lib.Frame()
-        f.images, f.H0, f.W0 = img.data_ptr(), img.shape[1], img.shape[2]
-        f.img_stride, f.row_stride = img.stride(0), img.stride(1)
-        # a float32 pose is applied in float32, as predict_frame does; cam_k then goes in the same type
-        pose = np.asarray(frame["cam_pose"] if g.dataset == 1 else frame["T_velo_2_cam"])
-        f.calib_f32 = 1 if pose.dtype == np.float32 else 0
-        cdt = np.float32 if f.calib_f32 else np.float64
-        if g.dataset == 1:
-            f.pose = host(np.linalg.inv(pose), cdt)
-            f.cam_k = host(frame["cam_k"], cdt) if "cam_k" in frame else None
-            f.vox_origin = host(frame["vox_origin"])
-            if g.has_depth:
-                d = torch.as_tensor(frame["depth"]).contiguous().cuda()
-                keep.append(d)
-                f.depth, f.depth_h, f.depth_w = d.data_ptr(), d.shape[0], d.shape[1]
-        else:
-            f.cam_k, f.pose = host(frame["cam_k"], cdt), host(pose, cdt)
-            if "vox_origin" in frame:
-                f.vox_origin = host(frame["vox_origin"])
-        if "scene_size" in frame:
-            f.scene_size = host(frame["scene_size"])
-        f.voxel_size = float(frame.get("voxel_size", 0.0))
-        f.flags = 0 if graph else _lib.FRAME_NO_GRAPH
-        if out is None:
-            out = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.uint16, device=img.device)
-        if conf is True:
-            conf = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.float16, device=img.device)
-        if conf is not None:
-            assert conf.dtype == torch.float16 and conf.is_cuda and conf.is_contiguous() and conf.numel() == out.numel()
-        if stream is not None:
-            # the inputs were copied and `out` allocated on the current stream; they must live until `stream` is done
-            stream.wait_stream(torch.cuda.current_stream())
-            for t in [k for k in keep if isinstance(k, torch.Tensor)] + [out] + ([] if conf is None else [conf]):
-                t.record_stream(stream)
-        st = (stream or torch.cuda.current_stream()).cuda_stream
+        occd_model_run_frame_conf; the result is then (map, conf).  On a slab rank other than 0 nothing is written
+        and the result is None; every rank must run every frame (with conf on every rank or on none)."""
+        root = self.comm is None or self.comm.rank == 0
+        f, keep, out, conf_t, st = _frame_call(self.geom, frame, out, stream, graph, conf, root)
         if conf is None:
-            _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), out.data_ptr(), C.c_void_p(st)),
-                       "occd_model_run_frame")
-            return out
-        _lib.check(_lib.lib().occd_model_run_frame_conf(self.handle, C.byref(f), out.data_ptr(), conf.data_ptr(),
-                                                        C.c_void_p(st)), "occd_model_run_frame_conf")
-        return out, conf
+            _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), _ptr(out), st), "occd_model_run_frame")
+            return out if root else None
+        _lib.check(_lib.lib().occd_model_run_frame_conf(self.handle, C.byref(f), _ptr(out), _ptr(conf_t), st),
+                   "occd_model_run_frame_conf")
+        return (out, conf_t) if root else None
 
     def close(self):
         if self.handle:
@@ -396,3 +424,71 @@ class LoadedModel:
             self.close()
         except Exception:  # noqa: BLE001
             pass
+
+
+def run_frame_group(models, frame, out=None, stream=None, graph=True, conf=None):
+    """one frame through every rank of a local group (LoadedModel r loaded with Comm.local(world)[r]), in lock step
+    on one stream (occd_model_run_frame_group) -> rank 0's whole map, or (map, conf), as LoadedModel.run_frame"""
+    hs = (C.c_void_p * len(models))(*[m.handle.value for m in models])
+    f, keep, out, conf_t, st = _frame_call(models[0].geom, frame, out, stream, graph, conf, True)
+    _lib.check(_lib.lib().occd_model_run_frame_group(hs, len(models), C.byref(f), _ptr(out), _ptr(conf_t), st),
+               "occd_model_run_frame_group")
+    return out if conf is None else (out, conf_t)
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _frame_call(g, frame, out, stream, graph, conf, root):
+    """the occd_frame of a predict_frame frame dict (with the host and device copies it points into, which must live
+    until the call returns), the outputs (allocated when not given; none on a slab rank other than 0) and the stream"""
+    img = torch.as_tensor(frame["img"])
+    if img.dim() == 3:
+        img = img.unsqueeze(0)
+    img = img.contiguous().cuda()
+    keep = [img]
+
+    def host(a, dt=np.float64):
+        a = np.ascontiguousarray(np.asarray(a, dt))
+        keep.append(a)
+        return a.ctypes.data
+
+    f = _lib.Frame()
+    f.images, f.H0, f.W0 = img.data_ptr(), img.shape[1], img.shape[2]
+    f.img_stride, f.row_stride = img.stride(0), img.stride(1)
+    # a float32 pose is applied in float32, as predict_frame does; cam_k then goes in the same type
+    pose = np.asarray(frame["cam_pose"] if g.dataset == 1 else frame["T_velo_2_cam"])
+    f.calib_f32 = 1 if pose.dtype == np.float32 else 0
+    cdt = np.float32 if f.calib_f32 else np.float64
+    if g.dataset == 1:
+        f.pose = host(np.linalg.inv(pose), cdt)
+        f.cam_k = host(frame["cam_k"], cdt) if "cam_k" in frame else None
+        f.vox_origin = host(frame["vox_origin"])
+        if g.has_depth:
+            d = torch.as_tensor(frame["depth"]).contiguous().cuda()
+            keep.append(d)
+            f.depth, f.depth_h, f.depth_w = d.data_ptr(), d.shape[0], d.shape[1]
+    else:
+        f.cam_k, f.pose = host(frame["cam_k"], cdt), host(pose, cdt)
+        if "vox_origin" in frame:
+            f.vox_origin = host(frame["vox_origin"])
+    if "scene_size" in frame:
+        f.scene_size = host(frame["scene_size"])
+    f.voxel_size = float(frame.get("voxel_size", 0.0))
+    f.flags = 0 if graph else _lib.FRAME_NO_GRAPH
+    if not root:
+        out = conf = None
+    else:
+        if out is None:
+            out = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.uint16, device=img.device)
+        if conf is True:
+            conf = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.float16, device=img.device)
+        if conf is not None:
+            assert conf.dtype == torch.float16 and conf.is_cuda and conf.is_contiguous() and conf.numel() == out.numel()
+    if stream is not None:
+        # the inputs were copied and `out` allocated on the current stream; they must live until `stream` is done
+        stream.wait_stream(torch.cuda.current_stream())
+        for t in [k for k in keep if isinstance(k, torch.Tensor)] + [t for t in (out, conf) if t is not None]:
+            t.record_stream(stream)
+    return f, keep, out, conf, C.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)

@@ -4,10 +4,13 @@ Frames are independent (SURVEY.md section 8e): the data path needs NO collective
 forward on its own frames.  torch.distributed (NCCL on GPUs, gloo in the CPU tests) is used only for the
 barrier around a timed region, the max-over-ranks reduction of device times and for gathering predictions.
 """
+import ctypes as C
 import os
 
 import torch
 import torch.distributed as dist
+
+from . import _lib
 
 
 def env_world():
@@ -61,6 +64,20 @@ def gather_counts(count, device=None):
 
 
 # --------------------------------------------------------------------------------------------------
+# The communication ops below run over torch.distributed (or, for SimSlabGroup, as copies between the ranks' plans).
+# While deploy.export records a plan (_lib.recording()), they instead emit the library's collective launch on the
+# model file's communicator (occd_comm_*, include/occdepth_b200.h), which the C runtime replays.
+class _CommOp:
+    def run(self, stream=None):
+        if _lib.recording():
+            return self._emit(_lib.lib(), stream)
+        return self._exchange()
+
+
+def _nbytes(t):
+    return t.numel() * t.element_size()
+
+
 # X-slab partition of ONE frame across ranks (BASELINE.json configs[2]): the voxel grid is split along X (the
 # camera-depth axis; SURVEY.md section 8e explains why not the literal Z), every 3-D activation carries `halo`
 # margin planes, and the only data-path communication is the neighbour exchange of those planes before a
@@ -110,7 +127,7 @@ def level_planes(lo, hi, k):
     return -(-hi // (1 << k)) - (lo >> k)
 
 
-class HaloExchangeOp:
+class HaloExchangeOp(_CommOp):
     """Plan op: fill the margins of a halo-carrying activation from the two X-neighbours (send/recv pairs).
     Neighbours may hold different numbers of planes: each side moves min(halo, planes) planes, and the plan only
     exchanges activations every rank holds at least `halo` planes of (Plan.need_halo), so both ends agree."""
@@ -122,9 +139,16 @@ class HaloExchangeOp:
         self.bytes = 2 * w * buf[0, 0].numel() * buf.element_size()
         self.send_left, self.recv_left = buf[0, h:h + w], buf[0, h - w:h]
         self.send_right, self.recv_right = buf[0, h + n - w:h + n], buf[0, h + n:h + n + w]
+        self.halo, self.planes = h, n
         self._keep = buf
 
-    def run(self, stream=None):
+    def _emit(self, L, stream):
+        buf = self._keep
+        assert buf.shape[0] == 1 and buf.is_contiguous()
+        return L.occd_comm_halo_exchange(_lib.MODEL_COMM, buf.data_ptr(), _nbytes(buf[0, 0]), self.halo, self.planes,
+                                         stream)
+
+    def _exchange(self):
         c = self.ctx
         ops = []
         if c.rank > 0:
@@ -137,18 +161,25 @@ class HaloExchangeOp:
                 req.wait()
 
 
-class AllGatherOp:
+class AllGatherOp(_CommOp):
     """Plan op: dst (full, contiguous) = concat over ranks of src (this rank's contiguous shard).  Shards are equal in
     size; a caller with uneven shards pads each to the largest (CPMegaVoxels.emit)."""
 
     def __init__(self, ctx, src, dst):
         self.ctx, self.src, self.dst, self.name, self.flops = ctx, src, dst, "all_gather", 0
+        self._keep = (src, dst)
 
-    def run(self, stream=None):
+    def _emit(self, L, stream):
+        assert self.src.is_contiguous() and self.dst.is_contiguous()
+        assert _nbytes(self.dst) == self.ctx.world * _nbytes(self.src)
+        return L.occd_comm_all_gather(_lib.MODEL_COMM, self.src.data_ptr(), self.dst.data_ptr(), _nbytes(self.src),
+                                      stream)
+
+    def _exchange(self):
         dist.all_gather_into_tensor(self.dst, self.src)
 
 
-class GatherRootOp:
+class GatherRootOp(_CommOp):
     """Plan op: rank 0 assembles the whole uint16 class map [1, X, Y, Z] from every rank's full-resolution X-slab
     src [1, hi - lo, Y, Z]; bounds[r] = (lo, hi) of rank r.  Rank 0 copies its own slab and receives the others straight
     into their planes of dst (one grouped send/recv); the other ranks send and take dst=None.  The bytes move as uint8,
@@ -164,12 +195,19 @@ class GatherRootOp:
         if ctx.rank == 0:
             self.parts = [dst[:, lo:hi] for lo, hi in bounds]          # contiguous: one frame, planes are outermost
         self.bytes = src.numel() * src.element_size()
+        self._keep = (src, dst)
 
     @staticmethod
     def _u8(t):
         return t.reshape(-1).view(torch.uint8)
 
-    def run(self, stream=None):
+    def _emit(self, L, stream):
+        bounds = (C.c_int * (2 * self.ctx.world))(*[b for lo_hi in self.bounds for b in lo_hi])
+        return L.occd_comm_gather_root(_lib.MODEL_COMM, self.src.data_ptr(),
+                                       None if self.dst is None else self.dst.data_ptr(), bounds,
+                                       _nbytes(self.src[0, 0]), stream)
+
+    def _exchange(self):
         c = self.ctx
         if c.rank == 0:
             self.parts[0].copy_(self.src)
@@ -234,7 +272,6 @@ class SimSlabGroup:
 
     @staticmethod
     def run_lockstep(plans, stream=None):
-        from . import _lib
         st = _lib.stream_ptr() if stream is None else stream
         n = len(plans[0].ops)
         assert all(len(p.ops) == n for p in plans), "ranks must build identical op sequences"
@@ -248,7 +285,7 @@ class _SimExchangeOp(HaloExchangeOp):
         super().__init__(ctx, cl)
         self.idx = idx
 
-    def run(self, stream=None):
+    def _exchange(self):
         peers = self.ctx.group.ex[self.idx]
         r = self.ctx.rank
         if r > 0:
@@ -262,7 +299,7 @@ class _SimAllGatherOp(AllGatherOp):
         super().__init__(ctx, src, dst)
         self.idx = idx
 
-    def run(self, stream=None):
+    def _exchange(self):
         peers = self.ctx.group.ag[self.idx]
         flat = self.dst.reshape(self.ctx.world, -1)
         for r in range(self.ctx.world):
@@ -274,7 +311,7 @@ class _SimGatherRootOp(GatherRootOp):
         super().__init__(ctx, src, dst, bounds)
         self.idx = idx
 
-    def run(self, stream=None):
+    def _exchange(self):
         if self.ctx.rank != 0:
             return
         peers = self.ctx.group.gr[self.idx]

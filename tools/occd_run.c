@@ -4,6 +4,7 @@
  * the library (occdepth_b200/lib/occd_run).
  *
  *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]
+ *            [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
  *
  * Inputs are raw little-endian files, one record per frame, frames back to back (no image decoder):
  *   IMAGES  N x V x H0 x W0 x 3 uint8, RGB, row-major (H0 x W0 default to the model's crop; --raw gives larger
@@ -14,13 +15,19 @@
  * Output: OUT_DIR/NNNNNN.label per frame, the uint16 class map (X x Y x Z, C order) as the KITTI submission writer
  * stores it; the labels are remapped when the model was exported with inv_map.  Prints ms per frame (device time
  * of occd_model_run_frame, from CUDA events) and the mean over the frames after the first.
+ *
+ * X-slab partition over W GPUs: one process per rank, each on its own device (e.g. CUDA_VISIBLE_DEVICES), MODEL the
+ * rank's file (deploy.export(..., slab_output="root")) and the same inputs on every rank.  Rank 0 writes the NCCL id
+ * to FILE, the other ranks wait for it; only rank 0 writes .label files.  LIBNCCL: where libnccl.so.2 is, when the
+ * loader does not find it by name.
  */
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <unistd.h>
 
-#include "occdepth_b200.h"
+#include "occdepth_b200_comm.h"
 
 #define CK(x)                                                                          \
   do {                                                                                 \
@@ -46,14 +53,43 @@ static int read_exact(FILE* f, void* dst, size_t n, const char* what) {
   return 1;
 }
 
+/* the NCCL id of a W-rank run: rank 0 makes it and writes FILE (whole, through a rename); the others wait for FILE */
+static int share_id(const char* path, int rank, const char* nccl_lib, char* id) {
+  if (rank == 0) {
+    if (occd_comm_unique_id(nccl_lib, id) != OCCD_OK) {
+      fprintf(stderr, "occd_run: occd_comm_unique_id: %s\n", occd_last_error());
+      return 0;
+    }
+    char tmp[4096];
+    snprintf(tmp, sizeof(tmp), "%s.tmp", path);
+    FILE* f = fopen(tmp, "wb");
+    if (!f || fwrite(id, 1, OCCD_COMM_ID_BYTES, f) != OCCD_COMM_ID_BYTES || fclose(f) != 0 || rename(tmp, path) != 0) {
+      fprintf(stderr, "occd_run: cannot write %s\n", path);
+      return 0;
+    }
+    return 1;
+  }
+  for (int t = 0; t < 6000; ++t) { /* 10 minutes */
+    FILE* f = fopen(path, "rb");
+    if (f) {
+      size_t n = fread(id, 1, OCCD_COMM_ID_BYTES, f);
+      fclose(f);
+      if (n == OCCD_COMM_ID_BYTES) return 1;
+    }
+    usleep(100000);
+  }
+  fprintf(stderr, "occd_run: rank %d: no NCCL id in %s\n", rank, path);
+  return 0;
+}
+
 int main(int argc, char** argv) {
   if (argc < 6) {
     fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]\n");
     return 2;
   }
   const char *model_path = argv[1], *img_path = argv[2], *calib_path = argv[3], *out_dir = argv[5];
-  const char* depth_path = NULL;
-  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0;
+  const char *depth_path = NULL, *id_path = NULL, *nccl_lib = NULL;
+  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0;
   for (int i = 6; i < argc; ++i) {
     if (!strcmp(argv[i], "--raw") && i + 2 < argc) {
       H0 = atoi(argv[++i]);
@@ -62,13 +98,33 @@ int main(int argc, char** argv) {
       depth_path = argv[++i];
     } else if (!strcmp(argv[i], "--no-graph")) {
       flags |= OCCD_FRAME_NO_GRAPH;
+    } else if (!strcmp(argv[i], "--world") && i + 1 < argc) {
+      world = atoi(argv[++i]);
+    } else if (!strcmp(argv[i], "--rank") && i + 1 < argc) {
+      rank = atoi(argv[++i]);
+    } else if (!strcmp(argv[i], "--nccl-id") && i + 1 < argc) {
+      id_path = argv[++i];
+    } else if (!strcmp(argv[i], "--nccl-lib") && i + 1 < argc) {
+      nccl_lib = argv[++i];
     } else {
       fprintf(stderr, "occd_run: unknown option %s\n", argv[i]);
       return 2;
     }
   }
+  if (world > 1 && (!id_path || rank < 0 || rank >= world)) {
+    fprintf(stderr, "occd_run: --world W needs --rank R (0 <= R < W) and --nccl-id FILE\n");
+    return 2;
+  }
   occd_model* m = NULL;
-  OK(occd_model_load(model_path, &m));
+  occd_comm* comm = NULL;
+  if (world > 1) {
+    char id[OCCD_COMM_ID_BYTES];
+    if (!share_id(id_path, rank, nccl_lib, id)) return 1;
+    OK(occd_comm_create(nccl_lib, id, rank, world, &comm));
+    OK(occd_model_load_slab(model_path, comm, &m));
+  } else {
+    OK(occd_model_load(model_path, &m));
+  }
   occd_model_geom g;
   OK(occd_model_info(m, &g));
   if (!H0) {
@@ -127,13 +183,14 @@ int main(int argc, char** argv) {
     f.depth_w = g.depth_w;
     f.flags = flags;
     CK(cudaEventRecord(e0, st));
-    OK(occd_model_run_frame(m, &f, (uint16_t*)d_map, st));
+    OK(occd_model_run_frame(m, &f, rank == 0 ? (uint16_t*)d_map : NULL, st));
     CK(cudaEventRecord(e1, st));
-    CK(cudaMemcpyAsync(h_map, d_map, map_bytes, cudaMemcpyDeviceToHost, st));
+    if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, e0, e1));
     if (i > 0) total += ms;
+    if (rank != 0) continue;
     char path[4096];
     snprintf(path, sizeof(path), "%s/%06d.label", out_dir, i);
     FILE* fo = fopen(path, "wb");
@@ -146,6 +203,7 @@ int main(int argc, char** argv) {
   }
   if (n > 1) printf("mean over frames 1..%d: %.3f ms per frame\n", n - 1, total / (n - 1));
   OK(occd_model_destroy(m));
+  if (comm) OK(occd_comm_destroy(comm));
   fclose(fi);
   fclose(fc);
   if (fd) fclose(fd);
