@@ -444,6 +444,11 @@ int occd_occupied_voxels(const uint16_t* class_map, const uint8_t* fov_mask, int
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,
                           int cs_in, int cs_out, int dh, int dw, float bf_scale, void* stream);
+/* the same with one depth map per batch item: item b reads the fp32 [dh][dw] map at depth + b * depth_stride floats.  */
+/* depth_stride 0 is occd_virtual_view_fwd exactly (item 0's map for every item); otherwise it must be >= dh * dw.    */
+int occd_virtual_view_items_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,
+                                int cs_in, int cs_out, int dh, int dw, float bf_scale, long long depth_stride,
+                                void* stream);
 
 /* -------------------------------------------------------------------------------------------- */
 /* Model files: one camera frame in, the class map out, without Python.  occdepth_b200.deploy.export writes the   */
@@ -509,6 +514,16 @@ int occd_model_run_frame(occd_model* m, const occd_frame* frame, uint16_t* class
 /* top class's softmax probability of every voxel (OCCD_OUT1_CLASS_U16_CONF).  OCCD_ERR_UNSUPPORTED for a model    */
 /* exported without confidence; occd_model_run_frame on a model exported with it writes the map only.              */
 int occd_model_run_frame_conf(occd_model* m, const occd_frame* frame, uint16_t* class_map, void* conf, void* stream);
+/* Batched model files (exported from a list of frames, OccDepth.predict_frames): one plan runs up to B frames.     */
+/* *batch = B, or 1 for a file exported from one frame.                                                             */
+int occd_model_batch(const occd_model* m, int* batch);
+/* frames[0..n) -> class_maps + i*X*Y*Z (DEVICE uint16), 1 <= n <= B, and with conf (DEVICE float16, or NULL for the */
+/* maps only; OCCD_ERR_UNSUPPORTED for a file without confidence) their confidences at conf + i*X*Y*Z.  Each item    */
+/* keeps its own calibration cache; items [n, B) keep what their buffers hold and their results are not copied.  The */
+/* B-frame plan runs whatever n is, with the graph rules of occd_model_run_frame.  On an unbatched file this is      */
+/* occd_model_run_frame(_conf) with n = 1.                                                                          */
+int occd_model_run_frames(occd_model* m, const occd_frame* frames, int n, uint16_t* class_maps, void* conf,
+                          void* stream);
 int occd_model_destroy(occd_model* m);
 
 /* Model files under the X-slab partition (DESIGN.md section 9): one file per rank, each holding that rank's plan of */

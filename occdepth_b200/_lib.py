@@ -155,6 +155,7 @@ SYMBOLS = {
     "occd_fc_fwd": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "occd_channel_scale": (C.c_int, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp]),
     "occd_virtual_view_fwd": (C.c_int, [_vp, _vp, _vp] + [_i] * 9 + [_f, _vp]),
+    "occd_virtual_view_items_fwd": (C.c_int, [_vp, _vp, _vp] + [_i] * 9 + [_f, _ll, _vp]),
     "occd_upsample_bilinear_ac": (C.c_int, [_vp, _vp] + [_i] * 11 + [_vp]),
     "occd_upsample_tapsum_ac": (C.c_int, [_vp, _vp, _vp] + [_i] * 15 + [_vp]),
     "occd_ssc_confusion": (C.c_int, [_vp, _i, _vp, _i, _ll, _i, _vp, _vp]),
@@ -167,6 +168,8 @@ SYMBOLS = {
     "occd_model_info": (C.c_int, [_vp, C.POINTER(ModelGeom)]),
     "occd_model_run_frame": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp]),
     "occd_model_run_frame_conf": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp, _vp]),
+    "occd_model_batch": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "occd_model_run_frames": (C.c_int, [_vp, C.POINTER(Frame), _i, _vp, _vp, _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "occd_comm_halo_exchange": (C.c_int, [_vp, _vp, _ll, _i, _i, _vp]),

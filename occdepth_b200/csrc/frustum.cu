@@ -245,11 +245,12 @@ namespace {
 // replaces OccDepth.generate_virtual_img (occdepth/models/OccDepth.py:233-260): F.interpolate(depth, bilinear,
 // align_corners=False) -> disparity bf/scale / depth (inf -> 0) -> base grid arange(-1,1,2/h) (pixel-CORNER
 // coordinates) shifted by disparity*2/w -> F.grid_sample(bilinear, border, align_corners=False).
-// The reference uses batch item 0's disparity for every item (:257); kept.
+// The reference uses batch item 0's disparity for every item (:257): depth_stride 0.  A batch of independent camera
+// frames gives item b the depth map at depth + b * depth_stride.
 template <typename T>
 __global__ void virtual_view_kernel(const T* __restrict__ in, T* __restrict__ out,
                                     const float* __restrict__ depth, int B, int h, int w, int CV, int cs_in,
-                                    int cs_out, int dh, int dw, float bf_scale) {
+                                    int cs_out, int dh, int dw, float bf_scale, long long depth_stride) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)B * h * w * CV;
   if (i >= total) return;
@@ -258,6 +259,7 @@ __global__ void virtual_view_kernel(const T* __restrict__ in, T* __restrict__ ou
   const int x = (int)(p % w); p /= w;
   const int y = (int)(p % h); p /= h;
   const int b = (int)p;
+  depth += b * depth_stride;
   // depth at (y, x) of the feature map: bilinear, align_corners=False (area_pixel_compute_source_index)
   const float sy = fmaxf(((float)y + 0.5f) * ((float)dh / (float)h) - 0.5f, 0.f);
   const float sx = fmaxf(((float)x + 0.5f) * ((float)dw / (float)w) - 0.5f, 0.f);
@@ -291,16 +293,36 @@ __global__ void virtual_view_kernel(const T* __restrict__ in, T* __restrict__ ou
 }
 }  // namespace
 
+namespace {
+int virtual_view(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C, int cs_in,
+                 int cs_out, int dh, int dw, float bf_scale, long long depth_stride, void* stream) {
+  const int CV = (C + 7) / 8;
+  const long long total = (long long)B * h * w * CV;
+  OCCD_DISPATCH_DTYPE(dtype, T, (virtual_view_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0,
+                                                           (cudaStream_t)stream>>>(
+                                     (const T*)in, (T*)out, depth, B, h, w, CV, cs_in, cs_out, dh, dw, bf_scale,
+                                     depth_stride)));
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+}  // namespace
+
 extern "C" int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w,
                                      int C, int cs_in, int cs_out, int dh, int dw, float bf_scale, void* stream) {
   OCCD_CHECK_ARG(in && out && depth && B > 0 && h > 0 && w > 0 && C > 0 && dh > 0 && dw > 0 && cs_in % 8 == 0 &&
                  cs_out % 8 == 0, "occd_virtual_view_fwd: args");
-  const int CV = (C + 7) / 8;
-  OCCD_CHECK_ARG(CV * 8 <= cs_in && CV * 8 <= cs_out, "occd_virtual_view_fwd: channel window");
-  const long long total = (long long)B * h * w * CV;
-  OCCD_DISPATCH_DTYPE(dtype, T, (virtual_view_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0,
-                                                           (cudaStream_t)stream>>>(
-                                     (const T*)in, (T*)out, depth, B, h, w, CV, cs_in, cs_out, dh, dw, bf_scale)));
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
+  OCCD_CHECK_ARG((C + 7) / 8 * 8 <= cs_in && (C + 7) / 8 * 8 <= cs_out, "occd_virtual_view_fwd: channel window");
+  return virtual_view(in, out, depth, dtype, B, h, w, C, cs_in, cs_out, dh, dw, bf_scale, 0, stream);
+}
+
+extern "C" int occd_virtual_view_items_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h,
+                                           int w, int C, int cs_in, int cs_out, int dh, int dw, float bf_scale,
+                                           long long depth_stride, void* stream) {
+  OCCD_CHECK_ARG(in && out && depth && B > 0 && h > 0 && w > 0 && C > 0 && dh > 0 && dw > 0 && cs_in % 8 == 0 &&
+                 cs_out % 8 == 0, "occd_virtual_view_items_fwd: args");
+  OCCD_CHECK_ARG((C + 7) / 8 * 8 <= cs_in && (C + 7) / 8 * 8 <= cs_out, "occd_virtual_view_items_fwd: channel window");
+  OCCD_CHECK_ARG(depth_stride == 0 || depth_stride >= (long long)dh * dw,
+                 "occd_virtual_view_items_fwd: depth_stride must be 0 (item 0's depth map for every item) or at least "
+                 "dh * dw (one map per item)");
+  return virtual_view(in, out, depth, dtype, B, h, w, C, cs_in, cs_out, dh, dw, bf_scale, depth_stride, stream);
 }

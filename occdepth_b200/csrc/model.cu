@@ -42,6 +42,11 @@ struct ArgOf<occd_model*> {  // a model handle cannot be stored in a file: only 
   static occd_model* get(const Arg&) { return nullptr; }
 };
 template <>
+struct ArgOf<const occd_model*> {
+  static constexpr char tag = 'n';
+  static const occd_model* get(const Arg&) { return nullptr; }
+};
+template <>
 struct ArgOf<occd_comm*> {  // the model's communicator (tag 'm'), filled in by occd_model_load_slab; or NULL ('n')
   static constexpr char tag = 'm';
   static occd_comm* get(const Arg& a) { return static_cast<occd_comm*>(a.p); }
@@ -117,8 +122,11 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_crp_relation_sums),     OCCD_ENTRY(occd_depth_cls_sums),
     OCCD_ENTRY(occd_occupied_voxels),       OCCD_ENTRY(occd_virtual_view_fwd),
     OCCD_ENTRY(occd_vox2pix_range_fwd),     OCCD_ENTRY(occd_argmax_classes_conf),
-    // takes a stream like the launches, so it has a signature here; its model handle can only be NULL
-    OCCD_ENTRY(occd_model_run_frame_conf),
+    OCCD_ENTRY(occd_virtual_view_items_fwd),
+    // take a stream like the launches (occd_model_batch is bound like them), so they have a signature here; their
+    // model handle can only be NULL
+    OCCD_ENTRY(occd_model_run_frame_conf),  OCCD_ENTRY(occd_model_run_frames),
+    OCCD_ENTRY(occd_model_batch),
     // the X-slab partition's collectives: the lock-step runner of a local group stops after each
     OCCD_ENTRY(occd_comm_halo_exchange),    OCCD_ENTRY(occd_comm_all_gather),
     OCCD_ENTRY(occd_comm_gather_root),
@@ -138,9 +146,11 @@ enum Role { ROLE_IMG, ROLE_PIX, ROLE_FOV, ROLE_PIX_Z, ROLE_DEPTH, ROLE_CAMS, ROL
 const char* kRoleNames[N_ROLES] = {"image", "pix", "fov", "pix_z", "depth", "camera tables", "scaled_pixel_size",
                                    "class map"};
 enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4,   // FLAG_CONF: the class-map role holds the map, then its
-       FLAG_SLAB = 16 };                                         // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
-                                                                 // FLAG_SLAB: one rank's plan, a slab block follows
-                                                                 // (bit 3 stays unassigned)
+       FLAG_SLAB = 16, FLAG_BATCH = 32 };                        // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
+                                                                 // FLAG_SLAB: one rank's plan, a slab block follows;
+                                                                 // FLAG_BATCH: a B-frame plan, a batch block follows
+                                                                 // the roles (bit 3 stays unassigned)
+const uint32_t kMaxBatch = 1024;
 const uint32_t kMaxWorld = 64;
 const size_t kArenaAlign = 512;  // the caching allocator's block alignment, which the plans were built with
 
@@ -223,9 +233,11 @@ struct occd_model {
   cudaStream_t capture_stream = nullptr;
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
-  std::vector<uint8_t> calib;  // the calibration the index buffers hold (KITTI)
-  bool calib_valid = false;
-  float cams[4 * 40], sps[4];
+  // per batch item: the calibration its index buffers hold (KITTI), and its FlospDepth tables on the host
+  uint32_t batch = 1;
+  std::vector<std::vector<uint8_t>> calib;
+  std::vector<char> calib_valid;
+  std::vector<float> cams, sps;
   // the X-slab partition (FLAG_SLAB): this rank, every rank's [lo, hi) planes of the lift grid, this rank's window of
   // the lift's voxel order, the one view it stages (-1: every view) and the whole map's X extent (rank 0's output)
   uint32_t rank = 0, world = 1, map_x = 0;
@@ -237,6 +249,8 @@ struct occd_model {
 
   bool slab() const { return (flags & FLAG_SLAB) != 0; }
   void* dev(int role) const { return arena + buf_off[roles[role].buffer] + roles[role].off; }
+  // item b's part of an input role, which holds `batch` items of equal length
+  void* dev(int role, uint32_t b) const { return static_cast<uint8_t*>(dev(role)) + roles[role].len / batch * b; }
   uint64_t map_bytes() const { return (uint64_t)out[0] * out[1] * out[2] * 2; }   // one uint16 class map
 };
 
@@ -296,6 +310,14 @@ int parse(occd_model* m) {
     m->roles[k].off = r.get<uint64_t>();
     m->roles[k].len = r.get<uint64_t>();
   }
+  if (m->flags & FLAG_BATCH) {
+    m->batch = r.get<uint32_t>();
+    if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (batch block)");
+    if (m->batch < 1 || m->batch > kMaxBatch)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: batch of " + std::to_string(m->batch) + " frames out of range");
+    if (m->flags & FLAG_SLAB)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: a batched file has no X-slab partition (flag bits 4 and 5)");
+  }
   if (m->flags & FLAG_SLAB) {
     m->rank = r.get<uint32_t>();
     m->world = r.get<uint32_t>();
@@ -317,7 +339,7 @@ int parse(occd_model* m) {
   if ((m->precision != OCCD_DTYPE_F32 && m->precision != OCCD_DTYPE_BF16) || m->dataset > 1 || m->V < 1 ||
       m->V > 4 || m->P < 1 || m->P > 64 || m->n_cams > 4 || m->img_cstride % 8 != 0)
     return fail(OCCD_ERR_FORMAT, "occd_model_load: header field out of range");
-  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB))
+  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB | FLAG_BATCH))
     return fail(OCCD_ERR_FORMAT, "occd_model_load: unknown header flag bits");
   if (m->slab()) {
     // every rank's slab, in rank order, tiles the lift grid's X planes; this rank's window is its slab's voxels
@@ -444,7 +466,8 @@ int parse(occd_model* m) {
   }
   if (r.pos != r.n) return fail(OCCD_ERR_FORMAT, "occd_model_load: trailing bytes after the records");
 
-  // under the slab partition: the staged view only, this rank's window of the indices, the whole map on rank 0 only
+  // under the slab partition: the staged view only, this rank's window of the indices, the whole map on rank 0 only;
+  // a batched file holds `batch` items of each
   const bool need[N_ROLES] = {true, true, true, true, (m->flags & FLAG_VIRTUAL) != 0,
                               (m->flags & FLAG_FLOSP_DEPTH) != 0, (m->flags & FLAG_FLOSP_DEPTH) != 0, m->rank == 0};
   const uint64_t N = m->slab() ? m->n_len : (uint64_t)m->grid[0] * m->grid[1] * m->grid[2];
@@ -457,10 +480,14 @@ int parse(occd_model* m) {
   for (int k = 0; k < N_ROLES; ++k) {
     const RoleRef& ro = m->roles[k];
     if (!need[k]) continue;
-    if (ro.buffer < 0 || !in_buffer((uint32_t)ro.buffer, ro.off, ro.len) || ro.len != want_len[k])
+    if (ro.buffer < 0 || !in_buffer((uint32_t)ro.buffer, ro.off, ro.len) || ro.len != want_len[k] * m->batch)
       return fail(OCCD_ERR_FORMAT, std::string("occd_model_load: the ") + kRoleNames[k] +
                                        " buffer does not match the header");
   }
+  m->calib.assign(m->batch, std::vector<uint8_t>());
+  m->calib_valid.assign(m->batch, 0);
+  m->cams.assign((size_t)m->batch * 4 * 40, 0.f);
+  m->sps.assign((size_t)m->batch * 4, 0.f);
   return OCCD_OK;
 }
 
@@ -577,21 +604,21 @@ void load_as_f32(const void* src, int n, float* dst) {
   for (int i = 0; i < n; ++i) dst[i] = (float)s[i];
 }
 
-// the datasets' camera-frame staging (OccDepth._stage_frame): images, depth, and -- for a new calibration -- the
-// projection indices and the FlospDepth tables
-int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
+// the datasets' camera-frame staging (OccDepth._stage_frames) of frame `f` into batch item b: images, depth, and -- for
+// a calibration other than the item's last -- the projection indices and the FlospDepth tables
+int stage(occd_model* m, const occd_frame* f, uint32_t b, cudaStream_t st) {
   static const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
   const bool nyu = m->dataset == 1;
   // under the partition's view sharding the rank stages its one view
   const void* images = static_cast<const uint8_t*>(f->images) + (m->view_sel > 0 ? m->view_sel * f->img_stride : 0);
   int rc = occd_stage_rgb_u8_cl(images, f->img_stride, f->row_stride, m->view_sel >= 0 ? 1 : (int)m->V, f->H0, f->W0,
-                                (int)m->img_h, (int)m->img_w, mean, stdv, m->dev(ROLE_IMG), (int)m->precision,
+                                (int)m->img_h, (int)m->img_w, mean, stdv, m->dev(ROLE_IMG, b), (int)m->precision,
                                 (int)m->img_cstride, st);
   if (rc != OCCD_OK) return rc;
   if (m->flags & FLAG_VIRTUAL) {
     OCCD_CHECK_ARG(f->depth != nullptr && f->depth_h == (int)m->depth_h && f->depth_w == (int)m->depth_w,
                    "occd_model_run_frame: the model takes a uint16 depth map of the size it was exported with");
-    rc = occd_depth_u16_to_f32(f->depth, static_cast<float*>(m->dev(ROLE_DEPTH)), (long long)m->depth_h * m->depth_w,
+    rc = occd_depth_u16_to_f32(f->depth, static_cast<float*>(m->dev(ROLE_DEPTH, b)), (long long)m->depth_h * m->depth_w,
                                8000.0, 10.0f, st);
     if (rc != OCCD_OK) return rc;
   }
@@ -623,9 +650,9 @@ int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
     put(origin, 24);
     put(scene, 24);
     put(&voxel, 8);
-    if (m->calib_valid && key == m->calib) return OCCD_OK;
-    m->calib_valid = false;
-    m->calib.swap(key);
+    if (m->calib_valid[b] && key == m->calib[b]) return OCCD_OK;
+    m->calib_valid[b] = 0;
+    m->calib[b].swap(key);
   }
   int dims[3];
   for (int k = 0; k < 3; ++k) dims[k] = (int)ceil(((origin[k] + scene[k]) - origin[k]) / voxel);  // volume_dims
@@ -659,15 +686,15 @@ int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
   const long long N = m->slab() ? (long long)m->n_len : (long long)m->grid[0] * m->grid[1] * m->grid[2];
   for (int v = 0; v < n_views; ++v) {
     const void* pose = f32_pose[v] ? (const void*)Ef[v] : (const void*)E[v];
-    long long* pix = static_cast<long long*>(m->dev(ROLE_PIX)) + (long long)v * N * m->P * 2;
-    unsigned char* fov = static_cast<unsigned char*>(m->dev(ROLE_FOV)) + (long long)v * N * m->P;
+    long long* pix = static_cast<long long*>(m->dev(ROLE_PIX, b)) + (long long)v * N * m->P * 2;
+    unsigned char* fov = static_cast<unsigned char*>(m->dev(ROLE_FOV, b)) + (long long)v * N * m->P;
     if (m->slab())
       rc = occd_vox2pix_range_fwd(pose, f32_pose[v], k32[v], o32, voxel, dims[0], dims[1], dims[2], (int)m->img_w,
-                                  (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z),
+                                  (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z, b),
                                   (long long)m->n_lo, N, st);
     else
       rc = occd_vox2pix_fwd(pose, f32_pose[v], k32[v], o32, voxel, dims[0], dims[1], dims[2], (int)m->img_w,
-                            (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z), st);
+                            (int)m->img_h, &m->pattern[0][0], (int)m->P, pix, fov, m->dev(ROLE_PIX_Z, b), st);
     if (rc != OCCD_OK) return rc;
   }
   if (m->flags & FLAG_FLOSP_DEPTH) {
@@ -680,9 +707,11 @@ int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
         kf[v * 9 + i] = (float)K[v][i];
       }
     int vn[3];
+    float* cams = m->cams.data() + (size_t)b * m->n_cams * 40;
+    float* sps = m->sps.data() + (size_t)b * m->n_cams;
     rc = occd_flosp_camera_tables((int)m->n_cams, f->calib_f32 ? (const void*)kf : (const void*)kd, f->pose,
-                                  f->calib_f32, nyu ? nullptr : m->G, nyu ? origin : nullptr, (int)m->ps, m->cams,
-                                  m->sps, vn);
+                                  f->calib_f32, nyu ? nullptr : m->G, nyu ? origin : nullptr, (int)m->ps, cams, sps,
+                                  vn);
     if (rc != OCCD_OK) return rc;
     // NYU re-derives FlospDepth's grid from each frame's origin; it must be the one the plan was built for (in
     // FlospDepth's own axis order, which is not the lift grid's)
@@ -691,11 +720,11 @@ int stage(occd_model* m, const occd_frame* f, cudaStream_t st) {
                          (unsigned)vn[2] == m->flosp_vn[2],
                      "occd_model_run_frame: this vox_origin gives FlospDepth another voxel grid than the model's");
     cudaError_t e;
-    if ((e = cudaMemcpyAsync(m->dev(ROLE_CAMS), m->cams, m->n_cams * 160, cudaMemcpyHostToDevice, st)) != cudaSuccess ||
-        (e = cudaMemcpyAsync(m->dev(ROLE_SPS), m->sps, m->n_cams * 4, cudaMemcpyHostToDevice, st)) != cudaSuccess)
+    if ((e = cudaMemcpyAsync(m->dev(ROLE_CAMS, b), cams, m->n_cams * 160, cudaMemcpyHostToDevice, st)) != cudaSuccess ||
+        (e = cudaMemcpyAsync(m->dev(ROLE_SPS, b), sps, m->n_cams * 4, cudaMemcpyHostToDevice, st)) != cudaSuccess)
       return cuda_fail(e, "occd_model_run_frame: camera tables");
   }
-  if (!nyu) m->calib_valid = true;
+  if (!nyu) m->calib_valid[b] = 1;
   return OCCD_OK;
 }
 
@@ -896,8 +925,8 @@ int execute(occd_model* owner, int flags, cudaStream_t st, Replay rep) {
   return OCCD_OK;
 }
 
-// stages the frame and replays the records (through the graph when there is one) on `stream`
-int run_records(occd_model* m, const occd_frame* f, cudaStream_t st) {
+// stages frames[0..n) into items [0, n) and replays the records (through the graph when there is one) on `stream`
+int run_records(occd_model* m, const occd_frame* frames, int n, cudaStream_t st) {
   if (m->comm) {
     int rank, world, kind;
     occd_comm_describe(m->comm, &rank, &world, &kind);
@@ -905,20 +934,23 @@ int run_records(occd_model* m, const occd_frame* f, cudaStream_t st) {
       return fail(OCCD_ERR_UNSUPPORTED, "occd_model_run_frame: a model on a local communicator runs with its group "
                                         "through occd_model_run_frame_group");
   }
-  int rc = stage(m, f, st);
-  if (rc != OCCD_OK) return rc;
-  return execute(m, f->flags, st, [m](cudaStream_t s) { return replay(m, s); });
+  for (int i = 0; i < n; ++i) {
+    int rc = stage(m, &frames[i], (uint32_t)i, st);
+    if (rc != OCCD_OK) return rc;
+  }
+  return execute(m, frames[0].flags, st, [m](cudaStream_t s) { return replay(m, s); });
 }
 
-// the whole map (and its confidence) of a model whose plan outputs one: every unpartitioned model, rank 0 of a slab
-int copy_out(const occd_model* m, uint16_t* class_map, void* conf, cudaStream_t st, const char* what) {
+// the whole maps of items [0, n) (and their confidences) of a model whose plan outputs them: every unpartitioned
+// model, rank 0 of a slab.  The class-map role is [B][map], or [2][B][map] with the confidence
+int copy_out(const occd_model* m, uint16_t* class_map, void* conf, int n, cudaStream_t st, const char* what) {
   if (m->rank != 0) return OCCD_OK;
   const char* roles = static_cast<const char*>(m->dev(ROLE_CLASSES));
   cudaError_t e;
-  if ((e = cudaMemcpyAsync(class_map, roles, m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+  if ((e = cudaMemcpyAsync(class_map, roles, m->map_bytes() * n, cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
     return cuda_fail(e, (std::string(what) + ": class map copy").c_str());
-  if (conf &&
-      (e = cudaMemcpyAsync(conf, roles + m->map_bytes(), m->map_bytes(), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+  if (conf && (e = cudaMemcpyAsync(conf, roles + m->map_bytes() * m->batch, m->map_bytes() * n,
+                                   cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
     return cuda_fail(e, (std::string(what) + ": confidence copy").c_str());
   return OCCD_OK;
 }
@@ -928,9 +960,9 @@ int copy_out(const occd_model* m, uint16_t* class_map, void* conf, cudaStream_t 
 extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t* class_map, void* stream) {
   OCCD_CHECK_ARG(m && f && f->images && (class_map || m->rank != 0), "occd_model_run_frame: null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = run_records(m, f, st);
+  int rc = run_records(m, f, 1, st);
   if (rc != OCCD_OK) return rc;
-  return copy_out(m, class_map, nullptr, st, "occd_model_run_frame");
+  return copy_out(m, class_map, nullptr, 1, st, "occd_model_run_frame");
 }
 
 extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uint16_t* class_map, void* conf,
@@ -942,9 +974,32 @@ extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uin
     return OCCD_ERR_UNSUPPORTED;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = run_records(m, f, st);
+  int rc = run_records(m, f, 1, st);
   if (rc != OCCD_OK) return rc;
-  return copy_out(m, class_map, conf, st, "occd_model_run_frame_conf");
+  return copy_out(m, class_map, conf, 1, st, "occd_model_run_frame_conf");
+}
+
+extern "C" int occd_model_batch(const occd_model* m, int* batch) {
+  OCCD_CHECK_ARG(m && batch, "occd_model_batch: null argument");
+  *batch = (int)m->batch;
+  return OCCD_OK;
+}
+
+extern "C" int occd_model_run_frames(occd_model* m, const occd_frame* frames, int n, uint16_t* class_maps, void* conf,
+                                     void* stream) {
+  OCCD_CHECK_ARG(m && frames && (class_maps || m->rank != 0), "occd_model_run_frames: null argument");
+  if (n < 1 || (uint32_t)n > m->batch)
+    return fail(OCCD_ERR_ARG, "occd_model_run_frames: " + std::to_string(n) + " frames, the model runs 1 to " +
+                                  std::to_string(m->batch));
+  for (int i = 0; i < n; ++i) OCCD_CHECK_ARG(frames[i].images, "occd_model_run_frames: a frame without images");
+  if (conf && !(m->flags & FLAG_CONF)) {
+    occd_set_last_error("occd_model_run_frames: the model was exported without confidence");
+    return OCCD_ERR_UNSUPPORTED;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = run_records(m, frames, n, st);
+  if (rc != OCCD_OK) return rc;
+  return copy_out(m, class_maps, conf, n, st, "occd_model_run_frames");
 }
 
 extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
@@ -965,7 +1020,7 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int r = 0; r < world; ++r) {
-    int rc = stage(ms[r], f, st);
+    int rc = stage(ms[r], f, 0, st);
     if (rc != OCCD_OK) return rc;
   }
   // rank 0 holds the group's graph; it is captured afresh when the group's models change
@@ -975,7 +1030,7 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
   int rc = execute(owner, f->flags, st, [ms, world](cudaStream_t s) { return replay_lockstep(ms, world, s); });
   if (rc != OCCD_OK) return rc;
   if (capture && owner->graph_exec) owner->graph_ranks.assign(ms, ms + world);
-  return copy_out(owner, class_map, conf, st, "occd_model_run_frame_group");
+  return copy_out(owner, class_map, conf, 1, st, "occd_model_run_frame_group");
 }
 
 extern "C" int occd_model_destroy(occd_model* m) {

@@ -25,11 +25,14 @@ ROLES = ("img", "pix", "fov", "pix_z", "depth", "cams", "sps", "classes")
 FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF, FLAG_SLAB = 1, 2, 4, 16  # FLAG_CONF: the class-map role holds the map,
                                                                    # then its float16 confidence; FLAG_SLAB: one
                                                                    # rank's plan of the X-slab partition
+FLAG_BATCH = 32                                                    # a B-frame plan of predict_frames (batch block)
 PATTERN_MAX = 64
 
 _STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
+# forwarded even while recording: queries, and the destructors -- a ConvOp or LoadedModel of another plan that the
+# garbage collector finalizes on the exporting thread during the recording run is released, not recorded
 _PASS_THROUGH = {"occd_last_error", "occd_abi_version", "occd_conv_plan_info", "occd_conv_plan_impl",
-                 "occd_conv_plan_schedule"}
+                 "occd_conv_plan_schedule", "occd_conv_plan_destroy", "occd_model_destroy"}
 
 
 class ExportError(RuntimeError):
@@ -176,7 +179,11 @@ class _Buffers:
 def export(model, path, frame, inv_map=None, confidence=False, slab_output=None):
     """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map, confidence=confidence)`
     for frames of this frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame
-    refuses, with the same messages.  Returns a dict of what was written (records, buffers, bytes).  With
+    refuses, with the same messages.  Returns a dict of what was written (records, buffers, bytes).
+
+    `frame` a list of B frames: the file of `model.predict_frames(frame, ...)`, B frames per run (header flag
+    FLAG_BATCH and a batch block; every role holds B items), which `occd_model_run_frames` replays for 1..B frames.
+    Refuses what predict_frames refuses; not with slab_output.  With
     `confidence` the file's class-map role holds the map and then its confidence (header flag FLAG_CONF), which
     `occd_model_run_frame_conf` reads; without it the file is what it always was.
 
@@ -189,7 +196,16 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     The recording stand-in replaces the library for the calling thread only, so other threads may keep serving
     through the library meanwhile; `model` itself must not run elsewhere during the export (as for predict_frame)."""
     from . import data as D
-    f = model._frame_checked(frame, slab_output)
+    batched = not isinstance(frame, dict)
+    if batched:
+        if slab_output is not None:
+            raise NotImplementedError("deploy.export: a batched model file (a list of frames) has no X-slab partition")
+        f = model._frames_checked(frame, True, confidence)[0]
+        B = len(frame)
+    else:
+        f = model._frame_checked(frame, slab_output)
+        B = 1
+    depth_items = f["virtual"] and B > 1
     slab = model.__dict__.get("slab_ctx")
     if slab_output == "slab":
         raise NotImplementedError("deploy.export: a model file holds the whole map on rank 0 (slab_output='root'); "
@@ -200,10 +216,11 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     with torch.cuda.device(dev), torch.no_grad():
         _lib._RECORDING.recorder = rec
         try:
-            ent = model._build(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"],
-                               classes=model._class_key(inv_map, confidence, slab is not None), capture=False)
+            ent = model._build(B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"],
+                               classes=model._class_key(inv_map, confidence, slab is not None), capture=False,
+                               depth_items=depth_items)
             plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
-            plan.pix_z = torch.zeros(pix.shape[2], dtype=torch.float64, device=dev)
+            plan.pix_z = torch.zeros(pix.shape[0], pix.shape[2], dtype=torch.float64, device=dev)
             state = getattr(plan, "flosp_state", None)
             tensors = []
             for op in plan.ops:
@@ -280,16 +297,19 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     out_dims = tuple(out.shape[-3:]) if out is not None else tuple(int(s) for s in model.full_scene_size)
     hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
                               1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0)
-                              | (FLAG_CONF if confidence else 0) | (FLAG_SLAB if slab is not None else 0),
+                              | (FLAG_CONF if confidence else 0) | (FLAG_SLAB if slab is not None else 0)
+                              | (FLAG_BATCH if batched else 0),
                               f["V"], f["H"], f["W"], model.project_scale),
            struct.pack("<7I", *S, *out_dims, f["P"]), pattern.astype("<i4").tobytes(),
            struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
                        *[float(v) for v in f["scene_size"]]),
            struct.pack("<2I", model.n_classes, 0 if lut is None else 1), lut_arr.astype("<i4").tobytes(),
-           struct.pack("<d3I", float(f["virtual_bf"]), *(depth0.shape if depth0 is not None else (0, 0)), n_cams),
+           struct.pack("<d3I", float(f["virtual_bf"]), *(depth0.shape[-2:] if depth0 is not None else (0, 0)), n_cams),
            struct.pack("<3I", *vn),
            G.astype("<f4").tobytes(), struct.pack("<I", img_cl.cstride)]
     hdr += [struct.pack("<iQQ", *r) for r in roles]
+    if batched:
+        hdr.append(struct.pack("<I", B))
     if slab is not None:
         # rank, world, every rank's [lo, hi) of the lift grid, this rank's index window, its staged view, the whole
         # map's X extent
@@ -399,6 +419,32 @@ class LoadedModel:
         _lib.check(_lib.lib().occd_model_info(self.handle, C.byref(g)), "occd_model_info")
         return g
 
+    def batch(self):
+        """frames per run: B of a file exported from a list of frames, 1 otherwise"""
+        b = C.c_int()
+        _lib.check(_lib.lib().occd_model_batch(self.handle, C.byref(b)), "occd_model_batch")
+        return b.value
+
+    def run_frames(self, frames, out=None, stream=None, graph=True, conf=None):
+        """1..B frames (as OccDepth.predict_frames takes them) through occd_model_run_frames -> uint16 [n, X, Y, Z] on
+        the current device, or (map, conf) with `conf` (a float16 [n, X, Y, Z] device tensor, or True)"""
+        n = len(frames)
+        calls = [_frame_call(self.geom, fr, None, None, graph, None, False) for fr in frames]
+        fa = (_lib.Frame * n)(*[c[0] for c in calls])
+        dev = calls[0][1][0].device                 # the first frame's images, on the device
+        if out is None:
+            out = torch.empty(n, self.geom.X, self.geom.Y, self.geom.Z, dtype=torch.uint16, device=dev)
+        if conf is True:
+            conf = torch.empty(out.shape, dtype=torch.float16, device=dev)
+        assert out.dtype == torch.uint16 and out.is_contiguous() and out.shape[0] == n
+        if conf is not None:
+            assert conf.dtype == torch.float16 and conf.is_contiguous() and conf.shape == out.shape
+        keep = [c[1] for c in calls]
+        st = _stream_for(stream, [t for c in keep for t in c if isinstance(t, torch.Tensor)] + [out, conf])
+        _lib.check(_lib.lib().occd_model_run_frames(self.handle, fa, n, _ptr(out), _ptr(conf), st),
+                   "occd_model_run_frames")
+        return out if conf is None else (out, conf)
+
     def run_frame(self, frame, out=None, stream=None, graph=True, conf=None):
         """frame: as OccDepth.predict_frame takes it (the uint8 images may be on the host or the device) -> the
         uint16 class map [1, X, Y, Z] on the current device, enqueued on `stream` (default: the current stream).
@@ -486,9 +532,15 @@ def _frame_call(g, frame, out, stream, graph, conf, root):
             conf = torch.empty(1, g.X, g.Y, g.Z, dtype=torch.float16, device=img.device)
         if conf is not None:
             assert conf.dtype == torch.float16 and conf.is_cuda and conf.is_contiguous() and conf.numel() == out.numel()
+    return f, keep, out, conf, _stream_for(stream, [k for k in keep if isinstance(k, torch.Tensor)] + [out, conf])
+
+
+def _stream_for(stream, tensors):
+    """the launch stream of a run; on a stream of the caller's, the inputs copied and outputs allocated on the current
+    stream must live until that stream is done"""
     if stream is not None:
-        # the inputs were copied and `out` allocated on the current stream; they must live until `stream` is done
         stream.wait_stream(torch.cuda.current_stream())
-        for t in [k for k in keep if isinstance(k, torch.Tensor)] + [t for t in (out, conf) if t is not None]:
-            t.record_stream(stream)
-    return f, keep, out, conf, C.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
+        for t in tensors:
+            if t is not None:
+                t.record_stream(stream)
+    return C.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)

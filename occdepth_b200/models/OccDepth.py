@@ -144,11 +144,13 @@ class OccDepth(_Base, B200Module):
             raise NotImplementedError(f"{self.trans_2d_to_3d} is not supported yet.")
 
     # ------------------------------------------------------------------------------------------
-    def _build(self, B, V, H, W, N, P, dev, batch, classes=None, capture=True):
+    def _build(self, B, V, H, W, N, P, dev, batch, classes=None, capture=True, depth_items=False):
         """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut, *options): the
         plan of predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor).  Options:
         "conf" -- `out` is uint16 [2, B, X, Y, Z], the map then the float16 bits of its confidence; "root" -- see
-        below.  capture=False: no CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says"""
+        below.  capture=False: no CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says.
+        depth_items: NYU's virtual view reads one depth map per batch item (a [B, dh, dw] buffer; predict_frames of
+        independent frames) instead of item 0's for the whole batch, as the reference's tensor batches do"""
         slab = self.__dict__.get("slab_ctx")
         plan = Plan(dev, slab=slab, precision=self.precision)
         ps = self.project_scale
@@ -220,14 +222,20 @@ class OccDepth(_Base, B200Module):
         if virtual:
             L = _lib.lib()
             gd = batch["gt_depth"]
-            depth0 = torch.zeros(gd.shape[2], gd.shape[3], dtype=torch.float32, device=dev)
+            dh, dw = gd.shape[2], gd.shape[3]
+            depth0 = torch.zeros(((B,) if depth_items else ()) + (dh, dw), dtype=torch.float32, device=dev)
             bf = float(batch["virtual_bf"][0])
             for s in scales:
                 vb = views[s]
                 _, _, h_s, w_s, _ = vb.shape
+                if depth_items:
+                    plan.add(FnOp(lambda st, vb=vb, h_s=h_s, w_s=w_s, s=s: L.occd_virtual_view_items_fwd(
+                        vb[0].data_ptr(), vb[1].data_ptr(), depth0.data_ptr(), plan.lib_dtype, B, h_s, w_s, Cf, Cp,
+                        Cp, dh, dw, bf / s, dh * dw, st), "virtual_view_1_%d" % s, keep=(vb, depth0)))
+                    continue
                 plan.add(FnOp(lambda st, vb=vb, h_s=h_s, w_s=w_s, s=s: L.occd_virtual_view_fwd(
                     vb[0].data_ptr(), vb[1].data_ptr(), depth0.data_ptr(), plan.lib_dtype, B, h_s, w_s, Cf, Cp, Cp,
-                    depth0.shape[0], depth0.shape[1], bf / s, st), "virtual_view_1_%d" % s, keep=(vb, depth0)))
+                    dh, dw, bf / s, st), "virtual_view_1_%d" % s, keep=(vb, depth0)))
         pix = torch.zeros(B, VL, N, P, 2, dtype=torch.int64, device=dev)
         fov = torch.zeros(B, VL, N, P, dtype=torch.bool, device=dev)
         x3d = plan.alloc(B, S[0], S[1], S[2], self.feature)
@@ -371,27 +379,33 @@ class OccDepth(_Base, B200Module):
             self.__dict__.pop("_build_only", None)
         return self
 
-    def _forward_on(self, batch, key, B, V, H, W, N, P, dev, stage):
-        """batch: what _build reads (shapes, the virtual view, vox_origin); stage(ent) fills the plan's inputs"""
+    def _forward_on(self, batch, key, B, V, H, W, N, P, dev, stage, n=None, depth_items=False):
+        """batch: what _build reads (shapes, the virtual view, vox_origin); stage(ent) fills the plan's inputs.
+        n: items [0, n) of every output (a short list of camera frames through a B-frame plan)"""
         ent = self._plans().get(key)
         if ent is None:
             self._plans().clear()              # weights changed / new shape: drop the stale snapshot
             with torch.no_grad():
-                ent = self._build(B, V, H, W, N, P, dev, batch)
+                ent = self._build(B, V, H, W, N, P, dev, batch, depth_items=depth_items)
             self._plans()[key] = ent
         if self.__dict__.get("_build_only"):
             return None
         stage(ent)
         ent[0].run()
-        return self._outputs(ent)
+        res = self._outputs(ent)
+        if n is not None and n != B:
+            res = {k: (v[:n] if isinstance(v, torch.Tensor) and v.dim() and v.shape[0] == B else v)
+                   for k, v in res.items()}
+        return res
 
-    def _classes_on(self, batch, key, B, V, H, W, N, P, dev, classes, stage):
+    def _classes_on(self, batch, key, B, V, H, W, N, P, dev, classes, stage, n=None, depth_items=False):
+        """n: return items [0, n) of the class map (a short list of camera frames through a B-frame plan)"""
         cache = self._class_plans()
         ent = cache.get(key)
         if ent is None:
             cache.clear()                      # one class-map plan: weights, shapes or inv_map changed
             with torch.no_grad():
-                ent = self._build(B, V, H, W, N, P, dev, batch, classes=classes)
+                ent = self._build(B, V, H, W, N, P, dev, batch, classes=classes, depth_items=depth_items)
             cache[key] = ent
         if self.__dict__.get("_build_only"):
             return None
@@ -399,14 +413,15 @@ class OccDepth(_Base, B200Module):
         ent[0].run()
         if ent[4] is None:                     # slab_output="root" on a rank other than 0
             return None
+        n = B if n is None else n
         if "conf" in classes[2:]:              # uint16 [2, ...]: the map, then the confidence's float16 bits
-            return ent[4][0].clone(), ent[4][1].clone().view(torch.float16)
-        return ent[4].clone()                  # the map lives in a plan-owned static buffer
+            return ent[4][0, :n].clone(), ent[4][1, :n].clone().view(torch.float16)
+        return ent[4][:n].clone()              # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
         """copy this batch's inputs into the static input buffers of plan entry `ent`"""
         plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
-        plan.calib_mark = None                 # the index buffers no longer hold a camera frame's calibration
+        plan.calib_mark = None                 # the index buffers no longer hold camera frames' calibrations
         B, V, _, H, W = img.shape
         CL.from_planar(img.reshape(B * V, 3, H, W) if view_sel is None else img[:, view_sel].reshape(B, 3, H, W),
                        out=img_cl)
@@ -556,30 +571,116 @@ class OccDepth(_Base, B200Module):
                     vox_origin=vox_origin, depth=depth, virtual=depth is not None, virtual_bf=bf, batch=batch,
                     calib=calib)
 
-    def _stage_frame(self, ent, f):
-        """the device side of predict_frame: stage frame `f` into the static input buffers of plan entry `ent`"""
+    def _stage_frame(self, ent, f, b=0):
+        """the device side of predict_frame / predict_frames: stage frame `f` into batch item b of the static input
+        buffers of plan entry `ent`.  The item's indices and camera tables are recomputed only when its calibration
+        differs from what the item's own buffers hold"""
         from .. import data as D
         plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
-        imgs = f["imgs"] if view_sel is None else f["imgs"][view_sel:view_sel + 1]
-        D.stage_rgb_u8(imgs, img_cl.buf, img_cl.lib_dtype, f["H"], f["W"])
-        if depth0 is not None:
-            if tuple(f["depth"].shape) != tuple(depth0.shape):
-                raise ValueError("OccDepth.predict_frame: depth map %r, the plan holds %r"
-                                 % (tuple(f["depth"].shape), tuple(depth0.shape)))
-            D.depth_u16_to_f32(f["depth"], depth0)
-        if f["calib"] is not None and f["calib"] == getattr(plan, "calib_mark", None):
-            return                              # same calibration: the indices and camera tables are in place
+        B = pix.shape[0]
+        if getattr(plan, "calib_mark", None) is None:
+            plan.calib_mark = [None] * B         # per item: the calibration its index buffers hold
         if getattr(plan, "pix_z", None) is None:
-            plan.pix_z = torch.empty(pix.shape[2], dtype=torch.float64, device=pix.device)   # vox2pix's depth output
+            plan.pix_z = torch.empty(B, pix.shape[2], dtype=torch.float64, device=pix.device)   # vox2pix's depths
+        imgs = f["imgs"] if view_sel is None else f["imgs"][view_sel:view_sel + 1]
+        n_img = imgs.shape[0]
+        D.stage_rgb_u8(imgs, img_cl.buf[b * n_img:(b + 1) * n_img], img_cl.lib_dtype, f["H"], f["W"])
+        if depth0 is not None:
+            d = depth0 if depth0.dim() == 2 else depth0[b]
+            if tuple(f["depth"].shape) != tuple(d.shape):
+                raise ValueError("OccDepth.predict_frame: depth map %r, the plan holds %r"
+                                 % (tuple(f["depth"].shape), tuple(d.shape)))
+            D.depth_u16_to_f32(f["depth"], d)
+        if f["calib"] is not None and f["calib"] == plan.calib_mark[b]:
+            return                              # same calibration: the indices and camera tables are in place
         # under the slab partition the index buffers hold this rank's window [n_lo, n_lo + N) of the lift's X-major
         # voxel order: the rank computes that window only, for every pose (NYU's virtual view too)
         window = None if plan.x_range is None else (n_lo, pix.shape[2])
         for v, (E, K) in enumerate(f["poses"]):
-            D.vox2pix_into(pix[0, v], fov[0, v], plan.pix_z, E, K, f["vox_origin"], f["voxel_size"], f["W"], f["H"],
+            D.vox2pix_into(pix[b, v], fov[b, v], plan.pix_z[b], E, K, f["vox_origin"], f["voxel_size"], f["W"], f["H"],
                            f["scene_size"], f["pattern_id"], voxel_range=window)
         if self.trans_2d_to_3d == "flosp_depth":
-            self.flosp_depth.stage_inputs(f["batch"], pix.device, plan.flosp_state)
-        plan.calib_mark = f["calib"]
+            self.flosp_depth.stage_inputs(f["batch"], pix.device, plan.flosp_state, item=b)
+        plan.calib_mark[b] = f["calib"]
+
+    # ---- batches of camera frames ----------------------------------------------------------------------------------
+    def predict_frames(self, frames, classes=True, inv_map=None, confidence=False):
+        """A list of 1..B camera frames (each what predict_frame takes) through one B-frame plan, B = len(frames): the
+        uint16 class maps [n, X, Y, Z] (with `confidence`: (map, conf)), or with classes=False the forward's output dict
+        with a leading n.  Every frame's result is bit for bit predict_frame's of that frame alone.
+
+        The frames must agree on the image count V, the crop `img_hw`, the grid geometry (voxel_size, scene_size,
+        pattern_id) and whether there is a depth map; calibration, pose, NYU's vox_origin and the raw image sizes may
+        differ (each frame's images are staged by their own launch).  NYU's virtual view reads each frame's own depth
+        map (all of the size the plan was built with).  One plan is cached per batch size and request; each batch item
+        keeps the calibration its index buffers hold, so a KITTI sequence computes the indices once per item.  Not
+        under enable_slab_parallel with more than one frame, nor for NYU with the FlospDepth prior with more than one
+        (its grid is rebuilt from item 0's vox_origin)."""
+        fs = self._frames_checked(frames, classes, confidence)
+        return self._run_frames(fs, len(fs), classes, inv_map, confidence)
+
+    def _frames_checked(self, frames, classes=True, confidence=False, batch=None, inputs=True):
+        """the refusals of predict_frames (host-side, before any frame is moved), then -- with `inputs` -- the frames
+        through `_frame_checked`"""
+        if isinstance(frames, dict) or not isinstance(frames, (list, tuple)):
+            raise TypeError("OccDepth.predict_frames: frames must be a list of frame dicts")
+        n = len(frames)
+        if n < 1 or (batch is not None and n > batch):
+            raise ValueError("OccDepth.predict_frames: %d frames, expected 1 to %s" % (n, "any" if batch is None
+                                                                                       else batch))
+        if confidence and not classes:
+            raise ValueError("OccDepth.predict_frames: confidence=True is the class map's confidence (classes=True)")
+        B = n if batch is None else batch
+        if self.__dict__.get("slab_ctx") is not None and B > 1:
+            raise NotImplementedError("OccDepth.predict_frames: the slab partition runs one frame per forward (batch "
+                                      "size 1), got %d" % B)
+        if self.infer_mode and self.trans_2d_to_3d == "flosp_depth":
+            raise NotImplementedError("OccDepth.predict_frames: infer_mode with flosp_depth takes the caller's sampling "
+                                      "grids, not camera matrices; use forward / predict_classes with a tensor batch")
+        if self.dataset == "NYU" and self.trans_2d_to_3d == "flosp_depth" and B > 1:
+            raise NotImplementedError("OccDepth.predict_frames: NYU with the FlospDepth prior rebuilds its grid from "
+                                      "item 0's vox_origin, so it runs one frame per call (no shipped configuration "
+                                      "uses it)")
+        sig0 = self._frame_signature(frames[0])
+        for i, fr in enumerate(frames[1:], 1):
+            sig = self._frame_signature(fr)
+            for k in sig0:
+                if sig[k] != sig0[k]:
+                    raise ValueError("OccDepth.predict_frames: frame %d's %s is %r, frame 0's %r (the frames of one "
+                                     "call share it)" % (i, k, sig[k], sig0[k]))
+        return [self._frame_checked(fr, None, classes) for fr in frames] if inputs else None
+
+    def _frame_signature(self, frame):
+        """what the frames of one predict_frames call must share, read on the host with predict_frame's defaults"""
+        nyu = self.dataset == "NYU"
+        shape = tuple(getattr(frame["img"], "shape", ()))
+        V = 1 if len(shape) == 3 else shape[-4] if len(shape) >= 4 else None
+        return {"V": V,
+                "img_hw": tuple(int(v) for v in frame.get("img_hw", (480, 640) if nyu else (370, 1220))),
+                "voxel_size": float(frame.get("voxel_size", 0.08 if nyu else 0.2 * self.project_scale)),
+                "scene_size": tuple(float(v) for v in frame.get("scene_size", (4.8, 4.8, 2.88) if nyu
+                                                                 else (51.2, 51.2, 6.4))),
+                "pattern_id": int(frame.get("pattern_id", 0)),
+                "depth": frame.get("depth") is not None}
+
+    def _run_frames(self, fs, B, classes, inv_map, confidence=False):
+        """frames fs (from _frames_checked) through the B-frame plan, B >= len(fs): the results of items [0, len(fs));
+        items [len(fs), B) keep what their buffers hold"""
+        f = fs[0]
+        dev = f["imgs"].device
+        depth_items = f["virtual"] and B > 1
+        # only a batch of camera frames with per-item depth maps gets a key of its own: every other plan is the one a
+        # tensor batch of the same shapes uses
+        key = self._plan_key(B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"]) \
+            + (("depth_items",) if depth_items else ())
+        stage = lambda ent: [self._stage_frame(ent, f, b) for b, f in enumerate(fs)]     # noqa: E731
+        with torch.cuda.device(dev):
+            if classes:
+                cls = self._class_key(inv_map, confidence)
+                return self._classes_on(f["batch"], key + cls, B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
+                                        stage, n=len(fs), depth_items=depth_items)
+            return self._forward_on(f["batch"], key, B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage,
+                                    n=len(fs), depth_items=depth_items)
 
     # ---- the occupied-voxel list: what every consumer of a class map builds from it first ----------------------
     def predict_voxels(self, batch_or_frame, inv_map=None, fov_mask=None, capacity=None, voxel_size=None,

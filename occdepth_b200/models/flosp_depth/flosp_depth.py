@@ -224,9 +224,9 @@ class FlospDepth(B200Module):
         """input buffers and depth distribution of the plan the last emit() built"""
         return self.__dict__["_state"]
 
-    def stage_inputs(self, batch, dev, state=None):
+    def stage_inputs(self, batch, dev, state=None, item=None):
         """copy this batch's camera tables (or infer_mode grids) into the buffers of `state` (default: the plan the
-        last emit() built)"""
+        last emit() built); item: a one-frame batch's tables go to that batch item of the plan"""
         state = self.plan_state() if state is None else state
         if self.infer_mode:
             g = state["grids"]
@@ -245,8 +245,13 @@ class FlospDepth(B200Module):
             # NYU: the voxel counts are re-derived from batch item 0's vox_origin every forward (flosp_depth.py:466-518)
             raise RuntimeError("FlospDepth: this batch's vox_origin gives a %r voxel grid, the plan was built for %r; "
                                "call invalidate_plans()" % (tuple(vn), state["vn"]))
-        state["cams"].copy_(cams, non_blocking=True)
-        state["sps"].copy_(sps, non_blocking=True)
+        if item is None:
+            state["cams"].copy_(cams, non_blocking=True)
+            state["sps"].copy_(sps, non_blocking=True)
+        else:
+            n = state["n_cams"]
+            state["cams"][item:item + 1].copy_(cams, non_blocking=True)
+            state["sps"][item * n:(item + 1) * n].copy_(sps, non_blocking=True)
 
     def depth_prob(self, state=None):
         return (self.plan_state() if state is None else state)["prob"]

@@ -152,11 +152,22 @@ class CameraPipeline:
     `output="voxels"` lists every frame's occupied voxels on the device (`OccDepth.predict_voxels`) and reads back the
     counts, the class histogram and the first `capacity` rows (flat index, class, voxel centre: 18 bytes a row; default
     capacity an eighth of the output grid) instead of the class map; `result(ticket)` trims them to the rows written
-    and says whether the frame held more (`truncated`).  `d2h_bytes` is what a frame reads back."""
+    and says whether the frame held more (`truncated`).  `d2h_bytes` is what a frame reads back.
+
+    `batch=B` runs `OccDepth.predict_frames` instead: `submit` takes a list of 1..B frames, copies them into B-frame
+    pinned and device buffers (each frame's slice sized from its own image) and runs the B-frame plan; `result(ticket)`
+    returns that submit's n maps [n, X, Y, Z] (or (map, conf)).  A short list -- the last of a stream -- runs the same
+    plan, and only its n results are read back.  Not with output="voxels" or slab_output."""
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
                  inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None,
-                 confidence=False):
+                 confidence=False, batch=None):
+        if batch is not None:
+            if isinstance(batch, bool) or not isinstance(batch, int) or batch < 1:
+                raise ValueError("CameraPipeline: batch must be None or a frame count >= 1, got %r" % (batch,))
+            if output is not None or slab_output is not None:
+                raise ValueError("CameraPipeline: batch=%d runs whole class maps (or logits) of unpartitioned plans; "
+                                 "output='voxels' and slab_output are not batched" % batch)
         if not torch.cuda.is_available():
             raise RuntimeError("CameraPipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         if output not in (None, "voxels"):
@@ -189,7 +200,9 @@ class CameraPipeline:
                 self.geometry[k] = v
         self.main = torch.cuda.current_stream(dev)
         self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
-        self.bufs = {"img": [None, None], "depth": [None, None]}     # (pinned host, device) flat byte buffers
+        self.bufs = {}                # name -> two (pinned host, device) flat byte buffers
+        self.batch = batch
+        self.counts = [0, 0]          # batch: the frames each result buffer holds
         self.dev_out, self.host_out = [None, None], [None, None]
         self.in_ready, self.in_free, self.host_free, self.out_ready, self.out_free = (
             [torch.cuda.Event(), torch.cuda.Event()] for _ in range(5))
@@ -223,7 +236,7 @@ class CameraPipeline:
         """copy host tensor x into pinned buffer j (once its previous H2D has finished), enqueue the H2D copy into
         device buffer j; returns the device view of x's shape"""
         nb = x.numel() * x.element_size()
-        buf = self.bufs[name][j]
+        buf = self.bufs.setdefault(name, [None, None])[j]
         if buf is None or buf[0].numel() < nb:
             torch.cuda.synchronize(self.dev)      # a larger raw image: nothing may still read the old buffers
             buf = (torch.empty(nb, dtype=torch.uint8).pin_memory(), torch.empty(nb, dtype=torch.uint8, device=self.dev))
@@ -236,8 +249,11 @@ class CameraPipeline:
         return dev
 
     def submit(self, frame):
-        """enqueue one camera frame (host arrays / tensors, see the class docstring).  Returns the ticket of the frame
-        submitted before this one -- its read-back overlaps this frame's forward -- or None."""
+        """enqueue one camera frame (host arrays / tensors, see the class docstring), or with `batch` a list of 1..B
+        frames.  Returns the ticket of the submit before this one -- its read-back overlaps this one's forward -- or
+        None."""
+        if self.batch is not None:
+            return self._submit_batch(frame)
         img = self._host(frame["img"], "img")
         if img.dim() == 5:
             if img.shape[0] != 1:
@@ -289,6 +305,57 @@ class CameraPipeline:
         self.n += 1
         return self.n - 2 if self.n >= 2 else None
 
+    def _submit_batch(self, frames):
+        """submit for batch=B: the frames' images (and depth maps) into slot j's per-item buffers, predict_frames'
+        B-frame plan, and the read-back of the first n results"""
+        m = self.model
+        fs = [dict(self.geometry, **fr) for fr in frames] if isinstance(frames, (list, tuple)) else frames
+        m._frames_checked(fs, self.classes, self.confidence, batch=self.batch, inputs=False)   # nothing moved yet
+        n = len(fs)
+        j = self.n & 1
+        self.host_free[j].synchronize()           # pinned buffers j: their previous H2D copies have been read
+        self.h2d_bytes = 0
+        with torch.cuda.stream(self.h2d):
+            self.h2d.wait_event(self.in_free[j])
+            for i, f in enumerate(fs):
+                img = self._host(f["img"], "img")
+                if img.dim() == 5:
+                    if img.shape[0] != 1:
+                        raise NotImplementedError("CameraPipeline.submit: frame %d holds %d frames; give one dict per "
+                                                  "frame" % (i, img.shape[0]))
+                    img = img[0]
+                f["img"] = self._stage_h2d("img%d" % i, j, img)
+                if f.get("depth") is not None:
+                    f["depth"] = self._stage_h2d("depth%d" % i, j, self._host(f["depth"], "depth"))
+            self.in_ready[j].record(self.h2d)
+            self.host_free[j].record(self.h2d)
+        self.main.wait_event(self.in_ready[j])
+        with torch.no_grad():
+            res = m._run_frames([m._frame_checked(f, None, self.classes) for f in fs], self.batch, self.classes,
+                                self.inv_map, self.confidence)
+        self.in_free[j].record(self.main)
+        if not self.classes:
+            res = res[self.out_key]
+        parts = list(res) if self.confidence else [res]
+        shape = (len(parts), self.batch) + tuple(parts[0].shape[1:])
+        if self.dev_out[j] is None or tuple(self.dev_out[j].shape) != shape:
+            self.out_free[j].synchronize()
+            self.dev_out[j] = torch.empty(shape, dtype=torch.uint16 if self.classes else parts[0].dtype,
+                                          device=self.dev)
+            self.host_out[j] = torch.empty(shape, dtype=self.dev_out[j].dtype).pin_memory()
+        self.main.wait_event(self.out_free[j])
+        for k, p in enumerate(parts):   # the results leave the allocator-owned tensors on the compute stream
+            self.dev_out[j][k, :n].copy_(p.view(torch.uint16) if p.dtype == torch.float16 else p)
+        self.out_ready[j].record(self.main)
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(self.out_ready[j])
+            for k in range(len(parts)):
+                self.host_out[j][k, :n].copy_(self.dev_out[j][k, :n], non_blocking=True)
+            self.out_free[j].record(self.d2h)
+        self.counts[j] = n
+        self.n += 1
+        return self.n - 2 if self.n >= 2 else None
+
     def _submit_voxels(self, f, j):
         """the tail of submit for output="voxels": list the frame into device list j, then read back the counts, the
         histogram and the first `capacity` rows in one batch of copies -- the host learns the count from that same
@@ -332,6 +399,9 @@ class CameraPipeline:
             return None
         j = ticket & 1
         self.out_free[j].synchronize()
+        if self.batch is not None:
+            h = self.host_out[j][:, :self.counts[j]]
+            return (h[0], h[1].view(torch.float16)) if self.confidence else h[0]
         if self.output == "voxels":
             h = {k: v.numpy() for k, v in self.host_out[j].items()}
             count = h["count"].astype("int64")

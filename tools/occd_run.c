@@ -14,7 +14,10 @@
  *   DEPTH   (NYU models with the virtual view) N x depth_h x depth_w uint16, the depth PNGs' values
  * Output: OUT_DIR/NNNNNN.label per frame, the uint16 class map (X x Y x Z, C order) as the KITTI submission writer
  * stores it; the labels are remapped when the model was exported with inv_map.  Prints ms per frame (device time
- * of occd_model_run_frame, from CUDA events) and the mean over the frames after the first.
+ * of occd_model_run_frames, from CUDA events) and the mean over the frames after the first.
+ *
+ * A batched model file (deploy.export of a list of B frames) runs the frames in groups of B, the last group short;
+ * the times are then per group, and the mean is per frame over the groups after the first.
  *
  * X-slab partition over W GPUs: one process per rank, each on its own device (e.g. CUDA_VISIBLE_DEVICES), MODEL the
  * rank's file (deploy.export(..., slab_output="root")) and the same inputs on every rank.  Rank 0 writes the NCCL id
@@ -127,6 +130,8 @@ int main(int argc, char** argv) {
   }
   occd_model_geom g;
   OK(occd_model_info(m, &g));
+  int B = 1;
+  OK(occd_model_batch(m, &B));
   if (!H0) {
     H0 = g.img_h;
     W0 = g.img_w;
@@ -147,61 +152,78 @@ int main(int argc, char** argv) {
     fprintf(stderr, "occd_run: cannot open the input files\n");
     return 1;
   }
-  unsigned char* h_img = (unsigned char*)malloc(img_bytes);
-  unsigned short* h_depth = (unsigned short*)malloc(depth_bytes ? depth_bytes : 1);
-  unsigned short* h_map = (unsigned short*)malloc(map_bytes);
-  double* calib = (double*)malloc(n_calib * sizeof(double));
+  unsigned char* h_img = (unsigned char*)malloc(img_bytes * B);
+  unsigned short* h_depth = (unsigned short*)malloc(depth_bytes ? depth_bytes * B : 1);
+  unsigned short* h_map = (unsigned short*)malloc(map_bytes * B);
+  double* calib = (double*)malloc(n_calib * sizeof(double) * B);
+  occd_frame* fs = (occd_frame*)calloc(B, sizeof(occd_frame));
   void *d_img, *d_depth = NULL, *d_map;
   cudaStream_t st;
   cudaEvent_t e0, e1;
-  CK(cudaMalloc(&d_img, img_bytes));
-  CK(cudaMalloc(&d_map, map_bytes));
-  if (g.has_depth) CK(cudaMalloc(&d_depth, depth_bytes));
+  CK(cudaMalloc(&d_img, img_bytes * B));
+  CK(cudaMalloc(&d_map, map_bytes * B));
+  if (g.has_depth) CK(cudaMalloc(&d_depth, depth_bytes * B));
   CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
   double total = 0;
-  for (int i = 0; i < n; ++i) {
-    if (!read_exact(fi, h_img, img_bytes, "IMAGES") || !read_exact(fc, calib, n_calib * 8, "CALIB") ||
-        (fd && !read_exact(fd, h_depth, depth_bytes, "DEPTH")))
-      return 1;
-    CK(cudaMemcpyAsync(d_img, h_img, img_bytes, cudaMemcpyHostToDevice, st));
-    if (fd) CK(cudaMemcpyAsync(d_depth, h_depth, depth_bytes, cudaMemcpyHostToDevice, st));
-    occd_frame f;
-    memset(&f, 0, sizeof(f));
-    f.images = d_img;
-    f.img_stride = (long long)H0 * W0 * 3;
-    f.row_stride = (long long)W0 * 3;
-    f.H0 = H0;
-    f.W0 = W0;
-    f.cam_k = calib;
-    f.pose = nyu ? calib + 9 : calib + 9 * g.V;
-    f.calib_f32 = 0;
-    f.vox_origin = nyu ? calib + 25 : NULL;
-    f.depth = (const uint16_t*)d_depth;
-    f.depth_h = g.depth_h;
-    f.depth_w = g.depth_w;
-    f.flags = flags;
+  int groups = 0;
+  for (int i0 = 0; i0 < n; i0 += B) {
+    const int k = n - i0 < B ? n - i0 : B;
+    for (int i = 0; i < k; ++i) {
+      unsigned char* img = h_img + img_bytes * i;
+      unsigned short* depth = h_depth + (depth_bytes / 2) * i;
+      double* cal = calib + n_calib * i;
+      if (!read_exact(fi, img, img_bytes, "IMAGES") || !read_exact(fc, cal, n_calib * 8, "CALIB") ||
+          (fd && !read_exact(fd, depth, depth_bytes, "DEPTH")))
+        return 1;
+      CK(cudaMemcpyAsync((char*)d_img + img_bytes * i, img, img_bytes, cudaMemcpyHostToDevice, st));
+      if (fd) CK(cudaMemcpyAsync((char*)d_depth + depth_bytes * i, depth, depth_bytes, cudaMemcpyHostToDevice, st));
+      occd_frame* f = &fs[i];
+      memset(f, 0, sizeof(*f));
+      f->images = (char*)d_img + img_bytes * i;
+      f->img_stride = (long long)H0 * W0 * 3;
+      f->row_stride = (long long)W0 * 3;
+      f->H0 = H0;
+      f->W0 = W0;
+      f->cam_k = cal;
+      f->pose = nyu ? cal + 9 : cal + 9 * g.V;
+      f->calib_f32 = 0;
+      f->vox_origin = nyu ? cal + 25 : NULL;
+      f->depth = d_depth ? (const uint16_t*)((char*)d_depth + depth_bytes * i) : NULL;
+      f->depth_h = g.depth_h;
+      f->depth_w = g.depth_w;
+      f->flags = flags;
+    }
     CK(cudaEventRecord(e0, st));
-    OK(occd_model_run_frame(m, &f, rank == 0 ? (uint16_t*)d_map : NULL, st));
+    OK(occd_model_run_frames(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
     CK(cudaEventRecord(e1, st));
-    if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes, cudaMemcpyDeviceToHost, st));
+    if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes * k, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, e0, e1));
-    if (i > 0) total += ms;
-    if (rank != 0) continue;
-    char path[4096];
-    snprintf(path, sizeof(path), "%s/%06d.label", out_dir, i);
-    FILE* fo = fopen(path, "wb");
-    if (!fo || fwrite(h_map, 1, map_bytes, fo) != map_bytes) {
-      fprintf(stderr, "occd_run: cannot write %s\n", path);
-      return 1;
+    if (i0 > 0) {
+      total += ms / k;
+      ++groups;
     }
-    fclose(fo);
-    printf("frame %d: %.3f ms\n", i, ms);
+    if (rank != 0) continue;
+    for (int i = 0; i < k; ++i) {
+      char path[4096];
+      snprintf(path, sizeof(path), "%s/%06d.label", out_dir, i0 + i);
+      FILE* fo = fopen(path, "wb");
+      if (!fo || fwrite(h_map + (map_bytes / 2) * i, 1, map_bytes, fo) != map_bytes) {
+        fprintf(stderr, "occd_run: cannot write %s\n", path);
+        return 1;
+      }
+      fclose(fo);
+    }
+    if (B == 1) printf("frame %d: %.3f ms\n", i0, ms);
+    else printf("frames %d..%d: %.3f ms\n", i0, i0 + k - 1, ms);
   }
-  if (n > 1) printf("mean over frames 1..%d: %.3f ms per frame\n", n - 1, total / (n - 1));
+  if (groups > 0) {
+    if (B == 1) printf("mean over frames 1..%d: %.3f ms per frame\n", n - 1, total / groups);
+    else printf("mean over groups 1..%d: %.3f ms per frame\n", groups, total / groups);
+  }
   OK(occd_model_destroy(m));
   if (comm) OK(occd_comm_destroy(comm));
   fclose(fi);
@@ -211,6 +233,7 @@ int main(int argc, char** argv) {
   free(h_depth);
   free(h_map);
   free(calib);
+  free(fs);
   cudaFree(d_img);
   cudaFree(d_map);
   if (d_depth) cudaFree(d_depth);
