@@ -281,6 +281,21 @@ int occd_normalize_rgb_u8(const void* in, float* out, int H0, int W0, int H, int
 int occd_stage_rgb_u8_cl(const void* in, long long img_stride, long long row_stride, int n, int H0, int W0, int H,
                          int W, const float* mean, const float* stdv, void* out, int out_dtype, int cstride,
                          void* stream);
+/* the same staging from what cameras and video decoders deliver, bit for bit what OpenCV makes on the host:         */
+/*   OCCD_PIX_RGB  as occd_stage_rgb_u8_cl; OCCD_PIX_BGR  pixels B, G, R (cv::cvtColor COLOR_BGR2RGB);                */
+/*   OCCD_PIX_NV12 a luma plane of H0 rows, then H0/2 rows of interleaved U, V at in + i*img_stride + uv_offset, both */
+/*                 with row_stride (cv::cvtColor COLOR_YUV2RGB_NV12: BT.601 limited range; H0, W0 even).             */
+/* maps (DEVICE float32, or NULL): per image [2][H][W] source x then y of every output pixel, image i's at            */
+/* maps + i*map_stride floats, 4-byte aligned: the converted image is rectified as cv::remap(INTER_LINEAR,           */
+/* BORDER_CONSTANT 0) does, each of the four taps converted first; taps outside H0 x W0 read 0.  The crop H x W is   */
+/* then the maps' size, and H0, W0 < 32767.  Without maps it is the top-left H x W of the image, as for RGB.         */
+#define OCCD_PIX_RGB 0
+#define OCCD_PIX_BGR 1
+#define OCCD_PIX_NV12 2
+int occd_stage_camera_u8_cl(const void* in, int format, long long img_stride, long long row_stride,
+                            long long uv_offset, int n, int H0, int W0, int H, int W, const float* maps,
+                            long long map_stride, const float* mean, const float* stdv, void* out, int out_dtype,
+                            int cstride, void* stream);
 /* NYU's depth map (data/NYU/nyu_dataset.py:42-48 load_depth): out[i] = float32(in[i] / divisor) (the division in   */
 /* float64), clamped to [0, max_depth] in float32; in: n uint16 (device), out: n float32 (device)                  */
 int occd_depth_u16_to_f32(const void* in, float* out, long long n, double divisor, float max_depth, void* stream);
@@ -524,6 +539,18 @@ int occd_model_batch(const occd_model* m, int* batch);
 /* occd_model_run_frame(_conf) with n = 1.                                                                          */
 int occd_model_run_frames(occd_model* m, const occd_frame* frames, int n, uint16_t* class_maps, void* conf,
                           void* stream);
+/* A frame in any camera format of occd_stage_camera_u8_cl.  frame.images holds the V images as that format lays     */
+/* them out: OCCD_PIX_RGB / OCCD_PIX_BGR (V, H0, W0, 3); OCCD_PIX_NV12 each image's luma rows (H0 x W0 bytes,         */
+/* H0 and W0 even), its interleaved U, V rows at images + i*img_stride + uv_offset, both with row_stride.  A model    */
+/* exported with rectification maps (DESIGN.md section 9) remaps every frame with them; the crop is then the maps'. */
+typedef struct {
+  occd_frame frame;
+  int pixel_format;             /* OCCD_PIX_*                                                               */
+  long long uv_offset;          /* NV12: bytes from an image's first luma row to its chroma plane           */
+} occd_frame_ex;
+/* occd_model_run_frames for frames of any camera format; occd_model_run_frame(s/_conf) are this call with RGB.      */
+int occd_model_run_frames_ex(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps, void* conf,
+                             void* stream);
 int occd_model_destroy(occd_model* m);
 
 /* Model files under the X-slab partition (DESIGN.md section 9): one file per rank, each holding that rank's plan of */

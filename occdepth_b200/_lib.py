@@ -14,6 +14,8 @@ _LIB = None
 MAX_SCALES = 4
 DTYPE_F32, DTYPE_BF16 = 0, 1
 DTYPE_U8, DTYPE_U16, DTYPE_I64 = 2, 3, 4
+PIX_RGB, PIX_BGR, PIX_NV12 = 0, 1, 2
+PIXEL_FORMATS = {"rgb": PIX_RGB, "bgr": PIX_BGR, "nv12": PIX_NV12}
 SFA_OUT_F32_PLANAR, SFA_OUT_BF16_CL, SFA_OUT_F32_CL, SFA_OUT_TF32_CL = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU, ACT_SIGMOID = 0, 1, 2, 3, 4
 
@@ -69,6 +71,11 @@ class Frame(C.Structure):
                 ("calib_f32", C.c_int), ("vox_origin", C.c_void_p), ("scene_size", C.c_void_p),
                 ("voxel_size", C.c_double), ("depth", C.c_void_p), ("depth_h", C.c_int), ("depth_w", C.c_int),
                 ("flags", C.c_int)]
+
+
+class FrameEx(C.Structure):
+    """occd_frame_ex"""
+    _fields_ = [("frame", Frame), ("pixel_format", C.c_int), ("uv_offset", C.c_longlong)]
 
 
 class ConvTap(C.Structure):
@@ -136,6 +143,8 @@ SYMBOLS = {
     "occd_argmax_classes_conf": (C.c_int, [_vp, _vp, _vp, _ll, _i, _ll, _vp, _vp]),
     "occd_normalize_rgb_u8": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "occd_stage_rgb_u8_cl": (C.c_int, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
+    "occd_stage_camera_u8_cl": (C.c_int, [_vp, _i, _ll, _ll, _ll, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _i,
+                                          _i, _vp]),
     "occd_depth_u16_to_f32": (C.c_int, [_vp, _vp, _ll, C.c_double, _f, _vp]),
     "occd_vox2pix_fwd": (C.c_int, [_vp, _i, _vp, _vp, C.c_double, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     "occd_vox2pix_range_fwd": (C.c_int, [_vp, _i, _vp, _vp, C.c_double, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp,
@@ -170,6 +179,7 @@ SYMBOLS = {
     "occd_model_run_frame_conf": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp, _vp]),
     "occd_model_batch": (C.c_int, [_vp, C.POINTER(C.c_int)]),
     "occd_model_run_frames": (C.c_int, [_vp, C.POINTER(Frame), _i, _vp, _vp, _vp]),
+    "occd_model_run_frames_ex": (C.c_int, [_vp, C.POINTER(FrameEx), _i, _vp, _vp, _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "occd_comm_halo_exchange": (C.c_int, [_vp, _vp, _ll, _i, _i, _vp]),

@@ -122,11 +122,11 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_crp_relation_sums),     OCCD_ENTRY(occd_depth_cls_sums),
     OCCD_ENTRY(occd_occupied_voxels),       OCCD_ENTRY(occd_virtual_view_fwd),
     OCCD_ENTRY(occd_vox2pix_range_fwd),     OCCD_ENTRY(occd_argmax_classes_conf),
-    OCCD_ENTRY(occd_virtual_view_items_fwd),
+    OCCD_ENTRY(occd_virtual_view_items_fwd), OCCD_ENTRY(occd_stage_camera_u8_cl),
     // take a stream like the launches (occd_model_batch is bound like them), so they have a signature here; their
     // model handle can only be NULL
     OCCD_ENTRY(occd_model_run_frame_conf),  OCCD_ENTRY(occd_model_run_frames),
-    OCCD_ENTRY(occd_model_batch),
+    OCCD_ENTRY(occd_model_batch),           OCCD_ENTRY(occd_model_run_frames_ex),
     // the X-slab partition's collectives: the lock-step runner of a local group stops after each
     OCCD_ENTRY(occd_comm_halo_exchange),    OCCD_ENTRY(occd_comm_all_gather),
     OCCD_ENTRY(occd_comm_gather_root),
@@ -146,10 +146,11 @@ enum Role { ROLE_IMG, ROLE_PIX, ROLE_FOV, ROLE_PIX_Z, ROLE_DEPTH, ROLE_CAMS, ROL
 const char* kRoleNames[N_ROLES] = {"image", "pix", "fov", "pix_z", "depth", "camera tables", "scaled_pixel_size",
                                    "class map"};
 enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4,   // FLAG_CONF: the class-map role holds the map, then its
-       FLAG_SLAB = 16, FLAG_BATCH = 32 };                        // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
+       FLAG_SLAB = 16, FLAG_BATCH = 32, FLAG_MAPS = 64 };        // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
                                                                  // FLAG_SLAB: one rank's plan, a slab block follows;
                                                                  // FLAG_BATCH: a B-frame plan, a batch block follows
-                                                                 // the roles (bit 3 stays unassigned)
+                                                                 // the roles (bit 3 stays unassigned); FLAG_MAPS: a
+                                                                 // rectification-maps role follows the roles
 const uint32_t kMaxBatch = 1024;
 const uint32_t kMaxWorld = 64;
 const size_t kArenaAlign = 512;  // the caching allocator's block alignment, which the plans were built with
@@ -219,6 +220,7 @@ struct occd_model {
   double voxel_size, vox_origin[3], scene_size[3], virtual_bf;
   float G[16];
   RoleRef roles[N_ROLES];
+  RoleRef maps{-1, 0, 0};  // FLAG_MAPS: the staged views' float32 [2][img_h][img_w] rectification maps
   // sections
   std::vector<uint64_t> buf_size, buf_off;
   std::vector<const uint8_t*> buf_data;  // into `file` (nullptr: zeros); only valid while loading
@@ -238,6 +240,7 @@ struct occd_model {
   std::vector<std::vector<uint8_t>> calib;
   std::vector<char> calib_valid;
   std::vector<float> cams, sps;
+  std::vector<occd_frame_ex> frames_ex;      // the RGB occd_frame_ex of each frame an occd_frame entry point is given
   // the X-slab partition (FLAG_SLAB): this rank, every rank's [lo, hi) planes of the lift grid, this rank's window of
   // the lift's voxel order, the one view it stages (-1: every view) and the whole map's X extent (rank 0's output)
   uint32_t rank = 0, world = 1, map_x = 0;
@@ -252,6 +255,7 @@ struct occd_model {
   // item b's part of an input role, which holds `batch` items of equal length
   void* dev(int role, uint32_t b) const { return static_cast<uint8_t*>(dev(role)) + roles[role].len / batch * b; }
   uint64_t map_bytes() const { return (uint64_t)out[0] * out[1] * out[2] * 2; }   // one uint16 class map
+  void* dev_maps() const { return arena + buf_off[maps.buffer] + maps.off; }
 };
 
 namespace {
@@ -310,6 +314,12 @@ int parse(occd_model* m) {
     m->roles[k].off = r.get<uint64_t>();
     m->roles[k].len = r.get<uint64_t>();
   }
+  if (m->flags & FLAG_MAPS) {
+    m->maps.buffer = r.get<int32_t>();
+    m->maps.off = r.get<uint64_t>();
+    m->maps.len = r.get<uint64_t>();
+    if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (maps role)");
+  }
   if (m->flags & FLAG_BATCH) {
     m->batch = r.get<uint32_t>();
     if (!r.ok) return fail(OCCD_ERR_FORMAT, "occd_model_load: truncated file (batch block)");
@@ -339,7 +349,7 @@ int parse(occd_model* m) {
   if ((m->precision != OCCD_DTYPE_F32 && m->precision != OCCD_DTYPE_BF16) || m->dataset > 1 || m->V < 1 ||
       m->V > 4 || m->P < 1 || m->P > 64 || m->n_cams > 4 || m->img_cstride % 8 != 0)
     return fail(OCCD_ERR_FORMAT, "occd_model_load: header field out of range");
-  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB | FLAG_BATCH))
+  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB | FLAG_BATCH | FLAG_MAPS))
     return fail(OCCD_ERR_FORMAT, "occd_model_load: unknown header flag bits");
   if (m->slab()) {
     // every rank's slab, in rank order, tiles the lift grid's X planes; this rank's window is its slab's voxels
@@ -484,6 +494,16 @@ int parse(occd_model* m) {
       return fail(OCCD_ERR_FORMAT, std::string("occd_model_load: the ") + kRoleNames[k] +
                                        " buffer does not match the header");
   }
+  if (m->flags & FLAG_MAPS) {
+    // one set of maps for every batch item: the staged views' [2][img_h][img_w] float32, 4-byte aligned in the arena
+    const RoleRef& ro = m->maps;
+    if (ro.buffer < 0)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: header flag bit 6 (rectification maps) without a maps buffer");
+    if (!in_buffer((uint32_t)ro.buffer, ro.off, ro.len) || ro.off % 4 != 0 ||
+        ro.len != (uint64_t)(m->view_sel >= 0 ? 1 : m->V) * 2 * m->img_h * m->img_w * 4)
+      return fail(OCCD_ERR_FORMAT, "occd_model_load: the rectification maps buffer does not match the header");
+  }
+  m->frames_ex.assign(m->batch, occd_frame_ex{});
   m->calib.assign(m->batch, std::vector<uint8_t>());
   m->calib_valid.assign(m->batch, 0);
   m->cams.assign((size_t)m->batch * 4 * 40, 0.f);
@@ -606,14 +626,17 @@ void load_as_f32(const void* src, int n, float* dst) {
 
 // the datasets' camera-frame staging (OccDepth._stage_frames) of frame `f` into batch item b: images, depth, and -- for
 // a calibration other than the item's last -- the projection indices and the FlospDepth tables
-int stage(occd_model* m, const occd_frame* f, uint32_t b, cudaStream_t st) {
+int stage(occd_model* m, const occd_frame_ex* fx, uint32_t b, cudaStream_t st) {
   static const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
+  const occd_frame* f = &fx->frame;
   const bool nyu = m->dataset == 1;
-  // under the partition's view sharding the rank stages its one view
+  // under the partition's view sharding the rank stages its one view (a slab file's maps are that view's)
   const void* images = static_cast<const uint8_t*>(f->images) + (m->view_sel > 0 ? m->view_sel * f->img_stride : 0);
-  int rc = occd_stage_rgb_u8_cl(images, f->img_stride, f->row_stride, m->view_sel >= 0 ? 1 : (int)m->V, f->H0, f->W0,
-                                (int)m->img_h, (int)m->img_w, mean, stdv, m->dev(ROLE_IMG, b), (int)m->precision,
-                                (int)m->img_cstride, st);
+  const float* maps = (m->flags & FLAG_MAPS) ? static_cast<const float*>(m->dev_maps()) : nullptr;
+  int rc = occd_stage_camera_u8_cl(images, fx->pixel_format, f->img_stride, f->row_stride, fx->uv_offset,
+                                   m->view_sel >= 0 ? 1 : (int)m->V, f->H0, f->W0, (int)m->img_h, (int)m->img_w, maps,
+                                   2LL * m->img_h * m->img_w, mean, stdv, m->dev(ROLE_IMG, b), (int)m->precision,
+                                   (int)m->img_cstride, st);
   if (rc != OCCD_OK) return rc;
   if (m->flags & FLAG_VIRTUAL) {
     OCCD_CHECK_ARG(f->depth != nullptr && f->depth_h == (int)m->depth_h && f->depth_w == (int)m->depth_w,
@@ -926,7 +949,7 @@ int execute(occd_model* owner, int flags, cudaStream_t st, Replay rep) {
 }
 
 // stages frames[0..n) into items [0, n) and replays the records (through the graph when there is one) on `stream`
-int run_records(occd_model* m, const occd_frame* frames, int n, cudaStream_t st) {
+int run_records(occd_model* m, const occd_frame_ex* frames, int n, cudaStream_t st) {
   if (m->comm) {
     int rank, world, kind;
     occd_comm_describe(m->comm, &rank, &world, &kind);
@@ -938,7 +961,13 @@ int run_records(occd_model* m, const occd_frame* frames, int n, cudaStream_t st)
     int rc = stage(m, &frames[i], (uint32_t)i, st);
     if (rc != OCCD_OK) return rc;
   }
-  return execute(m, frames[0].flags, st, [m](cudaStream_t s) { return replay(m, s); });
+  return execute(m, frames[0].frame.flags, st, [m](cudaStream_t s) { return replay(m, s); });
+}
+
+// the occd_frame entry points: frames[0..n) as RGB occd_frame_ex, in the model's own array (nothing allocated)
+const occd_frame_ex* rgb_frames(occd_model* m, const occd_frame* frames, int n) {
+  for (int i = 0; i < n; ++i) m->frames_ex[i] = occd_frame_ex{frames[i], OCCD_PIX_RGB, 0};
+  return m->frames_ex.data();
 }
 
 // the whole maps of items [0, n) (and their confidences) of a model whose plan outputs them: every unpartitioned
@@ -960,7 +989,7 @@ int copy_out(const occd_model* m, uint16_t* class_map, void* conf, int n, cudaSt
 extern "C" int occd_model_run_frame(occd_model* m, const occd_frame* f, uint16_t* class_map, void* stream) {
   OCCD_CHECK_ARG(m && f && f->images && (class_map || m->rank != 0), "occd_model_run_frame: null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = run_records(m, f, 1, st);
+  int rc = run_records(m, rgb_frames(m, f, 1), 1, st);
   if (rc != OCCD_OK) return rc;
   return copy_out(m, class_map, nullptr, 1, st, "occd_model_run_frame");
 }
@@ -974,7 +1003,7 @@ extern "C" int occd_model_run_frame_conf(occd_model* m, const occd_frame* f, uin
     return OCCD_ERR_UNSUPPORTED;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = run_records(m, f, 1, st);
+  int rc = run_records(m, rgb_frames(m, f, 1), 1, st);
   if (rc != OCCD_OK) return rc;
   return copy_out(m, class_map, conf, 1, st, "occd_model_run_frame_conf");
 }
@@ -985,21 +1014,34 @@ extern "C" int occd_model_batch(const occd_model* m, int* batch) {
   return OCCD_OK;
 }
 
+namespace {
+
+int run_frames(const char* who, occd_model* m, const occd_frame* frames, const occd_frame_ex* frames_ex, int n,
+               uint16_t* class_maps, void* conf, void* stream) {
+  const std::string w(who);
+  if (!(m && (frames || frames_ex) && (class_maps || m->rank != 0))) return fail(OCCD_ERR_ARG, w + ": null argument");
+  if (n < 1 || (uint32_t)n > m->batch)
+    return fail(OCCD_ERR_ARG, w + ": " + std::to_string(n) + " frames, the model runs 1 to " +
+                                  std::to_string(m->batch));
+  for (int i = 0; i < n; ++i)
+    if (!(frames ? frames[i].images : frames_ex[i].frame.images)) return fail(OCCD_ERR_ARG, w + ": a frame without images");
+  if (conf && !(m->flags & FLAG_CONF)) return fail(OCCD_ERR_UNSUPPORTED, w + ": the model was exported without confidence");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = run_records(m, frames ? rgb_frames(m, frames, n) : frames_ex, n, st);
+  if (rc != OCCD_OK) return rc;
+  return copy_out(m, class_maps, conf, n, st, who);
+}
+
+}  // namespace
+
 extern "C" int occd_model_run_frames(occd_model* m, const occd_frame* frames, int n, uint16_t* class_maps, void* conf,
                                      void* stream) {
-  OCCD_CHECK_ARG(m && frames && (class_maps || m->rank != 0), "occd_model_run_frames: null argument");
-  if (n < 1 || (uint32_t)n > m->batch)
-    return fail(OCCD_ERR_ARG, "occd_model_run_frames: " + std::to_string(n) + " frames, the model runs 1 to " +
-                                  std::to_string(m->batch));
-  for (int i = 0; i < n; ++i) OCCD_CHECK_ARG(frames[i].images, "occd_model_run_frames: a frame without images");
-  if (conf && !(m->flags & FLAG_CONF)) {
-    occd_set_last_error("occd_model_run_frames: the model was exported without confidence");
-    return OCCD_ERR_UNSUPPORTED;
-  }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = run_records(m, frames, n, st);
-  if (rc != OCCD_OK) return rc;
-  return copy_out(m, class_maps, conf, n, st, "occd_model_run_frames");
+  return run_frames("occd_model_run_frames", m, frames, nullptr, n, class_maps, conf, stream);
+}
+
+extern "C" int occd_model_run_frames_ex(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps,
+                                        void* conf, void* stream) {
+  return run_frames("occd_model_run_frames_ex", m, nullptr, frames, n, class_maps, conf, stream);
 }
 
 extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
@@ -1019,8 +1061,9 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
     return OCCD_ERR_UNSUPPORTED;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const occd_frame_ex fx{*f, OCCD_PIX_RGB, 0};
   for (int r = 0; r < world; ++r) {
-    int rc = stage(ms[r], f, 0, st);
+    int rc = stage(ms[r], &fx, 0, st);
     if (rc != OCCD_OK) return rc;
   }
   // rank 0 holds the group's graph; it is captured afresh when the group's models change

@@ -84,31 +84,84 @@ extern "C" int occd_normalize_rgb_u8(const void* in, float* out, int H0, int W0,
   return OCCD_OK;
 }
 
+namespace {
+
+// the staging launcher of every pixel format; `who` names the entry point in the refusals
+template <int FMT, bool MAPS>
+int stage_camera(const char* who, const void* in, long long img_stride, long long row_stride, long long uv_offset,
+                 int n, int H0, int W0, int H, int W, const float* maps, long long map_stride, const float* mean,
+                 const float* stdv, void* out, int out_dtype, int cstride, void* stream) {
+  auto refuse = [&](const char* what) {
+    char msg[160];
+    snprintf(msg, sizeof msg, "%s: %s", who, what);
+    occd_set_last_error(msg);
+    return OCCD_ERR_ARG;
+  };
+  if (!(in && out && mean && stdv)) return refuse("null argument");
+  if (!(n > 0 && H > 0 && W > 0 && H0 > 0 && W0 > 0 && (MAPS || (H <= H0 && W <= W0))))
+    return refuse("the crop must lie inside the image");
+  if (FMT == nrm::PIX_NV12) {
+    if (H0 % 2 || W0 % 2) return refuse("an NV12 image has an even height and width");
+    // luma rows [0, H0), then H0 / 2 chroma rows of W0 bytes from uv_offset
+    const long long luma = (long long)(H0 - 1) * row_stride + W0, chroma = (long long)(H0 / 2 - 1) * row_stride + W0;
+    if (!(row_stride >= W0 && uv_offset >= luma && (n == 1 || img_stride >= uv_offset + chroma)))
+      return refuse("the chroma plane overlaps the luma rows, or the strides overlap the rows / images");
+  } else if (!(row_stride >= 3LL * W0 && (n == 1 || img_stride >= (long long)(H0 - 1) * row_stride + 3LL * W0))) {
+    return refuse("strides overlap the rows / images");
+  }
+  if (MAPS) {
+    if (reinterpret_cast<uintptr_t>(maps) % 4 != 0) return refuse("maps must be 4-byte aligned float32");
+    if (!(n == 1 || map_stride >= 2LL * H * W)) return refuse("map_stride overlaps the images' maps");
+    if (H0 >= 32767 || W0 >= 32767) return refuse("a remapped image is under 32767 pixels a side");
+  }
+  if (!(cstride >= 8 && cstride % 8 == 0)) return refuse("cstride must be a multiple of 8");
+  if (reinterpret_cast<uintptr_t>(out) % 16 != 0) return refuse("out must be 16-byte aligned");
+  nrm::StageArgs a;
+  a.in = (const unsigned char*)in; a.img_stride = img_stride; a.row_stride = row_stride;
+  a.out = out; a.H = H; a.W = W; a.cstride = cstride;
+  for (int c = 0; c < 3; ++c) { a.mean[c] = mean[c]; a.stdv[c] = stdv[c]; }
+  a.uv_offset = uv_offset; a.H0 = H0; a.W0 = W0; a.maps = maps; a.map_stride = map_stride;
+  const long long total = (long long)n * H * W;
+  if ((total + 255) / 256 > 2147483647LL) return refuse("too many pixels");
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (out_dtype == OCCD_DTYPE_BF16) nrm::stage_camera_kernel<__nv_bfloat16, FMT, MAPS><<<grid, 256, 0, st>>>(a, total);
+  else if (out_dtype == OCCD_DTYPE_F32) nrm::stage_camera_kernel<float, FMT, MAPS><<<grid, 256, 0, st>>>(a, total);
+  else return refuse("dtype");
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+
+}  // namespace
+
 // occd_stage_rgb_u8_cl: n uint8 HWC images -> the forward's channels-last input [n][H][W][cstride], equal to
 // occd_planar_to_cl(occd_normalize_rgb_u8(image)) in one pass
 extern "C" int occd_stage_rgb_u8_cl(const void* in, long long img_stride, long long row_stride, int n, int H0, int W0,
                                     int H, int W, const float* mean, const float* stdv, void* out, int out_dtype,
                                     int cstride, void* stream) {
-  OCCD_CHECK_ARG(in && out && mean && stdv, "occd_stage_rgb_u8_cl: null argument");
-  OCCD_CHECK_ARG(n > 0 && H > 0 && W > 0 && H <= H0 && W <= W0,
-                 "occd_stage_rgb_u8_cl: the crop must lie inside the image");
-  OCCD_CHECK_ARG(row_stride >= 3LL * W0 && (n == 1 || img_stride >= (long long)(H0 - 1) * row_stride + 3LL * W0),
-                 "occd_stage_rgb_u8_cl: strides overlap the rows / images");
-  OCCD_CHECK_ARG(cstride >= 8 && cstride % 8 == 0, "occd_stage_rgb_u8_cl: cstride must be a multiple of 8");
-  OCCD_CHECK_ARG(reinterpret_cast<uintptr_t>(out) % 16 == 0, "occd_stage_rgb_u8_cl: out must be 16-byte aligned");
-  nrm::StageArgs a;
-  a.in = (const unsigned char*)in; a.img_stride = img_stride; a.row_stride = row_stride;
-  a.out = out; a.H = H; a.W = W; a.cstride = cstride;
-  for (int c = 0; c < 3; ++c) { a.mean[c] = mean[c]; a.stdv[c] = stdv[c]; }
-  const long long total = (long long)n * H * W;
-  OCCD_CHECK_ARG((total + 255) / 256 <= 2147483647LL, "occd_stage_rgb_u8_cl: too many pixels");
-  const unsigned grid = (unsigned)((total + 255) / 256);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (out_dtype == OCCD_DTYPE_BF16) nrm::stage_rgb_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(a, total);
-  else if (out_dtype == OCCD_DTYPE_F32) nrm::stage_rgb_kernel<float><<<grid, 256, 0, st>>>(a, total);
-  else { occd_set_last_error("occd_stage_rgb_u8_cl: dtype"); return OCCD_ERR_ARG; }
-  OCCD_CHECK_LAUNCH();
-  return OCCD_OK;
+  return stage_camera<nrm::PIX_RGB, false>("occd_stage_rgb_u8_cl", in, img_stride, row_stride, 0, n, H0, W0, H, W,
+                                           nullptr, 0, mean, stdv, out, out_dtype, cstride, stream);
+}
+
+// occd_stage_camera_u8_cl: the same staging of RGB, BGR or NV12 images, optionally rectified by per-image maps
+extern "C" int occd_stage_camera_u8_cl(const void* in, int format, long long img_stride, long long row_stride,
+                                       long long uv_offset, int n, int H0, int W0, int H, int W, const float* maps,
+                                       long long map_stride, const float* mean, const float* stdv, void* out,
+                                       int out_dtype, int cstride, void* stream) {
+  static const char* who = "occd_stage_camera_u8_cl";
+#define OCCD_STAGE_FMT(F)                                                                                           \
+  return maps ? stage_camera<F, true>(who, in, img_stride, row_stride, uv_offset, n, H0, W0, H, W, maps, map_stride, \
+                                      mean, stdv, out, out_dtype, cstride, stream)                                 \
+              : stage_camera<F, false>(who, in, img_stride, row_stride, uv_offset, n, H0, W0, H, W, nullptr, 0,    \
+                                       mean, stdv, out, out_dtype, cstride, stream)
+  switch (format) {
+    case OCCD_PIX_RGB: OCCD_STAGE_FMT(nrm::PIX_RGB);
+    case OCCD_PIX_BGR: OCCD_STAGE_FMT(nrm::PIX_BGR);
+    case OCCD_PIX_NV12: OCCD_STAGE_FMT(nrm::PIX_NV12);
+  }
+#undef OCCD_STAGE_FMT
+  occd_set_last_error("occd_stage_camera_u8_cl: format must be OCCD_PIX_RGB, OCCD_PIX_BGR or OCCD_PIX_NV12");
+  return OCCD_ERR_ARG;
 }
 
 // occd_depth_u16_to_f32: NYU's load_depth (data/NYU/nyu_dataset.py:42-48) of a decoded uint16 depth PNG

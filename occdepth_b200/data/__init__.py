@@ -145,6 +145,53 @@ def stage_rgb_u8(imgs_u8, out, out_dtype, img_H, img_W, mean=IMAGENET_MEAN, std=
     _lib.check(rc, "occd_stage_rgb_u8_cl")
 
 
+def stage_camera_u8(imgs_u8, out, out_dtype, img_H, img_W, pixel_format="rgb", maps=None, mean=IMAGENET_MEAN,
+                    std=IMAGENET_STD):
+    """`stage_rgb_u8` of the images cameras and video decoders deliver, bit for bit what OpenCV makes of them on the
+    host first (`occd_stage_camera_u8_cl`):
+      pixel_format "rgb" / "bgr": imgs_u8 a CUDA uint8 (n, H0, W0, 3) tensor with 3-byte pixels (cv2.COLOR_BGR2RGB);
+                   "nv12": a CUDA uint8 (n, H0 * 3 / 2, W0) tensor, OpenCV's NV12 layout (the luma rows, then the
+                   interleaved U, V rows; rows of one stride, H0 and W0 even), converted as cv2.COLOR_YUV2RGB_NV12.
+      maps: None (the top-left img_H x img_W crop) or a CUDA float32 (n, 2, img_H, img_W) tensor of source x, y per
+            output pixel, each image's maps contiguous: the converted images are rectified as
+            cv2.remap(rgb, maps[i, 0], maps[i, 1], cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT) does.
+    Enqueued on the current stream, no allocation."""
+    fmt = _lib.PIXEL_FORMATS.get(pixel_format)
+    if fmt is None:
+        raise ValueError("stage_camera_u8: pixel_format must be one of %s, got %r"
+                         % (sorted(_lib.PIXEL_FORMATS), pixel_format))
+    if not (imgs_u8.is_cuda and imgs_u8.dtype == torch.uint8):
+        raise ValueError("stage_camera_u8: expected a CUDA uint8 tensor")
+    if fmt == _lib.PIX_NV12:
+        if not (imgs_u8.dim() == 3 and imgs_u8.stride(2) == 1 and imgs_u8.shape[1] % 3 == 0):
+            raise ValueError("stage_camera_u8: an NV12 batch is a uint8 (n, H0 * 3 / 2, W0) tensor with 1-byte pixels")
+        H0 = int(imgs_u8.shape[1]) * 2 // 3
+        uv_offset = H0 * imgs_u8.stride(1)
+    else:
+        if not (imgs_u8.dim() == 4 and imgs_u8.shape[3] == 3 and imgs_u8.stride(3) == 1 and imgs_u8.stride(2) == 3):
+            raise ValueError("stage_camera_u8: expected a uint8 (n, H, W, 3) tensor with 3-byte pixels")
+        H0, uv_offset = int(imgs_u8.shape[1]), 0
+    n, W0 = int(imgs_u8.shape[0]), int(imgs_u8.shape[2])
+    want_dt = {_lib.DTYPE_F32: torch.float32, _lib.DTYPE_BF16: torch.bfloat16}.get(int(out_dtype))
+    if not (out.is_cuda and out.dtype == want_dt and out.is_contiguous()
+            and out.numel() == n * img_H * img_W * out.shape[-1]):
+        raise ValueError("stage_camera_u8: out must be a contiguous CUDA tensor [n, ..., H, W, cstride]")
+    map_ptr, map_stride = None, 0
+    if maps is not None:
+        if not (maps.is_cuda and maps.dtype == torch.float32 and tuple(maps.shape) == (n, 2, img_H, img_W)
+                and maps[0].is_contiguous() and maps.device == imgs_u8.device):
+            raise ValueError("stage_camera_u8: maps must be a CUDA float32 (%d, 2, %d, %d) tensor on the images' "
+                             "device, each image's contiguous" % (n, img_H, img_W))
+        map_ptr, map_stride = maps.data_ptr(), maps.stride(0)
+    m32 = np.ascontiguousarray(np.asarray(mean, dtype=np.float32))
+    s32 = np.ascontiguousarray(np.asarray(std, dtype=np.float32))
+    rc = _lib.lib().occd_stage_camera_u8_cl(imgs_u8.data_ptr(), fmt, imgs_u8.stride(0), imgs_u8.stride(1), uv_offset,
+                                            n, H0, W0, int(img_H), int(img_W), map_ptr, map_stride,
+                                            m32.ctypes.data_as(C.c_void_p), s32.ctypes.data_as(C.c_void_p),
+                                            out.data_ptr(), int(out_dtype), int(out.shape[-1]), _lib.stream_ptr())
+    _lib.check(rc, "occd_stage_camera_u8_cl")
+
+
 NYU_DEPTH_SCALE, NYU_MAX_DEPTH = 8000.0, 10.0     # nyu_dataset.py:42-48
 
 

@@ -26,6 +26,7 @@ FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF, FLAG_SLAB = 1, 2, 4, 16  # FLAG_CONF:
                                                                    # then its float16 confidence; FLAG_SLAB: one
                                                                    # rank's plan of the X-slab partition
 FLAG_BATCH = 32                                                    # a B-frame plan of predict_frames (batch block)
+FLAG_MAPS = 64                                                     # the staged views' rectification maps (maps role)
 PATTERN_MAX = 64
 
 _STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
@@ -187,6 +188,11 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     `confidence` the file's class-map role holds the map and then its confidence (header flag FLAG_CONF), which
     `occd_model_run_frame_conf` reads; without it the file is what it always was.
 
+    A frame carrying "rect_maps" embeds them (header flag FLAG_MAPS and a maps role after the roles): a rig's
+    calibration is fixed per deployment, so the runtime rectifies every frame with them (a slab file holds its staged
+    view's only).  The frames of a batched export must then all carry the same maps.  Neither the frame's pixel
+    format nor its maps change the plan; the format is the caller's per run (`occd_model_run_frames_ex`).
+
     Under enable_slab_parallel, slab_output="root" (the only value a file carries) writes this rank's plan of
     `predict_frame(frame, slab_output="root", ...)`: every rank exports the same frame to its own path, and the
     files are loaded by `occd_model_load_slab` on each rank's communicator (header flag FLAG_SLAB and a slab block).
@@ -200,8 +206,13 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     if batched:
         if slab_output is not None:
             raise NotImplementedError("deploy.export: a batched model file (a list of frames) has no X-slab partition")
-        f = model._frames_checked(frame, True, confidence)[0]
-        B = len(frame)
+        fs = model._frames_checked(frame, True, confidence)
+        f, B = fs[0], len(frame)
+        for i, fi in enumerate(fs[1:], 1):
+            if (fi["maps"] is None) != (f["maps"] is None) or (fi["maps"] is not None
+                                                              and not torch.equal(fi["maps"], f["maps"])):
+                raise ValueError("deploy.export: frame %d's rect_maps differ from frame 0's; a model file holds one "
+                                 "set of maps for every frame" % i)
     else:
         f = model._frame_checked(frame, slab_output)
         B = 1
@@ -227,7 +238,10 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
                 _collect(getattr(op, "_keep", ()), tensors)
                 if isinstance(op, ConvOp):
                     tensors += [op.weight, op.bias]
-            _collect([img_cl, pix, fov, out, depth0, plan.pix_z, state], tensors)
+            maps = None
+            if f["maps"] is not None:         # the staged views' maps, in a buffer of their own
+                maps = (f["maps"] if view_sel is None else f["maps"][view_sel:view_sel + 1]).contiguous().clone()
+            _collect([img_cl, pix, fov, out, depth0, plan.pix_z, state, maps], tensors)
             torch.cuda.synchronize()
             bufs = _Buffers(tensors)
             contents = [bufs.contents(k) for k in range(len(bufs.iv))]     # before the run: activations are zero
@@ -298,7 +312,7 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
                               1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0)
                               | (FLAG_CONF if confidence else 0) | (FLAG_SLAB if slab is not None else 0)
-                              | (FLAG_BATCH if batched else 0),
+                              | (FLAG_BATCH if batched else 0) | (FLAG_MAPS if maps is not None else 0),
                               f["V"], f["H"], f["W"], model.project_scale),
            struct.pack("<7I", *S, *out_dims, f["P"]), pattern.astype("<i4").tobytes(),
            struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
@@ -308,6 +322,8 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
            struct.pack("<3I", *vn),
            G.astype("<f4").tobytes(), struct.pack("<I", img_cl.cstride)]
     hdr += [struct.pack("<iQQ", *r) for r in roles]
+    if maps is not None:
+        hdr.append(struct.pack("<iQQ", *role(maps)))
     if batched:
         hdr.append(struct.pack("<I", B))
     if slab is not None:
@@ -425,12 +441,27 @@ class LoadedModel:
         _lib.check(_lib.lib().occd_model_batch(self.handle, C.byref(b)), "occd_model_batch")
         return b.value
 
-    def run_frames(self, frames, out=None, stream=None, graph=True, conf=None):
+    def run_frames(self, frames, out=None, stream=None, graph=True, conf=None, pixel_format=None):
         """1..B frames (as OccDepth.predict_frames takes them) through occd_model_run_frames -> uint16 [n, X, Y, Z] on
-        the current device, or (map, conf) with `conf` (a float16 [n, X, Y, Z] device tensor, or True)"""
+        the current device, or (map, conf) with `conf` (a float16 [n, X, Y, Z] device tensor, or True).
+        Each frame's "pixel_format" ("rgb" by default, "bgr", or "nv12": then its "img" is uint8 (V, H0 * 3 / 2, W0),
+        OpenCV's NV12 layout) is staged through occd_model_run_frames_ex; `pixel_format` sets it for every frame, and a
+        frame whose own key says otherwise is refused.  The file's rectification maps apply: a frame carrying
+        "rect_maps" is refused."""
         n = len(frames)
-        calls = [_frame_call(self.geom, fr, None, None, graph, None, False) for fr in frames]
-        fa = (_lib.Frame * n)(*[c[0] for c in calls])
+        if pixel_format is not None and pixel_format not in _lib.PIXEL_FORMATS:
+            raise ValueError("LoadedModel.run_frames: pixel_format must be 'rgb', 'bgr' or 'nv12', got %r"
+                             % (pixel_format,))
+        fmts = [pixel_format or fr.get("pixel_format", "rgb") for fr in frames]
+        calls = [_frame_call(self.geom, fr, None, None, graph, None, False, fmt, "LoadedModel.run_frames")
+                 for fr, fmt in zip(frames, fmts)]
+        if all(fmt == "rgb" for fmt in fmts):
+            fa = (_lib.Frame * n)(*[c[0] for c in calls])
+            run = _lib.lib().occd_model_run_frames
+        else:
+            fa = (_lib.FrameEx * n)(*[_lib.FrameEx(c[0], _lib.PIXEL_FORMATS[fmt], c[1][0].stride(1) * c[0].H0)
+                                      for c, fmt in zip(calls, fmts)])
+            run = _lib.lib().occd_model_run_frames_ex
         dev = calls[0][1][0].device                 # the first frame's images, on the device
         if out is None:
             out = torch.empty(n, self.geom.X, self.geom.Y, self.geom.Z, dtype=torch.uint16, device=dev)
@@ -441,8 +472,7 @@ class LoadedModel:
             assert conf.dtype == torch.float16 and conf.is_contiguous() and conf.shape == out.shape
         keep = [c[1] for c in calls]
         st = _stream_for(stream, [t for c in keep for t in c if isinstance(t, torch.Tensor)] + [out, conf])
-        _lib.check(_lib.lib().occd_model_run_frames(self.handle, fa, n, _ptr(out), _ptr(conf), st),
-                   "occd_model_run_frames")
+        _lib.check(run(self.handle, fa, n, _ptr(out), _ptr(conf), st), run.__name__)
         return out if conf is None else (out, conf)
 
     def run_frame(self, frame, out=None, stream=None, graph=True, conf=None):
@@ -452,7 +482,8 @@ class LoadedModel:
         occd_model_run_frame_conf; the result is then (map, conf).  On a slab rank other than 0 nothing is written
         and the result is None; every rank must run every frame (with conf on every rank or on none)."""
         root = self.comm is None or self.comm.rank == 0
-        f, keep, out, conf_t, st = _frame_call(self.geom, frame, out, stream, graph, conf, root)
+        f, keep, out, conf_t, st = _frame_call(self.geom, frame, out, stream, graph, conf, root, "rgb",
+                                               "LoadedModel.run_frame")
         if conf is None:
             _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), _ptr(out), st), "occd_model_run_frame")
             return out if root else None
@@ -476,7 +507,8 @@ def run_frame_group(models, frame, out=None, stream=None, graph=True, conf=None)
     """one frame through every rank of a local group (LoadedModel r loaded with Comm.local(world)[r]), in lock step
     on one stream (occd_model_run_frame_group) -> rank 0's whole map, or (map, conf), as LoadedModel.run_frame"""
     hs = (C.c_void_p * len(models))(*[m.handle.value for m in models])
-    f, keep, out, conf_t, st = _frame_call(models[0].geom, frame, out, stream, graph, conf, True)
+    f, keep, out, conf_t, st = _frame_call(models[0].geom, frame, out, stream, graph, conf, True, "rgb",
+                                           "deploy.run_frame_group")
     _lib.check(_lib.lib().occd_model_run_frame_group(hs, len(models), C.byref(f), _ptr(out), _ptr(conf_t), st),
                "occd_model_run_frame_group")
     return out if conf is None else (out, conf_t)
@@ -486,12 +518,26 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def _frame_call(g, frame, out, stream, graph, conf, root):
-    """the occd_frame of a predict_frame frame dict (with the host and device copies it points into, which must live
-    until the call returns), the outputs (allocated when not given; none on a slab rank other than 0) and the stream"""
+def _frame_call(g, frame, out, stream, graph, conf, root, pixel_format, who):
+    """the occd_frame of a predict_frame frame dict whose images are in `pixel_format` (with the host and device
+    copies it points into, which must live until the call returns; keep[0] is the images), the outputs (allocated when
+    not given; none on a slab rank other than 0) and the stream.  The images must be the model's V views of that
+    format: the library reads them from their shape."""
+    if frame.get("pixel_format", pixel_format) != pixel_format:
+        raise ValueError("%s: the frame's pixel_format is %r, this call stages %r"
+                         % (who, frame["pixel_format"], pixel_format))
+    if frame.get("rect_maps") is not None:
+        raise ValueError("%s: a model file rectifies with the maps it was exported with; the frame's rect_maps would "
+                         "be ignored" % who)
     img = torch.as_tensor(frame["img"])
-    if img.dim() == 3:
+    nv12 = pixel_format == "nv12"
+    if img.dim() == (2 if nv12 else 3):
         img = img.unsqueeze(0)
+    if (img.dtype != torch.uint8 or img.shape[0] != g.V
+            or (img.dim() != 3 or img.shape[1] % 3 or img.shape[2] % 2 if nv12
+                else img.dim() != 4 or img.shape[3] != 3)):
+        raise ValueError("%s: frame['img'] must be the model's %d uint8 images, %s" % (
+            who, g.V, "(V, H * 3 / 2, W) NV12 with H and W even" if nv12 else "(V, H, W, 3) %s" % pixel_format.upper()))
     img = img.contiguous().cuda()
     keep = [img]
 
@@ -501,7 +547,9 @@ def _frame_call(g, frame, out, stream, graph, conf, root):
         return a.ctypes.data
 
     f = _lib.Frame()
-    f.images, f.H0, f.W0 = img.data_ptr(), img.shape[1], img.shape[2]
+    # NV12: the luma plane's size; the chroma rows follow it (uv_offset = H0 rows)
+    H0 = img.shape[1] * 2 // 3 if pixel_format == "nv12" else img.shape[1]
+    f.images, f.H0, f.W0 = img.data_ptr(), H0, img.shape[2]
     f.img_stride, f.row_stride = img.stride(0), img.stride(1)
     # a float32 pose is applied in float32, as predict_frame does; cam_k then goes in the same type
     pose = np.asarray(frame["cam_pose"] if g.dataset == 1 else frame["T_velo_2_cam"])

@@ -450,6 +450,14 @@ class OccDepth(_Base, B200Module):
                  depth PNG (H, W) when the model runs the virtual right view (nyu_dataset.py:116-200)
           optional geometry, fixed per dataset: "img_hw" (KITTI (370, 1220), NYU (480, 640)), "vox_origin" (KITTI
           (0, -25.6, -2)), "voxel_size" (KITTI 0.2 * project_scale, NYU 0.08), "scene_size", "pattern_id" (0)
+          camera formats (`occd_stage_camera_u8_cl`; bit for bit what OpenCV makes of the frame on the host):
+          "pixel_format": "rgb" (default), "bgr", or "nv12" -- then "img" is uint8 (V, H0 * 3 / 2, W0), OpenCV's
+                 NV12 layout (cv2.COLOR_YUV2RGB_NV12), H0 and W0 even
+          "rect_maps": float32 (V, 2, img_h, img_w), each view's cv2.initUndistortRectifyMap x and y maps: the images
+                 are rectified as cv2.remap(INTER_LINEAR, BORDER_CONSTANT) does, and "cam_k" is the rectified
+                 camera's.  Read in place on the device; host maps are copied every call.  NYU's depth map is not
+                 remapped: it must already be in the rectified camera's frame.
+          Neither changes the plan.
         The indices are recomputed only when the calibration differs from what the plan's index buffers hold (a KITTI
         sequence keeps one); NYU poses change every frame.  One frame per call.
 
@@ -505,20 +513,45 @@ class OccDepth(_Base, B200Module):
         img = frame["img"]
         if not isinstance(img, torch.Tensor):
             img = torch.from_numpy(np.ascontiguousarray(img))
-        if img.dim() == 5:
-            if img.shape[0] != 1:
-                raise NotImplementedError("OccDepth.predict_frame: one frame per call (batch size %d)" % img.shape[0])
-            img = img[0]
-        if img.dim() == 3:
-            img = img.unsqueeze(0)
-        if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] != 3:
-            raise ValueError("OccDepth.predict_frame: frame['img'] must be uint8 RGB (V, H, W, 3)")
-        if img.stride(3) != 1 or img.stride(2) != 3:
-            img = img.contiguous()
+        fmt = frame.get("pixel_format", "rgb")
+        if fmt not in _lib.PIXEL_FORMATS:
+            raise ValueError("OccDepth.predict_frame: frame['pixel_format'] must be 'rgb', 'bgr' or 'nv12', got %r"
+                             % (fmt,))
+        if fmt == "nv12":
+            if img.dim() == 2:
+                img = img.unsqueeze(0)
+            # 3 * H / 2 rows: a multiple of 3 exactly when H is even
+            if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[1] % 3 or img.shape[2] % 2:
+                raise ValueError("OccDepth.predict_frame: an NV12 frame['img'] must be uint8 (V, H * 3 / 2, W), "
+                                 "OpenCV's NV12 layout, with H and W even")
+            if img.stride(2) != 1:
+                img = img.contiguous()
+        else:
+            if img.dim() == 5:
+                if img.shape[0] != 1:
+                    raise NotImplementedError("OccDepth.predict_frame: one frame per call (batch size %d)"
+                                              % img.shape[0])
+                img = img[0]
+            if img.dim() == 3:
+                img = img.unsqueeze(0)
+            if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[3] != 3:
+                raise ValueError("OccDepth.predict_frame: frame['img'] must be uint8 RGB (V, H, W, 3)")
+            if img.stride(3) != 1 or img.stride(2) != 3:
+                img = img.contiguous()
         img = img.to(dev, non_blocking=True)
         V = int(img.shape[0])
         nyu = self.dataset == "NYU"
         H, W = (int(v) for v in frame.get("img_hw", (480, 640) if nyu else (370, 1220)))
+        maps = frame.get("rect_maps")
+        if maps is not None:
+            if not isinstance(maps, torch.Tensor):
+                maps = torch.from_numpy(np.ascontiguousarray(maps))
+            if maps.dtype != torch.float32 or tuple(maps.shape) != (V, 2, H, W):
+                raise ValueError("OccDepth.predict_frame: frame['rect_maps'] must be float32 (%d, 2, %d, %d): each "
+                                 "view's source x and y per pixel of the %d x %d crop" % (V, H, W, H, W))
+            maps = maps.to(dev, non_blocking=True)
+            if not maps[0].is_contiguous():
+                maps = maps.contiguous()
         g = dict(voxel_size=frame.get("voxel_size", 0.08 if nyu else 0.2 * self.project_scale),
                  scene_size=tuple(frame.get("scene_size", (4.8, 4.8, 2.88) if nyu else (51.2, 51.2, 6.4))),
                  pattern_id=int(frame.get("pattern_id", 0)))
@@ -567,9 +600,9 @@ class OccDepth(_Base, B200Module):
                              "%dx%dx%d" % (X, Y, Z, S[0], S[1], S[2]))
         if not 0 <= g["pattern_id"] < len(D.PIXEL_PATTERNS):
             raise IndexError("pattern_id out of range")
-        return dict(g, imgs=img, V=V, H=H, W=W, N=X * Y * Z, P=len(D.PIXEL_PATTERNS[g["pattern_id"]]), poses=poses,
-                    vox_origin=vox_origin, depth=depth, virtual=depth is not None, virtual_bf=bf, batch=batch,
-                    calib=calib)
+        return dict(g, imgs=img, pixel_format=fmt, maps=maps, V=V, H=H, W=W, N=X * Y * Z,
+                    P=len(D.PIXEL_PATTERNS[g["pattern_id"]]), poses=poses, vox_origin=vox_origin, depth=depth,
+                    virtual=depth is not None, virtual_bf=bf, batch=batch, calib=calib)
 
     def _stage_frame(self, ent, f, b=0):
         """the device side of predict_frame / predict_frames: stage frame `f` into batch item b of the static input
@@ -584,7 +617,12 @@ class OccDepth(_Base, B200Module):
             plan.pix_z = torch.empty(B, pix.shape[2], dtype=torch.float64, device=pix.device)   # vox2pix's depths
         imgs = f["imgs"] if view_sel is None else f["imgs"][view_sel:view_sel + 1]
         n_img = imgs.shape[0]
-        D.stage_rgb_u8(imgs, img_cl.buf[b * n_img:(b + 1) * n_img], img_cl.lib_dtype, f["H"], f["W"])
+        if f["pixel_format"] == "rgb" and f["maps"] is None:
+            D.stage_rgb_u8(imgs, img_cl.buf[b * n_img:(b + 1) * n_img], img_cl.lib_dtype, f["H"], f["W"])
+        else:
+            maps = f["maps"] if f["maps"] is None or view_sel is None else f["maps"][view_sel:view_sel + 1]
+            D.stage_camera_u8(imgs, img_cl.buf[b * n_img:(b + 1) * n_img], img_cl.lib_dtype, f["H"], f["W"],
+                              f["pixel_format"], maps)
         if depth0 is not None:
             d = depth0 if depth0.dim() == 2 else depth0[b]
             if tuple(f["depth"].shape) != tuple(d.shape):
@@ -654,7 +692,10 @@ class OccDepth(_Base, B200Module):
         """what the frames of one predict_frames call must share, read on the host with predict_frame's defaults"""
         nyu = self.dataset == "NYU"
         shape = tuple(getattr(frame["img"], "shape", ()))
-        V = 1 if len(shape) == 3 else shape[-4] if len(shape) >= 4 else None
+        if frame.get("pixel_format", "rgb") == "nv12":
+            V = 1 if len(shape) == 2 else shape[0] if len(shape) == 3 else None
+        else:
+            V = 1 if len(shape) == 3 else shape[-4] if len(shape) >= 4 else None
         return {"V": V,
                 "img_hw": tuple(int(v) for v in frame.get("img_hw", (480, 640) if nyu else (370, 1220))),
                 "voxel_size": float(frame.get("voxel_size", 0.08 if nyu else 0.2 * self.project_scale)),

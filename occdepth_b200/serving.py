@@ -157,11 +157,18 @@ class CameraPipeline:
     `batch=B` runs `OccDepth.predict_frames` instead: `submit` takes a list of 1..B frames, copies them into B-frame
     pinned and device buffers (each frame's slice sized from its own image) and runs the B-frame plan; `result(ticket)`
     returns that submit's n maps [n, X, Y, Z] (or (map, conf)).  A short list -- the last of a stream -- runs the same
-    plan, and only its n results are read back.  Not with output="voxels" or slab_output."""
+    plan, and only its n results are read back.  Not with output="voxels" or slab_output.
+
+    `pixel_format` ("rgb", "bgr" or "nv12") and `rect_maps` (float32 (V, 2, img_h, img_w)) are predict_frame's frame
+    keys for every frame that leaves them out: the images are converted and rectified on the device, as OpenCV would on
+    the host.  The maps are copied to the device once, here; an NV12 frame copies 1.5 bytes a pixel where RGB copies
+    3 (`h2d_bytes`)."""
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
                  inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None,
-                 confidence=False, batch=None):
+                 confidence=False, batch=None, pixel_format="rgb", rect_maps=None):
+        if pixel_format not in ("rgb", "bgr", "nv12"):
+            raise ValueError("CameraPipeline: pixel_format must be 'rgb', 'bgr' or 'nv12', got %r" % (pixel_format,))
         if batch is not None:
             if isinstance(batch, bool) or not isinstance(batch, int) or batch < 1:
                 raise ValueError("CameraPipeline: batch must be None or a frame count >= 1, got %r" % (batch,))
@@ -198,6 +205,15 @@ class CameraPipeline:
         for k, v in (("vox_origin", vox_origin), ("voxel_size", voxel_size), ("scene_size", scene_size)):
             if v is not None:
                 self.geometry[k] = v
+        if pixel_format != "rgb":
+            self.geometry["pixel_format"] = pixel_format
+        if rect_maps is not None:
+            import numpy as np
+            maps = torch.as_tensor(np.ascontiguousarray(rect_maps) if not isinstance(rect_maps, torch.Tensor)
+                                   else rect_maps)
+            if maps.dtype != torch.float32 or maps.dim() != 4 or tuple(maps.shape[1:]) != (2,) + tuple(img_hw):
+                raise ValueError("CameraPipeline: rect_maps must be float32 (V, 2, %d, %d)" % tuple(img_hw))
+            self.geometry["rect_maps"] = maps.to(dev).contiguous()
         self.main = torch.cuda.current_stream(dev)
         self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
         self.bufs = {}                # name -> two (pinned host, device) flat byte buffers
@@ -259,9 +275,13 @@ class CameraPipeline:
             if img.shape[0] != 1:
                 raise NotImplementedError("CameraPipeline.submit: one frame per submit (batch size %d)" % img.shape[0])
             img = img[0]
+        if frame.get("pixel_format", self.geometry.get("pixel_format")) == "nv12":
+            img = img.unsqueeze(0) if img.dim() == 2 else img          # (V, H0 * 3 / 2, W0)
+        elif img.dim() == 3:
+            img = img.unsqueeze(0)                                     # (V, H0, W0, 3)
         depth = frame.get("depth")
         depth = None if depth is None else self._host(depth, "depth")
-        V = int(img.shape[0]) if img.dim() == 4 else 1
+        V = int(img.shape[0])
         sel = self.model.slab_view(V, virtual=depth is not None)
         j = self.n & 1
         self.host_free[j].synchronize()           # pinned buffer j: its previous H2D copy has been read
@@ -274,7 +294,7 @@ class CameraPipeline:
                 f["img"] = self._stage_h2d("img", j, img)
             else:
                 # this rank's plan stages view `sel` only: copy that one, and let every view of the frame read it
-                f["img"] = self._stage_h2d("img", j, img[sel:sel + 1]).expand(V, -1, -1, -1)
+                f["img"] = self._stage_h2d("img", j, img[sel:sel + 1]).expand((V,) + tuple(img.shape[1:]))
             if depth is not None:
                 f["depth"] = self._stage_h2d("depth", j, depth)
             self.in_ready[j].record(self.h2d)

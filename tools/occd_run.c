@@ -3,18 +3,20 @@
  * Linked only against libocc_b200.so and the CUDA runtime; `python -m occdepth_b200._build` builds it next to
  * the library (occdepth_b200/lib/occd_run).
  *
- *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]
+ *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] [--depth DEPTH] [--no-graph]
  *            [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
  *
  * Inputs are raw little-endian files, one record per frame, frames back to back (no image decoder):
  *   IMAGES  N x V x H0 x W0 x 3 uint8, RGB, row-major (H0 x W0 default to the model's crop; --raw gives larger
- *           images, cropped to the top-left corner as the datasets do)
+ *           images, cropped to the top-left corner as the datasets do, or remapped by the file's rectification
+ *           maps); --format bgr: the same with pixels B, G, R; --format nv12: N x V x (H0 * 3 / 2) x W0, each image
+ *           OpenCV's NV12 layout (H0 luma rows, then H0 / 2 rows of interleaved U, V; H0 and W0 even)
  *   CALIB   N records of float64: KITTI  V x 9 cam_k, then V x 16 T_velo_2_cam (row-major)
  *                                  NYU    9 cam_k, 16 T_world_2_cam (the inverse of the camera pose), 3 vox_origin
  *   DEPTH   (NYU models with the virtual view) N x depth_h x depth_w uint16, the depth PNGs' values
  * Output: OUT_DIR/NNNNNN.label per frame, the uint16 class map (X x Y x Z, C order) as the KITTI submission writer
  * stores it; the labels are remapped when the model was exported with inv_map.  Prints ms per frame (device time
- * of occd_model_run_frames, from CUDA events) and the mean over the frames after the first.
+ * of occd_model_run_frames_ex, from CUDA events) and the mean over the frames after the first.
  *
  * A batched model file (deploy.export of a list of B frames) runs the frames in groups of B, the last group short;
  * the times are then per group, and the mean is per frame over the groups after the first.
@@ -87,16 +89,24 @@ static int share_id(const char* path, int rank, const char* nccl_lib, char* id) 
 
 int main(int argc, char** argv) {
   if (argc < 6) {
-    fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--depth DEPTH] [--no-graph]\n");
+    fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] "
+                    "[--depth DEPTH] [--no-graph]\n");
     return 2;
   }
   const char *model_path = argv[1], *img_path = argv[2], *calib_path = argv[3], *out_dir = argv[5];
   const char *depth_path = NULL, *id_path = NULL, *nccl_lib = NULL;
-  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0;
+  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0, format = OCCD_PIX_RGB;
   for (int i = 6; i < argc; ++i) {
     if (!strcmp(argv[i], "--raw") && i + 2 < argc) {
       H0 = atoi(argv[++i]);
       W0 = atoi(argv[++i]);
+    } else if (!strcmp(argv[i], "--format") && i + 1 < argc) {
+      const char* f = argv[++i];
+      format = !strcmp(f, "rgb") ? OCCD_PIX_RGB : !strcmp(f, "bgr") ? OCCD_PIX_BGR : !strcmp(f, "nv12") ? OCCD_PIX_NV12 : -1;
+      if (format < 0) {
+        fprintf(stderr, "occd_run: --format takes rgb, bgr or nv12\n");
+        return 2;
+      }
     } else if (!strcmp(argv[i], "--depth") && i + 1 < argc) {
       depth_path = argv[++i];
     } else if (!strcmp(argv[i], "--no-graph")) {
@@ -137,7 +147,9 @@ int main(int argc, char** argv) {
     W0 = g.img_w;
   }
   const int nyu = g.dataset == 1;
-  const size_t img_bytes = (size_t)g.V * H0 * W0 * 3;
+  // one image: 3 bytes a pixel, or NV12's 1.5
+  const size_t one_img = format == OCCD_PIX_NV12 ? (size_t)H0 * W0 * 3 / 2 : (size_t)H0 * W0 * 3;
+  const size_t img_bytes = (size_t)g.V * one_img;
   const size_t n_calib = nyu ? 9 + 16 + 3 : (size_t)g.V * 25;
   const size_t map_bytes = (size_t)g.X * g.Y * g.Z * 2;
   const size_t depth_bytes = (size_t)g.depth_h * g.depth_w * 2;
@@ -156,7 +168,7 @@ int main(int argc, char** argv) {
   unsigned short* h_depth = (unsigned short*)malloc(depth_bytes ? depth_bytes * B : 1);
   unsigned short* h_map = (unsigned short*)malloc(map_bytes * B);
   double* calib = (double*)malloc(n_calib * sizeof(double) * B);
-  occd_frame* fs = (occd_frame*)calloc(B, sizeof(occd_frame));
+  occd_frame_ex* fs = (occd_frame_ex*)calloc(B, sizeof(occd_frame_ex));
   void *d_img, *d_depth = NULL, *d_map;
   cudaStream_t st;
   cudaEvent_t e0, e1;
@@ -179,11 +191,13 @@ int main(int argc, char** argv) {
         return 1;
       CK(cudaMemcpyAsync((char*)d_img + img_bytes * i, img, img_bytes, cudaMemcpyHostToDevice, st));
       if (fd) CK(cudaMemcpyAsync((char*)d_depth + depth_bytes * i, depth, depth_bytes, cudaMemcpyHostToDevice, st));
-      occd_frame* f = &fs[i];
-      memset(f, 0, sizeof(*f));
+      memset(&fs[i], 0, sizeof(fs[i]));
+      fs[i].pixel_format = format;
+      fs[i].uv_offset = (long long)H0 * W0;  /* NV12: the chroma rows follow the luma plane */
+      occd_frame* f = &fs[i].frame;
       f->images = (char*)d_img + img_bytes * i;
-      f->img_stride = (long long)H0 * W0 * 3;
-      f->row_stride = (long long)W0 * 3;
+      f->img_stride = (long long)one_img;
+      f->row_stride = format == OCCD_PIX_NV12 ? (long long)W0 : (long long)W0 * 3;
       f->H0 = H0;
       f->W0 = W0;
       f->cam_k = cal;
@@ -196,7 +210,7 @@ int main(int argc, char** argv) {
       f->flags = flags;
     }
     CK(cudaEventRecord(e0, st));
-    OK(occd_model_run_frames(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
+    OK(occd_model_run_frames_ex(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
     CK(cudaEventRecord(e1, st));
     if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes * k, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
