@@ -257,13 +257,14 @@ int occd_copy_channels(const void* in, void* out, int dtype, long long positions
 /* the reference multiplies in the pose's own precision; cam_k 3x3 float32 row-major (the reference's   */
 /* intr.astype(float32)), vox_origin 3 float32, pattern P x 2 int (dx, dy).                             */
 /* DEVICE pointers: pix int64 [N][P][2] (x, y), fov bool [N][P], pix_z [N] in the pose's precision or   */
-/* NULL; N = X*Y*Z voxels in C order.                                                                  */
+/* NULL; N = X*Y*Z voxels in C order.  pix may be NULL: then only fov (and pix_z, if given) is written, */
+/* the same bytes as with pix (a FOV mask alone needs no [N][P][2] index scratch).  fov is required.    */
 int occd_vox2pix_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
                      double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern, int P,
                      long long* pix, unsigned char* fov, void* pix_z, void* stream);
 /* the same for voxels [v0, v0 + n) of that C order only (0 <= v0, 1 <= n, v0 + n <= X*Y*Z), written to pix [n][P][2], */
 /* fov [n][P], pix_z [n]: bit for bit that slice of occd_vox2pix_fwd's outputs.  An X-slab [x0, x1) of the grid is  */
-/* v0 = x0*Y*Z, n = (x1 - x0)*Y*Z.                                                                                  */
+/* v0 = x0*Y*Z, n = (x1 - x0)*Y*Z.  pix may be NULL, as for occd_vox2pix_fwd.                                      */
 int occd_vox2pix_range_fwd(const void* cam_E, int pose_is_f32, const float* cam_k, const float* vox_origin,
                            double voxel_size, int X, int Y, int Z, int img_W, int img_H, const int* pattern, int P,
                            long long* pix, unsigned char* fov, void* pix_z, long long v0, long long n, void* stream);
@@ -551,6 +552,26 @@ typedef struct {
 /* occd_model_run_frames for frames of any camera format; occd_model_run_frame(s/_conf) are this call with RGB.      */
 int occd_model_run_frames_ex(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps, void* conf,
                              void* stream);
+/* The occupied-voxel list (occd_occupied_voxels) of the maps the model's last run left on the device: items [0, n)  */
+/* of that run (1 <= n <= its n), empty = 0, ignore = 255, the labels remapped when the file has a class LUT.  The  */
+/* rows of each item are split by its fov_mask_1: vox2pix of the first view of the item's last staged calibration  */
+/* at the output resolution (voxel size / project_scale, the img_w x img_h crop, the centre pixel), computed on the */
+/* first listing after that calibration changed and kept otherwise.  NYU has no mask: every row counts as inside.   */
+/* Under the X-slab partition rank 0 (also a local group's, after occd_model_run_frame_group) lists the whole       */
+/* gathered map; the other ranks hold no map and are refused.  The mask (B x N bytes) and the work array are        */
+/* allocated at the first listing and held until occd_model_destroy (counted in device_bytes); nothing is allocated */
+/* per call.  Launches on `stream` only, outside the graph; nothing synchronises with the host.                    */
+typedef struct {
+  int capacity;        /* rows per frame, >= 0                                                                    */
+  double voxel_size;   /* edge of an output voxel for xyz; 0: 0.2 for KITTI, 0.08 for NYU                         */
+  const double* origin;/* HOST 3 doubles added to the centres, or NULL                                            */
+  int32_t* count;      /* DEVICE [n][2] in-FOV / out-of-FOV occupied voxels (the true counts, whatever capacity is) */
+  int32_t* hist;       /* DEVICE [n][64] occupied voxels per class id                                             */
+  int32_t* index;      /* DEVICE [n][capacity] flat voxel index                                                   */
+  uint16_t* cls;       /* DEVICE [n][capacity]                                                                    */
+  float* xyz;          /* DEVICE [n][capacity][3] voxel centres, or NULL: no coordinates                          */
+} occd_voxel_out;
+int occd_model_list_voxels(occd_model* m, int n, const occd_voxel_out* out, void* stream);
 int occd_model_destroy(occd_model* m);
 
 /* Model files under the X-slab partition (DESIGN.md section 9): one file per rank, each holding that rank's plan of */

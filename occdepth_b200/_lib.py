@@ -78,6 +78,12 @@ class FrameEx(C.Structure):
     _fields_ = [("frame", Frame), ("pixel_format", C.c_int), ("uv_offset", C.c_longlong)]
 
 
+class VoxelOut(C.Structure):
+    """occd_voxel_out"""
+    _fields_ = [("capacity", C.c_int), ("voxel_size", C.c_double), ("origin", C.c_void_p), ("count", C.c_void_p),
+                ("hist", C.c_void_p), ("index", C.c_void_p), ("cls", C.c_void_p), ("xyz", C.c_void_p)]
+
+
 class ConvTap(C.Structure):
     _fields_ = [("src", C.c_int), ("dz", C.c_int), ("dy", C.c_int), ("dx", C.c_int)]
 
@@ -180,6 +186,7 @@ SYMBOLS = {
     "occd_model_batch": (C.c_int, [_vp, C.POINTER(C.c_int)]),
     "occd_model_run_frames": (C.c_int, [_vp, C.POINTER(Frame), _i, _vp, _vp, _vp]),
     "occd_model_run_frames_ex": (C.c_int, [_vp, C.POINTER(FrameEx), _i, _vp, _vp, _vp]),
+    "occd_model_list_voxels": (C.c_int, [_vp, _i, C.POINTER(VoxelOut), _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "occd_comm_halo_exchange": (C.c_int, [_vp, _vp, _ll, _i, _i, _vp]),

@@ -127,6 +127,7 @@ const Entry kEntries[] = {
     // model handle can only be NULL
     OCCD_ENTRY(occd_model_run_frame_conf),  OCCD_ENTRY(occd_model_run_frames),
     OCCD_ENTRY(occd_model_batch),           OCCD_ENTRY(occd_model_run_frames_ex),
+    OCCD_ENTRY(occd_model_list_voxels),
     // the X-slab partition's collectives: the lock-step runner of a local group stops after each
     OCCD_ENTRY(occd_comm_halo_exchange),    OCCD_ENTRY(occd_comm_all_gather),
     OCCD_ENTRY(occd_comm_gather_root),
@@ -249,6 +250,21 @@ struct occd_model {
   int32_t view_sel = -1;
   occd_comm* comm = nullptr;                 // not owned
   std::vector<occd_model*> graph_ranks;      // a local group's graph (held by rank 0): the models it was captured over
+  // occd_model_list_voxels: the last run's n (0: none, or it failed), per item the first view's calibration as staged
+  // (KITTI) and whether the item's output-resolution FOV mask was computed from it; the mask [batch][N_out] and the
+  // listing's work array, allocated at the first listing
+  struct ViewCalib {
+    int f32;
+    double E[16];
+    float Ef[16], k32[9];
+    double origin[3], scene[3], voxel;
+  };
+  int last_n = 0;
+  std::vector<ViewCalib> view0;
+  std::vector<char> mask_valid;
+  uint8_t* list_mask = nullptr;
+  uint32_t* list_work = nullptr;
+  size_t list_bytes = 0;
 
   bool slab() const { return (flags & FLAG_SLAB) != 0; }
   void* dev(int role) const { return arena + buf_off[roles[role].buffer] + roles[role].off; }
@@ -506,6 +522,8 @@ int parse(occd_model* m) {
   m->frames_ex.assign(m->batch, occd_frame_ex{});
   m->calib.assign(m->batch, std::vector<uint8_t>());
   m->calib_valid.assign(m->batch, 0);
+  m->view0.assign(m->batch, occd_model::ViewCalib{});
+  m->mask_valid.assign(m->batch, 0);
   m->cams.assign((size_t)m->batch * 4 * 40, 0.f);
   m->sps.assign((size_t)m->batch * 4, 0.f);
   return OCCD_OK;
@@ -517,6 +535,8 @@ void release(occd_model* m) {
   for (occd_conv_plan* p : m->plans)
     if (p) occd_conv_plan_destroy(p);
   if (m->arena) cudaFree(m->arena);
+  if (m->list_mask) cudaFree(m->list_mask);
+  if (m->list_work) cudaFree(m->list_work);
   if (m->capture_stream) cudaStreamDestroy(m->capture_stream);
   delete m;
 }
@@ -676,6 +696,21 @@ int stage(occd_model* m, const occd_frame_ex* fx, uint32_t b, cudaStream_t st) {
     if (m->calib_valid[b] && key == m->calib[b]) return OCCD_OK;
     m->calib_valid[b] = 0;
     m->calib[b].swap(key);
+    // what occd_model_list_voxels projects the item's FOV mask from: the key above covers all of it, so an unchanged
+    // calibration (the early return) keeps both this copy and the mask made from it
+    occd_model::ViewCalib& c = m->view0[b];
+    c.f32 = f->calib_f32;
+    for (int i = 0; i < 16; ++i) {
+      if (f->calib_f32) c.Ef[i] = static_cast<const float*>(f->pose)[i];
+      else c.E[i] = static_cast<const double*>(f->pose)[i];
+    }
+    for (int i = 0; i < 9; ++i) c.k32[i] = (float)K[0][i];
+    for (int k = 0; k < 3; ++k) {
+      c.origin[k] = origin[k];
+      c.scene[k] = scene[k];
+    }
+    c.voxel = voxel;
+    m->mask_valid[b] = 0;
   }
   int dims[3];
   for (int k = 0; k < 3; ++k) dims[k] = (int)ceil(((origin[k] + scene[k]) - origin[k]) / voxel);  // volume_dims
@@ -900,7 +935,7 @@ extern "C" int occd_model_info(const occd_model* m, occd_model_geom* g) {
   g->depth_w = (int)m->depth_w;
   g->flosp_depth = (m->flags & FLAG_FLOSP_DEPTH) ? 1 : 0;
   g->graph = m->graph_exec ? 1 : 0;
-  g->device_bytes = (long long)m->arena_bytes;
+  g->device_bytes = (long long)(m->arena_bytes + m->list_bytes);
   g->voxel_size = m->voxel_size;
   for (int k = 0; k < 3; ++k) {
     g->vox_origin[k] = m->vox_origin[k];
@@ -957,11 +992,14 @@ int run_records(occd_model* m, const occd_frame_ex* frames, int n, cudaStream_t 
       return fail(OCCD_ERR_UNSUPPORTED, "occd_model_run_frame: a model on a local communicator runs with its group "
                                         "through occd_model_run_frame_group");
   }
+  m->last_n = 0;  // a failed run leaves nothing to list
   for (int i = 0; i < n; ++i) {
     int rc = stage(m, &frames[i], (uint32_t)i, st);
     if (rc != OCCD_OK) return rc;
   }
-  return execute(m, frames[0].frame.flags, st, [m](cudaStream_t s) { return replay(m, s); });
+  int rc = execute(m, frames[0].frame.flags, st, [m](cudaStream_t s) { return replay(m, s); });
+  if (rc == OCCD_OK) m->last_n = n;
+  return rc;
 }
 
 // the occd_frame entry points: frames[0..n) as RGB occd_frame_ex, in the model's own array (nothing allocated)
@@ -1062,6 +1100,7 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const occd_frame_ex fx{*f, OCCD_PIX_RGB, 0};
+  for (int r = 0; r < world; ++r) ms[r]->last_n = 0;
   for (int r = 0; r < world; ++r) {
     int rc = stage(ms[r], &fx, 0, st);
     if (rc != OCCD_OK) return rc;
@@ -1073,7 +1112,78 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
   int rc = execute(owner, f->flags, st, [ms, world](cudaStream_t s) { return replay_lockstep(ms, world, s); });
   if (rc != OCCD_OK) return rc;
   if (capture && owner->graph_exec) owner->graph_ranks.assign(ms, ms + world);
+  for (int r = 0; r < world; ++r) ms[r]->last_n = 1;
   return copy_out(owner, class_map, conf, 1, st, "occd_model_run_frame_group");
+}
+
+namespace {
+
+// item b's fov_mask_1 (KITTI): vox2pix of its first view at the output resolution, centre pixel, into list_mask
+int fov_mask_1(occd_model* m, uint32_t b, long long N, cudaStream_t st) {
+  const occd_model::ViewCalib& c = m->view0[b];
+  const double voxel = c.voxel / m->ps;
+  int dims[3];
+  for (int k = 0; k < 3; ++k) dims[k] = (int)ceil(((c.origin[k] + c.scene[k]) - c.origin[k]) / voxel);  // volume_dims
+  if ((long long)dims[0] * dims[1] * dims[2] != N)
+    return fail(OCCD_ERR_ARG, "occd_model_list_voxels: item " + std::to_string(b) + "'s geometry gives " +
+                                  std::to_string((long long)dims[0] * dims[1] * dims[2]) +
+                                  " voxels at the output resolution, the model predicts " + std::to_string(N));
+  const float o32[3] = {(float)c.origin[0], (float)c.origin[1], (float)c.origin[2]};
+  static const int centre[2] = {0, 0};  // the datasets' pattern 0
+  return occd_vox2pix_fwd(c.f32 ? (const void*)c.Ef : (const void*)c.E, c.f32, c.k32, o32, voxel, dims[0], dims[1],
+                          dims[2], (int)m->img_w, (int)m->img_h, centre, 1, nullptr, m->list_mask + (size_t)b * N,
+                          nullptr, st);
+}
+
+}  // namespace
+
+extern "C" int occd_model_list_voxels(occd_model* m, int n, const occd_voxel_out* out, void* stream) {
+  OCCD_CHECK_ARG(m && out, "occd_model_list_voxels: null argument");
+  OCCD_CHECK_ARG(out->count && out->hist && out->index && out->cls,
+                 "occd_model_list_voxels: count, hist, index and cls are required");
+  OCCD_CHECK_ARG(out->capacity >= 0, "occd_model_list_voxels: capacity must be >= 0");
+  OCCD_CHECK_ARG(out->voxel_size >= 0.0, "occd_model_list_voxels: voxel_size must be >= 0 (0: the dataset's default)");
+  if (m->rank != 0)
+    return fail(OCCD_ERR_ARG, "occd_model_list_voxels: rank " + std::to_string(m->rank) + " of the X-slab partition "
+                              "holds no map; rank 0 lists the whole map");
+  if (m->last_n == 0)
+    return fail(OCCD_ERR_ARG, "occd_model_list_voxels: no run yet (or the last run failed): nothing to list");
+  if (n < 1 || n > m->last_n)
+    return fail(OCCD_ERR_ARG, "occd_model_list_voxels: " + std::to_string(n) + " items, the last run ran 1 to " +
+                                  std::to_string(m->last_n));
+  const bool nyu = m->dataset == 1;
+  const long long N = (long long)m->out[0] * m->out[1] * m->out[2];
+  const long long work_len = OCCD_VOXEL_WORK_LEN((long long)m->batch, N);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  cudaError_t e;
+  // the scratch of every later listing, on the current device (the model's, as for the runs): the work array of
+  // `batch` items, and KITTI's masks
+  if (!m->list_work) {
+    if ((e = cudaMalloc(&m->list_work, (size_t)work_len * 4)) != cudaSuccess) {
+      m->list_work = nullptr;
+      return cuda_fail(e, "occd_model_list_voxels: cudaMalloc");
+    }
+    m->list_bytes += (size_t)work_len * 4;
+  }
+  if (!nyu && !m->list_mask) {
+    if ((e = cudaMalloc(&m->list_mask, (size_t)m->batch * N)) != cudaSuccess) {
+      m->list_mask = nullptr;
+      return cuda_fail(e, "occd_model_list_voxels: cudaMalloc");
+    }
+    m->list_bytes += (size_t)m->batch * N;
+  }
+  if (!nyu)
+    for (int b = 0; b < n; ++b) {
+      if (m->mask_valid[b]) continue;
+      int rc = fov_mask_1(m, (uint32_t)b, N, st);
+      if (rc != OCCD_OK) return rc;
+      m->mask_valid[b] = 1;
+    }
+  const double voxel = out->voxel_size > 0 ? out->voxel_size : nyu ? 0.08 : 0.2;
+  return occd_occupied_voxels(static_cast<const uint16_t*>(m->dev(ROLE_CLASSES)), nyu ? nullptr : m->list_mask, n,
+                              (int)m->out[0], (int)m->out[1], (int)m->out[2], 0, 0, 255, 64, out->capacity,
+                              reinterpret_cast<uint32_t*>(out->count), reinterpret_cast<uint32_t*>(out->hist),
+                              out->index, out->cls, out->xyz, voxel, out->origin, m->list_work, work_len, st);
 }
 
 extern "C" int occd_model_destroy(occd_model* m) {

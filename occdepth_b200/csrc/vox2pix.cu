@@ -38,7 +38,7 @@ int vox2pix_window(const char* who, const void* cam_E, int pose_is_f32, const fl
     occd_set_last_error(msg);
     return OCCD_ERR_ARG;
   };
-  if (!(cam_E && cam_k && vox_origin && pattern && pix && fov)) return refuse("null argument");
+  if (!(cam_E && cam_k && vox_origin && pattern && fov)) return refuse("null argument");  // pix may be NULL
   if (!(X > 0 && Y > 0 && Z > 0 && img_W > 0 && img_H > 0 && voxel_size > 0)) return refuse("dims");
   if (!(P >= 1 && P <= v2p::kMaxPattern)) return refuse("pattern size must be 1..25");
   const long long N = (long long)X * Y * Z;

@@ -27,7 +27,7 @@ struct Args {
   double voxel_size;
   int X, Y, Z, W, H, P;
   int pat[kMaxPattern][2];
-  long long* pix;        // [n][P][2] (x, y)
+  long long* pix;        // [n][P][2] (x, y), or null: only the mask (and pix_z) is written
   unsigned char* fov;    // [n][P] (numpy bool)
   T* pix_z;              // [n] or null
   long long v0 = 0;      // flat index of the window's first voxel; output i holds voxel v0 + i
@@ -125,8 +125,10 @@ V2P_HD void body(const Args<T>& a, long long n) {
   const long long yc = to_pix(add_rn(div_rn(mul_rn(cam[1], (T)a.fy), cam[2]), (T)a.cy));
   for (int p = 0; p < a.P; ++p) {
     const long long x = xc + a.pat[p][0], y = yc + a.pat[p][1];
-    a.pix[(n * a.P + p) * 2] = x;
-    a.pix[(n * a.P + p) * 2 + 1] = y;
+    if (a.pix) {
+      a.pix[(n * a.P + p) * 2] = x;
+      a.pix[(n * a.P + p) * 2 + 1] = y;
+    }
     a.fov[n * a.P + p] = (x >= 0 && x < a.W && y >= 0 && y < a.H && cam[2] > (T)0) ? 1 : 0;
   }
   if (a.pix_z) a.pix_z[n] = cam[2];

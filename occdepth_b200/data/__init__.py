@@ -51,7 +51,8 @@ def vox2pix_into(pix, fov, pix_z, cam_E, cam_k, vox_origin, voxel_size, img_W, i
     """vox2pix into caller-owned CUDA buffers (no allocation): pix int64 (N, P, 2), fov bool (N, P), pix_z: N values
     of the pose's precision (float32 for a float32 pose, else float64; any buffer of that many bytes).  Enqueued on
     the current stream of pix's device.  voxel_range=(v0, n): only voxels [v0, v0 + n) of the grid's C order (an
-    X-slab), written to buffers of n voxels -- that slice of the whole grid's result (`occd_vox2pix_range_fwd`)."""
+    X-slab), written to buffers of n voxels -- that slice of the whole grid's result (`occd_vox2pix_range_fwd`).
+    pix and pix_z may be None: a FOV mask alone, the same bytes, without the (N, P, 2) index scratch."""
     if not 0 <= int(pattern_id) < len(PIXEL_PATTERNS):
         raise IndexError("pattern_id out of range")        # the reference indexes the same 9-entry list
     X, Y, Z = (int(v) for v in volume_dims(vox_origin, voxel_size, scene_size))
@@ -67,13 +68,14 @@ def vox2pix_into(pix, fov, pix_z, cam_E, cam_k, vox_origin, voxel_size, img_W, i
         v0, N = (int(v) for v in voxel_range)
         if not (v0 >= 0 and N >= 1 and v0 + N <= X * Y * Z):
             raise ValueError("vox2pix_into: voxel_range (%d, %d) is not inside the %d-voxel grid" % (v0, N, X * Y * Z))
-    if (tuple(pix.shape) != (N, P, 2) or pix.dtype != torch.int64 or tuple(fov.shape) != (N, P)
-            or fov.dtype != torch.bool or not (pix.is_contiguous() and fov.is_contiguous())
-            or pix_z.numel() * pix_z.element_size() < N * (4 if f32_pose else 8)):
+    if ((pix is not None and (tuple(pix.shape) != (N, P, 2) or pix.dtype != torch.int64 or not pix.is_contiguous()))
+            or tuple(fov.shape) != (N, P) or fov.dtype != torch.bool or not fov.is_contiguous()
+            or (pix_z is not None and pix_z.numel() * pix_z.element_size() < N * (4 if f32_pose else 8))):
         raise ValueError("vox2pix_into: the buffers do not hold a (%d, %d) index grid" % (N, P))
     args = (E.ctypes.data_as(C.c_void_p), 1 if f32_pose else 0, k32.ctypes.data_as(C.c_void_p),
             o32.ctypes.data_as(C.c_void_p), float(voxel_size), X, Y, Z, int(img_W), int(img_H),
-            pat.ctypes.data_as(C.c_void_p), P, pix.data_ptr(), fov.data_ptr(), pix_z.data_ptr())
+            pat.ctypes.data_as(C.c_void_p), P, None if pix is None else pix.data_ptr(), fov.data_ptr(),
+            None if pix_z is None else pix_z.data_ptr())
     if voxel_range is None:
         _lib.check(_lib.lib().occd_vox2pix_fwd(*args, _lib.stream_ptr()), "occd_vox2pix_fwd")
     else:

@@ -429,6 +429,7 @@ class LoadedModel:
         self.handle = h
         self.comm = comm
         self.geom = self.info()
+        self._last_n = 0               # frames of the last run through this object (list_voxels' default n)
 
     def info(self):
         g = _lib.ModelGeom()
@@ -472,7 +473,9 @@ class LoadedModel:
             assert conf.dtype == torch.float16 and conf.is_contiguous() and conf.shape == out.shape
         keep = [c[1] for c in calls]
         st = _stream_for(stream, [t for c in keep for t in c if isinstance(t, torch.Tensor)] + [out, conf])
+        self._last_n = 0
         _lib.check(run(self.handle, fa, n, _ptr(out), _ptr(conf), st), run.__name__)
+        self._last_n = n
         return out if conf is None else (out, conf)
 
     def run_frame(self, frame, out=None, stream=None, graph=True, conf=None):
@@ -484,12 +487,54 @@ class LoadedModel:
         root = self.comm is None or self.comm.rank == 0
         f, keep, out, conf_t, st = _frame_call(self.geom, frame, out, stream, graph, conf, root, "rgb",
                                                "LoadedModel.run_frame")
+        self._last_n = 0
         if conf is None:
             _lib.check(_lib.lib().occd_model_run_frame(self.handle, C.byref(f), _ptr(out), st), "occd_model_run_frame")
+            self._last_n = 1
             return out if root else None
         _lib.check(_lib.lib().occd_model_run_frame_conf(self.handle, C.byref(f), _ptr(out), _ptr(conf_t), st),
                    "occd_model_run_frame_conf")
+        self._last_n = 1
         return (out, conf_t) if root else None
+
+    def list_voxels(self, n=None, capacity=None, voxel_size=None, vox_origin=None, xyz=True, out=None, stream=None):
+        """The occupied-voxel list of the maps the last run left on the device (occd_model_list_voxels) ->
+        voxels.VoxelList with B = n, enqueued on `stream` (default: the current stream); nothing is read back until
+        the caller asks the list for counts or rows.  Bit for bit OccDepth.predict_voxels of the frames that run saw:
+        rows split by each frame's fov_mask_1 (KITTI; NYU lists every row as inside), labels remapped when the file
+        was exported with inv_map.  Works after run_frame, run_frames and run_frame_group (on models[0]).
+
+        n: items [0, n) of the last run (default: all of them).  capacity: rows per frame (default N: never
+        truncates).  voxel_size: of the output grid (default 0.2 KITTI, 0.08 NYU); vox_origin: added to the centres;
+        xyz=False: no coordinates.  out: a VoxelList of an earlier call with the same n, capacity and xyz, whose
+        tensors are overwritten."""
+        from .voxels import VoxelList
+        g = self.geom
+        n = self._last_n if n is None else int(n)
+        N = g.X * g.Y * g.Z
+        cap = N if capacity is None else int(capacity)
+        if cap < 0:
+            raise ValueError("LoadedModel.list_voxels: capacity must be >= 0")
+        if vox_origin is not None and not xyz:
+            raise ValueError("LoadedModel.list_voxels: vox_origin without coordinates (xyz=False)")
+        origin = None
+        if vox_origin is not None:
+            origin = np.ascontiguousarray(np.asarray(vox_origin, dtype=np.float64).reshape(-1))
+            if origin.shape != (3,):
+                raise ValueError("LoadedModel.list_voxels: vox_origin must hold 3 values")
+        if out is not None and ((out.B, out.N, out.capacity) != (n, N, cap) or (out.xyz is not None) != bool(xyz)):
+            raise ValueError("LoadedModel.list_voxels: `out` was made for another n, capacity or xyz")
+        if out is None:
+            # n < 1 (or no run yet) is the library's to refuse; the list it is refused with still has one item
+            out = VoxelList(max(n, 1), N, cap, bool(xyz), torch.device("cuda", torch.cuda.current_device()))
+        out._counts = None
+        vo = _lib.VoxelOut(capacity=cap, voxel_size=0.0 if voxel_size is None else float(voxel_size),
+                           origin=None if origin is None else origin.ctypes.data, count=out.count.data_ptr(),
+                           hist=out.hist.data_ptr(), index=out.index.data_ptr(), cls=out.cls.data_ptr(),
+                           xyz=_ptr(out.xyz))
+        st = _stream_for(stream, [out.count, out.hist, out.index, out.cls, out.xyz])
+        _lib.check(_lib.lib().occd_model_list_voxels(self.handle, n, C.byref(vo), st), "occd_model_list_voxels")
+        return out
 
     def close(self):
         if self.handle:
@@ -509,8 +554,12 @@ def run_frame_group(models, frame, out=None, stream=None, graph=True, conf=None)
     hs = (C.c_void_p * len(models))(*[m.handle.value for m in models])
     f, keep, out, conf_t, st = _frame_call(models[0].geom, frame, out, stream, graph, conf, True, "rgb",
                                            "deploy.run_frame_group")
+    for m in models:
+        m._last_n = 0
     _lib.check(_lib.lib().occd_model_run_frame_group(hs, len(models), C.byref(f), _ptr(out), _ptr(conf_t), st),
                "occd_model_run_frame_group")
+    for m in models:
+        m._last_n = 1
     return out if conf is None else (out, conf_t)
 
 

@@ -10,6 +10,7 @@ the device (occdepth_b200.losses).  Training (`training_step`, backward, optimis
 scope.
 """
 import os
+from collections.abc import Mapping
 
 import torch
 import torch.nn as nn
@@ -744,7 +745,19 @@ class OccDepth(_Base, B200Module):
         rank's X-slab with the whole grid's flat indices and coordinates: the ranks' in-FOV rows concatenated in rank
         order, then their out-of-FOV rows, are the unpartitioned list.  A camera frame's default mask is then this
         rank's window of it, from `occd_vox2pix_range_fwd`.  slab_output="root": rank 0 lists the gathered whole map
-        (the unpartitioned list exactly), the other ranks return None."""
+        (the unpartitioned list exactly), the other ranks return None.
+
+        A list of camera frames runs through predict_frames' B-frame plan (B = len(list), the same plan and key) and
+        gives one VoxelList with B = n: frame i's counts, histogram and rows bit for bit those of predict_voxels of
+        frame i alone.  Each list position keeps its own default mask while its calibration stays the same; an
+        explicit fov_mask holds one mask per frame.  The frames are refused as predict_frames refuses them (so a list
+        under enable_slab_parallel is), and slab_output must be None."""
+        if isinstance(batch_or_frame, (list, tuple)):
+            return self._predict_voxels_list(batch_or_frame, inv_map, fov_mask, capacity, voxel_size, vox_origin, out,
+                                             slab_output)
+        if not isinstance(batch_or_frame, Mapping):
+            raise TypeError("OccDepth.predict_voxels: takes a tensor batch, a camera frame dict or a list of camera "
+                            "frames, got %s" % type(batch_or_frame).__name__)
         window_mask = None
         if "projected_pix_%d" % self.project_scale in batch_or_frame:
             y = self.predict_classes(batch_or_frame, inv_map)
@@ -764,16 +777,37 @@ class OccDepth(_Base, B200Module):
             return None
         return self._list_voxels(y, x_range, fov_mask, capacity, voxel_size, vox_origin, out, window_mask)
 
+    def _predict_voxels_list(self, frames, inv_map, fov_mask, capacity, voxel_size, vox_origin, out, slab_output):
+        """predict_voxels of a list of camera frames: the refusals (host-side, before any device work), the B-frame
+        plan, then one listing of its n maps"""
+        if slab_output is not None:
+            raise ValueError("OccDepth.predict_voxels: a list of frames takes no slab_output (the slab partition runs "
+                             "one frame per forward)")
+        for i, fr in enumerate(frames):
+            if not isinstance(fr, Mapping) or "projected_pix_%d" % self.project_scale in fr:
+                raise TypeError("OccDepth.predict_voxels: item %d of the list is not a camera frame dict" % i)
+        fs = self._frames_checked(frames)
+        y = self._run_frames(fs, len(fs), True, inv_map)
+        if y is None:                          # prepare(): the plan was built, nothing ran
+            return None
+        window_mask = None
+        if fov_mask is None:
+            if self.dataset == "NYU":
+                fov_mask = False
+            else:
+                window_mask = torch.stack([self._frame_fov_mask_1(f, None, b) for b, f in enumerate(fs)])
+        return self._list_voxels(y, None, fov_mask, capacity, voxel_size, vox_origin, out, window_mask)
+
     def _list_voxels(self, y, x_range, fov_mask, capacity, voxel_size, vox_origin, out, window_mask=None):
         """the list of class map `y` [B, Xl, Y, Z]: the whole grid, or planes x_range = [lo, hi) of it.  fov_mask holds
-        the whole grid per frame; window_mask (one frame) only y's planes of it"""
+        the whole grid per frame; window_mask ([B, ...] on the device) only y's planes of it"""
         from ..voxels import occupied_voxels
         B, _, Y, Z = y.shape
         lo, hi = (0, y.shape[1]) if x_range is None else x_range
         n_full = int(self.full_scene_size[0]) * Y * Z
         mask = None
         if window_mask is not None:
-            mask = window_mask.view(1, -1)
+            mask = window_mask.view(B, -1)
         elif fov_mask is not None and fov_mask is not False:
             frames = [fov_mask] if getattr(fov_mask, "ndim", 0) == 1 else list(fov_mask)
             rows = []
@@ -793,13 +827,18 @@ class OccDepth(_Base, B200Module):
         return occupied_voxels(y, mask, voxel_size=voxel_size, vox_origin=vox_origin, capacity=capacity,
                                index0=lo * Y * Z, out=out)
 
-    def _frame_fov_mask_1(self, f, x_range=None):
+    def _frame_fov_mask_1(self, f, x_range=None, item=None):
         """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
         resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only; x_range = [lo, hi): only those X
-        planes of it.  Kept with the calibration and window it was computed from."""
+        planes of it.  Kept with the calibration and window it was computed from: one mask for single frames, one per
+        list position `item` for lists of frames.  Computed without the pixel indices (`occd_vox2pix_fwd` with no
+        pix), as the model-file runtime computes it."""
         import numpy as np
         from .. import data as D
-        held = self.__dict__.get("_fov_mask_1")
+        if item is None:
+            held = self.__dict__.get("_fov_mask_1")
+        else:
+            held = self.__dict__.setdefault("_fov_masks_1", {}).get(item)
         key = (f["calib"], x_range)
         if f["calib"] is not None and held is not None and held[0] == key and held[1].device == f["imgs"].device:
             return held[1]
@@ -816,13 +855,14 @@ class OccDepth(_Base, B200Module):
         dev = f["imgs"].device
         E, K = f["poses"][0]
         with torch.cuda.device(dev):
-            pix = torch.empty(n, 1, 2, dtype=torch.int64, device=dev)
             fov = torch.empty(n, 1, dtype=torch.bool, device=dev)
-            pix_z = torch.empty(n, dtype=torch.float64, device=dev)
-            D.vox2pix_into(pix, fov, pix_z, E, K, f["vox_origin"], voxel, f["W"], f["H"], f["scene_size"], 0,
+            D.vox2pix_into(None, fov, None, E, K, f["vox_origin"], voxel, f["W"], f["H"], f["scene_size"], 0,
                            voxel_range=window)
         mask = fov.view(-1)
-        self.__dict__["_fov_mask_1"] = (key, mask)
+        if item is None:
+            self.__dict__["_fov_mask_1"] = (key, mask)
+        else:
+            self.__dict__["_fov_masks_1"][item] = (key, mask)
         return mask
 
     def _outputs(self, ent):

@@ -4,7 +4,7 @@
  * the library (occdepth_b200/lib/occd_run).
  *
  *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] [--depth DEPTH] [--no-graph]
- *            [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
+ *            [--voxels CAP] [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
  *
  * Inputs are raw little-endian files, one record per frame, frames back to back (no image decoder):
  *   IMAGES  N x V x H0 x W0 x 3 uint8, RGB, row-major (H0 x W0 default to the model's crop; --raw gives larger
@@ -17,6 +17,12 @@
  * Output: OUT_DIR/NNNNNN.label per frame, the uint16 class map (X x Y x Z, C order) as the KITTI submission writer
  * stores it; the labels are remapped when the model was exported with inv_map.  Prints ms per frame (device time
  * of occd_model_run_frames_ex, from CUDA events) and the mean over the frames after the first.
+ *
+ * --voxels CAP: after each run, occd_model_list_voxels lists the occupied voxels of every frame's map (CAP rows per
+ * frame at most; coordinates at the dataset's output voxel size, in the grid's frame) and OUT_DIR/NNNNNN.voxels gets,
+ * little-endian: int32 count[2] (occupied voxels inside / outside the FOV, the true counts), int32 hist[64] (per class
+ * id), then the R = min(CAP, count[0] + count[1]) written rows as int32 index[R], uint16 cls[R], float32 xyz[R][3]
+ * (in-FOV rows first, each group in ascending flat index).  The two counts are printed per frame.
  *
  * A batched model file (deploy.export of a list of B frames) runs the frames in groups of B, the last group short;
  * the times are then per group, and the mean is per frame over the groups after the first.
@@ -87,15 +93,42 @@ static int share_id(const char* path, int rank, const char* nccl_lib, char* id) 
   return 0;
 }
 
+/* OUT_DIR/NNNNNN.voxels of item i of a group of k listed frames: its counts and histogram from h (the group's k x 2
+ * counts, then k x 64 bins), its written rows read back from the device lists */
+static int write_voxels(const char* out_dir, int frame, int32_t* h, int k, int i, int cap, const int32_t* d_index,
+                        const uint16_t* d_cls, const float* d_xyz) {
+  const int32_t* count = h + 2 * i;
+  const int32_t* hist = h + 2 * k + 64 * i;
+  const long long total = (long long)count[0] + count[1];
+  const size_t r = (size_t)(total < cap ? total : cap);
+  char* rows = (char*)(h + 66 * k);  /* after the group's counts and bins */
+  if (cudaMemcpy(rows, d_index + (size_t)i * cap, r * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(rows + r * 4, d_cls + (size_t)i * cap, r * 2, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(rows + r * 6, d_xyz + (size_t)i * cap * 3, r * 12, cudaMemcpyDeviceToHost) != cudaSuccess) {
+    fprintf(stderr, "occd_run: reading back the voxel rows failed\n");
+    return 0;
+  }
+  char path[4096];
+  snprintf(path, sizeof(path), "%s/%06d.voxels", out_dir, frame);
+  FILE* fo = fopen(path, "wb");
+  if (!fo || fwrite(count, 4, 2, fo) != 2 || fwrite(hist, 4, 64, fo) != 64 || fwrite(rows, 1, r * 18, fo) != r * 18) {
+    fprintf(stderr, "occd_run: cannot write %s\n", path);
+    return 0;
+  }
+  fclose(fo);
+  printf("frame %d: %d voxels inside the FOV, %d outside\n", frame, count[0], count[1]);
+  return 1;
+}
+
 int main(int argc, char** argv) {
   if (argc < 6) {
     fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] "
-                    "[--depth DEPTH] [--no-graph]\n");
+                    "[--depth DEPTH] [--no-graph] [--voxels CAP]\n");
     return 2;
   }
   const char *model_path = argv[1], *img_path = argv[2], *calib_path = argv[3], *out_dir = argv[5];
   const char *depth_path = NULL, *id_path = NULL, *nccl_lib = NULL;
-  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0, format = OCCD_PIX_RGB;
+  int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0, format = OCCD_PIX_RGB, cap = -1;
   for (int i = 6; i < argc; ++i) {
     if (!strcmp(argv[i], "--raw") && i + 2 < argc) {
       H0 = atoi(argv[++i]);
@@ -109,6 +142,12 @@ int main(int argc, char** argv) {
       }
     } else if (!strcmp(argv[i], "--depth") && i + 1 < argc) {
       depth_path = argv[++i];
+    } else if (!strcmp(argv[i], "--voxels") && i + 1 < argc) {
+      cap = atoi(argv[++i]);
+      if (cap < 0) {
+        fprintf(stderr, "occd_run: --voxels takes a capacity >= 0\n");
+        return 2;
+      }
     } else if (!strcmp(argv[i], "--no-graph")) {
       flags |= OCCD_FRAME_NO_GRAPH;
     } else if (!strcmp(argv[i], "--world") && i + 1 < argc) {
@@ -175,6 +214,19 @@ int main(int argc, char** argv) {
   CK(cudaMalloc(&d_img, img_bytes * B));
   CK(cudaMalloc(&d_map, map_bytes * B));
   if (g.has_depth) CK(cudaMalloc(&d_depth, depth_bytes * B));
+  /* --voxels: the lists of a group, and one frame's on the host */
+  int32_t *d_count = NULL, *d_hist = NULL, *d_index = NULL, *h_vox = NULL;
+  uint16_t* d_cls = NULL;
+  float* d_xyz = NULL;
+  const size_t row_bytes = 4 + 2 + 12;
+  if (cap >= 0 && rank == 0) {
+    CK(cudaMalloc((void**)&d_count, (size_t)B * 2 * 4));
+    CK(cudaMalloc((void**)&d_hist, (size_t)B * 64 * 4));
+    CK(cudaMalloc((void**)&d_index, (size_t)B * cap * 4 + 4));
+    CK(cudaMalloc((void**)&d_cls, (size_t)B * cap * 2 + 2));
+    CK(cudaMalloc((void**)&d_xyz, (size_t)B * cap * 12 + 12));
+    h_vox = (int32_t*)malloc((size_t)B * 66 * 4 + (size_t)cap * row_bytes + 4);
+  }
   CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
@@ -213,6 +265,19 @@ int main(int argc, char** argv) {
     OK(occd_model_run_frames_ex(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
     CK(cudaEventRecord(e1, st));
     if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes * k, cudaMemcpyDeviceToHost, st));
+    if (h_vox) {
+      occd_voxel_out vo;
+      memset(&vo, 0, sizeof(vo));
+      vo.capacity = cap;
+      vo.count = d_count;
+      vo.hist = d_hist;
+      vo.index = d_index;
+      vo.cls = d_cls;
+      vo.xyz = d_xyz;
+      OK(occd_model_list_voxels(m, k, &vo, st));
+      CK(cudaMemcpyAsync(h_vox, d_count, (size_t)k * 2 * 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(h_vox + (size_t)k * 2, d_hist, (size_t)k * 64 * 4, cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaStreamSynchronize(st));
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, e0, e1));
@@ -230,6 +295,7 @@ int main(int argc, char** argv) {
         return 1;
       }
       fclose(fo);
+      if (h_vox && !write_voxels(out_dir, i0 + i, h_vox, k, i, cap, d_index, d_cls, d_xyz)) return 1;
     }
     if (B == 1) printf("frame %d: %.3f ms\n", i0, ms);
     else printf("frames %d..%d: %.3f ms\n", i0, i0 + k - 1, ms);
@@ -248,6 +314,12 @@ int main(int argc, char** argv) {
   free(h_map);
   free(calib);
   free(fs);
+  free(h_vox);
+  cudaFree(d_count);
+  cudaFree(d_hist);
+  cudaFree(d_index);
+  cudaFree(d_cls);
+  cudaFree(d_xyz);
   cudaFree(d_img);
   cudaFree(d_map);
   if (d_depth) cudaFree(d_depth);
