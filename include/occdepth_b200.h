@@ -137,6 +137,12 @@ int occd_cl_to_planar(const void* in, int in_dtype, float* out, long long B, int
                                    /* probability, 1 / sum_c exp(l_c - max l), computed in fp32 and rounded once;   */
                                    /* NaN where a value is NaN or +inf.  The map is bit-identical to mode 3's, the   */
                                    /* lut does not touch the confidence, and the same refusals apply                */
+#define OCCD_OUT1_CLASS_U16_PROBS 5 /* class map and every class's probability: uint16 [B][positions], the map of */
+                                    /* OCCD_OUT1_CLASS_U16, then float16 [B][Cout][positions] (the planar mode's    */
+                                    /* layout), p_c = exp(l_c - m) / s rounded once from fp32, with m and s of mode  */
+                                    /* 4 (the probability at the map's class is mode 4's confidence, bit for bit);   */
+                                    /* NaN in every channel where a value is NaN or +inf.  The map is bit-identical  */
+                                    /* to mode 3's, the lut remaps the map only, and the same refusals apply         */
 #define OCCD_CLASS_LUT_MAX 64
 
 typedef struct {
@@ -245,6 +251,13 @@ int occd_argmax_classes(const float* in, void* out, long long B, int C, long lon
 /* +inf); out as occd_argmax_classes writes it, lut applied to the class only                                   */
 int occd_argmax_classes_conf(const float* in, void* out, void* conf, long long B, int C, long long S, const int* lut,
                              void* stream);
+/* occd_argmax_classes plus every class's softmax probability: probs (2-byte aligned) gets the float16 bits of      */
+/* softmax(in[b][:][s]) at probs[b][c][s], OCCD_OUT1_CLASS_U16_PROBS's arithmetic with the channels taken in      */
+/* ascending order by one thread: the same bytes as a conv epilogue that takes them so, within one float16 ulp of  */
+/* one that merges two threads' sums (NaN in every channel where a logit is NaN or +inf); map as                   */
+/* occd_argmax_classes writes it, lut applied to the map only                                                      */
+int occd_class_probs(const float* logits, void* map, void* probs, long long B, int C, long long S, const int* lut,
+                     void* stream);
 /* copy a channel window (C % 8 == 0) between channels-last buffers (torch.cat of CRP3D.py:90)    */
 int occd_copy_channels(const void* in, void* out, int dtype, long long positions, int C, int in_cstride,
                        int in_coff, int out_cstride, int out_coff, void* stream);
@@ -552,6 +565,12 @@ typedef struct {
 /* occd_model_run_frames for frames of any camera format; occd_model_run_frame(s/_conf) are this call with RGB.      */
 int occd_model_run_frames_ex(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps, void* conf,
                              void* stream);
+/* occd_model_run_frames_ex plus every class's probability: probs (DEVICE float16 [n][C][X][Y][Z], 2-byte aligned,  */
+/* C = occd_model_geom.n_classes) gets the float16 softmax of each item (OCCD_OUT1_CLASS_U16_PROBS).  Only for a    */
+/* file exported with probabilities (header flag bit 8), else OCCD_ERR_UNSUPPORTED; the other run calls on such a  */
+/* file copy only the map.  On a slab rank other than 0 class_maps and probs may be NULL.                          */
+int occd_model_run_frames_probs(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps, void* probs,
+                                void* stream);
 /* The occupied-voxel list (occd_occupied_voxels) of the maps the model's last run left on the device: items [0, n)  */
 /* of that run (1 <= n <= its n), empty = 0, ignore = 255, the labels remapped when the file has a class LUT.  The  */
 /* rows of each item are split by its fov_mask_1: vox2pix of the first view of the item's last staged calibration  */
@@ -589,6 +608,11 @@ int occd_comm_all_gather(occd_comm* comm, const void* src, void* dst, long long 
 /* bounds[2r + 1]; src holds this rank's hi - lo planes of plane_bytes each.  dst is ignored on the other ranks.     */
 int occd_comm_gather_root(occd_comm* comm, const void* src, void* dst, const int* bounds, long long plane_bytes,
                           void* stream);
+/* occd_comm_gather_root of `items` arrays at once: src holds items x (hi - lo) planes, item-major, and rank 0's dst  */
+/* items x X planes (X = bounds[2 * world - 1]), so item i of rank r lands at planes [i * X + lo, i * X + hi).  One  */
+/* grouped exchange; items == 1 is occd_comm_gather_root                                                           */
+int occd_comm_gather_root_items(occd_comm* comm, const void* src, void* dst, const int* bounds, long long plane_bytes,
+                                int items, void* stream);
 
 /* FlospDepth's per-camera tables on the host (FlospDepth.camera_tables of occdepth_b200, flosp_depth.py:466-541),  */
 /* bit for bit: cams[v] = {rows 0..2 of T[v] @ grid_to_lidar, rows 0..2 of K4[v], identity ida} (40 floats) and      */

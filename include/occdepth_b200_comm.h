@@ -46,6 +46,10 @@ int occd_model_load_slab(const char* path, occd_comm* comm, occd_model** m);
  * class_map and conf (NULL: the map only) as rank 0's of occd_model_run_frame / _conf. */
 int occd_model_run_frame_group(occd_model* const* models, int world, const occd_frame* frame, uint16_t* class_map,
                                void* conf, void* stream);
+/* occd_model_run_frame_group of files exported with probabilities: rank 0's whole map and its float16 [C][X][Y][Z]  */
+/* probabilities (probs, DEVICE), as occd_model_run_frames_probs writes them.  OCCD_ERR_UNSUPPORTED without the flag. */
+int occd_model_run_frame_group_probs(occd_model* const* models, int world, const occd_frame* frame,
+                                     uint16_t* class_map, void* probs, void* stream);
 
 #ifdef __cplusplus
 }

@@ -48,7 +48,7 @@ class SfaParams(C.Structure):
 
 CONV_MAX_TAPS, CONV_MAX_SRC, CONV_MAX_GROUPS = 81, 3, 8
 CONV_IMPL_TC, CONV_IMPL_SIMT, CONV_IMPL_HALO, CONV_IMPL_HALOX, CONV_IMPL_TCX, CONV_IMPL_AUTO = 0, 1, 2, 3, 4, 5
-OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16, OUT1_CLASS_U16_CONF = 0, 1, 2, 3, 4
+OUT1_NONE, OUT1_CL, OUT1_F32_PLANAR, OUT1_CLASS_U16, OUT1_CLASS_U16_CONF, OUT1_CLASS_U16_PROBS = 0, 1, 2, 3, 4, 5
 CLASS_LUT_MAX = 64
 ERR_ARG, ERR_CUDA, ERR_UNSUPPORTED, ERR_FORMAT, ERR_IO = 1, 2, 3, 4, 5
 MODEL_FORMAT_VERSION = 1
@@ -147,6 +147,7 @@ SYMBOLS = {
     "occd_softmax_planar_to_cl": (C.c_int, [_vp, _vp, _i, _ll, _i, _ll, _i, _i, _vp]),
     "occd_argmax_classes": (C.c_int, [_vp, _vp, _ll, _i, _ll, _vp, _vp]),
     "occd_argmax_classes_conf": (C.c_int, [_vp, _vp, _vp, _ll, _i, _ll, _vp, _vp]),
+    "occd_class_probs": (C.c_int, [_vp, _vp, _vp, _ll, _i, _ll, _vp, _vp]),
     "occd_normalize_rgb_u8": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "occd_stage_rgb_u8_cl": (C.c_int, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "occd_stage_camera_u8_cl": (C.c_int, [_vp, _i, _ll, _ll, _ll, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _i,
@@ -187,11 +188,13 @@ SYMBOLS = {
     "occd_model_run_frames": (C.c_int, [_vp, C.POINTER(Frame), _i, _vp, _vp, _vp]),
     "occd_model_run_frames_ex": (C.c_int, [_vp, C.POINTER(FrameEx), _i, _vp, _vp, _vp]),
     "occd_model_list_voxels": (C.c_int, [_vp, _i, C.POINTER(VoxelOut), _vp]),
+    "occd_model_run_frames_probs": (C.c_int, [_vp, C.POINTER(FrameEx), _i, _vp, _vp, _vp]),
     "occd_model_destroy": (C.c_int, [_vp]),
     "occd_flosp_camera_tables": (C.c_int, [_i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "occd_comm_halo_exchange": (C.c_int, [_vp, _vp, _ll, _i, _i, _vp]),
     "occd_comm_all_gather": (C.c_int, [_vp, _vp, _vp, _ll, _vp]),
     "occd_comm_gather_root": (C.c_int, [_vp, _vp, _vp, _vp, _ll, _vp]),
+    "occd_comm_gather_root_items": (C.c_int, [_vp, _vp, _vp, _vp, _ll, _i, _vp]),
 }
 # include/occdepth_b200_comm.h: communicators and slab model files; none of these is a launch a model file records
 COMM_SYMBOLS = {
@@ -201,6 +204,7 @@ COMM_SYMBOLS = {
     "occd_comm_destroy": (C.c_int, [_vp]),
     "occd_model_load_slab": (C.c_int, [C.c_char_p, _vp, C.POINTER(C.c_void_p)]),
     "occd_model_run_frame_group": (C.c_int, [C.POINTER(C.c_void_p), _i, C.POINTER(Frame), _vp, _vp, _vp]),
+    "occd_model_run_frame_group_probs": (C.c_int, [C.POINTER(C.c_void_p), _i, C.POINTER(Frame), _vp, _vp, _vp]),
 }
 COMM_ID_BYTES = 128
 VOXEL_TILE = 2048

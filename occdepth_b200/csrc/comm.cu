@@ -71,6 +71,7 @@ struct Post {
   const char* src = nullptr;
   long long bytes = 0;        // halo / gather-root: plane bytes; all-gather: shard bytes
   int halo = 0, planes = 0;
+  int items = 1;              // gather-root: items of [planes][plane bytes] each, X-major within an item
   std::vector<int> bounds;
 };
 
@@ -120,7 +121,7 @@ int run_local(LocalGroup* g, cudaStream_t st) {
   const int W = g->world;
   const Post& p0 = g->posts[0];
   for (int r = 1; r < W; ++r)
-    if (g->posts[r].kind != p0.kind || g->posts[r].bytes != p0.bytes)
+    if (g->posts[r].kind != p0.kind || g->posts[r].bytes != p0.bytes || g->posts[r].items != p0.items)
       return fail(OCCD_ERR_ARG, std::string(kKindNames[p0.kind]) + ": local rank " + std::to_string(r) +
                                     " posted another collective or size than rank 0 (the ranks are out of step)");
   int rc = OCCD_OK;
@@ -144,9 +145,12 @@ int run_local(LocalGroup* g, cudaStream_t st) {
     for (int r = 0; r < W && rc == OCCD_OK; ++r)
       for (int q = 0; q < W && rc == OCCD_OK; ++q) rc = copy(g->posts[r].base + q * pb, g->posts[q].src, pb, st);
   } else {
+    const long long X = p0.bounds[2 * W - 1];
     for (int q = 0; q < W && rc == OCCD_OK; ++q) {
       const int lo = p0.bounds[2 * q], hi = p0.bounds[2 * q + 1];
-      rc = copy(p0.base + (long long)lo * pb, g->posts[q].src, (long long)(hi - lo) * pb, st);
+      for (int i = 0; i < p0.items && rc == OCCD_OK; ++i)
+        rc = copy(p0.base + (i * X + lo) * pb, g->posts[q].src + (long long)i * (hi - lo) * pb, (long long)(hi - lo) * pb,
+                  st);
     }
   }
   return rc;
@@ -278,39 +282,66 @@ extern "C" int occd_comm_all_gather(occd_comm* c, const void* src, void* dst, lo
   return r == 0 ? OCCD_OK : nccl_fail(c, r, "occd_comm_all_gather");
 }
 
-extern "C" int occd_comm_gather_root(occd_comm* c, const void* src, void* dst, const int* bounds,
-                                     long long plane_bytes, void* stream) {
-  OCCD_CHECK_COMM(c, "occd_comm_gather_root");
-  OCCD_CHECK_ARG(src && bounds && plane_bytes > 0 && (c->rank != 0 || dst), "occd_comm_gather_root: bad arguments");
+namespace {
+
+// occd_comm_gather_root(_items): src [items][this rank's planes][plane_bytes] -> rank 0's dst [items][X][plane_bytes]
+int gather_root(occd_comm* c, const void* src, void* dst, const int* bounds, long long plane_bytes, int items,
+                cudaStream_t st, const char* who) {
+  const std::string w(who);
+  OCCD_CHECK_ARG(src && bounds && plane_bytes > 0 && items >= 1 && (c->rank != 0 || dst), (w + ": bad arguments").c_str());
   for (int r = 0; r < c->world; ++r)
     OCCD_CHECK_ARG(bounds[2 * r] == (r ? bounds[2 * r - 1] : 0) && bounds[2 * r + 1] > bounds[2 * r],
-                   "occd_comm_gather_root: the bounds must tile the planes from 0, rank by rank");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+                   (w + ": the bounds must tile the planes from 0, rank by rank").c_str());
   if (c->kind == OCCD_COMM_LOCAL) {
     Post p;
     p.kind = GATHER_ROOT;
     p.base = static_cast<char*>(dst);
     p.src = static_cast<const char*>(src);
     p.bytes = plane_bytes;
+    p.items = items;
     p.bounds.assign(bounds, bounds + 2 * c->world);
     return post(c, std::move(p), st);
   }
   const Nccl& N = c->nccl;
   char* d = static_cast<char*>(dst);
+  const char* sp = static_cast<const char*>(src);
+  const long long X = bounds[2 * c->world - 1];
   if (c->rank == 0) {
-    cudaError_t e = cudaMemcpyAsync(d, src, (size_t)((bounds[1] - bounds[0]) * plane_bytes), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) return fail(OCCD_ERR_CUDA, std::string("occd_comm_gather_root: ") + cudaGetErrorString(e));
+    const long long own = (bounds[1] - bounds[0]) * plane_bytes;
+    cudaError_t e = cudaMemcpy2DAsync(d, (size_t)(X * plane_bytes), src, (size_t)own, (size_t)own, (size_t)items,
+                                      cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return fail(OCCD_ERR_CUDA, w + ": " + cudaGetErrorString(e));
     if (c->world == 1) return OCCD_OK;
   }
+  // one grouped exchange: an item's planes are contiguous on both sides, so each item is one send / recv pair
   int r = N.group_start();
   if (c->rank == 0) {
-    for (int q = 1; q < c->world && r == 0; ++q)
-      r = N.recv(d + bounds[2 * q] * plane_bytes, (size_t)((bounds[2 * q + 1] - bounds[2 * q]) * plane_bytes),
-                 kNcclInt8, q, c->nc, st);
-  } else if (r == 0) {
-    r = N.send(src, (size_t)((bounds[2 * c->rank + 1] - bounds[2 * c->rank]) * plane_bytes), kNcclInt8, 0, c->nc, st);
+    for (int q = 1; q < c->world && r == 0; ++q) {
+      const long long n = (bounds[2 * q + 1] - bounds[2 * q]) * plane_bytes;
+      for (int i = 0; i < items && r == 0; ++i)
+        r = N.recv(d + (i * X + bounds[2 * q]) * plane_bytes, (size_t)n, kNcclInt8, q, c->nc, st);
+    }
+  } else {
+    const long long n = (bounds[2 * c->rank + 1] - bounds[2 * c->rank]) * plane_bytes;
+    for (int i = 0; i < items && r == 0; ++i) r = N.send(sp + i * n, (size_t)n, kNcclInt8, 0, c->nc, st);
   }
   const int r_end = N.group_end();
   if (r == 0) r = r_end;
-  return r == 0 ? OCCD_OK : nccl_fail(c, r, "occd_comm_gather_root");
+  return r == 0 ? OCCD_OK : nccl_fail(c, r, who);
+}
+
+}  // namespace
+
+extern "C" int occd_comm_gather_root(occd_comm* c, const void* src, void* dst, const int* bounds,
+                                     long long plane_bytes, void* stream) {
+  OCCD_CHECK_COMM(c, "occd_comm_gather_root");
+  return gather_root(c, src, dst, bounds, plane_bytes, 1, reinterpret_cast<cudaStream_t>(stream),
+                     "occd_comm_gather_root");
+}
+
+extern "C" int occd_comm_gather_root_items(occd_comm* c, const void* src, void* dst, const int* bounds,
+                                           long long plane_bytes, int items, void* stream) {
+  OCCD_CHECK_COMM(c, "occd_comm_gather_root_items");
+  return gather_root(c, src, dst, bounds, plane_bytes, items, reinterpret_cast<cudaStream_t>(stream),
+                     "occd_comm_gather_root_items");
 }

@@ -22,11 +22,47 @@ namespace {
 
 using namespace occd_conv;
 
+// the 8 accumulator sums of channel group g at one output position (conv_simt_kernel)
+template <typename T>
+__device__ __forceinline__ void simt_acc8(const SimtParams& p, int b, int od, int oh, int ow, int g, float* acc) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int tp = 0; tp < p.n_taps; ++tp) {
+    const int s = p.tap_src[tp];
+    const int id = od * p.stride[0] + p.tap_dz[tp] + p.src_d0;
+    const int ih = oh * p.stride[1] + p.tap_dy[tp];
+    const int iw = ow * p.stride[2] + p.tap_dx[tp];
+    if (id < 0 || id >= p.ID || ih < 0 || ih >= p.IH || iw < 0 || iw >= p.IW) continue;
+    const T* in = reinterpret_cast<const T*>(p.src[s]) +
+                  ((((long long)b * p.ID + id) * p.IH + ih) * p.IW + iw) * p.src_cstride[s] + p.src_coff[s];
+    const T* w = reinterpret_cast<const T*>(p.weight) +
+                 ((long long)b * p.w_batch_rows + (long long)tp * p.Cout_pad + g * 8) * p.Kpad;
+    const int C = p.src_C[s];
+    for (int c = 0; c < C; c += 8) {
+      float x[8];
+      Elem<T>::ld8(in + c, x);
+      if (c + 8 > C) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (c + i >= C) x[i] = 0.f;
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float wv[8];
+        Elem<T>::ld8_nc(w + (long long)j * p.Kpad + c, wv);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[j] = fmaf(x[i], wv[i], acc[j]);
+      }
+    }
+  }
+}
+
 // one thread per (output position, group of 8 channels); with a class-map output one thread per position walks every
-// channel group, so that one thread holds the position's arg-max
+// channel group, so that one thread holds the position's arg-max; with the probabilities it then walks them again,
+// recomputing each group's sums, and stores every channel's probability
 template <typename T>
 __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ SimtParams p) {
-  const bool cls = class_mode(p.epi.out1_mode), conf = p.epi.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
+  const bool cls = class_mode(p.epi.out1_mode), conf = class_softmax(p.epi.out1_mode);
   const int ngroups = cls ? 1 : p.epi.Cout_store / 8;
   const long long total = (long long)p.epi.B * p.epi.OD * p.epi.OH * p.epi.OW * ngroups;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -40,36 +76,7 @@ __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ 
   ClassArg ca = class_arg_init();
   for (int g = g0; g < g1; ++g) {
     float acc[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-    for (int tp = 0; tp < p.n_taps; ++tp) {
-      const int s = p.tap_src[tp];
-      const int id = od * p.stride[0] + p.tap_dz[tp] + p.src_d0;
-      const int ih = oh * p.stride[1] + p.tap_dy[tp];
-      const int iw = ow * p.stride[2] + p.tap_dx[tp];
-      if (id < 0 || id >= p.ID || ih < 0 || ih >= p.IH || iw < 0 || iw >= p.IW) continue;
-      const T* in = reinterpret_cast<const T*>(p.src[s]) +
-                    ((((long long)b * p.ID + id) * p.IH + ih) * p.IW + iw) * p.src_cstride[s] + p.src_coff[s];
-      const T* w = reinterpret_cast<const T*>(p.weight) +
-                   ((long long)b * p.w_batch_rows + (long long)tp * p.Cout_pad + g * 8) * p.Kpad;
-      const int C = p.src_C[s];
-      for (int c = 0; c < C; c += 8) {
-        float x[8];
-        Elem<T>::ld8(in + c, x);
-        if (c + 8 > C) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            if (c + i >= C) x[i] = 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float wv[8];
-          Elem<T>::ld8_nc(w + (long long)j * p.Kpad + c, wv);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[j] = fmaf(x[i], wv[i], acc[j]);
-        }
-      }
-    }
+    simt_acc8<T>(p, b, od, oh, ow, g, acc);
     if (!cls) {
       conv_epilogue_row<T, 8>(p.epi, b, od, oh, ow, g * 8, acc);
       continue;
@@ -79,7 +86,18 @@ __global__ void __launch_bounds__(128) conv_simt_kernel(const __grid_constant__ 
       if (g * 8 + i < p.epi.Cout)
         class_arg_take(ca, class_value<T>(p.epi, epi_pos(p.epi, b, od, oh, ow), g * 8 + i, acc[i]), g * 8 + i, conf);
   }
-  if (cls) class_store(p.epi, epi_pos(p.epi, b, od, oh, ow), ca);
+  if (!cls) return;
+  const long long ps = epi_pos(p.epi, b, od, oh, ow);
+  class_store(p.epi, ps, ca);
+  if (p.epi.out1_mode != OCCD_OUT1_CLASS_U16_PROBS) return;
+  for (int g = g0; g < g1; ++g) {
+    float acc[8];
+    simt_acc8<T>(p, b, od, oh, ow, g, acc);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (g * 8 + i < p.epi.Cout)
+        class_prob_store(p.epi, b, ps, g * 8 + i, class_value<T>(p.epi, ps, g * 8 + i, acc[i]), ca);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -506,8 +524,8 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int
     iters = (iters + n_groups - 1) / n_groups;   // tap groups: the mean group; every CTA gets its share of each
     const long long m_tiles0 = (long long)d->B * t.tiles_d * t.tiles_h * t.tiles_w * n_groups;
     const int n_sms = n_sms_current();
-    // (a class map, with or without its confidence, is costed as the planar logits it stands in for: every plan of
-    // one descriptor gets the same tiles, so the map equals the arg-max of the logits bit for bit)
+    // (a class map, with or without its confidence or probabilities, is costed as the planar logits it stands in
+    // for: every plan of one descriptor gets the same tiles, so the map equals the arg-max of the logits bit for bit)
     const double out_bytes_per_col = 128.0 * ((d->out0 ? pl->esize : 0) + (d->out1_mode == OCCD_OUT1_CL ? pl->esize : 0) +
                                               (d->out1_mode == OCCD_OUT1_F32_PLANAR || class_mode(d->out1_mode) ? 4 : 0));
     // per-tile mainloop and epilogue of an n-column tile that stores out_cols channels
@@ -534,6 +552,8 @@ static int tc_geometry(const occd_conv_desc* d, occd_conv_plan* pl, bool xp, int
   }
   PLAN_REQUIRE(!class_mode(d->out1_mode) || xp || t.N_tile >= d->Cout_pad,
                "a class map needs every output channel in one N tile");
+  PLAN_REQUIRE(d->out1_mode != OCCD_OUT1_CLASS_U16_PROBS || xp || t.N_tile <= kProbsMaxN,
+               "class probabilities need an N tile of at most 96 channels");
   PLAN_REQUIRE(xp ? TcxTiles::has(t.N_tile) : TcTiles::has(t.N_tile),
                xp ? "no kernel compiled for this Cout_pad (16, 32, 48, 64 or 80)" : "no kernel compiled for this N tile");
   t.rb = RB;

@@ -37,13 +37,15 @@ __device__ __forceinline__ long long epi_pos(const ConvEpi& e, int b, int od, in
   return epi_pos(e, b, od, oh, ow, e.oadd[0], e.oadd[1], e.oadd[2]);
 }
 
-// Running arg-max of the class-map output (OCCD_OUT1_CLASS_U16[_CONF]) over the channels one thread has seen, taken
+// Running arg-max of the class-map output (OCCD_OUT1_CLASS_U16[_CONF|_PROBS]) over the channels one thread has seen, taken
 // in ascending channel order.  The rule is argmax_classes_kernel's (elementwise.cu): the first index of the largest
 // value; a NaN in channel 0 wins, a NaN anywhere else is skipped.  A NaN channel 0 is held as +inf, which no later
 // value beats and which wins every tie by its index, so two threads' partial results merge with the same rule.
 // With a confidence (conf == true) the same pass keeps a running softmax of the raw values: m, their largest value
 // (NaN never becomes it), and s = sum exp(v - m).  The top-class probability is then 1 / s, and NaN where a value
 // is NaN (s is NaN) or +inf (m == +inf), or where every value is -inf (m == -inf): torch.softmax's NaN cases.
+// With the probabilities (OCCD_OUT1_CLASS_U16_PROBS) the same m and s are kept; once the row's result is complete
+// a second pass over its values writes exp(v - m) / s for every channel (class_arg_prob).
 // Host and device share the helpers, so that a CPU build can replay the epilogues' merge orders.
 struct ClassArg {
   float v;
@@ -51,7 +53,11 @@ struct ClassArg {
   float m, s;
 };
 __host__ __device__ __forceinline__ bool class_mode(int out1_mode) {
-  return out1_mode == OCCD_OUT1_CLASS_U16 || out1_mode == OCCD_OUT1_CLASS_U16_CONF;
+  return out1_mode >= OCCD_OUT1_CLASS_U16 && out1_mode <= OCCD_OUT1_CLASS_U16_PROBS;   // modes 3, 4 and 5
+}
+// the class-map modes that keep the running softmax beside the arg-max
+__host__ __device__ __forceinline__ bool class_softmax(int out1_mode) {
+  return out1_mode >= OCCD_OUT1_CLASS_U16_CONF && out1_mode <= OCCD_OUT1_CLASS_U16_PROBS;
 }
 __host__ __device__ __forceinline__ ClassArg class_arg_init() { return ClassArg{-INFINITY, 0x7fffffff, -INFINITY, 0.f}; }
 __host__ __device__ __forceinline__ void class_arg_take(ClassArg& a, float v, int c, bool conf) {
@@ -81,6 +87,11 @@ __host__ __device__ __forceinline__ void class_arg_join(ClassArg& a, const Class
 __host__ __device__ __forceinline__ float class_arg_conf(const ClassArg& a) {
   return (a.m == INFINITY || a.m == -INFINITY) ? NAN : 1.f / a.s;
 }
+// the probability of the class whose value is v, from a complete result: NaN wherever class_arg_conf is; at the
+// top class v == m, exp(0) == 1 and the quotient is class_arg_conf's bit for bit
+__host__ __device__ __forceinline__ float class_arg_prob(const ClassArg& a, float v) {
+  return (a.m == INFINITY || a.m == -INFINITY) ? NAN : expf(v - a.m) / a.s;
+}
 // the partial result of lane ^ mask joins this lane's (every lane of the warp calls it)
 __device__ __forceinline__ void class_arg_merge_xor(ClassArg& a, int mask, bool conf) {
   ClassArg b;
@@ -93,7 +104,8 @@ __device__ __forceinline__ void class_arg_merge_xor(ClassArg& a, int mask, bool 
   class_arg_join(a, b, conf);
 }
 // out1[pos]: the class map has the planar logits' spatial index, one uint16 per position; in OCCD_OUT1_CLASS_U16_CONF
-// the float16 confidence follows the whole map, at out1[B * positions + pos]
+// the float16 confidence follows the whole map, at out1[B * positions + pos]; in OCCD_OUT1_CLASS_U16_PROBS the
+// probabilities follow it (class_prob_store)
 __device__ __forceinline__ void class_store(const ConvEpi& e, long long pos, const ClassArg& a) {
   unsigned short* o = reinterpret_cast<unsigned short*>(e.out1);
   o[pos] = e.class_lut_use ? e.class_lut[a.c] : (unsigned short)a.c;
@@ -101,6 +113,16 @@ __device__ __forceinline__ void class_store(const ConvEpi& e, long long pos, con
     const __half_raw h = __float2half_rn(class_arg_conf(a));
     o[(long long)e.B * e.ODf * e.OHf * e.OWf + pos] = h.x;
   }
+}
+// the widest N tile whose row epilogue writes OCCD_OUT1_CLASS_U16_PROBS (see epilogue_rows)
+constexpr int kProbsMaxN = 96;
+// OCCD_OUT1_CLASS_U16_PROBS: the float16 probability of channel n (value v) at position pos of item b, at
+// out1[B * P + (b * Cout + n) * P + s] (P = positions, pos = b * P + s), from the complete result a
+__device__ __forceinline__ void class_prob_store(const ConvEpi& e, int b, long long pos, int n, float v,
+                                                 const ClassArg& a) {
+  const long long P = (long long)e.ODf * e.OHf * e.OWf;
+  const __half_raw h = __float2half_rn(class_arg_prob(a, v));
+  reinterpret_cast<unsigned short*>(e.out1)[(long long)e.B * P + pos + ((long long)b * (e.Cout - 1) + n) * P] = h.x;
 }
 // Pre-activation value of channel n at position pos from its accumulator sum: acc + bias + res1 (+ res2), the additions
 // of conv_epilogue_compute in its order, one channel at a time.  The class-map epilogues feed the arg-max with it
@@ -112,10 +134,10 @@ __device__ __forceinline__ float class_value(const ConvEpi& e, long long pos, in
   if (e.res2 && !e.res2_post) v += Elem<T>::up(reinterpret_cast<const T*>(e.res2)[pos * e.res2_cstride + e.res2_coff + n]);
   return v;
 }
-// class_value of the 8 channels [n0, n0 + 8) (n0 < Cout_store, a multiple of 8) with vector loads, taken into the
-// arg-max in ascending channel order
-template <typename T>
-__device__ __forceinline__ void class_take8(const ConvEpi& e, long long pos, int n0, const float* v, ClassArg& a) {
+// class_value of the 8 channels [n0, n0 + 8) (n0 < Cout_store, a multiple of 8) with vector loads, handed to
+// take(n, value) in ascending channel order
+template <typename T, typename Take>
+__device__ __forceinline__ void class_each8(const ConvEpi& e, long long pos, int n0, const float* v, Take&& take) {
   float x[8];
   const float4 b0 = __ldg(reinterpret_cast<const float4*>(e.bias + n0));
   const float4 b1 = __ldg(reinterpret_cast<const float4*>(e.bias + n0 + 4));
@@ -132,10 +154,9 @@ __device__ __forceinline__ void class_take8(const ConvEpi& e, long long pos, int
 #pragma unroll
     for (int i = 0; i < 8; ++i) x[i] += r[i];
   }
-  const bool conf = e.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
 #pragma unroll
   for (int i = 0; i < 8; ++i)
-    if (n0 + i < e.Cout) class_arg_take(a, x[i], n0 + i, conf);
+    if (n0 + i < e.Cout) take(n0 + i, x[i]);
 }
 
 // Epilogue arithmetic for one output position `pos` and NV consecutive channels [n0, n0+NV) held in v[] (fp32

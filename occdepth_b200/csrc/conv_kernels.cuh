@@ -129,7 +129,8 @@ __device__ __forceinline__ void stage8(float* st, const float (&acc)[N / 2], int
 // stores.  The caller gives the position of the thread's row; oa:
 // per-launch output offset (tap groups) or nullptr for e.oadd.  A class map needs the whole channel range in this
 // tile (n0 == 0, Cout <= N: plan creation refuses anything else); the two threads of a row merge their arg-max by
-// shuffle and the first one stores.
+// shuffle and the first one stores.  With the probabilities both threads of the row then stage their channels again
+// and store each channel's probability.
 template <typename T, int N, int LD>
 __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&acc)[N / 2], float* st, int bar_id,
                                               int warp4, int lane, int t, bool valid, int b, int od, int oh, int ow,
@@ -139,7 +140,7 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
   const int row = t / TPR, h = t % TPR;
   if (class_mode(e.out1_mode)) {
     // class map: every value joins the row's running arg-max (and softmax) as it leaves the staging buffer
-    const bool conf = e.out1_mode == OCCD_OUT1_CLASS_U16_CONF;
+    const bool conf = class_softmax(e.out1_mode);
     ClassArg ca = class_arg_init();
     const long long pos = valid ? epi_pos(e, b, od, oh, ow) : 0;
 #pragma unroll
@@ -158,6 +159,27 @@ __device__ __forceinline__ void epilogue_rows(const ConvEpi& e, const float (&ac
     }
     if constexpr (TPR == 2) class_arg_merge_xor(ca, 1, conf);
     if (valid && row < 64 && h == 0) class_store(e, pos, ca);
+    // the probabilities: the same rounds again, now that the row's softmax is complete (wider tiles hold too many
+    // accumulator registers for a second pass: plan creation refuses them the mode)
+    if constexpr (N <= kProbsMaxN) {
+      if (e.out1_mode == OCCD_OUT1_CLASS_U16_PROBS) {
+#pragma unroll
+        for (int c0 = 0; c0 < N; c0 += ROUND) {
+          tc::wg_sync(bar_id);
+#pragma unroll
+          for (int j = 0; j < ROUND / 8; ++j)
+            if (c0 + 8 * j < N) stage8<LD, N>(st, acc, (c0 >> 3) + j, 8 * j, warp4, lane);
+          tc::wg_sync(bar_id);
+          const int cc = c0 + VW * h;
+          if (valid && row < 64 && cc < N) {
+#pragma unroll 1
+            for (int i = 0; i < VW && n0 + cc + i < e.Cout; ++i)
+              class_prob_store(e, b, pos, n0 + cc + i, class_value<T>(e, pos, n0 + cc + i, st[row * LD + VW * h + i]),
+                               ca);
+          }
+        }
+      }
+    }
     return;
   }
   const bool fast = VW == 16 && epi_fast_ok(e);
@@ -220,7 +242,8 @@ struct XpRows {
 // one in the next or previous warp comes through the exchange buffer xb (xp_xchg_floats(d) floats, this
 // warpgroup's).  Chunks of 16 channels: two barriers each.  The sums of a row's 8-channel block are then gathered
 // into one lane of the quad (a 4 x 4 transpose of channel pairs by shuffle), which runs the row epilogue on them;
-// a class map instead takes them into the row's running arg-max (and softmax), and the two lanes of a row merge theirs.
+// a class map instead takes them into the row's running arg-max (and softmax), and the two lanes of a row merge theirs;
+// with the probabilities the chunk loop then runs again and both lanes store their channels' probabilities.
 template <typename T, int N>
 __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)[N / 2], float* xb, int bar_id,
                                             int warp4, int lane, int d, const XpRows& rows, int b) {
@@ -231,10 +254,10 @@ __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)
   const int wfl = 2 * d * 16;   // exchange floats per warp: [Q_0 of the last d rows, Q_2 of the first d rows][16]
   float* const mine = xb + warp4 * wfl;
   const bool my_valid = rows.valid;   // after the transpose this lane holds 8 channels of row 16 w + g + 8 (q >> 1)
-  // one copy of the chunk loop per output kind (CLS: class map), so that neither carries the other's registers
-  auto chunks = [&](auto cls) {
+  // one copy of the chunk loop per output kind (CLS: class map), so that neither carries the other's registers;
+  // a class map's values go to take(n, value)
+  auto chunks = [&](auto cls, auto&& take) {
     constexpr bool CLS = decltype(cls)::value;
-    ClassArg ca = class_arg_init();
     const long long pos = CLS && my_valid ? epi_pos(e, b, rows.od, rows.oh, rows.ow) : 0;
 #pragma unroll
     for (int c0 = 0; c0 < CP; c0 += 16) {
@@ -290,19 +313,26 @@ __device__ __forceinline__ void epilogue_xp(const ConvEpi& e, const float (&acc)
       for (int i = 0; i < 4; ++i) { w8[2 * i] = o[i].x; w8[2 * i + 1] = o[i].y; }
       const int n0 = c0 + 8 * (q & 1);
       if constexpr (CLS) {
-        if (my_valid && n0 < e.Cout) class_take8<T>(e, pos, n0, w8, ca);
+        if (my_valid && n0 < e.Cout) class_each8<T>(e, pos, n0, w8, take);
       } else {
         if (my_valid) conv_epilogue_row<T, 8>(e, b, rows.od, rows.oh, rows.ow, n0, w8);
       }
     }
-    if constexpr (CLS) {
-      // lanes q and q ^ 1 hold the two blocks of each chunk of one row
-      class_arg_merge_xor(ca, 1, e.out1_mode == OCCD_OUT1_CLASS_U16_CONF);
-      if ((q & 1) == 0 && my_valid) class_store(e, pos, ca);
-    }
   };
-  if (class_mode(e.out1_mode)) chunks(std::true_type{});
-  else chunks(std::false_type{});
+  if (class_mode(e.out1_mode)) {
+    const bool conf = class_softmax(e.out1_mode);
+    ClassArg ca = class_arg_init();
+    chunks(std::true_type{}, [&](int n, float v) { class_arg_take(ca, v, n, conf); });
+    // lanes q and q ^ 1 hold the two blocks of each chunk of one row
+    class_arg_merge_xor(ca, 1, conf);
+    if ((q & 1) == 0 && my_valid) class_store(e, epi_pos(e, b, rows.od, rows.oh, rows.ow), ca);
+    if (e.out1_mode == OCCD_OUT1_CLASS_U16_PROBS) {
+      const long long pos = my_valid ? epi_pos(e, b, rows.od, rows.oh, rows.ow) : 0;
+      chunks(std::true_type{}, [&](int n, float v) { class_prob_store(e, b, pos, n, v, ca); });
+    }
+  } else {
+    chunks(std::false_type{}, [](int, float) {});
+  }
 }
 
 __device__ __forceinline__ void pdl_prologue_done(int pdl) {

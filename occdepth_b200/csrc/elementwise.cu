@@ -100,6 +100,25 @@ __global__ void argmax_classes_conf_kernel(const float* __restrict__ in, unsigne
   conf[i] = h.x;
 }
 
+// argmax_classes_conf_kernel's pass, then a second one over the same logits that writes every class's probability
+// (OCCD_OUT1_CLASS_U16_PROBS's second part, probs[b][c][s])
+__global__ void class_probs_kernel(const float* __restrict__ in, unsigned short* __restrict__ out,
+                                   unsigned short* __restrict__ probs, int C, long long S, long long total,
+                                   const ClassLut lut) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const long long b = i / S, s = i - b * S;
+  const float* p = in + b * C * S + s;
+  ClassArg a = class_arg_init();
+  for (int c = 0; c < C; ++c) class_arg_take(a, p[(long long)c * S], c, true);
+  out[i] = lut.use ? lut.v[a.c] : (unsigned short)a.c;
+  unsigned short* q = probs + b * C * S + s;
+  for (int c = 0; c < C; ++c) {
+    const __half_raw h = __float2half_rn(class_arg_prob(a, p[(long long)c * S]));
+    q[(long long)c * S] = h.x;
+  }
+}
+
 int class_lut_of(const int* lut, int C, ClassLut* l) {
   l->use = lut ? 1 : 0;
   for (int c = 0; c < kMaxLut; ++c) l->v[c] = (lut && c < C) ? (unsigned short)lut[c] : 0;  // .astype(np.uint16)
@@ -134,6 +153,22 @@ extern "C" int occd_argmax_classes_conf(const float* in, void* out, void* conf, 
   class_lut_of(lut, C, &l);
   argmax_classes_conf_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       in, (unsigned short*)out, (unsigned short*)conf, C, S, total, l);
+  OCCD_CHECK_LAUNCH();
+  return OCCD_OK;
+}
+
+extern "C" int occd_class_probs(const float* logits, void* map, void* probs, long long B, int C, long long S,
+                                const int* lut, void* stream) {
+  OCCD_CHECK_ARG(logits && map && probs && B > 0 && C > 0 && C <= 65535 && S > 0, "occd_class_probs: args");
+  OCCD_CHECK_ARG(reinterpret_cast<uintptr_t>(map) % 2 == 0 && reinterpret_cast<uintptr_t>(probs) % 2 == 0,
+                 "occd_class_probs: map and probs must be 2-byte aligned");
+  OCCD_CHECK_ARG(!lut || C <= kMaxLut, "occd_class_probs: a label remap supports at most 64 classes");
+  const long long total = B * S;
+  OCCD_CHECK_ARG((total + 255) / 256 <= 2147483647LL, "occd_class_probs: too many positions");
+  ClassLut l;
+  class_lut_of(lut, C, &l);
+  class_probs_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      logits, (unsigned short*)map, (unsigned short*)probs, C, S, total, l);
   OCCD_CHECK_LAUNCH();
   return OCCD_OK;
 }

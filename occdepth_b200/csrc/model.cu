@@ -123,14 +123,15 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_occupied_voxels),       OCCD_ENTRY(occd_virtual_view_fwd),
     OCCD_ENTRY(occd_vox2pix_range_fwd),     OCCD_ENTRY(occd_argmax_classes_conf),
     OCCD_ENTRY(occd_virtual_view_items_fwd), OCCD_ENTRY(occd_stage_camera_u8_cl),
+    OCCD_ENTRY(occd_class_probs),
     // take a stream like the launches (occd_model_batch is bound like them), so they have a signature here; their
     // model handle can only be NULL
     OCCD_ENTRY(occd_model_run_frame_conf),  OCCD_ENTRY(occd_model_run_frames),
     OCCD_ENTRY(occd_model_batch),           OCCD_ENTRY(occd_model_run_frames_ex),
-    OCCD_ENTRY(occd_model_list_voxels),
+    OCCD_ENTRY(occd_model_list_voxels),     OCCD_ENTRY(occd_model_run_frames_probs),
     // the X-slab partition's collectives: the lock-step runner of a local group stops after each
     OCCD_ENTRY(occd_comm_halo_exchange),    OCCD_ENTRY(occd_comm_all_gather),
-    OCCD_ENTRY(occd_comm_gather_root),
+    OCCD_ENTRY(occd_comm_gather_root),     OCCD_ENTRY(occd_comm_gather_root_items),
 };
 
 bool is_collective(const Entry* e) { return strncmp(e->name, "occd_comm_", 10) == 0; }
@@ -147,7 +148,10 @@ enum Role { ROLE_IMG, ROLE_PIX, ROLE_FOV, ROLE_PIX_Z, ROLE_DEPTH, ROLE_CAMS, ROL
 const char* kRoleNames[N_ROLES] = {"image", "pix", "fov", "pix_z", "depth", "camera tables", "scaled_pixel_size",
                                    "class map"};
 enum { FLAG_FLOSP_DEPTH = 1, FLAG_VIRTUAL = 2, FLAG_CONF = 4,   // FLAG_CONF: the class-map role holds the map, then its
-       FLAG_SLAB = 16, FLAG_BATCH = 32, FLAG_MAPS = 64 };        // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
+       FLAG_SLAB = 16, FLAG_BATCH = 32, FLAG_MAPS = 64,           // float16 confidence (OCCD_OUT1_CLASS_U16_CONF);
+       FLAG_PROBS = 256 };                                       // FLAG_PROBS: the class-map role holds the B maps,
+                                                                 // then the B x C float16 probability planes
+                                                                 // (OCCD_OUT1_CLASS_U16_PROBS);
                                                                  // FLAG_SLAB: one rank's plan, a slab block follows;
                                                                  // FLAG_BATCH: a B-frame plan, a batch block follows
                                                                  // the roles (bit 3 stays unassigned); FLAG_MAPS: a
@@ -271,6 +275,10 @@ struct occd_model {
   // item b's part of an input role, which holds `batch` items of equal length
   void* dev(int role, uint32_t b) const { return static_cast<uint8_t*>(dev(role)) + roles[role].len / batch * b; }
   uint64_t map_bytes() const { return (uint64_t)out[0] * out[1] * out[2] * 2; }   // one uint16 class map
+  // map-sized planes per item in the class-map role: the map, and its confidence or its C probabilities
+  uint64_t maps_per_item() const {
+    return (flags & FLAG_PROBS) ? 1 + (uint64_t)n_classes : (flags & FLAG_CONF) ? 2 : 1;
+  }
   void* dev_maps() const { return arena + buf_off[maps.buffer] + maps.off; }
 };
 
@@ -365,8 +373,14 @@ int parse(occd_model* m) {
   if ((m->precision != OCCD_DTYPE_F32 && m->precision != OCCD_DTYPE_BF16) || m->dataset > 1 || m->V < 1 ||
       m->V > 4 || m->P < 1 || m->P > 64 || m->n_cams > 4 || m->img_cstride % 8 != 0)
     return fail(OCCD_ERR_FORMAT, "occd_model_load: header field out of range");
-  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB | FLAG_BATCH | FLAG_MAPS))
+  if (m->flags & ~(uint32_t)(FLAG_FLOSP_DEPTH | FLAG_VIRTUAL | FLAG_CONF | FLAG_SLAB | FLAG_BATCH | FLAG_MAPS |
+                             FLAG_PROBS))
     return fail(OCCD_ERR_FORMAT, "occd_model_load: unknown header flag bits");
+  if ((m->flags & FLAG_PROBS) && (m->flags & FLAG_CONF))
+    return fail(OCCD_ERR_FORMAT, "occd_model_load: header flag bits 2 (confidence) and 8 (probabilities) together: "
+                                 "the confidence is the probability at the map's class");
+  if ((m->flags & FLAG_PROBS) && (m->n_classes < 1 || m->n_classes > 65535))
+    return fail(OCCD_ERR_FORMAT, "occd_model_load: class probabilities need 1 to 65535 classes");
   if (m->slab()) {
     // every rank's slab, in rank order, tiles the lift grid's X planes; this rank's window is its slab's voxels
     const uint64_t plane = (uint64_t)m->grid[1] * m->grid[2];
@@ -502,7 +516,7 @@ int parse(occd_model* m) {
       (uint64_t)(m->view_sel >= 0 ? 1 : m->V) * m->img_h * m->img_w * m->img_cstride *
           (m->precision == OCCD_DTYPE_F32 ? 4 : 2),
       (uint64_t)VL * N * m->P * 16, (uint64_t)VL * N * m->P, N * 8, (uint64_t)m->depth_h * m->depth_w * 4,
-      (uint64_t)m->n_cams * 160, (uint64_t)m->n_cams * 4, m->map_bytes() * ((m->flags & FLAG_CONF) ? 2 : 1)};
+      (uint64_t)m->n_cams * 160, (uint64_t)m->n_cams * 4, m->map_bytes() * m->maps_per_item()};
   for (int k = 0; k < N_ROLES; ++k) {
     const RoleRef& ro = m->roles[k];
     if (!need[k]) continue;
@@ -1008,9 +1022,11 @@ const occd_frame_ex* rgb_frames(occd_model* m, const occd_frame* frames, int n) 
   return m->frames_ex.data();
 }
 
-// the whole maps of items [0, n) (and their confidences) of a model whose plan outputs them: every unpartitioned
-// model, rank 0 of a slab.  The class-map role is [B][map], or [2][B][map] with the confidence
-int copy_out(const occd_model* m, uint16_t* class_map, void* conf, int n, cudaStream_t st, const char* what) {
+// the whole maps of items [0, n) (and their confidences or probabilities) of a model whose plan outputs them: every
+// unpartitioned model, rank 0 of a slab.  The class-map role is [B][map], [2][B][map] with the confidence, or
+// [B][map] then [B][C][map] with the probabilities
+int copy_out(const occd_model* m, uint16_t* class_map, void* conf, int n, cudaStream_t st, const char* what,
+             void* probs = nullptr) {
   if (m->rank != 0) return OCCD_OK;
   const char* roles = static_cast<const char*>(m->dev(ROLE_CLASSES));
   cudaError_t e;
@@ -1019,6 +1035,9 @@ int copy_out(const occd_model* m, uint16_t* class_map, void* conf, int n, cudaSt
   if (conf && (e = cudaMemcpyAsync(conf, roles + m->map_bytes() * m->batch, m->map_bytes() * n,
                                    cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
     return cuda_fail(e, (std::string(what) + ": confidence copy").c_str());
+  if (probs && (e = cudaMemcpyAsync(probs, roles + m->map_bytes() * m->batch, m->map_bytes() * m->n_classes * n,
+                                    cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+    return cuda_fail(e, (std::string(what) + ": probabilities copy").c_str());
   return OCCD_OK;
 }
 
@@ -1055,7 +1074,7 @@ extern "C" int occd_model_batch(const occd_model* m, int* batch) {
 namespace {
 
 int run_frames(const char* who, occd_model* m, const occd_frame* frames, const occd_frame_ex* frames_ex, int n,
-               uint16_t* class_maps, void* conf, void* stream) {
+               uint16_t* class_maps, void* conf, void* stream, void* probs = nullptr) {
   const std::string w(who);
   if (!(m && (frames || frames_ex) && (class_maps || m->rank != 0))) return fail(OCCD_ERR_ARG, w + ": null argument");
   if (n < 1 || (uint32_t)n > m->batch)
@@ -1064,10 +1083,12 @@ int run_frames(const char* who, occd_model* m, const occd_frame* frames, const o
   for (int i = 0; i < n; ++i)
     if (!(frames ? frames[i].images : frames_ex[i].frame.images)) return fail(OCCD_ERR_ARG, w + ": a frame without images");
   if (conf && !(m->flags & FLAG_CONF)) return fail(OCCD_ERR_UNSUPPORTED, w + ": the model was exported without confidence");
+  if (probs && !(m->flags & FLAG_PROBS))
+    return fail(OCCD_ERR_UNSUPPORTED, w + ": the model was exported without probabilities");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int rc = run_records(m, frames ? rgb_frames(m, frames, n) : frames_ex, n, st);
   if (rc != OCCD_OK) return rc;
-  return copy_out(m, class_maps, conf, n, st, who);
+  return copy_out(m, class_maps, conf, n, st, who, probs);
 }
 
 }  // namespace
@@ -1082,22 +1103,32 @@ extern "C" int occd_model_run_frames_ex(occd_model* m, const occd_frame_ex* fram
   return run_frames("occd_model_run_frames_ex", m, nullptr, frames, n, class_maps, conf, stream);
 }
 
-extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
-                                          void* conf, void* stream) {
-  OCCD_CHECK_ARG(ms && world >= 1 && f && f->images && class_map, "occd_model_run_frame_group: null argument");
+extern "C" int occd_model_run_frames_probs(occd_model* m, const occd_frame_ex* frames, int n, uint16_t* class_maps,
+                                           void* probs, void* stream) {
+  if (m && !probs && m->rank == 0) return fail(OCCD_ERR_ARG, "occd_model_run_frames_probs: null argument");
+  if (m && !(m->flags & FLAG_PROBS))
+    return fail(OCCD_ERR_UNSUPPORTED, "occd_model_run_frames_probs: the model was exported without probabilities");
+  return run_frames("occd_model_run_frames_probs", m, nullptr, frames, n, class_maps, nullptr, stream, probs);
+}
+
+namespace {
+
+int run_frame_group(const char* who, occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
+                    void* conf, void* probs, void* stream) {
+  const std::string w(who);
+  if (!(ms && world >= 1 && f && f->images && class_map)) return fail(OCCD_ERR_ARG, w + ": null argument");
   for (int r = 0; r < world; ++r) {
-    OCCD_CHECK_ARG(ms[r] && ms[r]->comm, "occd_model_run_frame_group: every rank's model, loaded with a local "
-                                         "communicator, is needed");
-    int rank, w, kind;
-    occd_comm_describe(ms[r]->comm, &rank, &w, &kind);
-    OCCD_CHECK_ARG(kind == OCCD_COMM_LOCAL && rank == r && w == world &&
-                       occd_comm_group(ms[r]->comm) == occd_comm_group(ms[0]->comm),
-                   "occd_model_run_frame_group: models[r] must be rank r of one local group of `world` ranks");
+    if (!(ms[r] && ms[r]->comm))
+      return fail(OCCD_ERR_ARG, w + ": every rank's model, loaded with a local communicator, is needed");
+    int rank, wr, kind;
+    occd_comm_describe(ms[r]->comm, &rank, &wr, &kind);
+    if (!(kind == OCCD_COMM_LOCAL && rank == r && wr == world &&
+          occd_comm_group(ms[r]->comm) == occd_comm_group(ms[0]->comm)))
+      return fail(OCCD_ERR_ARG, w + ": models[r] must be rank r of one local group of `world` ranks");
   }
-  if (conf && !(ms[0]->flags & FLAG_CONF)) {
-    occd_set_last_error("occd_model_run_frame_group: the model was exported without confidence");
-    return OCCD_ERR_UNSUPPORTED;
-  }
+  if (conf && !(ms[0]->flags & FLAG_CONF)) return fail(OCCD_ERR_UNSUPPORTED, w + ": the model was exported without confidence");
+  if (probs && !(ms[0]->flags & FLAG_PROBS))
+    return fail(OCCD_ERR_UNSUPPORTED, w + ": the model was exported without probabilities");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const occd_frame_ex fx{*f, OCCD_PIX_RGB, 0};
   for (int r = 0; r < world; ++r) ms[r]->last_n = 0;
@@ -1113,7 +1144,20 @@ extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, cons
   if (rc != OCCD_OK) return rc;
   if (capture && owner->graph_exec) owner->graph_ranks.assign(ms, ms + world);
   for (int r = 0; r < world; ++r) ms[r]->last_n = 1;
-  return copy_out(owner, class_map, conf, 1, st, "occd_model_run_frame_group");
+  return copy_out(owner, class_map, conf, 1, st, who, probs);
+}
+
+}  // namespace
+
+extern "C" int occd_model_run_frame_group(occd_model* const* ms, int world, const occd_frame* f, uint16_t* class_map,
+                                          void* conf, void* stream) {
+  return run_frame_group("occd_model_run_frame_group", ms, world, f, class_map, conf, nullptr, stream);
+}
+
+extern "C" int occd_model_run_frame_group_probs(occd_model* const* ms, int world, const occd_frame* f,
+                                                uint16_t* class_map, void* probs, void* stream) {
+  if (!probs) return fail(OCCD_ERR_ARG, "occd_model_run_frame_group_probs: null argument");
+  return run_frame_group("occd_model_run_frame_group_probs", ms, world, f, class_map, nullptr, probs, stream);
 }
 
 namespace {

@@ -27,6 +27,8 @@ FLAG_FLOSP_DEPTH, FLAG_VIRTUAL, FLAG_CONF, FLAG_SLAB = 1, 2, 4, 16  # FLAG_CONF:
                                                                    # rank's plan of the X-slab partition
 FLAG_BATCH = 32                                                    # a B-frame plan of predict_frames (batch block)
 FLAG_MAPS = 64                                                     # the staged views' rectification maps (maps role)
+FLAG_PROBS = 256                                                   # the class-map role holds the B maps, then the
+                                                                   # B x C float16 probability planes
 PATTERN_MAX = 64
 
 _STREAM = object()        # the launch stream of the recording run: becomes the stream slot of a record
@@ -177,7 +179,7 @@ class _Buffers:
         return out.tobytes() if out.any() else None
 
 
-def export(model, path, frame, inv_map=None, confidence=False, slab_output=None):
+def export(model, path, frame, inv_map=None, confidence=False, slab_output=None, probabilities=False):
     """Write the model file of `model.predict_frame(frame, classes=True, inv_map=inv_map, confidence=confidence)`
     for frames of this frame's shape (image count and size, depth map size, voxel grid).  Refuses what predict_frame
     refuses, with the same messages.  Returns a dict of what was written (records, buffers, bytes).
@@ -186,7 +188,9 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     FLAG_BATCH and a batch block; every role holds B items), which `occd_model_run_frames` replays for 1..B frames.
     Refuses what predict_frames refuses; not with slab_output.  With
     `confidence` the file's class-map role holds the map and then its confidence (header flag FLAG_CONF), which
-    `occd_model_run_frame_conf` reads; without it the file is what it always was.
+    `occd_model_run_frame_conf` reads; without it the file is what it always was.  With `probabilities` the
+    class-map role holds the B maps and then the B x C float16 probability planes of `predict_frame(s)(...,
+    probabilities=True)` (header flag FLAG_PROBS), which `occd_model_run_frames_probs` reads.
 
     A frame carrying "rect_maps" embeds them (header flag FLAG_MAPS and a maps role after the roles): a rig's
     calibration is fixed per deployment, so the runtime rectifies every frame with them (a slab file holds its staged
@@ -206,7 +210,7 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     if batched:
         if slab_output is not None:
             raise NotImplementedError("deploy.export: a batched model file (a list of frames) has no X-slab partition")
-        fs = model._frames_checked(frame, True, confidence)
+        fs = model._frames_checked(frame, True, confidence, probabilities=probabilities)
         f, B = fs[0], len(frame)
         for i, fi in enumerate(fs[1:], 1):
             if (fi["maps"] is None) != (f["maps"] is None) or (fi["maps"] is not None
@@ -214,6 +218,8 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
                 raise ValueError("deploy.export: frame %d's rect_maps differ from frame 0's; a model file holds one "
                                  "set of maps for every frame" % i)
     else:
+        from .models.OccDepth import _check_class_request
+        _check_class_request("predict_frame", True, confidence, probabilities)
         f = model._frame_checked(frame, slab_output)
         B = 1
     depth_items = f["virtual"] and B > 1
@@ -228,7 +234,8 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
         _lib._RECORDING.recorder = rec
         try:
             ent = model._build(B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["batch"],
-                               classes=model._class_key(inv_map, confidence, slab is not None), capture=False,
+                               classes=model._class_key(inv_map, confidence, slab is not None, probabilities),
+                               capture=False,
                                depth_items=depth_items)
             plan, img_cl, pix, fov, out, depth0, n_lo, view_sel = ent
             plan.pix_z = torch.zeros(pix.shape[0], pix.shape[2], dtype=torch.float64, device=dev)
@@ -312,7 +319,8 @@ def export(model, path, frame, inv_map=None, confidence=False, slab_output=None)
     hdr = [MAGIC, struct.pack("<9I", _lib.MODEL_FORMAT_VERSION, _lib.lib().occd_abi_version(), plan.lib_dtype,
                               1 if nyu else 0, (FLAG_FLOSP_DEPTH if flosp else 0) | (FLAG_VIRTUAL if f["virtual"] else 0)
                               | (FLAG_CONF if confidence else 0) | (FLAG_SLAB if slab is not None else 0)
-                              | (FLAG_BATCH if batched else 0) | (FLAG_MAPS if maps is not None else 0),
+                              | (FLAG_BATCH if batched else 0) | (FLAG_MAPS if maps is not None else 0)
+                              | (FLAG_PROBS if probabilities else 0),
                               f["V"], f["H"], f["W"], model.project_scale),
            struct.pack("<7I", *S, *out_dims, f["P"]), pattern.astype("<i4").tobytes(),
            struct.pack("<7d", float(f["voxel_size"]), *[float(v) for v in f["vox_origin"]],
@@ -442,13 +450,15 @@ class LoadedModel:
         _lib.check(_lib.lib().occd_model_batch(self.handle, C.byref(b)), "occd_model_batch")
         return b.value
 
-    def run_frames(self, frames, out=None, stream=None, graph=True, conf=None, pixel_format=None):
+    def run_frames(self, frames, out=None, stream=None, graph=True, conf=None, pixel_format=None, probs=None):
         """1..B frames (as OccDepth.predict_frames takes them) through occd_model_run_frames -> uint16 [n, X, Y, Z] on
         the current device, or (map, conf) with `conf` (a float16 [n, X, Y, Z] device tensor, or True).
         Each frame's "pixel_format" ("rgb" by default, "bgr", or "nv12": then its "img" is uint8 (V, H0 * 3 / 2, W0),
         OpenCV's NV12 layout) is staged through occd_model_run_frames_ex; `pixel_format` sets it for every frame, and a
         frame whose own key says otherwise is refused.  The file's rectification maps apply: a frame carrying
-        "rect_maps" is refused."""
+        "rect_maps" is refused.  `probs` (a float16 [n, C, X, Y, Z] device tensor, or True) gets every class's
+        probability through occd_model_run_frames_probs (a file exported with probabilities); the result is then
+        (map, probs)."""
         n = len(frames)
         if pixel_format is not None and pixel_format not in _lib.PIXEL_FORMATS:
             raise ValueError("LoadedModel.run_frames: pixel_format must be 'rgb', 'bgr' or 'nv12', got %r"
@@ -456,13 +466,13 @@ class LoadedModel:
         fmts = [pixel_format or fr.get("pixel_format", "rgb") for fr in frames]
         calls = [_frame_call(self.geom, fr, None, None, graph, None, False, fmt, "LoadedModel.run_frames")
                  for fr, fmt in zip(frames, fmts)]
-        if all(fmt == "rgb" for fmt in fmts):
+        if all(fmt == "rgb" for fmt in fmts) and probs is None:
             fa = (_lib.Frame * n)(*[c[0] for c in calls])
             run = _lib.lib().occd_model_run_frames
         else:
             fa = (_lib.FrameEx * n)(*[_lib.FrameEx(c[0], _lib.PIXEL_FORMATS[fmt], c[1][0].stride(1) * c[0].H0)
                                       for c, fmt in zip(calls, fmts)])
-            run = _lib.lib().occd_model_run_frames_ex
+            run = _lib.lib().occd_model_run_frames_ex if probs is None else _lib.lib().occd_model_run_frames_probs
         dev = calls[0][1][0].device                 # the first frame's images, on the device
         if out is None:
             out = torch.empty(n, self.geom.X, self.geom.Y, self.geom.Z, dtype=torch.uint16, device=dev)
@@ -471,11 +481,19 @@ class LoadedModel:
         assert out.dtype == torch.uint16 and out.is_contiguous() and out.shape[0] == n
         if conf is not None:
             assert conf.dtype == torch.float16 and conf.is_contiguous() and conf.shape == out.shape
+        if probs is True:
+            probs = torch.empty((n, self.geom.n_classes) + tuple(out.shape[1:]), dtype=torch.float16, device=dev)
+        if probs is not None:
+            assert conf is None, "LoadedModel.run_frames: conf and probs are not taken together"
+            assert probs.dtype == torch.float16 and probs.is_contiguous()
+            assert tuple(probs.shape) == (n, self.geom.n_classes) + tuple(out.shape[1:])
         keep = [c[1] for c in calls]
-        st = _stream_for(stream, [t for c in keep for t in c if isinstance(t, torch.Tensor)] + [out, conf])
+        st = _stream_for(stream, [t for c in keep for t in c if isinstance(t, torch.Tensor)] + [out, conf, probs])
         self._last_n = 0
-        _lib.check(run(self.handle, fa, n, _ptr(out), _ptr(conf), st), run.__name__)
+        _lib.check(run(self.handle, fa, n, _ptr(out), _ptr(conf if probs is None else probs), st), run.__name__)
         self._last_n = n
+        if probs is not None:
+            return out, probs
         return out if conf is None else (out, conf)
 
     def run_frame(self, frame, out=None, stream=None, graph=True, conf=None):
@@ -548,18 +566,34 @@ class LoadedModel:
             pass
 
 
-def run_frame_group(models, frame, out=None, stream=None, graph=True, conf=None):
+def run_frame_group(models, frame, out=None, stream=None, graph=True, conf=None, probs=None):
     """one frame through every rank of a local group (LoadedModel r loaded with Comm.local(world)[r]), in lock step
-    on one stream (occd_model_run_frame_group) -> rank 0's whole map, or (map, conf), as LoadedModel.run_frame"""
+    on one stream (occd_model_run_frame_group) -> rank 0's whole map, or (map, conf), as LoadedModel.run_frame;
+    `probs` (a float16 [1, C, X, Y, Z] device tensor, or True) -> (map, probs) through
+    occd_model_run_frame_group_probs, for files exported with probabilities"""
     hs = (C.c_void_p * len(models))(*[m.handle.value for m in models])
     f, keep, out, conf_t, st = _frame_call(models[0].geom, frame, out, stream, graph, conf, True, "rgb",
                                            "deploy.run_frame_group")
+    g = models[0].geom
+    if probs is True:
+        probs = torch.empty(1, g.n_classes, g.X, g.Y, g.Z, dtype=torch.float16, device=out.device)
+    if probs is not None:
+        assert conf is None and probs.dtype == torch.float16 and probs.is_contiguous()
+        assert tuple(probs.shape) == (1, g.n_classes, g.X, g.Y, g.Z)
+        if stream is not None:
+            probs.record_stream(stream)
     for m in models:
         m._last_n = 0
-    _lib.check(_lib.lib().occd_model_run_frame_group(hs, len(models), C.byref(f), _ptr(out), _ptr(conf_t), st),
-               "occd_model_run_frame_group")
+    if probs is not None:
+        _lib.check(_lib.lib().occd_model_run_frame_group_probs(hs, len(models), C.byref(f), _ptr(out), _ptr(probs),
+                                                               st), "occd_model_run_frame_group_probs")
+    else:
+        _lib.check(_lib.lib().occd_model_run_frame_group(hs, len(models), C.byref(f), _ptr(out), _ptr(conf_t), st),
+                   "occd_model_run_frame_group")
     for m in models:
         m._last_n = 1
+    if probs is not None:
+        return out, probs
     return out if conf is None else (out, conf_t)
 
 

@@ -190,7 +190,7 @@ class ClassMapUnsupported(RuntimeError):
     """occd_conv_plan_create refused a class-map output (OCCD_ERR_UNSUPPORTED) for the kernel this launch runs on"""
 
 
-CLASS_MODES = ("classes", "classes_conf")     # ConvOp / Plan.conv out1 modes that write a class map
+CLASS_MODES = ("classes", "classes_conf", "classes_probs")     # ConvOp / Plan.conv out1 modes that write a class map
 
 
 class ConvOp:
@@ -205,7 +205,9 @@ class ConvOp:
         fp32 planar tensor [B, C1, D, H, W] (mode "planar", written at channel out1_coff), or the uint16 class map
         [B, D, H, W] of the pre-activation values (mode "classes", no out0; lut: Cout label ids or None, the remap of
         occd_argmax_classes), or that map followed by the float16 bits of its confidence, uint16 [2, B, D, H, W]
-        (mode "classes_conf").  Raises ClassMapUnsupported when the chosen kernel cannot write a class map.
+        (mode "classes_conf"), or the map followed by the float16 bits of every class's softmax probability, uint16
+        [(1 + Cout) * B, D, H, W] whose rows [B:] are the probabilities [B, Cout, D, H, W] (mode "classes_probs").
+        Raises ClassMapUnsupported when the chosen kernel cannot write a class map.
         groups: [(n_taps_of_group, (oadd_d, oadd_h, oadd_w))] -- several convolutions over the same sources in one
         launch, each with its own slice of `taps` and output offset (occd_conv_desc.n_groups; per-tap TC kernel)."""
         self.name = name
@@ -304,6 +306,10 @@ class ConvOp:
             assert out0 is None and out1.dtype == torch.uint16 and out1.is_contiguous()
             assert tuple(out1.shape) == (2, B) + fd
             d.out1_mode, d.out1 = _lib.OUT1_CLASS_U16_CONF, out1.data_ptr()
+        elif out1_mode == "classes_probs":
+            assert out0 is None and out1.dtype == torch.uint16 and out1.is_contiguous()
+            assert tuple(out1.shape) == ((1 + Cout) * B,) + fd
+            d.out1_mode, d.out1 = _lib.OUT1_CLASS_U16_PROBS, out1.data_ptr()
         self.desc = d
         self.flops = 2 * B * OD * OH * OW * Cout * sum(srcs[t[0]].C for t in taps)
         h = C.c_void_p()
@@ -423,7 +429,9 @@ class Plan:
         out1_mode="classes": out1 is a uint16 [B, D, H, W] class map (no out0), written by the conv's epilogue; where
         the kernel cannot do that, the logits go to a plan-owned fp32 buffer and occd_argmax_classes maps them.
         out1_mode="classes_conf": out1 is uint16 [2, B, D, H, W], the map and then the float16 bits of each position's
-        top-class softmax probability (the fallback: occd_argmax_classes_conf)."""
+        top-class softmax probability (the fallback: occd_argmax_classes_conf).
+        out1_mode="classes_probs": out1 is uint16 [(1 + Cout) * B, D, H, W], the map and then the float16 bits of every
+        class's softmax probability [B, Cout, D, H, W] (the fallback: occd_class_probs)."""
         s, p, d = _t3(stride), _t3(padding), _t3(dilation)
         B, ID, IH, IW = x.dims
         co, ci, kd, kh, kw = weight.shape
@@ -445,15 +453,16 @@ class Plan:
             try:
                 self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode=out1_mode, lut=lut, **kw))
             except ClassMapUnsupported:
-                self._class_map_fallback(x, taps, ws, bias, od, out1, lut, kw, out1_mode == "classes_conf")
+                self._class_map_fallback(x, taps, ws, bias, od, out1, lut, kw, out1_mode)
             return out
         self.add(ConvOp([x], taps, ws, bias, od, out1=out1, out1_mode=out1_mode, out1_coff=out1_coff, **kw))
         return out
 
-    def _class_map_fallback(self, x, taps, ws, bias, od, classes, lut, kw, conf=False):
+    def _class_map_fallback(self, x, taps, ws, bias, od, classes, lut, kw, mode="classes"):
         """the class map of a conv whose kernel cannot write one: planar fp32 logits into a plan-owned buffer, then
-        occd_argmax_classes (the same values and rule, so the same map); with `conf` occd_argmax_classes_conf, which
-        writes classes[0] and the confidence bits classes[1]"""
+        occd_argmax_classes (the same values and rule, so the same map); mode "classes_conf": occd_argmax_classes_conf,
+        which writes classes[0] and the confidence bits classes[1]; "classes_probs": occd_class_probs, which writes
+        the map classes[:B] and the probabilities' bits classes[B:]"""
         B = x.dims[0]
         co = int(bias.numel())
         logits = torch.empty((B, co) + tuple(od), dtype=torch.float32, device=self.device)
@@ -461,7 +470,12 @@ class Plan:
         L = _lib.lib()
         S = od[0] * od[1] * od[2]
         lut_c = None if lut is None else (C.c_int * len(lut))(*[int(v) for v in lut])
-        if conf:
+        if mode == "classes_probs":
+            self.add(FnOp(lambda st: L.occd_class_probs(logits.data_ptr(), classes[:B].data_ptr(),
+                                                        classes[B:].data_ptr(), B, co, S, lut_c, st),
+                          "occd_class_probs", keep=(logits, classes, lut_c)))
+            return
+        if mode == "classes_conf":
             self.add(FnOp(lambda st: L.occd_argmax_classes_conf(logits.data_ptr(), classes[0].data_ptr(),
                                                                 classes[1].data_ptr(), B, co, S, lut_c, st),
                           "occd_argmax_classes_conf", keep=(logits, classes, lut_c)))

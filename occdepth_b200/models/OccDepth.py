@@ -24,6 +24,7 @@ from .SFA import SFA, lift_multiscale
 from .unet2d import UNet2D
 from .unet3d_kitti import UNet3D as UNet3DKitti
 from .unet3d_nyu import UNet3D as UNet3DNYU
+from .modules import split_probs
 
 try:  # the reference derives from pl.LightningModule; use it when present so Trainer-based scripts keep working
     import pytorch_lightning as pl
@@ -43,6 +44,17 @@ def feature_hw(img_h, img_w, scale):
     while s < scale:
         h, w, s = (h + 1) // 2, (w + 1) // 2, s * 2
     return h, w
+
+
+def _check_class_request(who, classes, confidence, probabilities):
+    """the refusals of probabilities=True (every class's softmax probability beside the class map)"""
+    if not probabilities:
+        return
+    if not classes:
+        raise ValueError("OccDepth.%s: probabilities=True are the class map's probabilities (classes=True)" % who)
+    if confidence:
+        raise ValueError("OccDepth.%s: probabilities=True already hold the confidence (the probability at the map's "
+                         "class); ask for one of the two" % who)
 
 
 def _get(config, name, default=None):
@@ -148,8 +160,9 @@ class OccDepth(_Base, B200Module):
     def _build(self, B, V, H, W, N, P, dev, batch, classes=None, capture=True, depth_items=False):
         """the launch plan of one batch shape; classes: None (the forward's outputs) or ("classes", lut, *options): the
         plan of predict_classes, whose decoder ends in the uint16 class map (`out` is then that tensor).  Options:
-        "conf" -- `out` is uint16 [2, B, X, Y, Z], the map then the float16 bits of its confidence; "root" -- see
-        below.  capture=False: no CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says.
+        "conf" -- `out` is uint16 [2, B, X, Y, Z], the map then the float16 bits of its confidence; "probs" -- `out`
+        is uint16 [(1 + C) * B, X, Y, Z], the map then the float16 bits of every class's probability
+        (modules.split_probs); "root" -- see below.  capture=False: no CUDA graph (and no warm-up run), whatever OCCDEPTH_CUDA_GRAPH says.
         depth_items: NYU's virtual view reads one depth map per batch item (a [B, dh, dw] buffer; predict_frames of
         independent frames) instead of item 0's for the whole batch, as the reference's tensor batches do"""
         slab = self.__dict__.get("slab_ctx")
@@ -277,18 +290,20 @@ class OccDepth(_Base, B200Module):
         if classes is None:
             out = self.net_3d_decoder.emit(plan, x3d)
         else:
-            conf = "conf" in classes[2:]
-            out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1], confidence=conf)
+            conf, probs = "conf" in classes[2:], "probs" in classes[2:]
+            out = self.net_3d_decoder.emit(plan, x3d, classes=True, lut=classes[1], confidence=conf,
+                                           probabilities=probs)
             if "root" in classes[2:]:
                 # predict_frame(slab_output="root"): rank 0 gathers the ranks' slabs into the whole map (and its
-                # confidence: a second gather of the same shape), which is then this plan's output there; the other
-                # ranks' plans output nothing
+                # confidence: a second gather of the same shape; or its probabilities: the map and the C probability
+                # planes, 1 + C items of one gather), which is then this plan's output there; the other ranks' plans
+                # output nothing
                 bounds = [(lo * ps, hi * ps) for lo, hi in slab.bounds]       # every rank's plan.x_range
                 parts = [out[0], out[1]] if conf else [out]
                 whole = None
                 if slab.rank == 0:
-                    whole = torch.empty(((2,) if conf else ()) + (1, bounds[-1][1]) + tuple(out.shape[-2:]),
-                                        dtype=out.dtype, device=dev)
+                    lead = (2, 1) if conf else (out.shape[0],) if probs else (1,)
+                    whole = torch.empty(lead + (bounds[-1][1],) + tuple(out.shape[-2:]), dtype=out.dtype, device=dev)
                 for k, part in enumerate(parts):
                     plan.add(slab.gather_root_op(part, None if whole is None else (whole[k] if conf else whole),
                                                  bounds))
@@ -304,20 +319,25 @@ class OccDepth(_Base, B200Module):
     def forward(self, batch):
         return self._run(batch, None)
 
-    def predict_classes(self, batch, inv_map=None, confidence=False):
+    def predict_classes(self, batch, inv_map=None, confidence=False, probabilities=False):
         """uint16 class per voxel [B, X, Y, Z]: bit for bit `class_map(self(batch)["ssc_logit"], inv_map)`, but the
         classifier's epilogue writes the map, so no logits (and none of the forward's other outputs) are stored,
         converted or copied.  inv_map: one label id per class (at most 64), the submission writer's remap.  Its plan is
         cached apart from the forward's (alternating both rebuilds neither); under enable_slab_parallel this rank's
         X-slab.  confidence=True: returns (map, conf), conf float16 [B, X, Y, Z] each voxel's top-class softmax
         probability, max softmax(ssc_logit), computed by the same epilogue in fp32 and rounded once (NaN where a logit
-        is NaN or +inf; inv_map does not touch it).  The map is the same either way."""
-        return self._run(batch, self._class_key(inv_map, confidence))
+        is NaN or +inf; inv_map does not touch it).  probabilities=True: returns (map, probs), probs float16
+        [B, C, X, Y, Z] every class's softmax probability, softmax(ssc_logit, dim=1), from the same epilogue: exp(l - m)
+        / s in fp32 with the confidence's m and s, rounded once (NaN in every class where a logit is NaN or +inf; the
+        probability at the map's class is the confidence, bit for bit; inv_map remaps the map only).  The map is the
+        same either way."""
+        _check_class_request("predict_classes", True, confidence, probabilities)
+        return self._run(batch, self._class_key(inv_map, confidence, probabilities=probabilities))
 
-    def _class_key(self, inv_map, confidence=False, root=False):
+    def _class_key(self, inv_map, confidence=False, root=False, probabilities=False):
         """the `classes` argument of _build (and part of the class-map plan's cache key)"""
         return (("classes", self._class_lut(inv_map)) + (("conf",) if confidence else ())
-                + (("root",) if root else ()))
+                + (("probs",) if probabilities else ()) + (("root",) if root else ()))
 
     def _class_lut(self, inv_map):
         if inv_map is None:
@@ -417,6 +437,9 @@ class OccDepth(_Base, B200Module):
         n = B if n is None else n
         if "conf" in classes[2:]:              # uint16 [2, ...]: the map, then the confidence's float16 bits
             return ent[4][0, :n].clone(), ent[4][1, :n].clone().view(torch.float16)
+        if "probs" in classes[2:]:             # the map, then every class's float16 probability
+            cmap, probs = split_probs(ent[4], B)
+            return cmap[:n].clone(), probs[:n].clone()
         return ent[4][:n].clone()              # the map lives in a plan-owned static buffer
 
     def _stage(self, ent, batch, img, pp, fm, dev):
@@ -436,8 +459,10 @@ class OccDepth(_Base, B200Module):
             self.flosp_depth.stage_inputs(batch, dev, plan.flosp_state)
 
     # ---- camera frames: uint8 images and calibration in, the datasets' pre-processing on the device -------------
-    def predict_frame(self, frame, classes=True, inv_map=None, slab_output=None, confidence=False):
-        """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map` and `confidence` as in
+    def predict_frame(self, frame, classes=True, inv_map=None, slab_output=None, confidence=False,
+                      probabilities=False):
+        """One camera frame -> the class map (classes=True: uint16 [1, X, Y, Z], `inv_map`, `confidence` and
+        `probabilities` as in
         predict_classes) or the forward's output dict (classes=False), through the same cached plan a tensor batch of the same shapes
         uses.  Only the staging differs: the datasets' pre-processing (eval split, no augmentation) runs on the device
         and writes the plan's input buffers -- the images through `occd_stage_rgb_u8_cl`, the indices through
@@ -465,15 +490,16 @@ class OccDepth(_Base, B200Module):
         Under enable_slab_parallel every rank is handed the same frame and `slab_output` says which result it wants:
           "slab": this rank's X-slab, as predict_classes returns it (classes=False: the forward's per-rank dict);
           "root": (classes=True only) rank 0 returns the whole [1, X, Y, Z] map (with `confidence` the whole (map,
-                  conf)), bit for bit the unpartitioned one, gathered from the ranks' slabs; the other ranks return
-                  None.
+                  conf), with `probabilities` the whole (map, probs)), bit for bit the unpartitioned one, gathered from
+                  the ranks' slabs; the other ranks return None.
         Each rank stages its own view under view sharding (else every view), the whole depth map, and the indices of
         its X-slab only (`occd_vox2pix_range_fwd`).  Without slab_output the partition is refused; without the
         partition slab_output must be None."""
         if confidence and not classes:
             raise ValueError("OccDepth.predict_frame: confidence=True is the class map's confidence (classes=True)")
+        _check_class_request("predict_frame", classes, confidence, probabilities)
         return self._run_frame(self._frame_checked(frame, slab_output, classes), classes, inv_map, slab_output,
-                               confidence)
+                               confidence, probabilities)
 
     def _frame_checked(self, frame, slab_output=None, classes=True):
         """the refusals of the camera route, then `_frame_inputs`"""
@@ -496,13 +522,13 @@ class OccDepth(_Base, B200Module):
         self._check_mode(torch.empty(0, device=dev))
         return self._frame_inputs(frame, dev)
 
-    def _run_frame(self, f, classes, inv_map, slab_output=None, confidence=False):
+    def _run_frame(self, f, classes, inv_map, slab_output=None, confidence=False, probabilities=False):
         dev = f["imgs"].device
         key = self._plan_key(1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, f["virtual"], f["virtual_bf"])
         stage = lambda ent: self._stage_frame(ent, f)     # noqa: E731
         with torch.cuda.device(dev):
             if classes:
-                cls = self._class_key(inv_map, confidence, slab_output == "root")
+                cls = self._class_key(inv_map, confidence, slab_output == "root", probabilities)
                 return self._classes_on(f["batch"], key + cls, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
                                         stage)
             return self._forward_on(f["batch"], key, 1, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage)
@@ -643,9 +669,10 @@ class OccDepth(_Base, B200Module):
         plan.calib_mark[b] = f["calib"]
 
     # ---- batches of camera frames ----------------------------------------------------------------------------------
-    def predict_frames(self, frames, classes=True, inv_map=None, confidence=False):
+    def predict_frames(self, frames, classes=True, inv_map=None, confidence=False, probabilities=False):
         """A list of 1..B camera frames (each what predict_frame takes) through one B-frame plan, B = len(frames): the
-        uint16 class maps [n, X, Y, Z] (with `confidence`: (map, conf)), or with classes=False the forward's output dict
+        uint16 class maps [n, X, Y, Z] (with `confidence`: (map, conf); with `probabilities`: (map, probs), probs
+        float16 [n, C, X, Y, Z]), or with classes=False the forward's output dict
         with a leading n.  Every frame's result is bit for bit predict_frame's of that frame alone.
 
         The frames must agree on the image count V, the crop `img_hw`, the grid geometry (voxel_size, scene_size,
@@ -655,10 +682,10 @@ class OccDepth(_Base, B200Module):
         keeps the calibration its index buffers hold, so a KITTI sequence computes the indices once per item.  Not
         under enable_slab_parallel with more than one frame, nor for NYU with the FlospDepth prior with more than one
         (its grid is rebuilt from item 0's vox_origin)."""
-        fs = self._frames_checked(frames, classes, confidence)
-        return self._run_frames(fs, len(fs), classes, inv_map, confidence)
+        fs = self._frames_checked(frames, classes, confidence, probabilities=probabilities)
+        return self._run_frames(fs, len(fs), classes, inv_map, confidence, probabilities)
 
-    def _frames_checked(self, frames, classes=True, confidence=False, batch=None, inputs=True):
+    def _frames_checked(self, frames, classes=True, confidence=False, batch=None, inputs=True, probabilities=False):
         """the refusals of predict_frames (host-side, before any frame is moved), then -- with `inputs` -- the frames
         through `_frame_checked`"""
         if isinstance(frames, dict) or not isinstance(frames, (list, tuple)):
@@ -669,6 +696,7 @@ class OccDepth(_Base, B200Module):
                                                                                        else batch))
         if confidence and not classes:
             raise ValueError("OccDepth.predict_frames: confidence=True is the class map's confidence (classes=True)")
+        _check_class_request("predict_frames", classes, confidence, probabilities)
         B = n if batch is None else batch
         if self.__dict__.get("slab_ctx") is not None and B > 1:
             raise NotImplementedError("OccDepth.predict_frames: the slab partition runs one frame per forward (batch "
@@ -705,7 +733,7 @@ class OccDepth(_Base, B200Module):
                 "pattern_id": int(frame.get("pattern_id", 0)),
                 "depth": frame.get("depth") is not None}
 
-    def _run_frames(self, fs, B, classes, inv_map, confidence=False):
+    def _run_frames(self, fs, B, classes, inv_map, confidence=False, probabilities=False):
         """frames fs (from _frames_checked) through the B-frame plan, B >= len(fs): the results of items [0, len(fs));
         items [len(fs), B) keep what their buffers hold"""
         f = fs[0]
@@ -718,7 +746,7 @@ class OccDepth(_Base, B200Module):
         stage = lambda ent: [self._stage_frame(ent, f, b) for b, f in enumerate(fs)]     # noqa: E731
         with torch.cuda.device(dev):
             if classes:
-                cls = self._class_key(inv_map, confidence)
+                cls = self._class_key(inv_map, confidence, probabilities=probabilities)
                 return self._classes_on(f["batch"], key + cls, B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, cls,
                                         stage, n=len(fs), depth_items=depth_items)
             return self._forward_on(f["batch"], key, B, f["V"], f["H"], f["W"], f["N"], f["P"], dev, stage,
@@ -877,15 +905,18 @@ class OccDepth(_Base, B200Module):
         return res
 
     @staticmethod
-    def class_map(ssc_logit, inv_map=None, confidence=False):
+    def class_map(ssc_logit, inv_map=None, confidence=False, probabilities=False):
         """uint16 class per voxel from the fp32 logits [B, C, X, Y, Z] on the GPU -- what the reference's callers
         compute on the host after copying all logits back (`np.argmax(torch.softmax(pred["ssc_logit"], 1).cpu(),
         1).astype(np.uint16)`, scripts/generate_output.py:94-97; eval.py does the same).  168 MB of logits shrink to
         a 4 MB map before the device->host read.  `inv_map` (int array of C label ids, io_data.get_inv_map) applies the
         submission writer's remap `inv_map[y_pred].astype(np.uint16)` (generate_kitti_submission.py:79) in the same
         launch.  confidence=True: returns (map, conf), conf float16 [B, X, Y, Z] the top class's softmax probability
-        (occd_argmax_classes_conf; NaN where a logit is NaN or +inf; the remap does not touch it)."""
+        (occd_argmax_classes_conf; NaN where a logit is NaN or +inf; the remap does not touch it).
+        probabilities=True: returns (map, probs), probs float16 [B, C, X, Y, Z] every class's softmax probability
+        (occd_class_probs: bit for bit what predict_classes(probabilities=True) writes from the same logits)."""
         from .. import _lib
+        _check_class_request("class_map", True, confidence, probabilities)
         if not (ssc_logit.is_cuda and ssc_logit.dtype == torch.float32 and ssc_logit.dim() == 5):
             raise RuntimeError("OccDepth.class_map: expected CUDA fp32 logits [B, C, X, Y, Z]")
         x = ssc_logit.contiguous()
@@ -899,6 +930,11 @@ class OccDepth(_Base, B200Module):
             if lut.shape != (Cn,):
                 raise ValueError("OccDepth.class_map: inv_map must hold one label id per class")
         lut_p = None if lut is None else lut.ctypes.data
+        if probabilities:
+            probs = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+            _lib.check(_lib.lib().occd_class_probs(x.data_ptr(), out.data_ptr(), probs.data_ptr(), B, Cn, S, lut_p,
+                                                   _lib.stream_ptr()), "occd_class_probs")
+            return out, probs
         if confidence:
             conf = torch.empty(out.shape, dtype=torch.float16, device=x.device)
             _lib.check(_lib.lib().occd_argmax_classes_conf(x.data_ptr(), out.data_ptr(), conf.data_ptr(), B, Cn, S,

@@ -56,19 +56,33 @@ def _planar_out(plan, x, C_):
     return torch.empty(B, C_, D, H, W, dtype=torch.float32, device=plan.device)
 
 
-def _classifier(plan, x, w, b, name, classes, lut, res1=None, confidence=False):
+def _classifier(plan, x, w, b, name, classes, lut, res1=None, confidence=False, probabilities=False):
     """the head's last conv: fp32 planar logits [B, n_classes, D, H, W], or (classes) their uint16 arg-max map
     [B, D, H, W] (label ids lut[class] when lut is given) written by the same epilogue instead; with `confidence`
-    uint16 [2, B, D, H, W]: that map, then the float16 bits of each voxel's top-class softmax probability"""
+    uint16 [2, B, D, H, W]: that map, then the float16 bits of each voxel's top-class softmax probability; with
+    `probabilities` uint16 [(1 + n_classes) * B, D, H, W]: that map, then the float16 bits of every class's softmax
+    probability [B, n_classes, D, H, W] (split_probs)"""
     if classes:
         B, D, H, W = x.dims
-        shape, mode = ((2, B, D, H, W), "classes_conf") if confidence else ((B, D, H, W), "classes")
+        if probabilities:
+            shape, mode = ((1 + w.shape[0]) * B, D, H, W), "classes_probs"
+        elif confidence:
+            shape, mode = (2, B, D, H, W), "classes_conf"
+        else:
+            shape, mode = (B, D, H, W), "classes"
         out = torch.empty(shape, dtype=torch.uint16, device=plan.device)
         plan.conv(x, w, b, padding=1, res1=res1, out1=out, out1_mode=mode, lut=lut, no_out0=True, name=name)
         return out
     out = _planar_out(plan, x, w.shape[0])
     plan.conv(x, w, b, padding=1, res1=res1, out1=out, out1_mode="planar", no_out0=True, name=name)
     return out
+
+
+def split_probs(out, B):
+    """_classifier's `probabilities` output -> (uint16 map [B, D, H, W], float16 probabilities [B, C, D, H, W]),
+    views of `out`"""
+    C_ = out.shape[0] // B - 1
+    return out[:B], out[B:].view(torch.float16).view((B, C_) + tuple(out.shape[1:]))
 
 
 class ASPP(B200Module):
@@ -90,14 +104,15 @@ class SegmentationHead(B200Module):
         _aspp_params(self, planes, dilations_conv_list)
         self.conv_classes = nn.Conv3d(planes, nbr_classes, kernel_size=3, padding=1, stride=1)
 
-    def emit(self, plan, x, classes=False, lut=None, confidence=False):
+    def emit(self, plan, x, classes=False, lut=None, confidence=False, probabilities=False):
         """-> fp32 planar logits [B, n_classes, X, Y, Z] (written directly by the last conv's epilogue), or with
-        `classes` their uint16 class map [B, X, Y, Z] (`confidence`: see _classifier)"""
+        `classes` their uint16 class map [B, X, Y, Z] (`confidence`, `probabilities`: see _classifier)"""
         w, b = fold_bn(self.conv0.weight, self.conv0.bias, None)
         x0 = plan.conv(x, w, b, padding=1, act="relu", name="head.conv0")
         x1 = _emit_aspp(plan, self, x0, name="head.aspp")
         w, b = fold_bn(self.conv_classes.weight, self.conv_classes.bias, None)
-        return _classifier(plan, x1, w, b, "head.conv_classes", classes, lut, confidence=confidence)
+        return _classifier(plan, x1, w, b, "head.conv_classes", classes, lut, confidence=confidence,
+                           probabilities=probabilities)
 
     def forward(self, x_in):
         return self._run_planar(x_in)
@@ -113,9 +128,9 @@ class SegmentationHeadCascadeCLS(B200Module):
         self.occ_classes = nn.Conv3d(planes, occ_classes, kernel_size=3, padding=1, stride=1)
         self.softmax = nn.Softmax(dim=1)
 
-    def emit(self, plan, x, classes=False, lut=None, confidence=False):
+    def emit(self, plan, x, classes=False, lut=None, confidence=False, probabilities=False):
         """-> (ssc logits, occupancy logits), fp32 planar; with `classes` the ssc output is the uint16 class map
-        [B, X, Y, Z] (the occupancy logits still feed the softmax; `confidence`: see _classifier)"""
+        [B, X, Y, Z] (the occupancy logits still feed the softmax; `confidence`, `probabilities`: see _classifier)"""
         planes = self.conv0.out_channels
         w, b = fold_bn(self.conv0.weight, self.conv0.bias, None)
         x0 = plan.conv(x, w, b, padding=1, act="relu", name="head.conv0")
@@ -137,7 +152,7 @@ class SegmentationHeadCascadeCLS(B200Module):
         # `part` only feeds the second launch's epilogue add (never an MMA operand): stored unrounded in tf32 mode
         part = plan.conv(x1, w[:, :planes].contiguous(), b, padding=1, name="head.conv_classes.a", out0_exact=True)
         logits = _classifier(plan, sm, w[:, planes:].contiguous(), torch.zeros_like(b), "head.conv_classes.b", classes,
-                             lut, res1=part, confidence=confidence)
+                             lut, res1=part, confidence=confidence, probabilities=probabilities)
         return logits, x_occ
 
     def forward(self, x_in):

@@ -183,7 +183,9 @@ class GatherRootOp(_CommOp):
     """Plan op: rank 0 assembles the whole uint16 class map [1, X, Y, Z] from every rank's full-resolution X-slab
     src [1, hi - lo, Y, Z]; bounds[r] = (lo, hi) of rank r.  Rank 0 copies its own slab and receives the others straight
     into their planes of dst (one grouped send/recv); the other ranks send and take dst=None.  The bytes move as uint8,
-    whatever the map's element type."""
+    whatever the map's element type.  A leading extent of n > 1 gathers n items at once, src [n, hi - lo, Y, Z] into
+    dst [n, X, Y, Z] (a map followed by its class probabilities): still one grouped exchange, one send/recv pair per
+    item and rank (occd_comm_gather_root_items when recorded)."""
 
     def __init__(self, ctx, src, dst, bounds):
         self.ctx, self.name, self.flops = ctx, "gather_root", 0
@@ -193,7 +195,7 @@ class GatherRootOp(_CommOp):
         self.src, self.dst, self.bounds = src, dst, bounds
         self.parts = None
         if ctx.rank == 0:
-            self.parts = [dst[:, lo:hi] for lo, hi in bounds]          # contiguous: one frame, planes are outermost
+            self.parts = [dst[:, lo:hi] for lo, hi in bounds]          # per item contiguous: planes are outermost
         self.bytes = src.numel() * src.element_size()
         self._keep = (src, dst)
 
@@ -203,17 +205,22 @@ class GatherRootOp(_CommOp):
 
     def _emit(self, L, stream):
         bounds = (C.c_int * (2 * self.ctx.world))(*[b for lo_hi in self.bounds for b in lo_hi])
-        return L.occd_comm_gather_root(_lib.MODEL_COMM, self.src.data_ptr(),
-                                       None if self.dst is None else self.dst.data_ptr(), bounds,
-                                       _nbytes(self.src[0, 0]), stream)
+        dst = None if self.dst is None else self.dst.data_ptr()
+        if self.src.shape[0] > 1:
+            return L.occd_comm_gather_root_items(_lib.MODEL_COMM, self.src.data_ptr(), dst, bounds,
+                                                 _nbytes(self.src[0, 0]), self.src.shape[0], stream)
+        return L.occd_comm_gather_root(_lib.MODEL_COMM, self.src.data_ptr(), dst, bounds, _nbytes(self.src[0, 0]),
+                                       stream)
 
     def _exchange(self):
         c = self.ctx
+        items = self.src.shape[0]
         if c.rank == 0:
             self.parts[0].copy_(self.src)
-            ops = [dist.P2POp(dist.irecv, self._u8(self.parts[r]), r) for r in range(1, c.world)]
+            ops = [dist.P2POp(dist.irecv, self._u8(self.parts[r][i]), r) for r in range(1, c.world)
+                   for i in range(items)]
         else:
-            ops = [dist.P2POp(dist.isend, self._u8(self.src), 0)]
+            ops = [dist.P2POp(dist.isend, self._u8(self.src[i]), 0) for i in range(items)]
         for req in dist.batch_isend_irecv(ops):
             req.wait()
 

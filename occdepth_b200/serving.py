@@ -17,16 +17,21 @@ allocated per frame (a caching-allocator block that changes streams would serial
 With `classes=True` every frame runs `model.predict_classes(batch, inv_map)` instead: the classifier writes the
 uint16 class map [B, X, Y, Z] (4 MB at config 2) and that is what is read back, not the 168 MB of logits.  With
 `confidence=True` as well, the float16 top-class probability of every voxel is read back beside it and `result` returns
-(map, conf).
+(map, conf); with `probabilities=True` every class's float16 probability [B, C, X, Y, Z] is read back instead and
+`result` returns (map, probs).
 """
 import torch
 
 from .engine import require_cuda
 
 
-def _result_buffers(res):
+def _result_buffers(res, probabilities=False):
     """the device and pinned host buffers of one read-back slot: the result's shape, or for a (map, conf) pair one
-    uint16 [2, ...] buffer that holds the map and then the confidence's float16 bits"""
+    uint16 [2, ...] buffer that holds the map and then the confidence's float16 bits, or for a (map, probs) pair a
+    list of one buffer per part"""
+    if probabilities:
+        return ([torch.empty_like(t) for t in res],
+                [torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in res])
     if isinstance(res, tuple):
         dev = torch.empty((2,) + tuple(res[0].shape), dtype=torch.uint16, device=res[0].device)
     else:
@@ -35,28 +40,44 @@ def _result_buffers(res):
 
 
 def _copy_result(dst, res):
-    if isinstance(res, tuple):
+    """dst <- res: a result buffer (or a list of them, _result_buffers) from a device result or a device buffer"""
+    if isinstance(dst, list):
+        for d, r in zip(dst, res):
+            d.copy_(r, non_blocking=True)
+    elif isinstance(res, tuple):
         dst[0].copy_(res[0])
         dst[1].copy_(res[1].view(torch.uint16))
     else:
-        dst.copy_(res)
+        dst.copy_(res, non_blocking=True)
 
 
 def _host_result(host, confidence):
+    if isinstance(host, list):                 # (map, probs)
+        return tuple(host)
     return (host[0], host[1].view(torch.float16)) if confidence else host
+
+
+def _check_probabilities(who, classes, confidence, probabilities):
+    if probabilities and not classes:
+        raise ValueError("%s: probabilities=True are the class map's probabilities (classes=True)" % who)
+    if probabilities and confidence:
+        raise ValueError("%s: probabilities=True already hold the confidence (the probability at the map's class); "
+                         "ask for one of the two" % who)
 
 
 class FramePipeline:
     def __init__(self, model, img_shape, pix_shape, fov_shape, device=None, out_key="ssc_logit", classes=False,
-                 inv_map=None, confidence=False):
+                 inv_map=None, confidence=False, probabilities=False):
         if not torch.cuda.is_available():
             raise RuntimeError("FramePipeline: occdepth_b200 needs a CUDA (sm_90a) device")
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         require_cuda(torch.empty(0, device=dev), "FramePipeline")
         if confidence and not classes:
             raise ValueError("FramePipeline: confidence=True is the class map's confidence (classes=True)")
+        _check_probabilities("FramePipeline", classes, confidence, probabilities)
         self.model, self.dev, self.out_key = model, dev, out_key
         self.classes, self.inv_map, self.confidence = classes, inv_map, confidence
+        self.probabilities = probabilities
         self.key = "%d" % model.project_scale
         self.main = torch.cuda.current_stream(dev)
         self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
@@ -87,18 +108,19 @@ class FramePipeline:
         batch = {"img": buf["img"], "projected_pix_" + self.key: [buf["pix"]], "fov_mask_" + self.key: [buf["fov"]]}
         with torch.no_grad():
             if self.classes:
-                res = self.model.predict_classes(batch, self.inv_map, confidence=self.confidence)
+                res = self.model.predict_classes(batch, self.inv_map, confidence=self.confidence,
+                                                 probabilities=self.probabilities)
             else:
                 res = self.model(batch)[self.out_key]
         self.in_free[j].record(self.main)
         if self.dev_out[j] is None:
-            self.dev_out[j], self.host_out[j] = _result_buffers(res)
+            self.dev_out[j], self.host_out[j] = _result_buffers(res, self.probabilities)
         self.main.wait_event(self.out_free[j])
         _copy_result(self.dev_out[j], res)   # the result leaves the allocator-owned tensor on the compute stream
         self.out_ready[j].record(self.main)
         with torch.cuda.stream(self.d2h):
             self.d2h.wait_event(self.out_ready[j])
-            self.host_out[j].copy_(self.dev_out[j], non_blocking=True)
+            _copy_result(self.host_out[j], self.dev_out[j])
             self.out_free[j].record(self.d2h)
         self.n += 1
         return self.n - 2 if self.n >= 2 else None
@@ -108,7 +130,8 @@ class FramePipeline:
         return self.n - 1 if self.n else None
 
     def result(self, ticket):
-        """host tensor of a submitted frame (with `confidence`: (map, conf) views of one pinned buffer); blocks until
+        """host tensor of a submitted frame (with `confidence`: (map, conf) views of one pinned buffer; with
+        `probabilities`: (map, probs), two pinned buffers); blocks until
         its D2H read has finished.  The buffer is reused by the second submit after the one that produced it."""
         if ticket is None or ticket < self.n - 2 or ticket >= self.n:
             raise ValueError("FramePipeline.result: ticket %r is not one of the two frames in flight" % (ticket,))
@@ -142,7 +165,9 @@ class CameraPipeline:
     sampling grids, not camera matrices).
 
     `confidence=True` (with classes=True) reads back each voxel's float16 top-class probability beside the map into the
-    same pinned buffer; `result(ticket)` then returns (map, conf).
+    same pinned buffer; `result(ticket)` then returns (map, conf).  `probabilities=True` reads back every class's
+    float16 probability [n, C, X, Y, Z] beside the map instead (`OccDepth.predict_frame(probabilities=True)`), into
+    pinned buffers of their own; `result(ticket)` then returns (map, probs).  Not with output="voxels".
 
     Under enable_slab_parallel (one pipeline per rank, every rank submitting the same frames) `slab_output` is
     required and means what it does for predict_frame: "slab" reads back this rank's X-slab, "root" the whole class
@@ -166,7 +191,7 @@ class CameraPipeline:
 
     def __init__(self, model, img_hw, vox_origin=None, voxel_size=None, scene_size=None, pattern_id=0, classes=True,
                  inv_map=None, device=None, out_key="ssc_logit", output=None, capacity=None, slab_output=None,
-                 confidence=False, batch=None, pixel_format="rgb", rect_maps=None):
+                 confidence=False, batch=None, pixel_format="rgb", rect_maps=None, probabilities=False):
         if pixel_format not in ("rgb", "bgr", "nv12"):
             raise ValueError("CameraPipeline: pixel_format must be 'rgb', 'bgr' or 'nv12', got %r" % (pixel_format,))
         if batch is not None:
@@ -183,6 +208,10 @@ class CameraPipeline:
         if confidence and (output is not None or not classes):
             raise ValueError("CameraPipeline: confidence=True is the class map's confidence (classes=True, "
                              "output=None); the voxel list has no confidence column")
+        if probabilities and output is not None:
+            raise ValueError("CameraPipeline: probabilities=True read back the class map and every class's "
+                             "probability (output=None); the voxel list has no probability columns")
+        _check_probabilities("CameraPipeline", classes, confidence, probabilities)
         if slab_output not in (None, "slab", "root"):
             raise ValueError("CameraPipeline: slab_output must be None, 'slab' or 'root', got %r" % (slab_output,))
         slab = model.__dict__.get("slab_ctx")
@@ -201,6 +230,7 @@ class CameraPipeline:
         require_cuda(torch.empty(0, device=dev), "CameraPipeline")
         self.model, self.dev, self.out_key = model, dev, out_key
         self.classes, self.inv_map, self.confidence = classes, inv_map, confidence
+        self.probabilities = probabilities
         self.geometry = {"img_hw": tuple(img_hw), "pattern_id": int(pattern_id)}
         for k, v in (("vox_origin", vox_origin), ("voxel_size", voxel_size), ("scene_size", scene_size)):
             if v is not None:
@@ -304,23 +334,28 @@ class CameraPipeline:
             return self._submit_voxels(f, j)
         with torch.no_grad():
             res = self.model.predict_frame(f, classes=self.classes, inv_map=self.inv_map,
-                                           slab_output=self.slab_output, confidence=self.confidence)
+                                           slab_output=self.slab_output, confidence=self.confidence,
+                                           probabilities=self.probabilities)
         self.in_free[j].record(self.main)
         if not self.reads_back:
             self.n += 1
             return self.n - 2 if self.n >= 2 else None
         if not self.classes:
             res = res[self.out_key]
-        shape = (2,) + tuple(res[0].shape) if self.confidence else res.shape
-        if self.dev_out[j] is None or self.dev_out[j].shape != shape:
+        if self.probabilities:
+            shape, held = [t.shape for t in res], self.dev_out[j] and [t.shape for t in self.dev_out[j]]
+        else:
+            shape = (2,) + tuple(res[0].shape) if self.confidence else res.shape
+            held = None if self.dev_out[j] is None else self.dev_out[j].shape
+        if self.dev_out[j] is None or held != shape:
             self.out_free[j].synchronize()
-            self.dev_out[j], self.host_out[j] = _result_buffers(res)
+            self.dev_out[j], self.host_out[j] = _result_buffers(res, self.probabilities)
         self.main.wait_event(self.out_free[j])
         _copy_result(self.dev_out[j], res)   # the result leaves the allocator-owned tensor on the compute stream
         self.out_ready[j].record(self.main)
         with torch.cuda.stream(self.d2h):
             self.d2h.wait_event(self.out_ready[j])
-            self.host_out[j].copy_(self.dev_out[j], non_blocking=True)
+            _copy_result(self.host_out[j], self.dev_out[j])
             self.out_free[j].record(self.d2h)
         self.n += 1
         return self.n - 2 if self.n >= 2 else None
@@ -330,7 +365,8 @@ class CameraPipeline:
         B-frame plan, and the read-back of the first n results"""
         m = self.model
         fs = [dict(self.geometry, **fr) for fr in frames] if isinstance(frames, (list, tuple)) else frames
-        m._frames_checked(fs, self.classes, self.confidence, batch=self.batch, inputs=False)   # nothing moved yet
+        m._frames_checked(fs, self.classes, self.confidence, batch=self.batch, inputs=False,   # nothing moved yet
+                          probabilities=self.probabilities)
         n = len(fs)
         j = self.n & 1
         self.host_free[j].synchronize()           # pinned buffers j: their previous H2D copies have been read
@@ -352,10 +388,12 @@ class CameraPipeline:
         self.main.wait_event(self.in_ready[j])
         with torch.no_grad():
             res = m._run_frames([m._frame_checked(f, None, self.classes) for f in fs], self.batch, self.classes,
-                                self.inv_map, self.confidence)
+                                self.inv_map, self.confidence, self.probabilities)
         self.in_free[j].record(self.main)
         if not self.classes:
             res = res[self.out_key]
+        if self.probabilities:
+            return self._read_back_probs(res, j, n)
         parts = list(res) if self.confidence else [res]
         shape = (len(parts), self.batch) + tuple(parts[0].shape[1:])
         if self.dev_out[j] is None or tuple(self.dev_out[j].shape) != shape:
@@ -371,6 +409,23 @@ class CameraPipeline:
             self.d2h.wait_event(self.out_ready[j])
             for k in range(len(parts)):
                 self.host_out[j][k, :n].copy_(self.dev_out[j][k, :n], non_blocking=True)
+            self.out_free[j].record(self.d2h)
+        self.counts[j] = n
+        self.n += 1
+        return self.n - 2 if self.n >= 2 else None
+
+    def _read_back_probs(self, res, j, n):
+        """the tail of a batched submit with probabilities: the n (map, probs) items into B-item pinned buffers"""
+        if self.dev_out[j] is None:
+            self.dev_out[j] = [torch.empty((self.batch,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev)
+                               for t in res]
+            self.host_out[j] = [torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in self.dev_out[j]]
+        self.main.wait_event(self.out_free[j])
+        _copy_result([t[:n] for t in self.dev_out[j]], res)
+        self.out_ready[j].record(self.main)
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(self.out_ready[j])
+            _copy_result([t[:n] for t in self.host_out[j]], [t[:n] for t in self.dev_out[j]])
             self.out_free[j].record(self.d2h)
         self.counts[j] = n
         self.n += 1
@@ -407,7 +462,8 @@ class CameraPipeline:
         return self.n - 1 if self.n else None
 
     def result(self, ticket):
-        """host tensor (pinned) of a submitted frame, or with `confidence` (map, conf) views of one pinned buffer;
+        """host tensor (pinned) of a submitted frame, or with `confidence` (map, conf) views of one pinned buffer, or
+        with `probabilities` (map, probs) in two pinned buffers;
         blocks until its D2H read has finished.  The buffer is reused by
         the second submit after the one that produced it.  With output="voxels": a dict of numpy views of the pinned
         buffers, trimmed to the rows that were written -- "count" (inside, outside the FOV; the true counts), "hist",
@@ -419,6 +475,8 @@ class CameraPipeline:
             return None
         j = ticket & 1
         self.out_free[j].synchronize()
+        if self.batch is not None and self.probabilities:
+            return tuple(t[:self.counts[j]] for t in self.host_out[j])
         if self.batch is not None:
             h = self.host_out[j][:, :self.counts[j]]
             return (h[0], h[1].view(torch.float16)) if self.confidence else h[0]

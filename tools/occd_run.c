@@ -4,7 +4,7 @@
  * the library (occdepth_b200/lib/occd_run).
  *
  *   occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] [--depth DEPTH] [--no-graph]
- *            [--voxels CAP] [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
+ *            [--voxels CAP] [--probs FILE] [--world W --rank R --nccl-id FILE [--nccl-lib LIBNCCL]]
  *
  * Inputs are raw little-endian files, one record per frame, frames back to back (no image decoder):
  *   IMAGES  N x V x H0 x W0 x 3 uint8, RGB, row-major (H0 x W0 default to the model's crop; --raw gives larger
@@ -23,6 +23,10 @@
  * little-endian: int32 count[2] (occupied voxels inside / outside the FOV, the true counts), int32 hist[64] (per class
  * id), then the R = min(CAP, count[0] + count[1]) written rows as int32 index[R], uint16 cls[R], float32 xyz[R][3]
  * (in-FOV rows first, each group in ascending flat index).  The two counts are printed per frame.
+ *
+ * --probs FILE: a model exported with probabilities (deploy.export(..., probabilities=True)) runs through
+ * occd_model_run_frames_probs, and FILE gets every frame's float16 class probabilities, C x X x Y x Z (C order), frame
+ * after frame; the .label files are written as without it.
  *
  * A batched model file (deploy.export of a list of B frames) runs the frames in groups of B, the last group short;
  * the times are then per group, and the mean is per frame over the groups after the first.
@@ -123,11 +127,11 @@ static int write_voxels(const char* out_dir, int frame, int32_t* h, int k, int i
 int main(int argc, char** argv) {
   if (argc < 6) {
     fprintf(stderr, "usage: occd_run MODEL IMAGES CALIB N OUT_DIR [--raw H0 W0] [--format rgb|bgr|nv12] "
-                    "[--depth DEPTH] [--no-graph] [--voxels CAP]\n");
+                    "[--depth DEPTH] [--no-graph] [--voxels CAP] [--probs FILE]\n");
     return 2;
   }
   const char *model_path = argv[1], *img_path = argv[2], *calib_path = argv[3], *out_dir = argv[5];
-  const char *depth_path = NULL, *id_path = NULL, *nccl_lib = NULL;
+  const char *depth_path = NULL, *id_path = NULL, *nccl_lib = NULL, *probs_path = NULL;
   int n = atoi(argv[4]), H0 = 0, W0 = 0, flags = 0, world = 1, rank = 0, format = OCCD_PIX_RGB, cap = -1;
   for (int i = 6; i < argc; ++i) {
     if (!strcmp(argv[i], "--raw") && i + 2 < argc) {
@@ -148,6 +152,8 @@ int main(int argc, char** argv) {
         fprintf(stderr, "occd_run: --voxels takes a capacity >= 0\n");
         return 2;
       }
+    } else if (!strcmp(argv[i], "--probs") && i + 1 < argc) {
+      probs_path = argv[++i];
     } else if (!strcmp(argv[i], "--no-graph")) {
       flags |= OCCD_FRAME_NO_GRAPH;
     } else if (!strcmp(argv[i], "--world") && i + 1 < argc) {
@@ -206,6 +212,16 @@ int main(int argc, char** argv) {
   unsigned char* h_img = (unsigned char*)malloc(img_bytes * B);
   unsigned short* h_depth = (unsigned short*)malloc(depth_bytes ? depth_bytes * B : 1);
   unsigned short* h_map = (unsigned short*)malloc(map_bytes * B);
+  /* --probs: C float16 planes of the map's size per frame */
+  const size_t probs_bytes = probs_path ? map_bytes * g.n_classes : 0;
+  void* d_probs = NULL;
+  unsigned short* h_probs = probs_path ? (unsigned short*)malloc(probs_bytes * B) : NULL;
+  FILE* fp = probs_path && rank == 0 ? fopen(probs_path, "wb") : NULL;
+  if (probs_path && rank == 0 && !fp) {
+    fprintf(stderr, "occd_run: cannot open %s\n", probs_path);
+    return 1;
+  }
+  if (probs_path && rank == 0) CK(cudaMalloc(&d_probs, probs_bytes * B));
   double* calib = (double*)malloc(n_calib * sizeof(double) * B);
   occd_frame_ex* fs = (occd_frame_ex*)calloc(B, sizeof(occd_frame_ex));
   void *d_img, *d_depth = NULL, *d_map;
@@ -262,9 +278,13 @@ int main(int argc, char** argv) {
       f->flags = flags;
     }
     CK(cudaEventRecord(e0, st));
-    OK(occd_model_run_frames_ex(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
+    if (probs_path)
+      OK(occd_model_run_frames_probs(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, d_probs, st));
+    else
+      OK(occd_model_run_frames_ex(m, fs, k, rank == 0 ? (uint16_t*)d_map : NULL, NULL, st));
     CK(cudaEventRecord(e1, st));
     if (rank == 0) CK(cudaMemcpyAsync(h_map, d_map, map_bytes * k, cudaMemcpyDeviceToHost, st));
+    if (fp) CK(cudaMemcpyAsync(h_probs, d_probs, probs_bytes * k, cudaMemcpyDeviceToHost, st));
     if (h_vox) {
       occd_voxel_out vo;
       memset(&vo, 0, sizeof(vo));
@@ -286,6 +306,10 @@ int main(int argc, char** argv) {
       ++groups;
     }
     if (rank != 0) continue;
+    if (fp && fwrite(h_probs, 1, probs_bytes * k, fp) != probs_bytes * k) {
+      fprintf(stderr, "occd_run: cannot write %s\n", probs_path);
+      return 1;
+    }
     for (int i = 0; i < k; ++i) {
       char path[4096];
       snprintf(path, sizeof(path), "%s/%06d.label", out_dir, i0 + i);
@@ -309,6 +333,12 @@ int main(int argc, char** argv) {
   fclose(fi);
   fclose(fc);
   if (fd) fclose(fd);
+  if (fp && fclose(fp) != 0) {
+    fprintf(stderr, "occd_run: cannot write %s\n", probs_path);
+    return 1;
+  }
+  free(h_probs);
+  if (d_probs) cudaFree(d_probs);
   free(h_img);
   free(h_depth);
   free(h_map);
