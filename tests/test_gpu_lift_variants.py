@@ -12,6 +12,7 @@ import torch
 import torch.nn.functional as F
 
 import gpu_cases as G
+import launch_replay as LR
 
 # bounds relative to max |ref|: twice the largest figure measured on an H100 (OCCDEPTH_PARITY_DIR), never looser than
 # the one-store bound G.TOL for rounded outputs.  fp32 outputs differ from the reference only in operation order.
@@ -85,48 +86,8 @@ def _case(i, dt, V, C_, kern):
 CASES = _cases()
 
 
-# ---- float64 restatement of the lift -------------------------------------------------------------------------------
-def lift_ref(feats, divs, pix, fov, perm=None, prior=None, scale_const=1.0):
-    """feats: per scale float64 [V, h, w, C]; pix [V, N, P, 2] int64; fov [V, N, P] bool -> float64 [N, C] in output
-    voxel order.  Per scale and view: mean over the in-FOV points of feat[(y // div) * w + (x // div)] (floor
-    division; an index outside the map contributes zero but its point still counts), mask = any point in FOV; views
-    are combined by the pairwise cosine soft-assignment of SFA.forward; scales are summed."""
-    V, N, P, _ = pix.shape
-    Cc = feats[0].shape[3]
-    out = torch.zeros(N, Cc, dtype=torch.float64)
-    for f, d in zip(feats, divs):
-        h, w = f.shape[1], f.shape[2]
-        idx = torch.div(pix[..., 1], d, rounding_mode="floor") * w + torch.div(pix[..., 0], d, rounding_mode="floor")
-        inmap = (idx >= 0) & (idx < h * w)
-        fs, ms = [], []
-        for v in range(V):
-            g = f[v].reshape(h * w, Cc)[idx[v].clamp(0, h * w - 1)]                # [N, P, C]
-            g = g * (fov[v] & inmap[v]).unsqueeze(-1).double()
-            cnt = fov[v].sum(1)
-            fs.append(g.sum(1) / cnt.clamp_min(1).unsqueeze(-1).double())
-            ms.append((cnt > 0).double())
-        if V == 1:
-            out += fs[0]
-            continue
-        acc = torch.zeros_like(out)
-        for a in range(V):
-            for b in range(a + 1, V):
-                cos = (fs[a] * fs[b]).sum(1) / (fs[a].norm(dim=1).clamp_min(1e-8) * fs[b].norm(dim=1).clamp_min(1e-8))
-                cos = cos * ms[a] * ms[b]
-                wa = cos + (ms[a] > ms[b]).double()
-                wb = cos + (ms[b] > ms[a]).double()
-                acc += wa.unsqueeze(1) * fs[a] + wb.unsqueeze(1) * fs[b]
-        out += acc / (V * (V - 1))
-    n = torch.arange(N)
-    no = n
-    if perm is not None:
-        S1, S2 = perm
-        no = (n // (S1 * S2) * S1 + n % S1) * S2 + (n // S1) % S2
-    res = torch.empty_like(out)
-    res[no] = out
-    if prior is not None:
-        res = res * prior.double().unsqueeze(1) * scale_const
-    return res
+# ---- float64 restatement of the lift: launch_replay.lift_ref -----------------------------------------------------------
+lift_ref = LR.lift_ref
 
 
 def make_inputs(case):

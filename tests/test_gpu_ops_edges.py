@@ -9,6 +9,7 @@ import torch
 import torch.nn.functional as F
 
 import gpu_cases as G
+import launch_replay as LR
 
 pytestmark = pytest.mark.gpu
 
@@ -304,45 +305,10 @@ def _cameras(V):
 
 
 def _frustum_grid_f64(T, K4, ida):
-    """oracle.functional.frustum_grid restated in float64"""
-    X, Y, Z = GRID
-    d = torch.float64
-    pmin, pmax = torch.tensor(PC_MIN, dtype=d), torch.tensor(PC_MAX, dtype=d)
-    Gm = torch.eye(4, dtype=d)
-    Gm[0, 0], Gm[1, 1], Gm[2, 2] = (pmax - pmin) / torch.tensor([X, Y, Z], dtype=d)
-    Gm[:3, 3] = pmin
-    i, j, k = torch.meshgrid(torch.arange(X, dtype=d), torch.arange(Y, dtype=d), torch.arange(Z, dtype=d),
-                             indexing="ij")
-    vox = torch.stack([i, j, k, torch.ones_like(i)], -1)
-    vox[..., :3] += 0.5
-
-    def dehom(p):
-        z = p[..., -1:]
-        return p[..., :-1] * torch.where(z.abs() > 1e-8, 1.0 / (z + 1e-8), torch.ones_like(z))
-
-    cam = dehom(vox @ (T.double() @ Gm).t())
-    pt = F.pad(cam, [0, 1], value=1.0) @ K4.double()[:3].t()
-    img = dehom(pt)
-    depth = pt[..., 2] - K4[2, 3].double()
-    bin_size = 2 * (DMAX - DMIN) / (DN * (1 + DN))
-    idx = -0.5 + 0.5 * torch.sqrt(1 + 8 * (depth - DMIN) / bin_size)
-    fg = dehom(F.pad(torch.cat([img, idx.unsqueeze(-1)], -1), [0, 1], value=1.0) @ ida.double().t())
-    fg = fg / (torch.tensor([IMG_HW[1], IMG_HW[0], DN], dtype=d) - 1) * 2 - 1
-    fg[~torch.isfinite(fg)] = -2
-    return fg.unsqueeze(0)
+    return LR.frustum_grid_f64(T.double() @ _grid_to_lidar().double(), K4, ida, GRID, IMG_HW, DN, DMIN, DMAX)
 
 
-def _sample_mean(depth, grids, mean_mode):
-    """F.grid_sample of each view's depth volume and of an all-ones volume, then the masked mean"""
-    V = depth.shape[0]
-    fs = [F.grid_sample(depth[v][None, None], grids[v], mode="bilinear", padding_mode="zeros", align_corners=False)
-          for v in range(V)]
-    ms = [F.grid_sample(torch.ones_like(depth[v])[None, None], grids[v], mode="bilinear", padding_mode="zeros",
-                        align_corners=False) for v in range(V)]
-    agg, m = sum(fs), sum(ms)
-    if V > 1 and mean_mode:
-        agg = torch.where(m > 0, agg / m, agg)
-    return agg.reshape(-1), m.reshape(-1)
+_sample_mean = LR.sample_mean
 
 
 def _to_kernel_order(r, perm_xzy):
