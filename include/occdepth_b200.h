@@ -215,7 +215,9 @@ int occd_conv_run(const occd_conv_plan* plan, void* stream);
 /* class-map plans (OCCD_OUT1_CLASS_U16): lut (HOST pointer, n == Cout <= 64 ints) or NULL: the map holds     */
 /* uint16(lut[class]) -- the inv_map remap of occd_argmax_classes -- from the next occd_conv_run on             */
 int occd_conv_plan_set_class_lut(occd_conv_plan* plan, const int* lut, int n);
-/* introspection for tests / profiling: tile box (TD,TH,TW), N tile, K chunk, stages, grid          */
+/* introspection for tests / profiling: tile box (TD,TH,TW), N tile, K chunk, stages, grid, and      */
+/* info8[7]: TC / TCX plans the number of output tiles; HALO / HALOX plans 1 when the x-packed halo   */
+/* kernel runs its plane ring, 0 when it runs the box mainloop (HALO: always 0); SIMT plans 0        */
 int occd_conv_plan_info(const occd_conv_plan* plan, int* info8);
 /* the kernel (OCCD_CONV_IMPL_*, never _AUTO) the plan runs on                                      */
 int occd_conv_plan_impl(const occd_conv_plan* plan, int* impl);

@@ -816,14 +816,14 @@ extern "C" int occd_conv_plan_info(const occd_conv_plan* pl, int* info) {
     const HaloParams& h = pl->halo;
     info[0] = h.BD; info[1] = h.BH; info[2] = h.BW; info[3] = h.N_tile; info[4] = pl->kc;
     info[5] = h.stages * 100 + h.nM; info[6] = (int)pl->grid.x;
-    info[7] = h.epi.B * h.d * h.d * h.d * h.tilesD * h.tilesH * h.tilesW;
+    info[7] = 0;   // no plane ring
     return OCCD_OK;
   }
   if (pl->impl == OCCD_CONV_IMPL_HALOX) {
     const HaloxParams& h = pl->halox;
     info[0] = h.BD; info[1] = h.BH; info[2] = h.PW; info[3] = h.N_tile; info[4] = pl->kc;
     info[5] = h.stages * 100 + h.nM; info[6] = (int)pl->grid.x;
-    info[7] = h.epi.B * h.d * h.d * h.tilesD * h.tilesH;
+    info[7] = h.ring;   // 1: plane ring, 0: box mainloop
     return OCCD_OK;
   }
   info[0] = pl->tc.TD; info[1] = pl->tc.TH; info[2] = pl->tc.TW; info[3] = pl->tc.N_tile;

@@ -327,11 +327,16 @@ class ConvOp:
                        "occd_conv_plan_set_class_lut(%s)" % name)
 
     def info(self):
+        """occd_conv_plan_info as a dict: the tile box TD / TH / TW, N_tile, KC (K chunk channels), stages
+        (stages * 100 + stage group or M tiles per box), grid_x (CTAs), then grid_y (output tiles) for TC / TCX plans
+        or ring (1: the x-packed halo kernel's plane ring, 0: its box mainloop) for HALO / HALOX plans; and the
+        schedule ('cooperative', 'pingpong', or 'none' for SIMT)"""
         arr = (C.c_int * 8)()
         _lib.check(_lib.lib().occd_conv_plan_info(self.handle, arr), "occd_conv_plan_info")
         sched = C.c_int()
         _lib.check(_lib.lib().occd_conv_plan_schedule(self.handle, C.byref(sched)), "occd_conv_plan_schedule")
-        info = dict(zip(("TD", "TH", "TW", "N_tile", "KC", "stages", "grid_x", "grid_y"), list(arr)))
+        last = "ring" if self.impl in (_lib.CONV_IMPL_HALO, _lib.CONV_IMPL_HALOX) else "grid_y"
+        info = dict(zip(("TD", "TH", "TW", "N_tile", "KC", "stages", "grid_x", last), list(arr)))
         info["schedule"] = {0: "none", 1: "cooperative", 2: "pingpong"}[sched.value]
         return info
 

@@ -19,9 +19,13 @@ Shared by tests/test_conv_replay_host.py and tests/test_gpu_conv_replay.py (a pl
                   longest could not; L = 1.1 for SiLU (its largest slope), else 1; a(v) = |v| for SiLU, 1 for the
                   sigmoid, 0 for the exact activations
   check_op(...)   every output of the launch through check(); TF32 bit pattern of tf32 stores; the class map, where
-                  a differing class needs a float64 gap within the accumulation bound; and NOTHING ELSE MOVES: every
+                  a differing class needs a float64 gap within the accumulation bound; the float16 confidence (out1
+                  mode 4) and probabilities (mode 5) through check_prob(), taken at the class the map holds, and in
+                  mode 5 the map's class holding the largest probability bit for bit; and NOTHING ELSE MOVES: every
                   byte of every reachable storage equals the snapshot except channels [coff, coff + roundup(Cout, 8))
-                  of the output window at the launch's output positions (planar out1: [out1_coff, out1_coff + Cout)).
+                  of the output window at the launch's output positions (planar out1: [out1_coff, out1_coff + Cout);
+                  class modes: the uint16 map [B P] (P positions), then [B P] of confidence or [B Cout P] of
+                  probabilities at out1[B P + (b Cout + n) P + s]).
                   The pad channels [Cout, roundup(Cout, 8)) are checked like any other: they hold what the epilogue
                   makes of a zero accumulator (zero without activation and residual -- DESIGN.md section 3).
 
@@ -33,6 +37,13 @@ configurations, both precisions, forward + class-map + two slab rank plans: 1276
   largest (|got - ref| - 1/2 ulp - L C_ACC sqrt(K) S) / a(v):         bf16 SiLU (tanh.approx) 3.1e-6;
       below zero for the tf32 SiLU and both sigmoids (__expf / __fdividef): the accumulation term already covers
       them, so they get no term of their own
+
+The confidence and probabilities (check_prob):  |got - p| <= 1/2 ulp_f16(p + d) + d,  d = p (delta_c + sum_j p_j
+delta_j) + A_SM p, with p the float64 softmax of v over the Cout classes and delta_j = C_ACC sqrt(K) S_j the bound on
+class value j (an fp32 sum plus bias and residuals, never rounded to the storage type).  A_SM would cover expf, the fp32
+sum over the classes and the division; the largest (|got - p| - 1/2 ulp_f16 - d + A_SM p) / p over both sweeps is below
+zero (shipped: tf32 -4.6e-7, bf16 -3.3e-7; menu: tf32 -7.9e-6, bf16 -8.7e-6), so, like the exact activations, they
+get no term of their own: A_SM = 0.
 """
 import types
 import zlib
@@ -45,11 +56,14 @@ ACT_NAME = {_lib.ACT_NONE: "none", _lib.ACT_RELU: "relu", _lib.ACT_LEAKY: "leaky
             _lib.ACT_SIGMOID: "sigmoid"}
 IMPL_NAME = {_lib.CONV_IMPL_TC: "tc", _lib.CONV_IMPL_SIMT: "simt", _lib.CONV_IMPL_HALO: "halo",
              _lib.CONV_IMPL_HALOX: "halox", _lib.CONV_IMPL_TCX: "tcx"}
-MANT = {"tf32": 10, "bf16": 7, "fp32": 23}          # explicit mantissa bits of the storage types
+MANT = {"tf32": 10, "bf16": 7, "fp32": 23, "f16": 10}          # explicit mantissa bits of the storage types
+EMIN = {"f16": -14}                                            # smallest normal exponent (default: fp32's -126)
 
 C_ACC = {"tf32": 6.0e-8, "bf16": 5.0e-8}
 A_ACT = {"tf32": dict(), "bf16": dict(silu=5.0e-6)}
 ACT_SLOPE = dict(silu=1.1)
+A_SM = {"tf32": 0.0, "bf16": 0.0}
+OBSERVED = {}        # sweep -> precision -> observed maxima (check / check_prob stats) of the GPU sweeps of a session
 
 
 def _ceil_div(a, b):
@@ -116,7 +130,7 @@ def quantize(x, store, mode=None):
 def ulp_store(x, store):
     """spacing of the storage type at magnitude x (float64, >= 0); 0 at 0"""
     _, e = torch.frexp(x)
-    e = (e - 1).clamp_min(-126) - MANT[store]
+    e = (e - 1).clamp_min(EMIN.get(store, -126)) - MANT[store]
     return torch.where(x > 0, torch.ldexp(torch.ones_like(x), e), torch.zeros_like(x))
 
 
@@ -330,6 +344,9 @@ def check(got, ref, S, K, store, precision, act="none", v=None, where=None, c_ac
     return bad, err - bound, stats
 
 
+CLASS_OUT1 = (_lib.OUT1_CLASS_U16, _lib.OUT1_CLASS_U16_CONF, _lib.OUT1_CLASS_U16_PROBS)
+
+
 def _merge(stats, new):
     for k, val in new.items():
         stats[k] = max(stats.get(k, val), val)
@@ -398,17 +415,35 @@ def check_op(op, snap, R, info=None):
         if bool(bad.any()):
             fails.append(describe("out1 (planar)", D, bad, excess, got, R.v[..., :Cout], info))
         put_back(op.out1.permute(0, 2, 3, 4, 1), slice(c0, c0 + Cout))
-    elif D["out1_mode"] == _lib.OUT1_CLASS_U16:
+    elif D["out1_mode"] in CLASS_OUT1:
         assert full                 # a class map needs no tap groups, and no planned one is written on a sub-grid
-        got = _bits(op.out1).to(torch.int64) & 0xFFFF
-        msg = check_classes(got, R.v[..., :Cout], R.S[..., :Cout], snap.lut, C_ACC[prec] * snap.K ** 0.5)
+        mode = D["out1_mode"]
+        B = D["B"]
+        u16 = op.out1.reshape(-1, *D["Of"])          # [B] map rows, then [B] confidence or [B * Cout] probability rows
+        c_acc = C_ACC[prec] * snap.K ** 0.5
+        got = _bits(u16[:B]).to(torch.int64) & 0xFFFF
+        msg = check_classes(got, R.v[..., :Cout], R.S[..., :Cout], snap.lut, c_acc)
         if msg:
             fails.append(msg)
-        a, b = view(op.out1), snap.of(op.out1)
-        if full:
-            a.copy_(b)
-        else:
-            _bits(a)[:, m] = _bits(b)[:, m]
+        if mode != _lib.OUT1_CLASS_U16:
+            P, d = softmax_bound(R.v[..., :Cout], R.S[..., :Cout], c_acc)
+            k = chosen_class(got, R.v[..., :Cout], snap.lut)
+            if mode == _lib.OUT1_CLASS_U16_CONF:
+                what, half = "confidence", u16[B:2 * B].view(torch.float16).unsqueeze(-1)
+                P, d = P.gather(-1, k[..., None]), d.gather(-1, k[..., None])
+            else:
+                what, half = "probabilities", u16[B:].view(torch.float16).view(B, Cout, *D["Of"]).movedim(1, -1)
+                at = half.gather(-1, k[..., None])
+                top = half.max(-1, keepdim=True).values
+                if not bool((_bits(at.contiguous()) == _bits(top.contiguous())).all()):
+                    fails.append("probabilities: at %d position(s) the map's class does not hold the largest "
+                                 "probability bit for bit (the top class's value is the confidence 1 / s)"
+                                 % int((at != top).sum()))
+            bad, excess, st = check_prob(half.to(f64), P, d, A_SM[prec])
+            _merge(stats, st)
+            if bool(bad.any()):
+                fails.append(describe(what, D, bad, excess, half, P, info))
+        view(op.out1).copy_(snap.of(op.out1))
     for key, live in restored.items():
         if not torch.equal(_bits(live), _bits(snap.store[key])):
             role = [r for r, t in reach(op) if t.untyped_storage().data_ptr() == key]
@@ -443,6 +478,52 @@ def check_classes(got, v, S, lut, c_acc):
     return ("class map: %d position(s) hold a class whose float64 value is below the largest by more than the "
             "accumulation bound; first (b, d, h, w) = %s: got %d, want %d"
             % (at.shape[0], tuple(at[0].tolist()), int(got[tuple(at[0])]), int(ids[cls[tuple(at[0])]])))
+
+
+def class_softmax(v):
+    """float64 softmax over the last axis: p_c = exp(v_c - max v) / sum_j exp(v_j - max v)"""
+    e = torch.exp(v - v.max(-1, keepdim=True).values)
+    return e / e.sum(-1, keepdim=True)
+
+
+def softmax_bound(v, S, c_acc):
+    """-> (p, d): the float64 probabilities of the class values v [..., Cout], and d, the bound on how far the error of
+    the device's values moves them.  The device's values carry at most delta_j = c_acc S_j each (they are fp32 sums,
+    never rounded to the storage type); since dp_c = p_c (dv_c - sum_j p_j dv_j), p_c moves by at most
+    p_c (delta_c + sum_j p_j delta_j)."""
+    p = class_softmax(v)
+    delta = c_acc * S
+    return p, p * (delta + (p * delta).sum(-1, keepdim=True))
+
+
+def chosen_class(got, v, lut):
+    """the class index behind each map entry (through lut when set; among classes sharing a label, the largest v), or
+    the float64 arg-max where no class has the entry's label"""
+    if lut is None:
+        ids = torch.arange(v.shape[-1], device=v.device)
+    else:
+        ids = torch.tensor(lut, device=v.device)
+    match = ids == got[..., None]
+    k = torch.where(match, v, torch.full_like(v, -float("inf"))).argmax(-1)
+    return torch.where(match.any(-1), k, v.argmax(-1))
+
+
+def check_prob(got, p, d_val, a_sm):
+    """float16 probabilities: |got - p| <= 1/2 ulp_f16(p + d) + d, d = d_val + a_sm p (got, p, d_val: float64 of one
+    shape, d_val from softmax_bound; a NaN fails).  a_sm p covers expf, the fp32 sum over the classes and the
+    division.  -> (bad, excess, stats): stats 'softmax', the largest (|got - p| - 1/2 ulp_f16 - d_val) / p, what a_sm
+    has to cover, and 'softmax_raw', the same without d_val"""
+    d = d_val + a_sm * p
+    err = (got - p).abs()
+    bound = 0.5 * ulp_store(p + d, "f16") + d
+    bad = ~(err <= bound)
+    e = err - 0.5 * ulp_store(torch.maximum(p, got.abs()), "f16")
+    stats = {}
+    pos = p > 0
+    if bool(pos.any()):
+        stats["softmax"] = float(((e - d_val)[pos] / p[pos]).max())
+        stats["softmax_raw"] = float((e[pos] / p[pos]).max())
+    return bad, err - bound, stats
 
 
 def describe(what, D, bad, excess, got, ref, info):

@@ -231,8 +231,9 @@ def test_planar_and_class_map_out1():
 
 # ---------------------------------------------------------------------------------------------------------------
 # the comparator
-def emulate(op, snap, ref, v=None, out0=None, mode=None):
-    """store into the op's live buffers what a correct device stores (mode: the rounding, default the type's own)"""
+def emulate(op, snap, ref, v=None, out0=None, mode=None, probs=None):
+    """store into the op's live buffers what a correct device stores (mode: the rounding, default the type's own;
+    probs: the class probabilities [..., Cout] to store in place of the float64 softmax of v)"""
     D, prec, Cw, m = snap.D, snap.precision, ref.Cw, ref.mask
     v = ref.v if v is None else v
     if D["out0"]:
@@ -246,11 +247,26 @@ def emulate(op, snap, ref, v=None, out0=None, mode=None):
     elif D["out1_mode"] == _lib.OUT1_F32_PLANAR:
         win = cl_last(op.out1)[..., D["out1_coff"]:D["out1_coff"] + D["Cout"]]
         win[:, m] = v[..., :D["Cout"]][:, m].float()
-    elif D["out1_mode"] == _lib.OUT1_CLASS_U16:
-        cls = v[..., :D["Cout"]].argmax(-1)
-        if snap.lut is not None:
-            cls = torch.tensor(snap.lut)[cls]
-        R._bits(op.out1)[:, m] = cls[:, m].to(torch.int16)
+    elif D["out1_mode"] in R.CLASS_OUT1:
+        B, Cout = D["B"], D["Cout"]
+        u16 = op.out1.reshape(-1, *D["Of"])
+        k = v[..., :Cout].argmax(-1)
+        cls = k if snap.lut is None else torch.tensor(snap.lut)[k]
+        R._bits(u16[:B])[:, m] = cls[:, m].to(torch.int16)
+        p = R.class_softmax(v[..., :Cout]) if probs is None else probs
+        if D["out1_mode"] == _lib.OUT1_CLASS_U16_CONF:
+            R._bits(u16[B:2 * B])[:, m] = f16_bits(p.gather(-1, k[..., None])[..., 0], mode)[:, m]
+        elif D["out1_mode"] == _lib.OUT1_CLASS_U16_PROBS:
+            R._bits(u16[B:]).view(B, Cout, *D["Of"])[:] = f16_bits(p, mode).movedim(-1, 1)
+
+
+def f16_bits(p, mode=None):
+    """float16 bits of p (float64 >= 0): nearest even, or toward zero for mode 'trunc'"""
+    h = p.to(torch.float16)
+    bits = R._bits(h).clone()
+    if mode == "trunc":
+        bits -= (h.to(f64) > p).to(torch.int16)
+    return bits
 
 
 def _case(precision, out1=True):
@@ -363,6 +379,116 @@ def test_comparator_rejects_stray_writes_and_dirty_pad_channels():
     buf[at] = float(buf[at]) + 2.0 ** -9
     fails, _ = R.check_op(op, snap, ref)
     assert len(fails) == 1 and "(0, 1, 1, 1, 20)" in fails[0], fails
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# class confidence (mode 4) and class probabilities (mode 5)
+CLS_B, CLS_C, CLS_DIMS = 2, 12, (4, 5, 6)
+CLS_P = CLS_DIMS[0] * CLS_DIMS[1] * CLS_DIMS[2]
+
+
+def _class_case(mode, precision="tf32", lut=None):
+    """3x3x3 conv of 2 items onto 12 classes writing the map and its confidence (mode 'classes_conf') or every
+    probability ('classes_probs'); out1 is the front of a uint16 storage one element longer, so that a store past
+    its (rows * B * positions) region lands in the storage"""
+    plan = Plan(torch.device("cpu"), precision=precision)
+    w, b = g16(CLS_C, 16, 3, 3, 3, scale=0.3), g16(CLS_C, seed=2)
+    x = plan.alloc(CLS_B, *CLS_DIMS, 16)
+    rows = (2 if mode == "classes_conf" else 1 + CLS_C) * CLS_B
+    store = torch.zeros(rows * CLS_P + 1, dtype=torch.uint16)
+    shape = (2, CLS_B) if mode == "classes_conf" else (rows,)
+    plan.conv(x, w, b, padding=1, out1=store[:rows * CLS_P].view(*shape, *CLS_DIMS), out1_mode=mode, no_out0=True,
+              lut=lut)
+    op = plan.ops[-1]
+    assert op.out1_mode == mode, "the driverless kernel writes no class map"
+    snap, ref = prepared(op, seed=5)
+    return op, snap, ref, w, b, store
+
+
+def test_class_softmax_reference_against_torch():
+    op, snap, ref, w, b, _ = _class_case("classes_probs")
+    v = F.conv3d(src64(snap), w.to(f64), b.to(f64), 1, 1)
+    close(ref.v[..., :CLS_C], cl_last(v))
+    close(R.class_softmax(ref.v[..., :CLS_C]), cl_last(torch.softmax(v, 1)))
+    g = torch.Generator().manual_seed(3)
+    u = torch.randn(7, 33, generator=g, dtype=f64) * 30           # wide spreads: probabilities far below 2^-24
+    close(R.class_softmax(u), torch.softmax(u, -1))
+    p, d = R.softmax_bound(ref.v[..., :CLS_C], ref.S[..., :CLS_C], 1e-6)
+    assert float((p.sum(-1) - 1).abs().max()) < 1e-12 and bool((d > 0).all())
+
+
+@pytest.mark.parametrize("lut", [None, tuple(range(40, 40 + CLS_C))])
+@pytest.mark.parametrize("mode", ["classes_conf", "classes_probs"])
+@pytest.mark.parametrize("precision", ["tf32", "bf16"])
+def test_comparator_class_probs_accepts_the_rounded_result_and_an_fp32_softmax(precision, mode, lut):
+    op, snap, ref, _, _, _ = _class_case(mode, precision, lut)
+    emulate(op, snap, ref)
+    fails, stats = R.check_op(op, snap, ref)
+    assert fails == [], fails
+    assert stats["softmax_raw"] <= 0 and stats["softmax"] <= 0, stats
+    # fp32 values and an fp32 softmax that sums the classes in the opposite order
+    v32 = ref.v[..., :CLS_C].float()
+    e = torch.exp(v32 - v32.max(-1, keepdim=True).values)
+    s = torch.zeros_like(e[..., 0])
+    for c in reversed(range(CLS_C)):
+        s = s + e[..., c]
+    emulate(op, snap, ref, probs=(e / s[..., None]).to(f64))
+    fails, stats = R.check_op(op, snap, ref)
+    assert fails == [], fails
+    assert stats["softmax"] <= R.A_SM[precision], stats
+
+
+@pytest.mark.parametrize("mode", ["classes_conf", "classes_probs"])
+def test_comparator_class_probs_rejects_one_ulp_and_truncation(mode):
+    what = "confidence" if mode == "classes_conf" else "probabilities"
+    op, snap, ref, _, _, _ = _class_case(mode)
+    emulate(op, snap, ref, mode="trunc")
+    fails, _ = R.check_op(op, snap, ref)
+    assert len(fails) == 1 and fails[0].startswith(what + ":"), fails
+    emulate(op, snap, ref)
+    assert R.check_op(op, snap, ref)[0] == []
+    # one float16 ulp on one stored value above 0.1 that is not the largest of its position
+    u16 = op.out1.reshape(-1, *CLS_DIMS)[CLS_B:]
+    half = u16.view(torch.float16)
+    top = half.view(CLS_B, -1, *CLS_DIMS).max(1, keepdim=True).values.expand(-1, u16.shape[0] // CLS_B, -1, -1, -1)
+    cand = (half.view(CLS_B, -1, *CLS_DIMS) > 0.1) & ((half.view(CLS_B, -1, *CLS_DIMS) < top) | (mode == "classes_conf"))
+    at = tuple(cand.nonzero()[0].tolist())
+    R._bits(u16).view(CLS_B, -1, *CLS_DIMS)[at] += 1
+    fails, _ = R.check_op(op, snap, ref)
+    assert len(fails) == 1 and fails[0].startswith(what + ": 1 element(s) beyond the bound"), fails
+
+
+def test_comparator_class_probs_rejects_the_wrong_item_stride():
+    """item 1's probabilities stored at out1[B P + pos + n P] (no b (Cout - 1) P): over item 0's rows, one row down"""
+    op, snap, ref, _, _, _ = _class_case("classes_probs")
+    emulate(op, snap, ref)
+    p = R.class_softmax(ref.v[..., :CLS_C])
+    rows = op.out1.reshape(-1, CLS_P)
+    b = 1
+    for n in range(CLS_C):
+        R._bits(rows)[CLS_B + b + n] = f16_bits(p[b, ..., n]).reshape(-1)
+    fails, _ = R.check_op(op, snap, ref)
+    assert any(f.startswith("probabilities:") for f in fails), fails
+
+
+def test_comparator_class_conf_rejects_swapped_halves():
+    op, snap, ref, _, _, _ = _class_case("classes_conf")
+    emulate(op, snap, ref)
+    u16 = op.out1
+    u16.copy_(torch.stack([u16[1].clone(), u16[0].clone()]))          # [2, B, D, H, W]: map, then confidence
+    fails, _ = R.check_op(op, snap, ref)
+    assert any(f.startswith("class map:") for f in fails) and any(f.startswith("confidence:") for f in fails), fails
+
+
+@pytest.mark.parametrize("mode", ["classes_conf", "classes_probs"])
+def test_comparator_class_probs_rejects_a_store_past_the_region(mode):
+    op, snap, ref, _, _, store = _class_case(mode)
+    emulate(op, snap, ref)
+    assert R.check_op(op, snap, ref)[0] == []
+    assert op.out1.numel() == store.numel() - 1
+    R._bits(store)[-1] = 0x3C00                          # 1.0 in float16, one element past the map and probabilities
+    fails, _ = R.check_op(op, snap, ref)
+    assert len(fails) == 1 and "moved outside the output window" in fails[0], fails
 
 
 def test_signature_tells_launches_apart():

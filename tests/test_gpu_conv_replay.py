@@ -32,8 +32,8 @@ SLAB = {"kitti_b3_f32_flospdepth_2080ti": (4, 1), "nyu_b7_f200_v100": (3, 1)}
 _MODEL = {}
 _SEEN = set()
 _COVER = {}          # (kernel, schedule, N tile, rb) -> launches replayed
-_CLASS_MAP = set()   # kernels whose class-map epilogue ran
-_MAX = {}            # precision -> observed maxima (conv_replay.check)
+_CLASS_MAP = set()   # (kernel, out1 mode) of every class-map epilogue that ran
+_MAX = R.OBSERVED.setdefault("conv_replay", {})   # precision -> observed maxima (conv_replay.check, check_prob)
 _RAN = {}            # (name, precision) -> (launches, replayed, seconds)
 
 
@@ -92,8 +92,8 @@ def _replay(plan, what, precision, failures, count):
         kernel = R.IMPL_NAME[op.impl]
         key = (kernel, info["schedule"], info["N_tile"], info["KC"] * op.srcs[0].esize)
         _COVER[key] = _COVER.get(key, 0) + 1
-        if snap.D["out1_mode"] == _lib.OUT1_CLASS_U16:
-            _CLASS_MAP.add(kernel)
+        if snap.D["out1_mode"] in R.CLASS_OUT1:
+            _CLASS_MAP.add((kernel, snap.D["out1_mode"]))
         R._merge(_MAX.setdefault(precision, {}), stats)
         if fails:
             failures.append("%s, launch %r on the %s kernel (%s schedule):\n    %s\n    signature: %r"
@@ -113,7 +113,10 @@ def test_every_planned_convolution_alone(monkeypatch, name, precision):
     failures, count = [], [0, 0]
     # the class-map plan of every other configuration remaps its labels
     lut = tuple((7 * i + 3) % 251 for i in range(m.n_classes)) if NAMES.index(name) % 2 else None
-    variants = [("forward", dict()), ("predict_classes", dict(classes=("classes", lut)))]
+    # the confidence and probability plans add only their classifier launch: the others deduplicate by signature
+    variants = [("forward", dict()), ("predict_classes", dict(classes=("classes", lut))),
+                ("predict_classes(confidence=True)", dict(classes=m._class_key(lut, confidence=True))),
+                ("predict_classes(probabilities=True)", dict(classes=m._class_key(lut, probabilities=True)))]
     if name in SLAB:
         world, rank = SLAB[name]
         variants.append(("slab rank %d of %d" % (rank, world), dict(slab=SimSlabGroup(world, halo=3).ctxs[rank])))
@@ -141,17 +144,18 @@ def test_coverage_and_constants():
     total = sum(v[2] for v in _RAN.values())
     print("\nconv replay coverage (%s, power limit %s; %d distinct launches, %.0f s wall for the sweep):\n%s"
           % (gpu, power, len(_SEEN), total, "\n".join(lines)))
-    print("class-map epilogue on: %s" % sorted(_CLASS_MAP))
+    print("class-map epilogue (kernel, out1 mode) on: %s" % sorted(_CLASS_MAP))
     for p in sorted(_MAX):
-        print("observed maxima [%s] (acc per sqrt(K) S): %s   constants: C_ACC %.3g, A_ACT %s"
-              % (p, {k: "%.3g" % v for k, v in sorted(_MAX[p].items())}, R.C_ACC[p], R.A_ACT[p]))
+        print("observed maxima [%s] (acc per sqrt(K) S): %s   constants: C_ACC %.3g, A_ACT %s, A_SM %.3g"
+              % (p, {k: "%.3g" % v for k, v in sorted(_MAX[p].items())}, R.C_ACC[p], R.A_ACT[p], R.A_SM[p]))
         G.record("conv_replay", p, gpu=gpu, power_limit=power, wall_s=round(total), launches=len(_SEEN),
                  coverage=["%s/%s/N%d/rb%d" % k for k in sorted(_COVER)], **_MAX[p])
     kernels = {k[0] for k in _COVER}
     assert {"tc", "tcx", "halo", "halox"} <= kernels, kernels
     assert {"cooperative", "pingpong"} <= {k[1] for k in _COVER}
-    assert _CLASS_MAP, "no class-map epilogue was replayed"
+    assert {m for _, m in _CLASS_MAP} == set(R.CLASS_OUT1), _CLASS_MAP
     for p in ("tf32", "bf16"):
         assert R.C_ACC[p] <= 2 * _MAX[p]["acc"], (p, _MAX[p])
         for act, a in R.A_ACT[p].items():
             assert a <= 2 * max(_MAX[p].get(act, 0.0), 0.0), (p, act, a, _MAX[p])
+        assert R.A_SM[p] <= 2 * max(_MAX[p]["softmax"], 0.0), (p, R.A_SM[p], _MAX[p])
