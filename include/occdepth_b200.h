@@ -471,6 +471,41 @@ int occd_occupied_voxels(const uint16_t* class_map, const uint8_t* fov_mask, int
                          int32_t* index, uint16_t* cls, float* xyz, double voxel_size, const double* origin,
                          uint32_t* work, long long work_len, void* stream);
 
+/* -------------------------------------------------------------------------------------------- */
+/* Scene maps: frames' class probabilities fused into one persistent voxel map (naive Bayes: the per-voxel       */
+/* posterior is proportional to prod_t p_t(c), so its log is a sum of ln p_t(c) and softmax over that sum is the */
+/* normalised posterior).  A map is an axis-aligned grid in a caller-chosen map frame: origin (3 float64), voxel */
+/* (float64 edge), dims MX x MY x MZ, holding acc fp32 [C][MX][MY][MZ] (summed log-probabilities, start 0) and   */
+/* count int32 [MX][MY][MZ] (frames that observed the voxel, start 0).  acc is a logits tensor:                 */
+/* occd_argmax_classes / _conf / occd_class_probs read it as [1][C][MX*MY*MZ].                                   */
+/* Integrating one frame.  probs: DEVICE float16, C class planes of a frame grid with origin grid_origin (HOST, 3 */
+/* float64), edge grid_voxel and dims GX x GY x GZ along its own x, y, z; strides (HOST, 4 long long): elements   */
+/* between classes, then between x, y and z neighbours inside a plane (KITTI's output is [x][y][z]; NYU's is      */
+/* [x][z][y]).  R (HOST, 12 float64): rows 0..2 of inverse(T), T the rigid 4x4 frame grid's frame -> map frame   */
+/* (KITTI: world <- velodyne_t; NYU: map <- world).  For each map voxel (i, j, k) in box (HOST, 6 int: i_lo, i_hi, */
+/* j_lo, j_hi, k_lo, k_hi, half-open, inside the map), in float64 without FMA contraction:                       */
+/*   c = ((idx + 0.5) * voxel) + origin;  q_r = ((R[r][0] c_x + R[r][1] c_y) + R[r][2] c_z) + R[r][3];           */
+/*   f = floor((q - grid_origin) / grid_voxel)                                                                    */
+/* The voxel is observed when 0 <= f < (GX, GY, GZ), fov_mask (DEVICE bytes at the class plane's offsets, or     */
+/* NULL) is nonzero at f, and none of its C probabilities is NaN.  Then, in fp32 with full-precision logf,       */
+/* acc[c] += logf(fmaxf(p_c, min_prob)) for every class, and count += 1.  Nothing else is written.  The box only  */
+/* bounds the launch: any box holding every observed voxel gives the same bytes, the whole map included         */
+/* ({0, MX, 0, MY, 0, MZ}); the smallest safe one is the frame grid's 8 corners taken to the map frame, their   */
+/* bounding box in map indices widened by one voxel and clipped to the map.  n_classes <= 64, min_prob in       */
+/* (0, 1].  One launch, one writer per voxel: the same inputs give the same bytes.                               */
+int occd_scene_map_integrate(float* acc, int32_t* count, int n_classes, int MX, int MY, int MZ, double voxel,
+                             const double* origin, const void* probs, const long long* strides,
+                             const uint8_t* fov_mask, int GX, int GY, int GZ, const double* grid_origin,
+                             double grid_voxel, const double* R, float min_prob, const int* box, void* stream);
+/* Shift by whole voxels d (HOST, 3 int): voxel idx of (acc_out, count_out) is voxel idx + d of (acc, count), and */
+/* voxels that come into view hold acc = 0, count = 0.  Out of place (the outputs must be other buffers of the    */
+/* same shape); the caller moves the origin by d * voxel.  One launch.                                           */
+int occd_scene_map_shift(const float* acc, const int32_t* count, float* acc_out, int32_t* count_out, int n_classes,
+                         int MX, int MY, int MZ, const int* d, void* stream);
+/* map (uint16 [n], e.g. occd_argmax_classes of acc) = unknown (a uint16 id) wherever count == 0: an unobserved */
+/* voxel's acc is all zero and would read as class 0.  One launch.                                               */
+int occd_scene_map_mark_unobserved(void* map, const int32_t* count, long long n, int unknown, void* stream);
+
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,

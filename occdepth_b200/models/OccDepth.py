@@ -855,6 +855,49 @@ class OccDepth(_Base, B200Module):
         return occupied_voxels(y, mask, voxel_size=voxel_size, vox_origin=vox_origin, capacity=capacity,
                                index0=lo * Y * Z, out=out)
 
+    # ---- scene maps: a sequence's class probabilities fused into one voxel map --------------------------------------
+    def fuse_frames(self, scene_map, frames, poses, fov=True):
+        """Integrate camera frames into `scene_map` (fusion.SceneMap): predict_frames(frames, probabilities=True) (a
+        single frame dict: predict_frame), then scene_map.integrate of item i with poses[i] (a single pose for a single
+        frame), in list order.  poses[i]: the rigid 4x4 taking frame i's output grid frame to the map frame -- KITTI:
+        world <- velodyne_t; NYU, whose grid is in world coordinates: map <- world.
+        The frame grid is the output grid: corner `vox_origin`, edge voxel_size / project_scale, dims
+        full_scene_size, stored [x][y][z] (NYU: [x][z][y]).  fov=True masks KITTI frames with their `fov_mask_1`
+        (kept per list position while the calibration stays the same, as predict_voxels keeps it); NYU has no mask.
+        Returns scene_map, or None when nothing ran (prepare()).  Not under enable_slab_parallel."""
+        if self.__dict__.get("slab_ctx") is not None:
+            raise NotImplementedError("OccDepth.fuse_frames: scene maps fuse whole frames, not the slab partition's "
+                                      "X-slabs")
+        one = isinstance(frames, Mapping)
+        pose_list = [poses] if one else poses
+        if not one and isinstance(frames, (list, tuple)) and len(pose_list) != len(frames):
+            raise ValueError("OccDepth.fuse_frames: %d poses for %d frames" % (len(pose_list), len(frames)))
+        from ..fusion import SceneMap, check_pose
+        if not isinstance(scene_map, SceneMap):
+            raise TypeError("OccDepth.fuse_frames: scene_map must be a fusion.SceneMap")
+        if scene_map.n_classes != self.n_classes:
+            raise ValueError("OccDepth.fuse_frames: the map holds %d classes, the model predicts %d"
+                             % (scene_map.n_classes, self.n_classes))
+        for p in pose_list:                    # refused before any frame runs
+            check_pose(p)
+        if one:
+            fs = [self._frame_checked(frames)]
+            res = self._run_frame(fs[0], True, None, None, False, True)
+        else:
+            fs = self._frames_checked(frames, probabilities=True)
+            res = self._run_frames(fs, len(fs), True, None, False, True)
+        if res is None:                        # prepare(): the plan was built, nothing ran
+            return None
+        _, probs = res
+        nyu = self.dataset == "NYU"
+        for b, f in enumerate(fs):
+            mask = None
+            if fov and not nyu:
+                mask = self._frame_fov_mask_1(f, None, None if one else b)
+            scene_map.integrate(probs[b], pose_list[b], f["vox_origin"], f["voxel_size"] / self.project_scale,
+                                axes="xzy" if nyu else "xyz", fov_mask=mask)
+        return scene_map
+
     def _frame_fov_mask_1(self, f, x_range=None, item=None):
         """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
         resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only; x_range = [lo, hi): only those X
