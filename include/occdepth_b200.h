@@ -506,6 +506,37 @@ int occd_scene_map_shift(const float* acc, const int32_t* count, float* acc_out,
 /* voxel's acc is all zero and would read as class 0.  One launch.                                               */
 int occd_scene_map_mark_unobserved(void* map, const int32_t* count, long long n, int unknown, void* stream);
 
+/* -------------------------------------------------------------------------------------------- */
+/* Camera views: each pixel's first visible voxel in a class map, as the camera sees it (the views the           */
+/* visualisation scripts draw from, scripts/visualization/kitti_vis_pred.py, NYU_vis_pred.py).  class_map: DEVICE */
+/* uint16 [B][GX*GY*GZ] (e.g. what occd_model_run_frames or occd_argmax_classes wrote, or a scene map's classes); */
+/* the grid's x, y, z have dims GX, GY, GZ, corner origin (HOST, 3 float64) and edge voxel; strides (HOST, 3     */
+/* long long): elements between x, y and z neighbours inside one map (KITTI [x][y][z]: {GY*GZ, GZ, 1}; NYU        */
+/* [x][z][y]: {GZ*GY, 1, GY}).  cameras (HOST, B*V*12 float64): camera v of map b at (b*V + v)*12, M row-major   */
+/* (3x3) then o (3): M = R^-1 K^-1 and o = -R^-1 t for E = [R | t] taking the grid frame to the camera frame     */
+/* (KITTI T_velo_2_cam, NYU world -> cam; R^-1 = R^T for a rigid E), K with last row (0, 0, 1), so o is the      */
+/* camera centre and a ray's parameter t is camera-frame z.  Pixel (u, v), u the column, is the image point (u, v) */
+/* (pixel centres at integers, as the reference's cam2pix rounds).  In float64 without FMA contraction:          */
+/*   d_r = ((M[r][0] u + M[r][1] v) + M[r][2]);  boundary i of axis a at t_a(i) = ((origin_a + i voxel) - o_a) r_a, */
+/*   r_a = 1 / d_a, recomputed from the integer index every time.  An axis with d_a == 0 is never stepped and keeps */
+/*   the ray only if origin_a <= o_a < origin_a + G_a voxel.  [t_lo, t_hi]: the slab test over the other axes;     */
+/*   t0 = max(t_lo, near), t_end = min(t_hi, far), a miss if t0 >= t_end.  First voxel: floor((o + t0 d - origin) */
+/*   / voxel) clamped into [0, G_a - 1].  Walk: a voxel of class c with c != empty and c != ignore is the hit;    */
+/*   else step the axis with the least next boundary time (ties: x, then y, then z), a miss when that time is >=   */
+/*   t_end, when the index leaves the grid, or after GX + GY + GZ + 3 voxels.  Entry time: t0 for the first voxel,  */
+/*   max(the previous entry time, the crossed boundary's time) after it.  Every min / max is a plain comparison.  */
+/* Outputs [B][V][H][W], each optional (NULL; at least one): cls uint16 = the hit's class (empty on a miss), depth  */
+/* float32 = its entry time rounded once (+inf on a miss), index int32 = its element offset in its map            */
+/* i*s_x + j*s_y + k*s_z, the flat index occd_occupied_voxels lists (-1 on a miss).  B*V <= 32 cameras travel in  */
+/* the kernel parameters (no host-to-device copy: the launch captures into a CUDA graph); at most 2^31 - 1 voxels */
+/* per map; near finite >= 0, far > near (+inf allowed).  One launch on `stream`; the same inputs give the same   */
+/* bytes.                                                                                                          */
+#define OCCD_RENDER_MAX_CAMERAS 32
+int occd_render_classes(const uint16_t* class_map, int B, int GX, int GY, int GZ, const long long* strides,
+                        const double* origin, double voxel, int V, const double* cameras, int W, int H, int empty,
+                        int ignore, double near_t, double far_t, uint16_t* cls, float* depth, int32_t* index,
+                        void* stream);
+
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */
 int occd_virtual_view_fwd(const void* in, void* out, const float* depth, int dtype, int B, int h, int w, int C,

@@ -25,30 +25,30 @@ from . import _lib
 MAX_CLASSES = 64        # the class-map kernels' LUT cap
 
 
-def _vec3(v, what):
+def _vec3(v, what, who="SceneMap"):
     a = np.asarray(v, dtype=np.float64).reshape(-1)
     if a.shape != (3,) or not np.isfinite(a).all():
-        raise ValueError("SceneMap: %s must hold 3 finite values" % what)
+        raise ValueError("%s: %s must hold 3 finite values" % (who, what))
     return a
 
 
-def check_pose(pose):
-    """(T, inverse(T)) in float64 of a finite, invertible 4x4 pose; ValueError otherwise"""
+def check_pose(pose, who="SceneMap.integrate", what="pose"):
+    """(T, inverse(T)) in float64 of a finite, invertible 4x4 pose; ValueError otherwise, naming `who` and `what`"""
     if isinstance(pose, torch.Tensor):
         pose = pose.detach().cpu().double().numpy()
     T = np.asarray(pose, dtype=np.float64)
     if T.shape != (4, 4) or not np.isfinite(T).all():
-        raise ValueError("SceneMap.integrate: pose must be a finite 4x4 matrix")
+        raise ValueError("%s: %s must be a finite 4x4 matrix" % (who, what))
     try:
         R = np.linalg.inv(T)
     except np.linalg.LinAlgError:
-        raise ValueError("SceneMap.integrate: pose is singular") from None
+        raise ValueError("%s: %s is singular" % (who, what)) from None
     if not np.isfinite(R).all():
-        raise ValueError("SceneMap.integrate: pose is singular")
+        raise ValueError("%s: %s is singular" % (who, what))
     return T, R
 
 
-def plane_layout(shape, axes):
+def plane_layout(shape, axes, who="SceneMap.integrate"):
     """(GX, GY, GZ) along the frame grid's x, y, z and their element strides, for one contiguous class plane of
     storage shape (D0, D1, D2): KITTI's output is [x][y][z] ("xyz"), NYU's [x][z][y] ("xzy")"""
     D0, D1, D2 = (int(v) for v in shape)
@@ -56,7 +56,7 @@ def plane_layout(shape, axes):
         return (D0, D1, D2), (D1 * D2, D2, 1)
     if axes == "xzy":
         return (D0, D2, D1), (D1 * D2, 1, D2)
-    raise ValueError("SceneMap.integrate: axes must be 'xyz' or 'xzy', got %r" % (axes,))
+    raise ValueError("%s: axes must be 'xyz' or 'xzy', got %r" % (who, axes))
 
 
 def frame_box(T, grid_origin, grid_voxel, grid_dims, origin, voxel, dims):
@@ -219,3 +219,19 @@ class SceneMap:
         with torch.cuda.device(self.device):
             return occupied_voxels(cmap, voxel_size=self.voxel, vox_origin=self.origin, capacity=capacity,
                                    ignore=int(unknown), out=out)
+
+    def render(self, E, K, size, inv_map=None, unknown=255, near=0.0, far=float("inf")):
+        """The map as a camera sees it: `render.render_classes` of `classes(inv_map, unknown)` with the map's origin
+        and voxel ("xyz").  E: the 4x4 map frame -> camera frame (or (1, V, 4, 4) for V cameras), K the 3x3
+        intrinsics, size = (W, H).  Unobserved voxels are transparent (ignore = unknown); class 0 is empty.
+        Returns View(classes, depth, index), each [1, V, H, W]."""
+        from .render import check_request, render_classes
+        unknown = int(unknown)
+        if not 0 <= unknown <= 65535:
+            raise ValueError("SceneMap.render: unknown must be a uint16 class id")
+        args = dict(E=E, K=K, size=size, grid_origin=self.origin, grid_voxel=self.voxel, ignore=unknown, near=near,
+                    far=far, who="SceneMap.render")
+        check_request(1, self.dims, **args)           # every refusal before classes() launches
+        cmap = self.classes(inv_map, unknown)
+        with torch.cuda.device(self.device):
+            return render_classes(cmap, **args)

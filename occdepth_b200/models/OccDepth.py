@@ -898,6 +898,64 @@ class OccDepth(_Base, B200Module):
                                 axes="xzy" if nyu else "xyz", fov_mask=mask)
         return scene_map
 
+    # ---- camera views: the prediction as each frame's cameras see it -----------------------------------------------
+    def predict_view(self, frame_or_frames, inv_map=None, views=(0,), near=0.0, far=float("inf")):
+        """predict_frame (a frame dict) or predict_frames (a list), through their class-map plan and key, then
+        `render.render_classes` of each frame's map from its own cameras: f["poses"][v] for v in `views` (KITTI: the
+        frame's T_velo_2_cam[v] and cam_k[v]; NYU: world -> cam, and with a depth map view 1 is the virtual right
+        view), at the frame's crop W x H.  The grid is the output grid: corner vox_origin, edge voxel_size /
+        project_scale, stored [x][y][z] (NYU [x][z][y]); class 0 is empty, 255 is transparent.  Returns (class map,
+        View) with the view [n, len(views), H, W], or None when nothing ran (prepare()).  Nothing synchronises.  At
+        most 32 frames x views; not under enable_slab_parallel."""
+        import operator
+        import numpy as np
+        from .. import render as R
+        if self.__dict__.get("slab_ctx") is not None:
+            raise NotImplementedError("OccDepth.predict_view: camera views render whole frames, not the slab "
+                                      "partition's X-slabs")
+        try:
+            views = tuple(operator.index(v) for v in views)
+        except TypeError:
+            raise ValueError("OccDepth.predict_view: views must be a sequence of view indices") from None
+        one = isinstance(frame_or_frames, Mapping)
+        if not one and not isinstance(frame_or_frames, (list, tuple)):
+            raise TypeError("OccDepth.predict_view: takes a camera frame dict or a list of them")
+        n = 1 if one else len(frame_or_frames)
+        if not views or n * len(views) > R.MAX_CAMERAS:
+            raise ValueError("OccDepth.predict_view: %d frames x %d views, 1 to %d cameras per call"
+                             % (n, len(views), R.MAX_CAMERAS))
+        fs = [self._frame_checked(frame_or_frames)] if one else self._frames_checked(frame_or_frames)
+        nyu = self.dataset == "NYU"
+        axes = "xzy" if nyu else "xyz"
+        storage = tuple(int(s) for s in self.full_scene_size)
+        reqs = []                              # every refusal before the plan runs
+        for f in fs:
+            if min(views) < 0 or max(views) >= len(f["poses"]):
+                raise ValueError("OccDepth.predict_view: views %r of a frame with %d cameras"
+                                 % (views, len(f["poses"])))
+            E = np.stack([f["poses"][v][0] for v in views])[None]
+            K = np.stack([f["poses"][v][1] for v in views])[None]
+            reqs.append(dict(E=E, K=K, size=(f["W"], f["H"]), grid_origin=f["vox_origin"],
+                             grid_voxel=f["voxel_size"] / self.project_scale, axes=axes, near=near, far=far,
+                             who="OccDepth.predict_view"))
+            R.check_request(1, storage, **reqs[-1])
+        y = self._run_frame(fs[0], True, inv_map) if one else self._run_frames(fs, len(fs), True, inv_map)
+        if y is None:                          # prepare(): the plan was built, nothing ran
+            return None
+        with torch.cuda.device(y.device):
+            same = all(np.array_equal(np.asarray(r["grid_origin"], np.float64),
+                                      np.asarray(reqs[0]["grid_origin"], np.float64)) and
+                       r["grid_voxel"] == reqs[0]["grid_voxel"] for r in reqs)
+            if same:                           # one launch for the whole batch (a KITTI sequence)
+                a = dict(reqs[0], E=np.concatenate([r["E"] for r in reqs]), K=np.concatenate([r["K"] for r in reqs]))
+                return y, R.render_classes(y, **a)
+            H, W = fs[0]["H"], fs[0]["W"]       # NYU frames with their own vox_origin: one launch per frame
+            out = R.View(*(torch.empty((len(fs), len(views), H, W), dtype=dt, device=y.device)
+                           for dt in (torch.uint16, torch.float32, torch.int32)))
+            for b, r in enumerate(reqs):
+                R.render_classes(y[b:b + 1], **r, out=R.View(*(x[b:b + 1] for x in out)))
+            return y, out
+
     def _frame_fov_mask_1(self, f, x_range=None, item=None):
         """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
         resolution (kitti_dataset.py:259-273 with scale_3d = 1), centre pixel only; x_range = [lo, hi): only those X
