@@ -536,6 +536,32 @@ int occd_render_classes(const uint16_t* class_map, int B, int GX, int GY, int GZ
                         const double* origin, double voxel, int V, const double* cameras, int W, int H, int empty,
                         int ignore, double near_t, double far_t, uint16_t* cls, float* depth, int32_t* index,
                         void* stream);
+/* Soft camera views: each ray composited front to back through per-voxel class probabilities instead of stopping  */
+/* at the first arg-max hit.  probs: DEVICE float16 [B][C][GX*GY*GZ] (what occd_model_run_frames_probs or          */
+/* occd_class_probs wrote), class planes contiguous, strides inside a plane as above; 1 <= C <= 64, channel `empty` */
+/* (< C) is the probability that the voxel is free.  class_map: DEVICE uint16 [B][GX*GY*GZ] with the same layout, or */
+/* NULL; a voxel whose class there is `ignore` is skipped (a scene map's unobserved voxels).  The walk is            */
+/* occd_render_classes' (same voxels, order, entry times t, near / far, exit and step cap), and no voxel stops it   */
+/* on its class.  Per visited voxel, in float32 with one correctly rounded operation per step (no FMA), T = 1,      */
+/* D = -0 (addition's identity, so a lone term keeps its sign) and S[c] = 0 at the start:                           */
+/*   skip it if class_map holds `ignore` there; e = p[empty]; skip it if e == 1 (no other channel is read);         */
+/*   S[c] = S[c] + T p[c] for every c != empty;  Tn = T e, w = T - Tn, D = D + w (float)t, T = Tn;                   */
+/*   stop after it once T <= t_min (t_min in [0, 1); 0 walks every voxel that does not empty T).                    */
+/* Voxel i is occupied with probability 1 - p_i(empty), independently, and then has class c with weight p_i(c): T   */
+/* is the chance the ray got past every voxel so far, T p_i(c) the chance voxel i is the first occupied one and has */
+/* class c, so the channels below sum to 1 when each voxel's probabilities do.  Probabilities are not clamped to    */
+/* [0, 1]; NaN propagates.  Outputs [B][V][H][W], each optional (NULL; at least one): opacity float32 = 1 - T;      */
+/* depth float32 = D / opacity, the expected entry depth of the first surface (+inf where opacity <= 0); probs_out */
+/* float16 [B][V][C][H][W]: channel empty = T (the ray leaves unblocked), channel c = S[c], each rounded once; cls */
+/* uint16 = the first largest float32 channel (from channel 0, replaced only on a strict >), remapped to           */
+/* uint16(lut[cls]) when lut (HOST, C ints) is given, as occd_argmax_classes remaps.  On one-hot probabilities with */
+/* the arg-max map as class_map this is occd_render_classes' cls and depth bit for bit, opacity 1 on a hit and 0   */
+/* on a miss.  Cameras, W, H, near and far as occd_render_classes.  One launch on `stream`; the same inputs give   */
+/* the same bytes.                                                                                                   */
+int occd_render_probs(const void* probs, int B, int C, int GX, int GY, int GZ, const long long* strides,
+                      const uint16_t* class_map, int ignore, int empty, const double* origin, double voxel, int V,
+                      const double* cameras, int W, int H, double near_t, double far_t, float t_min, const int* lut,
+                      uint16_t* cls, float* depth, float* opacity, void* probs_out, void* stream);
 
 /* virtual right view for single-view RGB-D inputs: OccDepth.generate_virtual_img (OccDepth.py:233-260). */
 /* in/out: channels-last [B][h][w][cs] of `dtype`; depth: fp32 [dh][dw] of batch item 0; bf_scale = bf / scale_2d */

@@ -186,6 +186,8 @@ SYMBOLS = {
     "occd_scene_map_mark_unobserved": (C.c_int, [_vp, _vp, _ll, _i, _vp]),
     "occd_render_classes": (C.c_int, [_vp, _i, _i, _i, _i, _vp, _vp, C.c_double, _i, _vp, _i, _i, _i, _i, C.c_double,
                                       C.c_double, _vp, _vp, _vp, _vp]),
+    "occd_render_probs": (C.c_int, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, C.c_double, _i, _vp, _i, _i,
+                                    C.c_double, C.c_double, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
     "occd_model_load": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
     "occd_model_info": (C.c_int, [_vp, C.POINTER(ModelGeom)]),
     "occd_model_run_frame": (C.c_int, [_vp, C.POINTER(Frame), _vp, _vp]),

@@ -125,7 +125,7 @@ const Entry kEntries[] = {
     OCCD_ENTRY(occd_virtual_view_items_fwd), OCCD_ENTRY(occd_stage_camera_u8_cl),
     OCCD_ENTRY(occd_class_probs),           OCCD_ENTRY(occd_scene_map_integrate),
     OCCD_ENTRY(occd_scene_map_shift),       OCCD_ENTRY(occd_scene_map_mark_unobserved),
-    OCCD_ENTRY(occd_render_classes),
+    OCCD_ENTRY(occd_render_classes),        OCCD_ENTRY(occd_render_probs),
     // take a stream like the launches (occd_model_batch is bound like them), so they have a signature here; their
     // model handle can only be NULL
     OCCD_ENTRY(occd_model_run_frame_conf),  OCCD_ENTRY(occd_model_run_frames),

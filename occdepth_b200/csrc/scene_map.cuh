@@ -49,6 +49,35 @@ SMAP_HD double div_rn(double a, double b) {
   return a / b;
 #endif
 }
+// the float32 twins: one correctly rounded IEEE single operation each, never contracted into an FMA
+SMAP_HD float fmul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+SMAP_HD float fadd_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+SMAP_HD float fsub_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+SMAP_HD float fdiv_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fdiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
 
 // element offset inside a class plane of the frame voxel that map voxel (i, j, k) falls in, or -1 when its centre
 // lies outside the frame grid.  f[3] receives the frame index (also when outside; NaN-free since R is finite)

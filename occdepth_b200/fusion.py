@@ -235,3 +235,29 @@ class SceneMap:
         cmap = self.classes(inv_map, unknown)
         with torch.cuda.device(self.device):
             return render_classes(cmap, **args)
+
+    def render_probs(self, E, K, size, inv_map=None, unknown=255, near=0.0, far=float("inf"),
+                     min_transmittance=1e-4):
+        """The fused posterior as a camera sees it: `render.render_probs` of `classes(inv_map, unknown,
+        probabilities=True)`, with that map as class_map and ignore = unknown, so unobserved voxels are transparent
+        (rather than opaque at 1 / C per class); class 0 is empty.  inv_map remaps the returned classes only.
+        Returns SoftView(classes, depth, opacity, probs), each [1, V, ...]."""
+        from .render import check_request, render_probs
+        unknown = int(unknown)
+        if not 0 <= unknown <= 65535:
+            raise ValueError("SceneMap.render_probs: unknown must be a uint16 class id")
+        t_min = float(np.float32(min_transmittance))
+        if not 0.0 <= t_min < 1.0:
+            raise ValueError("SceneMap.render_probs: min_transmittance must be in [0, 1), got %r" % (min_transmittance,))
+        lut = None
+        if inv_map is not None:
+            lut = np.asarray(inv_map).reshape(-1)
+            if lut.shape != (self.n_classes,):
+                raise ValueError("SceneMap.render_probs: inv_map must hold one label id per class (%d)"
+                                 % self.n_classes)
+        args = dict(E=E, K=K, size=size, grid_origin=self.origin, grid_voxel=self.voxel, ignore=unknown, near=near,
+                    far=far, who="SceneMap.render_probs")
+        check_request(1, self.dims, **args, n_classes=self.n_classes)    # every refusal before classes() launches
+        cmap, probs = self.classes(inv_map, unknown, probabilities=True)
+        with torch.cuda.device(self.device):
+            return render_probs(probs, **args, class_map=cmap, min_transmittance=t_min, inv_map=lut)

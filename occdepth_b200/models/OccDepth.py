@@ -899,14 +899,18 @@ class OccDepth(_Base, B200Module):
         return scene_map
 
     # ---- camera views: the prediction as each frame's cameras see it -----------------------------------------------
-    def predict_view(self, frame_or_frames, inv_map=None, views=(0,), near=0.0, far=float("inf")):
+    def predict_view(self, frame_or_frames, inv_map=None, views=(0,), near=0.0, far=float("inf"), soft=False,
+                     min_transmittance=1e-4):
         """predict_frame (a frame dict) or predict_frames (a list), through their class-map plan and key, then
         `render.render_classes` of each frame's map from its own cameras: f["poses"][v] for v in `views` (KITTI: the
         frame's T_velo_2_cam[v] and cam_k[v]; NYU: world -> cam, and with a depth map view 1 is the virtual right
         view), at the frame's crop W x H.  The grid is the output grid: corner vox_origin, edge voxel_size /
         project_scale, stored [x][y][z] (NYU [x][z][y]); class 0 is empty, 255 is transparent.  Returns (class map,
         View) with the view [n, len(views), H, W], or None when nothing ran (prepare()).  Nothing synchronises.  At
-        most 32 frames x views; not under enable_slab_parallel."""
+        most 32 frames x views; not under enable_slab_parallel.
+        soft=True: the same frames through predict_frame(s)' probabilities plan and key instead, then
+        `render.render_probs` of each frame's float16 probabilities (empty = class 0, `min_transmittance`, inv_map
+        remapping the view's classes as it remaps the map): returns (class map, probs, SoftView)."""
         import operator
         import numpy as np
         from .. import render as R
@@ -938,23 +942,45 @@ class OccDepth(_Base, B200Module):
             reqs.append(dict(E=E, K=K, size=(f["W"], f["H"]), grid_origin=f["vox_origin"],
                              grid_voxel=f["voxel_size"] / self.project_scale, axes=axes, near=near, far=far,
                              who="OccDepth.predict_view"))
-            R.check_request(1, storage, **reqs[-1])
+            R.check_request(1, storage, **reqs[-1], n_classes=self.n_classes if soft else None)
+        if soft:
+            t_min = float(np.float32(min_transmittance))
+            if not 0.0 <= t_min < 1.0:
+                raise ValueError("OccDepth.predict_view: min_transmittance must be in [0, 1), got %r"
+                                 % (min_transmittance,))
+            lut = self._class_lut(inv_map)
+            res = self._run_frame(fs[0], True, inv_map, None, False, True) if one else \
+                self._run_frames(fs, len(fs), True, inv_map, False, True)
+            if res is None:                    # prepare(): the plan was built, nothing ran
+                return None
+            return res[0], res[1], self._frame_views(R.render_probs, res[1], reqs, min_transmittance=t_min,
+                                                     inv_map=lut)
         y = self._run_frame(fs[0], True, inv_map) if one else self._run_frames(fs, len(fs), True, inv_map)
         if y is None:                          # prepare(): the plan was built, nothing ran
             return None
-        with torch.cuda.device(y.device):
+        return y, self._frame_views(R.render_classes, y, reqs)
+
+    @staticmethod
+    def _frame_views(render, x, reqs, **kw):
+        """`render` (render.render_classes or render_probs) of x [n, ...] from frame i's cameras reqs[i]: one launch
+        when the frames share their grid (a KITTI sequence), else one per frame (NYU frames with their own
+        vox_origin), each into its slice of the same outputs"""
+        import numpy as np
+        with torch.cuda.device(x.device):
             same = all(np.array_equal(np.asarray(r["grid_origin"], np.float64),
                                       np.asarray(reqs[0]["grid_origin"], np.float64)) and
                        r["grid_voxel"] == reqs[0]["grid_voxel"] for r in reqs)
-            if same:                           # one launch for the whole batch (a KITTI sequence)
+            if same:
                 a = dict(reqs[0], E=np.concatenate([r["E"] for r in reqs]), K=np.concatenate([r["K"] for r in reqs]))
-                return y, R.render_classes(y, **a)
-            H, W = fs[0]["H"], fs[0]["W"]       # NYU frames with their own vox_origin: one launch per frame
-            out = R.View(*(torch.empty((len(fs), len(views), H, W), dtype=dt, device=y.device)
-                           for dt in (torch.uint16, torch.float32, torch.int32)))
-            for b, r in enumerate(reqs):
-                R.render_classes(y[b:b + 1], **r, out=R.View(*(x[b:b + 1] for x in out)))
-            return y, out
+                return render(x, **a, **kw)
+            first = render(x[:1], **reqs[0], **kw)
+            out = type(first)(*(torch.empty((len(reqs),) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+                                for t in first))
+            for o, t in zip(out, first):
+                o[:1].copy_(t)
+            for b, r in enumerate(reqs[1:], 1):
+                render(x[b:b + 1], **r, **kw, out=type(first)(*(o[b:b + 1] for o in out)))
+            return out
 
     def _frame_fov_mask_1(self, f, x_range=None, item=None):
         """bool [N] on the device: the first view's `fov_mask_1` of camera frame `f`, i.e. vox2pix at the output
